@@ -282,6 +282,18 @@ int kb200_host_cholqr_factors(int p, const double *G, double *R, double *Rinv);
 int kb200_host_householder_signs(int p, const double *top, double *s);
 /* y = A x.  variant: 0 auto, 1 row-per-thread LDG kernel, 2 TMA-staged kernel. */
 int kb200_spmv_csr(void *ctx, void *csr, const void *x, void *y, int variant);
+/* W = A X on row-major n x p device panels (the SpMM of block_gmres).  variant: 0 auto (what block_gmres runs),
+ * 1 p-threads-per-row kernel, 2 TMA-staged (p in {2,4,8,16,32} and a fitting tile plan, else -1 and last_error).
+ * Synchronises before returning. */
+int kb200_spmm_csr(void *ctx, void *csr, int p, const void *X, void *Y, int variant);
+/* One panel operation of a block workspace on device pointers, which may point into larger allocations (the
+ * Householder fallback of the panel QR runs them on row ranges).  op 0: G = L^T Out (L = Next, or Out when Next is
+ * NULL); 1: Out = beta Out + alpha In S; 2: op 1 then op 0 in one pass.  S, G: p x p column-major, device.
+ * 1 <= rows <= the workspace's n.  path 0: the solver's own dispatch; 1 DMMA (Float64, p in {8,16,32}); 2 SIMT;
+ * 3 SIMT with prefetch; 4 SIMT alternative lanes-per-row (p in {8,16}); 5 tiled generic (any p).  Unavailable
+ * combinations return -1.  Synchronises before returning. */
+int krylov_b200_block_panel_op(void *ws, int op, int path, int rows, double alpha, const void *In, const void *S,
+                               double beta, void *Out, const void *Next, void *G);
 /* staging plan of a CSR object: out[0]=ntiles out[1]=tile_cap out[2]=max_row out[3]=tma_ok out[4]=stages out[5]=grid out[6]=smem_bytes */
 int kb200_csr_plan(void *csr, long long *out7);
 

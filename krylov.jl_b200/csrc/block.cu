@@ -717,10 +717,15 @@ template <class T, int P> static void launch_spmm_tma(Ctx& c, const Csr<T>& A, c
   const int grid = std::min(std::min(occ, A.ctas_per_sm) * sm_count(), std::max(1, A.ntiles));
   spmm_tma_kernel<T, P><<<grid, kTileThreads, A.smem_bytes, c.stream>>>(A, X, Y);
 }
-template <class T> static void k_spmm(Ctx& c, const Csr<T>& A, int p, const T* X, T* Y) {
+// variant: 0 auto (what block_gmres runs), 1 the p-threads-per-row kernel, 2 TMA-staged (throws when p has no
+// specialization or the tile plan does not fit)
+template <class T> static void k_spmm(Ctx& c, const Csr<T>& A, int p, const T* X, T* Y, int variant = 0) {
+  if (variant < 0 || variant > 2) throw std::runtime_error("SpMM variant must be 0, 1 or 2");
+  if (variant == 2 && !A.tma_ok) throw std::runtime_error("TMA-staged SpMM requested but the tile plan does not fit shared memory");
   if (A.n <= 0) return;
   static const char* spmm_env = getenv("KB200_SPMM");          // "rows": force the generic kernel (A/B runs)
-  if (A.tma_ok && !getenv("KB200_BLOCK_GENERIC") && !(spmm_env && !strcmp(spmm_env, "rows"))) {
+  const bool auto_tma = variant == 0 && A.tma_ok && !getenv("KB200_BLOCK_GENERIC") && !(spmm_env && !strcmp(spmm_env, "rows"));
+  if (variant == 2 || auto_tma) {
     bool done = true;
     switch (p) {
       case 2: launch_spmm_tma<T, 2>(c, A, X, Y); break;
@@ -731,6 +736,7 @@ template <class T> static void k_spmm(Ctx& c, const Csr<T>& A, int p, const T* X
       default: done = false;
     }
     if (done) { KB_CUDA(cudaGetLastError()); c.launches++; return; }
+    if (variant == 2) throw std::runtime_error("TMA-staged SpMM exists for p = 2, 4, 8, 16, 32 only");
   }
   spmm_rows_kernel<T><<<stream_grid((long long)A.n * p, 1, 8), kBlock, 0, c.stream>>>(A, p, X, Y);
   KB_CUDA(cudaGetLastError()); c.launches++;
@@ -739,16 +745,15 @@ template <class T> static void k_rows_diag(Ctx& c, int n, int p, const T* d, con
   rows_diag_kernel<T><<<stream_grid((long long)n * p, 1, 8), kBlock, 0, c.stream>>>((long long)n * p, p, d, in, out, ldiv ? 1 : 0);
   KB_CUDA(cudaGetLastError()); c.launches++;
 }
-// tensor-core dispatch (Float64, p = 8 / 16 / 32).  KB200_BLOCK_MMA=0 keeps the SIMT kernels (A/B runs, tests),
-// KB200_BLOCK_MMA=16 only p = 16 / 32 (p = 8 stays on the SIMT kernel)
+// tensor-core dispatch (Float64, p = 8 / 16 / 32).  ws.mma_mode (KB200_BLOCK_MMA) 0 keeps the SIMT kernels (A/B
+// runs, tests), 16 only p = 16 / 32 (p = 8 stays on the SIMT kernel)
 template <class T, bool UPDATE, bool GRAM>
 static bool launch_mma(BlockWorkspace<T>&, T, const T*, const T*, T, T*, const T*, T*, int) { return false; }
 template <bool UPDATE, bool GRAM>
 static bool launch_mma_f64(BlockWorkspace<double>& ws, double alpha, const double* In, const double* S, double beta, double* Out,
                            const double* Next, double* G, int rows) {
   Ctx& c = ws.ctx;
-  static const char* env = getenv("KB200_BLOCK_MMA");
-  static const int mode = env ? atoi(env) : 1;
+  const int mode = ws.mma_mode;
   if (mode == 0) return false;
   const int p = ws.p;
   if (!(p == 16 || p == 32 || (p == 8 && mode != 16))) return false;
@@ -774,9 +779,9 @@ static bool launch_fast(BlockWorkspace<T>& ws, T alpha, const T* In, const T* S,
   if (ws.generic_kernels) return false;
   if (launch_mma<T, UPDATE, GRAM>(ws, alpha, In, S, beta, Out, Next, G, rows)) return true;
   const int grid = ws.fast_grid;
-  // KB200_FAST_TPR=alt selects the second lanes-per-row shape of P = 8 / 16 (sweeps, profiles/sweep_block.py)
-  static const bool alt = getenv("KB200_FAST_TPR") != nullptr;
-  static const bool prefetch = getenv("KB200_FAST_PREFETCH") != nullptr;   // software-pipelined row loads (sweeps)
+  // the second lanes-per-row shape of P = 8 / 16 (sweeps, profiles/sweep_block.py) and software-pipelined row loads
+  const bool alt = ws.fast_alt_tpr;
+  const bool prefetch = ws.fast_prefetch;
 #define KB_FAST(PV, TV)                                                                                                   \
   do {                                                                                                                    \
     if (prefetch)                                                                                                         \
@@ -809,13 +814,15 @@ template <class T> static void k_panel_tn(BlockWorkspace<T>& ws, const T* V, con
   panel_tn_kernel<T><<<ws.grid, kBlock, smem, c.stream>>>(rows, p, V, Q, ws.part, c.tickets + 6, G);
   KB_CUDA(cudaGetLastError()); c.launches++;
 }
-template <class T> static void k_panel_nn_tn(BlockWorkspace<T>& ws, T alpha, const T* In, const T* S, T beta, T* Out, const T* Next, T* G) {
+template <class T> static void k_panel_nn_tn(BlockWorkspace<T>& ws, T alpha, const T* In, const T* S, T beta, T* Out, const T* Next, T* G,
+                                             int rows = -1) {
   Ctx& c = ws.ctx;
   const int p = ws.p;
-  if (launch_fast<T, true, true>(ws, alpha, In, S, beta, Out, Next, G, ws.n)) return;
+  if (rows < 0) rows = ws.n;
+  if (launch_fast<T, true, true>(ws, alpha, In, S, beta, Out, Next, G, rows)) return;
   const size_t smem = sizeof(T) * ((size_t)3 * kPanelTileElems + (size_t)p * p);
   ensure_dyn_smem((const void*)panel_nn_tn_kernel<T>, 96 * 1024);
-  panel_nn_tn_kernel<T><<<ws.grid, kBlock, smem, c.stream>>>(ws.n, p, alpha, In, S, beta, Out, Next, ws.part, c.tickets + 6, G);
+  panel_nn_tn_kernel<T><<<ws.grid, kBlock, smem, c.stream>>>(rows, p, alpha, In, S, beta, Out, Next, ws.part, c.tickets + 6, G);
   KB_CUDA(cudaGetLastError()); c.launches++;
 }
 template <class T> static void k_panel_nn(BlockWorkspace<T>& ws, T alpha, const T* In, const T* S, T beta, T* Out, int rows = -1) {
@@ -1020,6 +1027,10 @@ template <class T> BlockWorkspace<T>* block_ws_create(int m, int n, int p, int m
     ws->grid = panel_grid<T>(n, p);
     ws->fast_grid = std::max(1, std::min(sm_count() * 2, (int)(((long long)n + kBlock - 1) / kBlock)));
     ws->generic_kernels = getenv("KB200_BLOCK_GENERIC") != nullptr;     // tests: force the tiled any-p kernels
+    const char* mma_env = getenv("KB200_BLOCK_MMA");
+    ws->mma_mode = mma_env ? atoi(mma_env) : 1;
+    ws->fast_prefetch = getenv("KB200_FAST_PREFETCH") != nullptr;
+    ws->fast_alt_tpr = getenv("KB200_FAST_TPR") != nullptr;
     // partial Gram matrices: one p x p block per CTA of whichever panel kernel runs (tiled, register-resident, or the
     // tensor-core kernels with up to 3 CTAs of 8 warps per SM, one 8-row tile per warp)
     const int mma_grid = std::max(1, std::min(sm_count() * 3, (int)((((long long)n + 7) / 8 + kMmaWarps - 1) / kMmaWarps)));
@@ -1067,6 +1078,49 @@ template <class T> void block_warm_start(BlockWorkspace<T>& ws, const T* X0_colm
 template <class T> void block_get_X(BlockWorkspace<T>& ws, T* X_colmajor_dev) {
   k_transpose<T>(ws.ctx, ws.n, ws.p, ws.X, X_colmajor_dev);
   ws.ctx.sync();
+}
+
+template <class T> void block_spmm(Ctx& c, const Csr<T>& A, int p, const T* X, T* Y, int variant) {
+  if (p < 1 || p > kMaxBlockP) throw std::runtime_error("block size p must be in 1..32");
+  k_spmm<T>(c, A, p, X, Y, variant);
+  c.sync();
+}
+
+// One panel operation through the solver's own launchers.  path 0 keeps the workspace's dispatch; the others set
+// the dispatch fields for this call only: 1 DMMA, 2 SIMT, 3 SIMT with prefetch, 4 SIMT with the alternative
+// lanes-per-row shape, 5 tiled.
+template <class T>
+void block_panel_op(BlockWorkspace<T>& ws, int op, int path, int rows, T alpha, const T* In, const T* S, T beta, T* Out, const T* Next,
+                    T* G) {
+  const int p = ws.p;
+  const bool simt_p = p == 2 || p == 4 || p == 8 || p == 16 || p == 32;
+  bool ok = path == 0 || path == 5;
+  if (path == 1) ok = sizeof(T) == sizeof(double) && (p == 8 || p == 16 || p == 32);
+  if (path == 2 || path == 3) ok = simt_p;
+  if (path == 4) ok = p == 8 || p == 16;
+  if (!ok) throw std::runtime_error("no panel kernel for this path, dtype and block size");
+  if (op < 0 || op > 2) throw std::runtime_error("op must be 0, 1 or 2");
+  if (rows < 1 || rows > ws.n) throw std::runtime_error("rows must be in 1..n of the workspace");
+  if (!Out || (op != 1 && !G) || (op != 0 && (!In || !S))) throw std::runtime_error("missing operand");
+  const bool generic = ws.generic_kernels, prefetch = ws.fast_prefetch, alt = ws.fast_alt_tpr;
+  const int mma = ws.mma_mode;
+  if (path != 0) {
+    ws.generic_kernels = path == 5;
+    ws.mma_mode = path == 1 ? 1 : 0;
+    ws.fast_prefetch = path == 3;
+    ws.fast_alt_tpr = path == 4;
+  }
+  auto restore = [&]() { ws.generic_kernels = generic; ws.fast_prefetch = prefetch; ws.fast_alt_tpr = alt; ws.mma_mode = mma; };
+  try {
+    if (op == 0) k_panel_tn<T>(ws, Next ? Next : Out, Out, G, rows);
+    else if (op == 1) k_panel_nn<T>(ws, alpha, In, S, beta, Out, rows);
+    else k_panel_nn_tn<T>(ws, alpha, In, S, beta, Out, Next, G, rows);
+    ws.ctx.sync();
+  } catch (...) {
+    restore();
+    throw;
+  }
+  restore();
 }
 
 // ===========================================================================
@@ -1277,7 +1331,9 @@ void block_gmres_solve(BlockWorkspace<T>& ws, const BlockOp<T>& A, const T* B_co
   template void block_ws_destroy<T>(BlockWorkspace<T>*);                                                         \
   template void block_gmres_solve<T>(BlockWorkspace<T>&, const BlockOp<T>&, const T*, const BlockOp<T>&, const BlockOp<T>&, const SolveOpts&); \
   template void block_warm_start<T>(BlockWorkspace<T>&, const T*);                                               \
-  template void block_get_X<T>(BlockWorkspace<T>&, T*);
+  template void block_get_X<T>(BlockWorkspace<T>&, T*);                                                          \
+  template void block_spmm<T>(Ctx&, const Csr<T>&, int, const T*, T*, int);                                      \
+  template void block_panel_op<T>(BlockWorkspace<T>&, int, int, int, T, const T*, const T*, T, T*, const T*, T*);
 INST(double)
 INST(float)
 #undef INST

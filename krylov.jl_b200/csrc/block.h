@@ -41,7 +41,12 @@ struct BlockWorkspace {
   T *hX = nullptr, *hY = nullptr;                       // pinned panels for host block callbacks
   int grid = 1;                                         // tiled generic kernels
   int fast_grid = 1;                                    // register-resident kernels (p = 2, 4, 8, 16, 32)
-  bool generic_kernels = false;
+  // panel-kernel choice: set from the environment by block_ws_create (A/B runs, sweeps), overridden for one call by
+  // block_panel_op
+  bool generic_kernels = false;                         // KB200_BLOCK_GENERIC: the tiled any-p kernels only
+  int mma_mode = 1;                                     // KB200_BLOCK_MMA: 0 no DMMA, 16 DMMA for p = 16 / 32 only
+  bool fast_prefetch = false;                           // KB200_FAST_PREFETCH: software-pipelined SIMT row loads
+  bool fast_alt_tpr = false;                            // KB200_FAST_TPR: second lanes-per-row shape of p = 8 / 16
   long long qr_fallbacks = 0;
 };
 
@@ -52,5 +57,10 @@ template <class T> void block_gmres_solve(BlockWorkspace<T>& ws, const BlockOp<T
                                           const BlockOp<T>& N, const SolveOpts& o);
 template <class T> void block_warm_start(BlockWorkspace<T>& ws, const T* X0_colmajor_dev);
 template <class T> void block_get_X(BlockWorkspace<T>& ws, T* X_colmajor_dev);
+// Single kernels of the solver, for tests (kb200_spmm_csr, krylov_b200_block_panel_op in krylov_b200.h).  Both
+// synchronise before returning and throw on a combination that has no kernel.
+template <class T> void block_spmm(Ctx& c, const Csr<T>& A, int p, const T* X, T* Y, int variant);
+template <class T> void block_panel_op(BlockWorkspace<T>& ws, int op, int path, int rows, T alpha, const T* In, const T* S, T beta,
+                                       T* Out, const T* Next, T* G);
 
 }  // namespace kb

@@ -1067,6 +1067,33 @@ int kb200_spmv_csr(void* ctx, void* csr, const void* x, void* y, int variant) {
   } catch (const std::exception& e) { return fail("kb200_spmv_csr", e); }
 }
 
+int kb200_spmm_csr(void* ctx, void* csr, int p, const void* X, void* Y, int variant) {
+  try {
+    if (!ctx || !csr) throw std::runtime_error("bad arguments");
+    Ctx& c = *(Ctx*)ctx;
+    CsrAny* a = (CsrAny*)csr;
+    if (a->dtype == KRYLOV_FLOAT64) block_spmm<double>(c, a->d, p, (const double*)X, (double*)Y, variant);
+    else block_spmm<float>(c, a->f, p, (const float*)X, (float*)Y, variant);
+    return 0;
+  } catch (const std::exception& e) { return fail("kb200_spmm_csr", e); }
+}
+
+int krylov_b200_block_panel_op(void* ws, int op, int path, int rows, double alpha, const void* In, const void* S, double beta,
+                               void* Out, const void* Next, void* G) {
+  try {
+    Handle* h = lookup_block(ws);
+    if (!h) return fail("krylov_b200_block_panel_op", "unknown block workspace handle");
+    KB_CUDA(cudaSetDevice(ctx_of(h).device));
+    if (h->dtype == KRYLOV_FLOAT64)
+      block_panel_op<double>(*BW<double>(h), op, path, rows, alpha, (const double*)In, (const double*)S, beta, (double*)Out,
+                             (const double*)Next, (double*)G);
+    else
+      block_panel_op<float>(*BW<float>(h), op, path, rows, (float)alpha, (const float*)In, (const float*)S, (float)beta, (float*)Out,
+                            (const float*)Next, (float*)G);
+    return 0;
+  } catch (const std::exception& e) { return fail("krylov_b200_block_panel_op", e); }
+}
+
 int kb200_csr_plan(void* csr, long long* out) {
   CsrAny* a = (CsrAny*)csr;
   if (!a || !out) return -1;

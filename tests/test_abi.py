@@ -29,6 +29,19 @@ def test_header_symbols_are_exported_and_bound():
         assert n in _lib.SIGNATURES, f"{n} has no ctypes signature"
 
 
+def test_signature_argument_counts_match_header():
+    """Each ctypes signature takes as many arguments as the header's prototype (the kernel test entry points
+    kb200_spmm_csr and krylov_b200_block_panel_op among them)."""
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "krylov_b200.h")).read(), flags=re.S)
+    protos = dict(re.findall(r"\b((?:krylov|kb200)_[a-z0-9_A-Z]+)\s*\(([^()]*)\)\s*;", src))
+    for name in ("kb200_spmm_csr", "krylov_b200_block_panel_op", "kb200_spmv_csr"):
+        assert name in protos
+    for name, params in protos.items():
+        params = params.strip()
+        n = 0 if params in ("", "void") else params.count(",") + 1
+        assert len(_lib.SIGNATURES[name][1]) == n, name
+
+
 def test_default_option_sentinels():               # test_api.c:105-118
     L = _lib.lib()
     o = L.krylov_default_options()

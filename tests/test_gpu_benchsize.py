@@ -11,6 +11,9 @@ import scipy.sparse as sp
 
 pytestmark = pytest.mark.gpu
 F64_TOL = 1e-6
+# block_gmres! on the host oracle (one thread): p = 8 on get_div_grad(215) takes about 14 s for 2 block iterations and
+# 33 s for 4; p = 32 on get_div_grad(127) about 40 s for 2.
+BLOCK_ITERS_P8, BLOCK_ITERS_P32 = 4, 2
 
 
 def _mat(csr):
@@ -98,6 +101,28 @@ def test_cfg4_bicgstab_f32_random5e6_history_matches_oracle(kb, O):
     assert np.all(devA <= tol + 1e-6), devA.max()
     assert devA[:3].max() <= 1e-4, devA[:3]
     ws.free()
+
+
+@pytest.mark.parametrize("N,p,iters", [(215, 8, BLOCK_ITERS_P8), (127, 32, BLOCK_ITERS_P32)])
+def test_block_gmres_benchsize_history_matches_oracle(kb, O, N, p, iters):
+    """block_gmres! at the sizes profiles/bench_block.py times: p = 8 on get_div_grad(215) (n = 9 938 375, n = 7 mod 8:
+    ragged last tiles of every panel kernel, hundreds of partial Gram blocks per reduction) and p = 32 on
+    get_div_grad(127) (n = 2 048 383), a fixed number of block iterations (atol = rtol = 0), seeded random B.
+    Iteration count, status and the residual history within 1e-6 of the oracle, X within 1e-6."""
+    from krylov_b200 import problems as P
+    A = _mat(P.div_grad_csr(N))
+    n = N ** 3
+    B = np.random.default_rng(N).standard_normal((n, p))
+    Xo, so = O.block_gmres(A, B, memory=iters, atol=0.0, rtol=0.0, itmax=iters)
+    assert so["niter"] == iters
+    ws = kb.BlockGmresWorkspace(n, n, p, memory=iters)
+    ws.solve(A, B, atol=0.0, rtol=0.0, itmax=iters, history=True)
+    st, X = ws.stats, ws.x
+    ws.free()
+    assert st.niter == so["niter"] and st.status == so["status"]
+    assert len(st.residuals) == len(so["residuals"])
+    assert _rel(st.residuals, so["residuals"]).max() <= F64_TOL
+    assert np.linalg.norm(X - Xo) <= F64_TOL * np.linalg.norm(Xo)
 
 
 def test_device_assembled_random_csr_equals_scipy_assembly(kb):

@@ -27,38 +27,31 @@ def _check(st, X, so, Xo, tol=1e-6):
     assert np.linalg.norm(X - Xo) <= 1e-6 * np.linalg.norm(Xo)
 
 
-@pytest.mark.parametrize("generic", [False, True, "prefetch", "simt", "mma8"])
-@pytest.mark.parametrize("p", [1, 2, 3, 4, 5, 8, 16, 32])
-def test_block_gmres_block_sizes(kb, O, p, generic, monkeypatch):
+def _with_n729(cases):
+    """kron_unsymmetric(8) (n = 512) under the case's own id, kron_unsymmetric(9) (n = 729) under id + "-729"."""
+    out = []
+    for N in (8, 9):
+        for c in cases:
+            vals = c if isinstance(c, tuple) else (c,)
+            ident = "-".join(str(v) for v in vals) + ("-729" if N == 9 else "")
+            out.append(pytest.param(*vals, N, id=ident))
+    return out
+
+
+@pytest.mark.parametrize("p,generic,N", _with_n729([(p, g) for g in (False, True, "prefetch", "simt", "mma8")
+                                                     for p in (1, 2, 3, 4, 5, 8, 16, 32)]))
+def test_block_gmres_block_sizes(kb, O, p, generic, N, monkeypatch):
     """Float64 p = 8, 16, 32 run the tensor-core panel kernels (mma.sync m8n8k4.f64; "simt" = KB200_BLOCK_MMA=0 keeps
     every p on the register-resident SIMT kernels, "mma8" = KB200_BLOCK_MMA=16 only p = 8); p = 2, 4 the SIMT ones (with
     or without software-pipelined row loads); every other p (and KB200_BLOCK_GENERIC=1) the tiled any-p kernels.
-    All against the oracle."""
+    All against the oracle, at n = 512 (a multiple of every tile and pass width) and n = 729 (ragged last tiles)."""
     if generic in ("simt", "mma8") and p not in (8, 16, 32):
         pytest.skip("variant only changes p = 8 / 16 / 32")
-    if generic in ("prefetch", "simt", "mma8"):
-        import subprocess, sys, textwrap
-        # the switch is read once per process: run this variant in a child
-        code = textwrap.dedent(f"""
-            import sys; sys.path[:0] = {[ROOT, os.path.join(ROOT, "krylov.jl_b200"), os.path.join(ROOT, "tests")]!r}
-            import numpy as np, scipy.sparse as sp
-            import krylov_b200 as kb
-            from oracle import oracle as O
-            A, _ = O.kron_unsymmetric(8); A = sp.csr_matrix(A)
-            B = A @ np.random.default_rng(0).standard_normal((A.shape[0], {p}))
-            X, st = kb.block_gmres(A, B, memory=6, history=True)
-            Xo, so = O.block_gmres(A, B, memory=6)
-            assert st.niter == so["niter"] and st.status == so["status"]
-            assert np.allclose(st.residuals, so["residuals"], rtol=1e-6, atol=1e-9 * so["residuals"][0])
-            assert np.linalg.norm(X - Xo) <= 1e-6 * np.linalg.norm(Xo)
-        """)
-        extra = {"prefetch": dict(KB200_FAST_PREFETCH="1"), "simt": dict(KB200_BLOCK_MMA="0"), "mma8": dict(KB200_BLOCK_MMA="16")}[generic]
-        out = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **extra), capture_output=True, text=True)
-        assert out.returncode == 0, out.stderr[-2000:]
-        return
-    if generic:
-        monkeypatch.setenv("KB200_BLOCK_GENERIC", "1")
-    A, _ = O.kron_unsymmetric(8)
+    env = {True: dict(KB200_BLOCK_GENERIC="1"), "prefetch": dict(KB200_FAST_PREFETCH="1"), "simt": dict(KB200_BLOCK_MMA="0"),
+           "mma8": dict(KB200_BLOCK_MMA="16")}.get(generic, {})
+    for k, v in env.items():                    # read when the workspace is created
+        monkeypatch.setenv(k, v)
+    A, _ = O.kron_unsymmetric(N)
     A = sp.csr_matrix(A)
     B = A @ _rhs(A.shape[0], p)
     X, st = kb.block_gmres(A, B, memory=6, history=True)
@@ -114,13 +107,13 @@ def test_block_gmres_float32_callbacks_and_torch(kb, O):
         kb.block_gmres(A, B, callback=lambda w: "string")
 
 
-@pytest.mark.parametrize("p", [3, 4, 8])
-def test_device_householder_path_matches_oracle_on_full_rank_blocks(kb, O, p, monkeypatch):
+@pytest.mark.parametrize("p,N", _with_n729([3, 4, 8, 16, 32]))
+def test_device_householder_path_matches_oracle_on_full_rank_blocks(kb, O, p, N, monkeypatch):
     """KB200_QR_FORCE_HOUSEHOLDER=1 sends EVERY panel QR through the slow path (LAPACK's dgeqr2 + dorg2r run as column
-    operations on row ranges of the device panel).  On full-rank blocks that path must give LAPACK's factors, so the
-    whole solve matches the oracle at the usual 1e-6."""
+    operations on row ranges of the device panel, at odd row offsets; the DMMA kernels for p = 8 / 16 / 32).  On
+    full-rank blocks that path must give LAPACK's factors, so the whole solve matches the oracle at the usual 1e-6."""
     monkeypatch.setenv("KB200_QR_FORCE_HOUSEHOLDER", "1")
-    A, _ = O.kron_unsymmetric(8)
+    A, _ = O.kron_unsymmetric(N)
     A = sp.csr_matrix(A)
     B = A @ _rhs(A.shape[0], p, 3)
     ws = kb.BlockGmresWorkspace(A.shape[0], A.shape[0], p, memory=6)
@@ -130,6 +123,20 @@ def test_device_householder_path_matches_oracle_on_full_rank_blocks(kb, O, p, mo
     Xo, so = O.block_gmres(A, B, memory=6)
     assert nfall >= st.niter
     _check(st, X, so, Xo)
+
+
+@pytest.mark.parametrize("N", [8, 9])
+@pytest.mark.parametrize("p", [8, 16, 32])
+def test_block_gmres_float32_wide_blocks(kb, O, p, N):
+    """Float32 panels at p = 8, 16, 32 (SIMT kernels: the DMMA path is Float64 only), with the checks of the p = 4
+    Float32 case above: solved within one iteration of the Float32 oracle, true residual small."""
+    A, _ = O.kron_unsymmetric(N)
+    A = sp.csr_matrix(A)
+    B = A @ _rhs(A.shape[0], p, 2)
+    X, st = kb.block_gmres(A, B.astype(np.float32), memory=8, history=True)
+    Xo, so = O.block_gmres(A, B, memory=8, dtype=np.float32)
+    assert st.solved and abs(st.niter - so["niter"]) <= 1, (st.niter, so["niter"])
+    assert np.linalg.norm(B - A @ X.astype(np.float64)) / np.linalg.norm(B) <= 5e-3
 
 
 @pytest.mark.parametrize("p", [3, 4])
