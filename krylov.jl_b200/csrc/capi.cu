@@ -6,6 +6,7 @@
 // (solver, dtype); free returns 1 for an unknown handle.  Unlike the reference
 // (global typed Dicts, documented as not thread-safe) the handle table is a
 // single mutex-protected map.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <memory>
@@ -39,6 +40,8 @@ struct Handle {
   int p = 0;
   void* ws = nullptr;
   std::shared_ptr<CsrAny> csr;
+  std::shared_ptr<CsrAny> csrT;        // LSQR / LSMR: A^T of the attached operator, built on first use ...
+  const CsrAny* csrT_for = nullptr;    // ... for this operator
   void* Mdiag = nullptr;
   void* Ndiag = nullptr;
   void* Pblk[2] = {nullptr, nullptr};      // block-Jacobi M / N: dense diagonal blocks (device) ...
@@ -73,7 +76,7 @@ int fail(const char* where, const char* msg) {
 
 bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
-         s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES;
+         s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR;
 }
 
 int pick_device() {
@@ -103,6 +106,11 @@ int n_of(Handle* h) {
   if (h->block) return h->dtype == KRYLOV_FLOAT64 ? BW<double>(h)->n : BW<float>(h)->n;
   return h->dtype == KRYLOV_FLOAT64 ? W<double>(h)->n : W<float>(h)->n;
 }
+int m_of(Handle* h) {
+  if (h->block) return n_of(h);
+  return h->dtype == KRYLOV_FLOAT64 ? W<double>(h)->m : W<float>(h)->m;
+}
+bool is_ls(const Handle* h) { return !h->block && is_ls_kind(h->solver); }
 template <class T> Csr<T>& csr_of(CsrAny& a);
 template <> Csr<double>& csr_of<double>(CsrAny& a) { return a.d; }
 template <> Csr<float>& csr_of<float>(CsrAny& a) { return a.f; }
@@ -114,6 +122,7 @@ template <class T> void destroy_handle(Handle* h) {
     if (ws->ctx.stream) cudaStreamSynchronize(ws->ctx.stream);
   }
   h->csr.reset();
+  h->csrT.reset();
   dev_free(h->Mdiag); dev_free(h->Ndiag);
   for (int w = 0; w < 2; w++) { dev_free(h->Pblk[w]); dev_free(h->Pblk_inv[w]); }
   if (h->hx) cudaFreeHost(h->hx);
@@ -122,12 +131,12 @@ template <class T> void destroy_handle(Handle* h) {
   delete h;
 }
 
-// Bring a caller vector (host or device, per device_kind) into a device buffer.
+// Bring a caller vector of length m (b; c of the square solvers) into a device buffer (host or device, per device_kind).
 template <class T> const T* stage_in(Handle* h, Workspace<T>* ws, const void* src, T*& buf) {
   if (!src) return nullptr;
   if (h->device_kind == KRYLOV_CUDA) return (const T*)src;
-  if (!buf) buf = dev_alloc<T>((size_t)ws->n);
-  KB_CUDA(cudaMemcpyAsync(buf, src, sizeof(T) * (size_t)ws->n, cudaMemcpyHostToDevice, ws->ctx.stream));
+  if (!buf) buf = dev_alloc<T>((size_t)ws->m);
+  KB_CUDA(cudaMemcpyAsync(buf, src, sizeof(T) * (size_t)ws->m, cudaMemcpyHostToDevice, ws->ctx.stream));
   return buf;
 }
 
@@ -138,9 +147,10 @@ template <class T> LinOp<T> make_cb_op(Handle* h, Workspace<T>* ws, KrylovMatvec
   op.fn = fn; op.userdata = ud;
   if (h->device_kind == KRYLOV_CUDA) { op.kind = LinOp<T>::DEV_CB; return op; }
   op.kind = LinOp<T>::HOST_CB;
-  if (!h->hx) {
-    KB_CUDA(cudaHostAlloc(&h->hx, sizeof(T) * (size_t)ws->n, cudaHostAllocDefault));
-    KB_CUDA(cudaHostAlloc(&h->hy, sizeof(T) * (size_t)ws->n, cudaHostAllocDefault));
+  if (!h->hx) {   // rectangular operators stage both lengths through the same buffers
+    const size_t len = (size_t)std::max(ws->m, ws->n);
+    KB_CUDA(cudaHostAlloc(&h->hx, sizeof(T) * len, cudaHostAllocDefault));
+    KB_CUDA(cudaHostAlloc(&h->hy, sizeof(T) * len, cudaHostAllocDefault));
   }
   op.hx = (T*)h->hx; op.hy = (T*)h->hy;
   return op;
@@ -161,6 +171,7 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   if (h->solver == S_DIOM || h->solver == S_DQGMRES) s.reorthogonalization = o->reorthogonalization != 0;      // _typed_solve_mn_reorth!
   s.cr_gamma = std::isnan(h->ext.cr_gamma) ? -1 : h->ext.cr_gamma;
   if (h->solver == S_MINRES) { s.lambda = o->lambda; s.linesearch = o->linesearch != 0; }
+  if (is_ls_kind(h->solver)) { s.lambda = o->lambda; s.radius = o->radius; }   // _typed_solve_ls_mn_radius! (c_stores.jl:403-423)
   // _typed_solve_gmres! serves GMRES, FGMRES and FOM (c_stores.jl:376-398)
   if (h->solver == S_GMRES || h->solver == S_FGMRES || h->solver == S_FOM) {
     s.restart = o->restart != 0; s.reorthogonalization = o->reorthogonalization != 0;
@@ -170,6 +181,8 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   s.ldiv = h->ext.ldiv != 0;
   s.etol = std::isnan(h->ext.etol) ? -1 : h->ext.etol;
   s.conlim = std::isnan(h->ext.conlim) ? -1 : h->ext.conlim;
+  s.axtol = std::isnan(h->ext.axtol) ? -1 : h->ext.axtol;
+  s.btol = std::isnan(h->ext.btol) ? -1 : h->ext.btol;
   s.fused = h->ext.fused;
   s.persist = h->ext.fused != 2;       // fused == 2: fused CG keeps the two-launch kernels (A/B measurements, tests)
   s.batch = h->ext.batch;
@@ -177,6 +190,57 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   s.callback_user = h->ext.callback_user;
   s.time_kernels = h->ext.time_kernels;
   return s;
+}
+
+// A^T of a CSR operator as a new object on context c (host-side transpose, once per operator)
+std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src) {
+  HostCsr hs, ht;
+  if (src.dtype == KRYLOV_FLOAT64) csr_to_host<double>(c, src.d, hs); else csr_to_host<float>(c, src.f, hs);
+  transpose_csr(hs, ht);
+  auto a = std::make_shared<CsrAny>();
+  a->dtype = src.dtype; a->owner_ctx = &c;
+  if (a->dtype == KRYLOV_FLOAT64) csr_from_host<double>(c, a->d, ht); else csr_from_host<float>(c, a->f, ht);
+  return a;
+}
+
+// lsqr! / lsmr! (c_stores.jl:403-423): b has m entries, x has n; A maps n -> m and needs its adjoint
+template <class T>
+int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, void* ud,
+                const KrylovOptions* opts) {
+  Workspace<T>* ws = W<T>(h);
+  KB_CUDA(cudaSetDevice(ws->ctx.device));
+  SolveOpts so = map_opts(h, opts);
+  const int m = ws->m, n = ws->n;
+  LinOp<T> A, At;
+  if (fA) {
+    if (!fAt) throw std::runtime_error("lsqr and lsmr apply the adjoint of A: matvec_At must be given with matvec_A");
+    A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
+    At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
+  } else if (h->csr) {
+    const Csr<T>& C = csr_of<T>(*h->csr);
+    if (C.n != m || C.max_col >= n)
+      throw std::runtime_error("CSR operator: size inconsistent with the workspace ((m, n) = (" + std::to_string(m) + ", " +
+                               std::to_string(n) + "), operator rows = " + std::to_string(C.n) + ", largest column = " +
+                               std::to_string(C.max_col) + ")");
+    if (!h->csrT || h->csrT_for != h->csr.get()) {
+      h->csrT.reset();
+      h->csrT = transpose_any(ws->ctx, *h->csr);
+      h->csrT_for = h->csr.get();
+    }
+    A.kind = LinOp<T>::CSR; A.csr = &C; A.n = m;
+    At.kind = LinOp<T>::CSR; At.csr = &csr_of<T>(*h->csrT); At.n = n;
+  } else {
+    throw std::runtime_error("no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr");
+  }
+  LinOp<T> M = make_cb_op<T>(h, ws, fM, ud), N = make_cb_op<T>(h, ws, fN, ud);
+  M.n = m; N.n = n;                      // M acts on the m-dimensional data space, N on the n-dimensional solution space
+  if (!fM && h->Mdiag) { M.kind = LinOp<T>::DIAG; M.diag = (const T*)h->Mdiag; }
+  if (!fN && h->Ndiag) { N.kind = LinOp<T>::DIAG; N.diag = (const T*)h->Ndiag; }
+  if (!b) throw std::runtime_error("b is NULL");
+  const T* bd = stage_in<T>(h, ws, b, ws->bbuf);
+  if (h->solver == S_LSQR) lsqr_solve<T>(*ws, A, At, bd, M, N, so);
+  else lsmr_solve<T>(*ws, A, At, bd, M, N, so);
+  return 0;
 }
 
 template <class T>
@@ -243,6 +307,7 @@ template <class T> int do_get_x(Handle* h, void* x, int n) {
 
 template <class T> int do_warm_start(Handle* h, const void* x0, int n) {
   Workspace<T>* ws = W<T>(h);
+  if (is_ls_kind(h->solver)) throw std::runtime_error("lsqr and lsmr do not support warm-start (they take no x0)");
   if (n != ws->n) throw std::runtime_error("x0 should have size n");
   KB_CUDA(cudaSetDevice(ws->ctx.device));
   // c_stores.jl:218-229: allocate dx if empty, copy, set the flag
@@ -265,7 +330,8 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
       {"x", ws->x}, {"dx", ws->dx}, {"r", ws->r}, {"p", ws->p}, {"Ap", ws->Ap}, {"z", ws->z}, {"npc_dir", ws->npc_dir},
       {"v", ws->kind == S_MINRES ? (ws->vv ? ws->vv : ws->r2) : ws->v}, {"s", ws->s}, {"qd", ws->qd}, {"t", ws->t}, {"yz", ws->yz},
       {"r1", ws->r1}, {"r2", ws->r2}, {"w1", ws->w1}, {"w2", ws->w2}, {"y", ws->y}, {"w", ws->w}, {"q", ws->q},
-      {"u", ws->u}, {"ts", ws->ts}, {"vw", ws->vw}, {"Mv", ws->Mv}, {"Mv_prev", ws->Mv_prev}, {"Mv_next", ws->Mv_next}};
+      {"u", ws->u}, {"ts", ws->ts}, {"vw", ws->vw}, {"Mv", ws->Mv}, {"Mv_prev", ws->Mv_prev}, {"Mv_next", ws->Mv_next},
+      {"Nv", ws->Nv}, {"Mu", ws->Mu}, {"Av", ws->Av}, {"Atu", ws->Atu}, {"h", ws->h}, {"hbar", ws->hbar}};
   for (auto& e : tab) if (!strcmp(e.n, nm)) return e.p;
   if (nm[0] == 'P' && nm[1]) { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->Z.size()) return ws->Z[i - 1]; return nullptr; }
   if (!strcmp(nm, "Ar")) return ws->Ap;
@@ -322,10 +388,12 @@ void krylov_get_version(int* major, int* minor, int* patch) {
 
 int krylov_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, KrylovMatvec matvec_M, KrylovMatvec matvec_N,
                  const void* b, const void* c, void* userdata, const KrylovOptions* opts) {
-  (void)matvec_At;   // none of CG / MINRES / GMRES / BiCGSTAB uses the adjoint
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_solve", "unknown workspace handle");
+    if (is_ls(h))                    // the square solvers never apply the adjoint
+      return h->dtype == KRYLOV_FLOAT64 ? do_solve_ls<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts)
+                                        : do_solve_ls<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts);
     return h->dtype == KRYLOV_FLOAT64 ? do_solve<double>(h, matvec_A, matvec_M, matvec_N, b, c, userdata, opts)
                                       : do_solve<float>(h, matvec_A, matvec_M, matvec_N, b, c, userdata, opts);
   } catch (const std::exception& e) { return fail("krylov_solve", e); }
@@ -552,12 +620,15 @@ int krylov_b200_set_operator_csr(void* ws, int n, long long nnz, const void* row
     a->dtype = h->dtype;
     Ctx& cx = ctx_of(h);
     KB_CUDA(cudaSetDevice(cx.device));
-    if (n != n_of(h)) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
+    // n: number of rows (m of an LSQR / LSMR workspace, whose operator has the workspace's n columns)
+    if (n != m_of(h)) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
+    const int ncols = is_ls(h) ? n_of(h) : -1;
     if (h->dtype == KRYLOV_FLOAT64)
-      csr_upload<double>(cx, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0);
+      csr_upload<double>(cx, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, ncols);
     else
-      csr_upload<float>(cx, a->f, n, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0);
+      csr_upload<float>(cx, a->f, n, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0, ncols);
     h->csr = a;
+    h->csrT.reset();
     return 0;
   } catch (const std::exception& e) { return fail("krylov_b200_set_operator_csr", e); }
 }
@@ -567,6 +638,7 @@ int krylov_b200_share_operator(void* ws, void* src) {
   if (!h || !s) return fail("krylov_b200_share_operator", "unknown workspace handle");
   if (!s->csr || s->dtype != h->dtype) return fail("krylov_b200_share_operator", "source has no CSR operator of this dtype");
   h->csr = s->csr;
+  h->csrT.reset();
   return 0;
 }
 
@@ -576,6 +648,7 @@ int krylov_b200_attach_csr(void* ws, void* csr) {
   CsrAny* a = (CsrAny*)csr;
   if (a->dtype != h->dtype) return fail("krylov_b200_attach_csr", "dtype mismatch");
   h->csr = std::shared_ptr<CsrAny>(std::shared_ptr<CsrAny>(), a);   // non-owning alias
+  h->csrT.reset();
   return 0;
 }
 
@@ -586,7 +659,7 @@ int krylov_b200_set_preconditioner_diag(void* ws, int which, const void* d, int 
     void*& slot = which == 0 ? h->Mdiag : h->Ndiag;
     if (!d) { dev_free(slot); slot = nullptr; return 0; }
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
-    const int n = n_of(h);
+    const int n = which == 0 ? m_of(h) : n_of(h);     // LSQR / LSMR: M has m entries, N has n
     KB_CUDA(cudaSetDevice(ctx_of(h).device));
     if (!slot) slot = dev_alloc<char>(esz * (size_t)n);
     KB_CUDA(cudaMemcpy(slot, d, esz * (size_t)n, location ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
@@ -604,6 +677,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
     h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0;
     if (!blocks) return 0;
+    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on LSQR / LSMR workspaces");
     if (bs < 2 || bs > 8) return fail("krylov_b200_set_preconditioner_blockdiag", "block size must be in 2..8");
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
     const int n = n_of(h);
@@ -631,7 +705,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
 KrylovB200Options krylov_b200_default_options(void) {
   KrylovB200Options o;
   memset(&o, 0, sizeof(o));
-  o.etol = NAN; o.conlim = NAN; o.fused = 1; o.cr_gamma = NAN;
+  o.etol = NAN; o.conlim = NAN; o.fused = 1; o.cr_gamma = NAN; o.axtol = NAN; o.btol = NAN;
   return o;
 }
 
@@ -822,6 +896,7 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_b200_dist_init", "unknown workspace handle");
+    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned LSQR / LSMR solves are not available");
     return h->dtype == KRYLOV_FLOAT64 ? dist_init_t<double>(h, rank, world, nhalo, halo_rank, halo_off)
                                       : dist_init_t<float>(h, rank, world, nhalo, halo_rank, halo_off);
   } catch (const std::exception& e) { return fail("krylov_b200_dist_init", e); }
@@ -902,7 +977,13 @@ void* kb200_alloc(long long bytes) {
 }
 int kb200_free(void* p) { dev_free(p); return 0; }
 int kb200_h2d(void* dst, const void* src, long long bytes) {
-  return cudaMemcpy(dst, src, (size_t)bytes, cudaMemcpyHostToDevice) == cudaSuccess ? 0 : fail("kb200_h2d", "cudaMemcpy failed");
+  // From pageable memory cudaMemcpy returns once the data is staged, possibly before the last DMA lands; the
+  // contexts' streams are non-blocking and do not wait for the legacy stream, so a kernel launched next could read
+  // (or be overwritten by) the tail of the copy.  Wait for it here: the data is in place when the call returns.
+  if (cudaMemcpy(dst, src, (size_t)bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaStreamSynchronize(cudaStreamLegacy) != cudaSuccess)
+    return fail("kb200_h2d", "cudaMemcpy failed");
+  return 0;
 }
 int kb200_d2h(void* dst, const void* src, long long bytes) {
   return cudaMemcpy(dst, src, (size_t)bytes, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : fail("kb200_d2h", "cudaMemcpy failed");
@@ -959,6 +1040,24 @@ void* kb200_csr_create(void* ctx, int dtype, int n, long long nnz, const void* r
     return a;
   } catch (const std::exception& e) { fail("kb200_csr_create", e); return nullptr; }
 }
+void* kb200_csr_create_rect(void* ctx, int dtype, int m, int n, long long nnz, const void* rowptr, const void* colind,
+                            const void* values, int index_base, int index_bytes, int location) {
+  try {
+    if (!ctx) throw std::runtime_error("bad arguments");
+    if (n < 0) throw std::runtime_error("negative number of columns");
+    Ctx& c = *(Ctx*)ctx;
+    CsrAny* a = new CsrAny();
+    a->dtype = dtype; a->owner_ctx = &c;
+    try {
+      if (dtype == KRYLOV_FLOAT64) csr_upload<double>(c, a->d, m, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, n);
+      else if (dtype == KRYLOV_FLOAT32) csr_upload<float>(c, a->f, m, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0, n);
+      else throw std::runtime_error("unsupported dtype");
+      const int max_col = dtype == KRYLOV_FLOAT64 ? a->d.max_col : a->f.max_col;
+      if (max_col >= n) throw std::runtime_error("CSR operator: column index " + std::to_string(max_col) + " outside the " + std::to_string(n) + " columns");
+    } catch (...) { delete a; throw; }
+    return a;
+  } catch (const std::exception& e) { fail("kb200_csr_create_rect", e); return nullptr; }
+}
 void kb200_csr_destroy(void* csr) { delete (CsrAny*)csr; }
 
 // Matrix Market ingestion and the transposed operator (mtx.cu)
@@ -1000,6 +1099,15 @@ int kb200_csr_info(void* csr, int* n, long long* nnz) {
   CsrAny* a = (CsrAny*)csr;
   if (!a) return -1;
   if (n) *n = a->dtype == KRYLOV_FLOAT64 ? a->d.n : a->f.n;
+  if (nnz) *nnz = a->dtype == KRYLOV_FLOAT64 ? a->d.nnz : a->f.nnz;
+  return 0;
+}
+
+int kb200_csr_shape(void* csr, int* m, int* n, long long* nnz) {
+  CsrAny* a = (CsrAny*)csr;
+  if (!a) return -1;
+  if (m) *m = a->dtype == KRYLOV_FLOAT64 ? a->d.n : a->f.n;
+  if (n) *n = a->dtype == KRYLOV_FLOAT64 ? a->d.ncols : a->f.ncols;
   if (nnz) *nnz = a->dtype == KRYLOV_FLOAT64 ? a->d.nnz : a->f.nnz;
   return 0;
 }
@@ -1061,6 +1169,9 @@ int kb200_spmv_csr(void* ctx, void* csr, const void* x, void* y, int variant) {
   try {
     Ctx& c = *(Ctx*)ctx;
     CsrAny* a = (CsrAny*)csr;
+    const int max_col = a->dtype == KRYLOV_FLOAT64 ? a->d.max_col : a->f.max_col;
+    const int ncols = a->dtype == KRYLOV_FLOAT64 ? a->d.ncols : a->f.ncols;
+    if (max_col >= ncols) throw std::runtime_error("column index outside the operator's columns");
     if (a->dtype == KRYLOV_FLOAT64) k_spmv<double>(c, a->d, (const double*)x, (double*)y, variant);
     else k_spmv<float>(c, a->f, (const float*)x, (float*)y, variant);
     return 0;

@@ -28,7 +28,7 @@ __global__ void __launch_bounds__(kTileThreads, 3) spmv_epi_tma(Csr<T> A, G xg, 
 #pragma unroll
   for (int k = 0; k < K; k++) d[k] = T(0);
   spmv_tiles_run<T>(
-      A, smem, xg, NoRowBegin(), [&](int row, T acc, int) { epi(row, acc, d); });
+      A, smem, gather_for_cta(xg), NoRowBegin(), [&](int row, T acc, int) { epi(row, acc, d); });
   T mine[K], tot[K];
 #pragma unroll
   for (int k = 0; k < K; k++) mine[k] = block_sum(d[k], sm);
@@ -46,11 +46,12 @@ __global__ void __launch_bounds__(kBlock) spmv_epi_rows(Csr<T> A, G xg, Epi epi,
   T d[K];
 #pragma unroll
   for (int k = 0; k < K; k++) d[k] = T(0);
+  const G g = gather_for_cta(xg);
   const int stride = gridDim.x * blockDim.x;
   for (int row = blockIdx.x * blockDim.x + threadIdx.x; row < A.n; row += stride) {
     const int kb = A.rowptr[row], ke = A.rowptr[row + 1];
     T acc = T(0);
-    for (int k = kb; k < ke; k++) acc = add_rn(acc, mul_rn(A.val[k], xg(A.colind[k])));
+    for (int k = kb; k < ke; k++) acc = add_rn(acc, mul_rn(A.val[k], g(A.colind[k])));
     epi(row, acc, d);
   }
   T mine[K], tot[K];
@@ -603,6 +604,108 @@ template <class T> T cr_fused_directions(Workspace<T>& ws, T beta) {
   return out[0];
 }
 
+// ===========================================================================
+// LSQR / LSMR  (src/lsqr.jl:297-317,361-362, src/lsmr.jl:309-328,352-365, M = N = I, no trust region)
+// kdiv!(u, beta) = kscal!(1/beta, u) is left pending: Mu stays unscaled in memory and both of its readers apply
+// s_u = 1/beta (the scaled gather of P2 and the Mu read of the next P1), which are the two roundings the reference
+// performs.  v === Nv is scaled in place by P3, as kdiv!(v, alpha) does.
+// ===========================================================================
+template <class T> struct LsqState { T alpha, beta, s_u, ww; int beta_zero; };
+
+template <class T> struct LsqP1Epi {      // Mu = A v - alpha (Mu s_u) ; ||Mu||^2   (kaxpby!(m, one, Av, -alpha, Mu))
+  T* mu; const LsqState<T>* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T u = mul_rn(mu[row], s->s_u);
+    const T nm = add_rn(mul_rn(T(1), acc), mul_rn(-s->alpha, u));
+    mu[row] = nm;
+    d[0] += nm * nm;
+  }
+};
+template <class T> struct LsqP1Fin {      // beta = ||Mu|| ; s_u = 1/beta (1 when beta = 0: kdiv! is skipped)
+  LsqState<T>* s;
+  __device__ void operator()(const T* tot) const {
+    const T beta = sqrt_rn(tot[0]);
+    s->beta = beta;
+    s->beta_zero = beta == T(0);
+    s->s_u = beta == T(0) ? T(1) : div_rn(T(1), beta);
+  }
+};
+template <class T, bool WW> struct LsqP2Epi {   // Nv = A^T u - beta Nv ; ||Nv||^2 ; LSQR: <w, w> of the old w
+  T* nv; const T* w; const LsqState<T>* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    if (WW) { const T wr = w[row]; d[1] += wr * wr; }
+    if (s->beta_zero) return;                     // beta = 0: the reference skips this product (lsqr.jl:303)
+    const T nn = add_rn(mul_rn(T(1), acc), mul_rn(-s->beta, nv[row]));
+    nv[row] = nn;
+    d[0] += nn * nn;
+  }
+};
+template <class T, int K> struct LsqP2Fin {
+  LsqState<T>* s;
+  __device__ void operator()(const T* tot) const {
+    if (K > 1) s->ww = tot[K - 1];
+    if (!s->beta_zero) s->alpha = sqrt_rn(tot[0]);
+  }
+};
+template <class T> struct LsqrP3Body {    // v = Nv / alpha ; x += sigma w ; w = v - tau w   (lsqr.jl:315,361-362)
+  T* v; T* x; T* w; T inv_alpha, sigma, tau; int scale_v;
+  __device__ __forceinline__ void operator()(int i, T*) const {
+    T vi = v[i];
+    if (scale_v) { vi = mul_rn(inv_alpha, vi); v[i] = vi; }
+    const T wi = w[i];
+    x[i] = add_rn(x[i], mul_rn(sigma, wi));
+    w[i] = add_rn(mul_rn(T(1), vi), mul_rn(-tau, wi));
+  }
+};
+template <class T> struct LsmrP3Body {    // v = Nv / alpha ; hbar = h - delta hbar ; x += sigma hbar ; h = v - tau h ; ||x||^2
+  T* v; T* x; T* h; T* hbar; T inv_alpha, sigma, tau, delta; int scale_v;   // (lsmr.jl:325,352,364-365,399)
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    T vi = v[i];
+    if (scale_v) { vi = mul_rn(inv_alpha, vi); v[i] = vi; }
+    const T hi = h[i];
+    const T hb = add_rn(mul_rn(T(1), hi), mul_rn(-delta, hbar[i]));
+    hbar[i] = hb;
+    const T xn = add_rn(x[i], mul_rn(sigma, hb));
+    x[i] = xn;
+    h[i] = add_rn(mul_rn(T(1), vi), mul_rn(-tau, hi));
+    d[0] += xn * xn;
+  }
+};
+
+template <class T>
+void lsq_fused_bidiag(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, bool want_ww, T* beta, T* alpha_out,
+                      T* ww) {
+  Ctx& c = ws.ctx;
+  typedef LsqState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  if (init) {                     // Mu holds u_1 already scaled (the initialisation runs on the primitives)
+    memset(H, 0, sizeof(St));
+    H->alpha = alpha; H->s_u = T(1);
+    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+  }
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.Nv}, LsqP1Epi<T>{ws.Mu, S}, LsqP1Fin<T>{S}, 4);
+  const XScaled<T> ug{ws.Mu, &S->s_u, T(1)};
+  if (want_ww) launch_spmv_epi_g<T, 2>(c, At, ug, LsqP2Epi<T, true>{ws.Nv, ws.w, S}, LsqP2Fin<T, 2>{S}, 4);
+  else launch_spmv_epi_g<T, 1>(c, At, ug, LsqP2Epi<T, false>{ws.Nv, ws.w, S}, LsqP2Fin<T, 1>{S}, 4);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  c.sync();
+  *beta = H[1].beta; *alpha_out = H[1].alpha; *ww = H[1].ww;
+}
+
+template <class T> T lsq_fused_update(Workspace<T>& ws, bool lsmr, bool scale_v, T inv_alpha, T sigma, T tau, T delta) {
+  Ctx& c = ws.ctx;
+  if (!lsmr) {
+    launch_stream<T, 0>(c, ws.n, LsqrP3Body<T>{ws.Nv, ws.x, ws.w, inv_alpha, sigma, tau, scale_v ? 1 : 0}, NoFin(), 5);
+    return T(0);
+  }
+  T* out = sib_slots<T>(c);
+  launch_stream<T, 1>(c, ws.n, LsmrP3Body<T>{ws.Nv, ws.x, ws.h, ws.hbar, inv_alpha, sigma, tau, delta, scale_v ? 1 : 0},
+                      StoreFin<T, 1>{out}, 5);
+  T xx[1]; sib_read<T, 1>(c, xx);
+  return std::sqrt(xx[0]);
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -621,7 +724,9 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void cr_fused_step<T>(Workspace<T>&, const Csr<T>&, T, T*, T*, T*, T*);                                   \
   template T cr_fused_directions<T>(Workspace<T>&, T);                                                               \
   template void fused_multi_axpy<T>(Workspace<T>&, T*, int, const T*, T* const*);                                    \
-  template void gmres_fused_update_x<T>(Workspace<T>&, T*, int, const T*);
+  template void gmres_fused_update_x<T>(Workspace<T>&, T*, int, const T*);                                          \
+  template void lsq_fused_bidiag<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, bool, T*, T*, T*);        \
+  template T lsq_fused_update<T>(Workspace<T>&, bool, bool, T, T, T, T);
 INST(double)
 INST(float)
 #undef INST

@@ -9,6 +9,7 @@
 //   solvers.cu    host control flow of cg!/gmres!/bicgstab!/minres! on the primitives
 //   siblings.cu   cgs!, cg_lanczos!, fom!, fgmres!, dqgmres!, diom!, cr! on the same kernels (SURVEY.md 8f-3)
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
+//   lsq.cu        host control flow of lsqr!/lsmr! on rectangular operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
 #pragma once
@@ -76,12 +77,14 @@ inline void dist_nan_guard(Ctx& c, double v) { if (c.dcomm && v != v) dist_check
 
 // ---------------------------------------------------------------------------
 // CSR operator resident in HBM (int32 indices, 0-based, columns ascending).
+// n rows; ncols columns (= n for square operators, the only kind the square solvers take).
 // ---------------------------------------------------------------------------
 constexpr int kTileRows = 256;   // rows per TMA-staged tile (= consumer threads per CTA)
 
 template <class T>
 struct Csr {
   int n = 0;
+  int ncols = 0;
   long long nnz = 0;
   int* rowptr = nullptr;    // n+1 (+ pad)
   int* colind = nullptr;    // nnz (+ pad)
@@ -98,8 +101,9 @@ struct Csr {
   int ctas_per_sm = 0;      // resident CTAs per SM the ring was sized for
 };
 
+// ncols < 0: square (ncols = n)
 template <class T> void csr_upload(Ctx& c, Csr<T>& A, int n, long long nnz, const void* rowptr, const void* colind,
-                                   const T* val, int index_base, int index_bytes, bool on_device);
+                                   const T* val, int index_base, int index_bytes, bool on_device, int ncols = -1);
 template <class T> void csr_free(Csr<T>& A);
 template <class T> void csr_plan(Ctx& c, Csr<T>& A);
 // y = A x.  variant: 0 auto (TMA-staged when the plan allows), 1 force row-per-thread LDG, 2 force TMA-staged
@@ -125,7 +129,8 @@ struct LinOp {
   void* userdata = nullptr;
   T* hx = nullptr;               // pinned staging for HOST_CB
   T* hy = nullptr;
-  int n = 0;
+  int n = 0;                     // length of y (and of x unless nin is set)
+  int nin = 0;                   // HOST_CB of a rectangular operator: length of x (0: n)
   bool is_identity() const { return kind == NONE; }
 };
 template <class T> void op_apply(Ctx& c, const LinOp<T>& op, const T* x, T* y, bool ldiv = false);
@@ -142,8 +147,9 @@ struct SolveOpts {
   bool history = false;
   double radius = 0;                // CG
   bool linesearch = false;          // CG, MINRES
-  double lambda = 0;                // MINRES
-  double etol = -1, conlim = -1;    // MINRES (<0 => defaults)
+  double lambda = 0;                // MINRES, LSQR, LSMR
+  double etol = -1, conlim = -1;    // MINRES, LSQR, LSMR (<0 => defaults)
+  double axtol = -1, btol = -1;     // LSQR, LSMR (<0 => sqrt(eps(T)))
   bool restart = false;             // GMRES, FOM, FGMRES
   bool reorthogonalization = false; // GMRES, FOM, FGMRES
   bool check_curvature = false;     // CG-Lanczos
@@ -170,7 +176,9 @@ struct Stats {
 
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
-                  S_CGS = 11, S_CG_LANCZOS = 100 };
+                  S_CGS = 11, S_LSQR = 21, S_LSMR = 22, S_CG_LANCZOS = 100 };
+// the least-squares solvers: A is m x n, b has m entries and x has n
+inline bool is_ls_kind(int k) { return k == S_LSQR || k == S_LSMR; }
 
 // One workspace per (solver, dtype): owns every device vector of the solver
 // (src/krylov_workspaces.jl; SURVEY.md appendix B for fields and aliasing).
@@ -190,10 +198,12 @@ struct Workspace {
   T *w = nullptr, *q = nullptr, *pp = nullptr;                                        // GMRES / FOM / FGMRES (+ V)
   T *u = nullptr, *ts = nullptr, *vw = nullptr;                                       // CGS (+ r, p, q, yz)
   T *Mv = nullptr, *Mv_prev = nullptr, *Mv_next = nullptr;                            // CG-Lanczos (+ p, vv)
+  T *Nv = nullptr, *Mu = nullptr, *Av = nullptr, *Atu = nullptr;                     // LSQR / LSMR (+ w, u, v; Mu, Av, u: m)
+  T *h = nullptr, *hbar = nullptr;                                                   // LSMR
   std::vector<T*> V;
   std::vector<T*> Z;                   // FGMRES: Z[k] = N_k V[k];  DQGMRES / DIOM: the direction stack P
   std::vector<T> c, sgiv, zg, R;       // GMRES host-side Givens data
-  std::vector<T> err_vec;              // MINRES window
+  std::vector<T> err_vec;              // MINRES, LSQR, LSMR window
   int memory = 20, window = 5;
   int inner_iter = 0;
   const T* mdiag_fused = nullptr;      // diagonal of M for the fused CG kernels (set per solve; nullptr: M = I)
@@ -253,6 +263,11 @@ template <class T> void fgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const 
 template <class T> void dqgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void diom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
+// Least squares on an m x n operator (lsq.cu).  At: the adjoint (a CSR operator holding A^T, or a callback m -> n).
+template <class T> void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                   const LinOp<T>& N, const SolveOpts& o);
+template <class T> void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                   const LinOp<T>& N, const SolveOpts& o);
 
 // Fused CG (cg_fused.cu).  Returns false if the configuration is not eligible
 // (caller falls back to the generic primitive path, still on the GPU).
@@ -287,6 +302,14 @@ template <class T> void cr_fused_step(Workspace<T>& ws, const Csr<T>& A, T alpha
 template <class T> T cr_fused_directions(Workspace<T>& ws, T beta);
 template <class T> void gmres_fused_update_x(Workspace<T>& ws, T* xr, int k, const T* y);
 int gmres_fused_max();
+// LSQR / LSMR (fused_phases.cu), M = N = I, A and A^T CSR operators, no trust region.  Golub-Kahan step: P1 (SpMV on A
+// with Mu <- A v - alpha Mu and ||Mu||^2) and P2 (SpMV on A^T with Nv <- A^T u - beta Nv, ||Nv||^2 and, for LSQR,
+// <w, w>), then one read-back of {beta, alpha, <w, w>}.  `init`: first iteration, sets the device scalars from the host.
+template <class T> void lsq_fused_bidiag(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, bool want_ww,
+                                         T* beta, T* alpha_out, T* ww);
+// P3.  LSQR: v = Nv / alpha (scale_v), x += sigma w, w = v - tau w.  LSMR (lsmr = true, w = h):
+// v = Nv / alpha (scale_v), hbar = h - delta hbar, x += sigma hbar, h = v - tau h; returns ||x|| (LSMR only).
+template <class T> T lsq_fused_update(Workspace<T>& ws, bool lsmr, bool scale_v, T inv_alpha, T sigma, T tau, T delta);
 
 double now_seconds();
 

@@ -1,0 +1,511 @@
+// lsq.cu -- host control flow of lsqr! (src/lsqr.jl:174-440) and lsmr! (src/lsmr.jl:178-455) on an m x n operator.
+// Both run the Golub-Kahan bidiagonalization: one product with A and one with A^H per iteration.  The primitive path
+// restates the reference line by line over blas1.cu / spmv.cu (11 launches per LSQR iteration, 12 per LSMR one).  When
+// A is a CSR operator, M = N = I and there is no trust region, the fused path runs the same iteration as 3 launches
+// (fused_phases.cu: P1 on A, P2 on A^T, P3 over n) and one read-back (LSMR: two, its tests need ||x|| after P3).  The
+// scalar recurrences, stopping tests and status strings run on the host, unchanged.
+#include <algorithm>
+#include <cmath>
+#include <cstdio>
+#include <limits>
+
+#include "solver_common.h"
+
+namespace kb {
+
+namespace {
+
+// allocate_if for a vector of length len (u, Mu and Av have m entries)
+template <class T> void allocate_len(Workspace<T>& ws, T*& v, int len) {
+  const double t0 = now_seconds();
+  if (!v) v = dev_alloc<T>((size_t)len);
+  ws.stats.allocation_timer += now_seconds() - t0;
+}
+
+// knorm_elliptic(n, x, y) (src/krylov_utils.jl:319)
+template <class T> T knorm_elliptic(Ctx& c, int n, const T* x, const T* y) {
+  return x == y ? k_nrm2<T>(c, n, x) : std::sqrt(k_dot<T>(c, n, x, y));
+}
+
+template <class T> T err_window_norm(const std::vector<T>& e) {   // knorm(window, err_vec)
+  T ssq = 0;
+  for (T v : e) ssq += v * v;
+  return std::sqrt(ssq);
+}
+
+// Step to the trust-region boundary along d (lsqr.jl:355-358, lsmr.jl:358-361): returns the clipped sigma.
+template <class T> T clip_to_boundary(Ctx& c, int n, const T* x, const T* d, T* z, T radius, T sigma, bool& on_boundary) {
+  LinOp<T> I;
+  T t1, t2;
+  const int e = to_boundary<T>(c, n, x, d, z, radius, T(0), I, false, &t1, &t2);
+  if (e == 2) throw std::runtime_error("zero direction");
+  if (e == 3) throw std::runtime_error("outside of the trust region");
+  if (e) throw std::runtime_error("The quadratic `q` doesn't have real roots.");
+  const T tmax = std::max(t1, t2), tmin = std::min(t1, t2);
+  on_boundary = sigma > tmax || sigma < tmin;
+  return sigma > 0 ? std::min(sigma, tmax) : std::max(sigma, tmin);
+}
+
+struct Setup {
+  bool MisI, NisI, fused;
+};
+
+// Common prologue: argument checks, lazily allocated vectors, x = 0, Mu = b, u = M Mu, beta_1.
+template <class T>
+Setup lsq_prologue(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                   const SolveOpts& o, T* beta1) {
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  Setup s;
+  s.MisI = M.is_identity(); s.NisI = N.is_identity();
+  s.fused = o.fused && A.kind == LinOp<T>::CSR && At.kind == LinOp<T>::CSR && s.MisI && s.NisI && !(o.radius > 0);
+  allocate_len(ws, ws.Mu, m);
+  allocate_len(ws, ws.Nv, n);
+  if (!s.MisI) allocate_len(ws, ws.u, m);
+  if (!s.NisI) allocate_len(ws, ws.v, n);
+  if (!s.fused) { allocate_len(ws, ws.Av, m); allocate_len(ws, ws.Atu, n); }
+  ws.stats.reset();
+  ws.stats.Anorm = NAN;
+  k_fill<T>(c, n, ws.x, T(0));
+  k_copy<T>(c, m, ws.Mu, b);
+  T* u = s.MisI ? ws.Mu : ws.u;
+  if (!s.MisI) op_apply(c, M, ws.Mu, u, o.ldiv);
+  *beta1 = m > 0 ? knorm_elliptic<T>(c, m, u, ws.Mu) : T(0);
+  return s;
+}
+
+// Golub-Kahan start: u /= beta_1, Nv = A^H u, v = N Nv (lsqr.jl:230-234).
+template <class T> void lsq_start(Workspace<T>& ws, const Setup& s, const LinOp<T>& At, const LinOp<T>& N, bool ldiv, T beta1) {
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  T* u = s.MisI ? ws.Mu : ws.u;
+  k_scal<T>(c, m, T(1) / beta1, u);
+  if (!s.MisI) k_scal<T>(c, m, T(1) / beta1, ws.Mu);
+  if (s.fused) {
+    op_apply(c, At, u, ws.Nv);                  // kmul!(Aᴴu, Aᴴ, u) ; kcopy!(n, Nv, Aᴴu) without the copy
+  } else {
+    op_apply(c, At, u, ws.Atu);
+    k_copy<T>(c, n, ws.Nv, ws.Atu);
+  }
+  if (!s.NisI) op_apply(c, N, ws.Nv, ws.v, ldiv);
+}
+
+// One Golub-Kahan step on the primitives (lsqr.jl:299-318): returns the new beta; alpha is updated when beta != 0.
+// `on_beta` runs between the two products (LSQR's Anorm update).
+template <class T, class OnBeta>
+T lsq_bidiag_step(Workspace<T>& ws, const Setup& s, const LinOp<T>& A, const LinOp<T>& At, const LinOp<T>& M, const LinOp<T>& N,
+                  bool ldiv, T& alpha, OnBeta on_beta) {
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  T* u = s.MisI ? ws.Mu : ws.u;
+  T* v = s.NisI ? ws.Nv : ws.v;
+  op_apply(c, A, v, ws.Av);
+  k_axpby<T>(c, m, T(1), ws.Av, -alpha, ws.Mu);
+  if (!s.MisI) op_apply(c, M, ws.Mu, u, ldiv);
+  const T beta = knorm_elliptic<T>(c, m, u, ws.Mu);
+  if (beta != 0) {
+    k_scal<T>(c, m, T(1) / beta, u);
+    if (!s.MisI) k_scal<T>(c, m, T(1) / beta, ws.Mu);
+    on_beta(beta);
+    op_apply(c, At, u, ws.Atu);
+    k_axpby<T>(c, n, T(1), ws.Atu, -beta, ws.Nv);
+    if (!s.NisI) op_apply(c, N, ws.Nv, v, ldiv);
+    alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+    if (alpha != 0) {
+      k_scal<T>(c, n, T(1) / alpha, v);
+      if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+    }
+  }
+  return beta;
+}
+
+struct Exit {
+  bool solved = false, tired = false, ill_cond = false, ill_cond_mach = false, ill_cond_lim = false;
+  bool zero_resid = false, fwd_err = false, on_boundary = false, user_exit = false, overtimed = false;
+  const char* status() const {   // termination status, in the reference's order of precedence (lsqr.jl:423-431)
+    const char* st = "unknown";
+    if (tired) st = "maximum number of iterations exceeded";
+    if (ill_cond_mach) st = "condition number seems too large for this machine";
+    if (ill_cond_lim) st = "condition number exceeds tolerance";
+    if (solved) st = "found approximate minimum least-squares solution";
+    if (zero_resid) st = "found approximate zero-residual solution";
+    if (fwd_err) st = "truncated forward error small enough";
+    if (on_boundary) st = "on trust-region boundary";
+    if (user_exit) st = "user-requested exit";
+    if (overtimed) st = "time limit exceeded";
+    return st;
+  }
+};
+
+template <class T> void early_exit(Workspace<T>& ws, double start_time, const char* status) {
+  ws.ctx.sync();
+  ws.stats.niter = 0; ws.stats.solved = true; ws.stats.inconsistent = false;
+  ws.stats.timer = now_seconds() - start_time;
+  ws.stats.status = status;
+}
+
+template <class T> int ls_itmax(const Workspace<T>& ws, int itmax) {
+  if (itmax != 0) return itmax;
+  const long long mn = (long long)ws.m + ws.n;
+  return mn > 2147483647LL ? 2147483647 : (int)mn;
+}
+
+}  // namespace
+
+// ===========================================================================
+// lsqr!  (src/lsqr.jl:174-440)
+// ===========================================================================
+template <class T>
+void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                const SolveOpts& o) {
+  const double start_time = now_seconds();
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("LSQR: system of %d equations in %d variables\n", m, n);
+  const T lambda = (T)o.lambda, lambda2 = lambda * lambda;
+  const T conlim = o.conlim < 0 ? T(1) / std::sqrt(eps_of<T>()) : (T)o.conlim;
+  const T ctol = conlim > 0 ? T(1) / conlim : T(0);
+  const T etol = tol_of<T>(o.etol), axtol = tol_of<T>(o.axtol), btol = tol_of<T>(o.btol);
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol), radius = (T)o.radius;
+  Stats& stats = ws.stats;
+  std::vector<T>& err_vec = ws.err_vec;
+
+  T beta1;
+  const Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta1);
+  if (beta1 == 0) {
+    early_exit(ws, start_time, "x is a zero-residual solution");
+    if (history) { stats.residuals.push_back(0); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  T beta = beta1;
+  lsq_start<T>(ws, s, At, N, ldiv, beta1);
+  T* v = s.NisI ? ws.Nv : ws.v;
+  T Anorm2 = k_dot<T>(c, n, v, ws.Nv);
+  T Anorm = std::sqrt(Anorm2);
+  T alpha = Anorm;
+  T Acond = 0, xNorm = 0, xNorm2 = 0, dNorm2 = 0, c2 = -1, s2 = 0, z = 0;
+  T xENorm2 = 0, err_lbnd = 0;
+  const int window = (int)err_vec.size();
+  std::fill(err_vec.begin(), err_vec.end(), T(0));
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+  if (o.verbose > 0) {
+    printf("%5s  %7s  %7s  %7s  %7s  %7s  %7s  %7s  %7s  %5s\n", "k", "α", "β", "‖r‖", "‖Aᴴr‖", "compat", "backwrd", "‖A‖", "κ(A)", "timer");
+    printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)beta1, (double)alpha, (double)beta1,
+           (double)alpha, 0.0, 1.0, (double)Anorm, (double)Acond, now_seconds() - start_time);
+  }
+  T rNorm = beta1, r1Norm = rNorm, r2Norm = rNorm, res2 = 0;
+  (void)r1Norm;
+  if (history) stats.residuals.push_back(r2Norm);
+  T ArNorm = alpha * beta;
+  const T ArNorm0 = ArNorm;
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  if (alpha == 0) {                                          // Aᴴb = 0: x = 0 is a minimum least-squares solution
+    early_exit(ws, start_time, "x is a minimum least-squares solution");
+    return;
+  }
+  k_scal<T>(c, n, T(1) / alpha, v);
+  if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+  k_copy<T>(c, n, ws.w, v);
+
+  T phibar = beta1, rhobar = alpha;
+  Exit ex;
+  const bool solved_lim0 = ArNorm / (Anorm * rNorm) <= axtol;
+  const bool solved_mach0 = T(1) + ArNorm / (Anorm * rNorm) <= T(1);
+  ex.solved = solved_mach0 || solved_lim0;
+  ex.tired = iter >= itmax;
+  ex.zero_resid = (T(1) + rNorm / beta1 <= T(1)) || (rNorm / beta1 <= axtol);
+
+  while (!(ex.solved || ex.tired || ex.ill_cond || ex.user_exit || ex.overtimed)) {
+    iter = iter + 1;
+    T ww = 0;
+    bool scale_v = false;
+    if (s.fused) {
+      // P1 + P2 and one read-back of {beta, alpha, <w, w>}; v /= alpha is applied by P3
+      T alpha_new;
+      lsq_fused_bidiag<T>(ws, *A.csr, *At.csr, iter == 1, alpha, true, &beta, &alpha_new, &ww);
+      if (beta != 0) {
+        Anorm2 = Anorm2 + alpha * alpha + beta * beta;       // = ‖B_{k-1}‖²
+        if (lambda > 0) Anorm2 += lambda2;
+        alpha = alpha_new;
+        scale_v = alpha != 0;
+      }
+    } else {
+      beta = lsq_bidiag_step<T>(ws, s, A, At, M, N, ldiv, alpha, [&](T bt) {
+        Anorm2 = Anorm2 + alpha * alpha + bt * bt;
+        if (lambda > 0) Anorm2 += lambda2;
+      });
+    }
+
+    // 1. Eliminate the regularization parameter.
+    T c1, s1, rhobar1;
+    sym_givens<T>(rhobar, lambda, &c1, &s1, &rhobar1);
+    const T psi = s1 * phibar;
+    phibar = c1 * phibar;
+    // 2. Eliminate beta.
+    T cs, sn, rho;
+    sym_givens<T>(rhobar1, beta, &cs, &sn, &rho);
+    const T phi = cs * phibar;
+    phibar = sn * phibar;
+
+    xENorm2 = xENorm2 + phi * phi;
+    err_vec[iter % window] = phi;
+    if (iter >= window) err_lbnd = err_window_norm(err_vec);
+
+    const T tau = sn * phi;
+    const T theta = sn * alpha;
+    rhobar = -cs * alpha;
+    if (!s.fused) ww = k_dot<T>(c, n, ws.w, ws.w);
+    dNorm2 += ww / (rho * rho);
+
+    T sigma = phi / rho;
+    if (radius > 0) sigma = clip_to_boundary<T>(c, n, ws.x, ws.w, v, radius, sigma, ex.on_boundary);
+
+    if (s.fused) {
+      lsq_fused_update<T>(ws, false, scale_v, T(1) / alpha, sigma, theta / rho, T(0));
+    } else {
+      k_axpy<T>(c, n, sigma, ws.w, ws.x);                       // x = x + ϕ / ρ * w
+      k_axpby<T>(c, n, T(1), v, -theta / rho, ws.w);            // w = v - θ / ρ * w
+    }
+
+    // plane rotation on the right: estimate of ‖x‖
+    const T delta = s2 * rho;
+    const T gammabar = -c2 * rho;
+    const T rhs = phi - delta * z;
+    const T zbar = rhs / gammabar;
+    xNorm = std::sqrt(xNorm2 + zbar * zbar);
+    T gamma;
+    sym_givens<T>(gammabar, theta, &c2, &s2, &gamma);
+    z = rhs / gamma;
+    xNorm2 += z * z;
+
+    Anorm = std::sqrt(Anorm2);
+    Acond = Anorm * std::sqrt(dNorm2);
+    const T res1 = phibar * phibar;
+    res2 += psi * psi;
+    rNorm = std::sqrt(res1 + res2);
+
+    ArNorm = alpha * std::fabs(tau);
+    if (history) stats.Aresiduals.push_back(ArNorm);
+
+    const T r1sq = rNorm * rNorm - lambda2 * xNorm2;
+    r1Norm = std::sqrt(std::fabs(r1sq));
+    if (r1sq < 0) r1Norm = -r1Norm;
+    r2Norm = rNorm;
+    if (history) stats.residuals.push_back(r2Norm);
+
+    const T test1 = rNorm / beta1;
+    const T test2 = ArNorm / (Anorm * rNorm);
+    const T test3 = T(1) / Acond;
+    const T t1 = test1 / (T(1) + Anorm * xNorm / beta1);
+    const T rNormtol = btol + axtol * Anorm * xNorm / beta1;
+    if (kdisplay(iter, o.verbose))
+      printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)alpha, (double)beta, (double)rNorm,
+             (double)ArNorm, (double)test1, (double)test2, (double)Anorm, (double)Acond, now_seconds() - start_time);
+
+    ex.ill_cond_mach = (T(1) + test3 <= T(1));
+    const bool solved_mach = (T(1) + test2 <= T(1));
+    const bool zero_resid_mach = (T(1) + t1 <= T(1));
+    if (o.callback) { c.sync(); stats.niter = iter; ex.user_exit = o.callback(&ws, o.callback_user) != 0; }
+    ex.tired = iter >= itmax;
+    ex.ill_cond_lim = (test3 <= ctol);
+    const bool solved_lim = (test2 <= axtol);
+    const bool solved_opt = ArNorm <= atol + rtol * ArNorm0;
+    const bool zero_resid_lim = (test1 <= rNormtol);
+    if (iter >= window) ex.fwd_err = err_lbnd <= etol * std::sqrt(xENorm2);
+    ex.ill_cond = ex.ill_cond_mach || ex.ill_cond_lim;
+    ex.zero_resid = zero_resid_mach || zero_resid_lim;
+    ex.solved = solved_mach || solved_lim || solved_opt || ex.zero_resid || ex.fwd_err || ex.on_boundary;
+    ex.overtimed = (now_seconds() - start_time) > o.timemax;
+  }
+  if (o.verbose > 0) printf("\n");
+  c.sync();
+  stats.niter = iter; stats.solved = ex.solved; stats.inconsistent = !ex.zero_resid;
+  stats.timer = now_seconds() - start_time;
+  stats.status = ex.status();
+}
+
+// ===========================================================================
+// lsmr!  (src/lsmr.jl:178-455)
+// ===========================================================================
+template <class T>
+void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                const SolveOpts& o) {
+  const double start_time = now_seconds();
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("LSMR: system of %d equations in %d variables\n", m, n);
+  const T lambda = (T)o.lambda;
+  const T conlim = o.conlim < 0 ? T(1) / std::sqrt(eps_of<T>()) : (T)o.conlim;
+  const T ctol = conlim > 0 ? T(1) / conlim : T(0);
+  const T etol = tol_of<T>(o.etol), axtol = tol_of<T>(o.axtol), btol = tol_of<T>(o.btol);
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol), radius = (T)o.radius;
+  Stats& stats = ws.stats;
+  std::vector<T>& err_vec = ws.err_vec;
+
+  T beta1;
+  const Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta1);
+  if (beta1 == 0) {
+    early_exit(ws, start_time, "x is a zero-residual solution");
+    if (history) { stats.residuals.push_back(0); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  T beta = beta1;
+  lsq_start<T>(ws, s, At, N, ldiv, beta1);
+  T* v = s.NisI ? ws.Nv : ws.v;
+  T alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+
+  T zetabar = alpha * beta, alphabar = alpha, rho = 1, rhobar = 1, cbar = 1, sbar = 0;
+  T betadd = beta, betad = 0, rhodold = 1, tautildeold = 0, thetatilde = 0, zeta = 0, d = 0;
+  T Anorm2 = alpha * alpha, maxrbar = 0;
+  T minrbar = std::min(std::numeric_limits<T>::max(), (T)1.0e+100);
+  T Acond = maxrbar / minrbar, Anorm = std::sqrt(Anorm2), xNorm = 0;
+  T rNorm = beta;
+  if (history) stats.residuals.push_back(rNorm);
+  T ArNorm = alpha * beta;
+  const T ArNorm0 = ArNorm;
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  T xENorm2 = 0, err_lbnd = 0;
+  const int window = (int)err_vec.size();
+  std::fill(err_vec.begin(), err_vec.end(), T(0));
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+  if (o.verbose > 0) {
+    printf("%5s  %7s  %7s  %7s  %7s  %8s  %8s  %7s  %5s\n", "k", "‖r‖", "‖Aᴴr‖", "β", "α", "cos", "sin", "‖A‖²", "timer");
+    printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %.2fs\n", iter, (double)beta1, (double)alpha, (double)beta1,
+           (double)alpha, 0.0, 1.0, (double)Anorm2, now_seconds() - start_time);
+  }
+  if (alpha == 0) {                                          // Aᴴb = 0: x = 0 is a minimum least-squares solution
+    early_exit(ws, start_time, "x is a minimum least-squares solution");
+    stats.Anorm = Anorm;
+    return;
+  }
+  k_scal<T>(c, n, T(1) / alpha, v);
+  if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+  k_copy<T>(c, n, ws.h, v);
+  k_fill<T>(c, n, ws.hbar, T(0));
+
+  Exit ex;
+  ex.solved = (rNorm <= axtol);
+  ex.tired = iter >= itmax;
+
+  while (!(ex.solved || ex.tired || ex.ill_cond || ex.user_exit || ex.overtimed)) {
+    iter = iter + 1;
+    bool scale_v = false;
+    if (s.fused) {
+      T alpha_new, unused;
+      lsq_fused_bidiag<T>(ws, *A.csr, *At.csr, iter == 1, alpha, false, &beta, &alpha_new, &unused);
+      if (beta != 0) { alpha = alpha_new; scale_v = alpha != 0; }
+    } else {
+      beta = lsq_bidiag_step<T>(ws, s, A, At, M, N, ldiv, alpha, [](T) {});
+    }
+
+    // Continue QR factorization
+    T chat, shat, alphahat;
+    sym_givens<T>(alphabar, lambda, &chat, &shat, &alphahat);
+    const T rhoold = rho;
+    T cs, sn;
+    sym_givens<T>(alphahat, beta, &cs, &sn, &rho);
+    const T thetanew = sn * alpha;
+    alphabar = cs * alpha;
+
+    const T rhobarold = rhobar;
+    const T zetaold = zeta;
+    const T thetabar = sbar * rho;
+    const T rhotemp = cbar * rho;
+    sym_givens<T>(rhotemp, thetanew, &cbar, &sbar, &rhobar);
+    zeta = cbar * zetabar;
+    zetabar = -sbar * zetabar;
+
+    xENorm2 = xENorm2 + zeta * zeta;
+    err_vec[iter % window] = zeta;
+    if (iter >= window) err_lbnd = err_window_norm(err_vec);
+
+    // Update h, hbar and x.
+    const T delta = thetabar * rho / (rhoold * rhobarold);   // δₖ = θbarₖ * ρₖ / (ρₖ₋₁ * ρbarₖ₋₁)
+    T sigma = zeta / (rho * rhobar);
+    if (s.fused) {
+      xNorm = lsq_fused_update<T>(ws, true, scale_v, T(1) / alpha, sigma, thetanew / rho, delta);
+    } else {
+      k_axpby<T>(c, n, T(1), ws.h, -delta, ws.hbar);            // ĥₖ = hₖ - δₖ * ĥₖ₋₁
+      if (radius > 0) sigma = clip_to_boundary<T>(c, n, ws.x, ws.hbar, v, radius, sigma, ex.on_boundary);
+      k_axpy<T>(c, n, sigma, ws.hbar, ws.x);                    // xₖ = xₖ₋₁ + σₖ * ĥₖ
+      k_axpby<T>(c, n, T(1), v, -thetanew / rho, ws.h);         // hₖ₊₁ = vₖ₊₁ - (θₖ₊₁/ρₖ) * hₖ
+    }
+
+    // Estimate ‖r‖.
+    const T betaacute = chat * betadd;
+    const T betacheck = -shat * betadd;
+    const T betahat = cs * betaacute;
+    betadd = -sn * betaacute;
+    const T thetatildeold = thetatilde;
+    T ctildeold, stildeold, rhotildeold;
+    sym_givens<T>(rhodold, thetabar, &ctildeold, &stildeold, &rhotildeold);
+    thetatilde = stildeold * rhobar;
+    rhodold = ctildeold * rhobar;
+    betad = -stildeold * betad + ctildeold * betahat;
+    tautildeold = (zetaold - thetatildeold * tautildeold) / rhotildeold;
+    const T taud = (zeta - thetatilde * tautildeold) / rhodold;
+    d = d + betacheck * betacheck;
+    rNorm = std::sqrt(d + (betad - taud) * (betad - taud) + betadd * betadd);
+    if (history) stats.residuals.push_back(rNorm);
+
+    // Estimate ‖A‖.
+    Anorm2 += beta * beta;
+    Anorm = std::sqrt(Anorm2);
+    Anorm2 += alpha * alpha;
+
+    // Estimate cond(A).
+    maxrbar = std::max(maxrbar, rhobarold);
+    if (iter > 1) minrbar = std::min(minrbar, rhobarold);
+    Acond = std::max(maxrbar, rhotemp) / std::min(minrbar, rhotemp);
+
+    // Test for convergence.
+    ArNorm = std::fabs(zetabar);
+    if (history) stats.Aresiduals.push_back(ArNorm);
+    if (!s.fused) xNorm = k_nrm2<T>(c, n, ws.x);
+
+    const T test1 = rNorm / beta1;
+    const T test2 = ArNorm / (Anorm * rNorm);
+    const T test3 = T(1) / Acond;
+    const T t1 = test1 / (T(1) + Anorm * xNorm / beta1);
+    const T rNormtol = btol + axtol * Anorm * xNorm / beta1;
+    if (kdisplay(iter, o.verbose))
+      printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm, (double)beta,
+             (double)alpha, (double)cs, (double)sn, (double)Anorm2, now_seconds() - start_time);
+
+    ex.ill_cond_mach = (T(1) + test3 <= T(1));
+    const bool solved_mach = (T(1) + test2 <= T(1));
+    const bool zero_resid_mach = (T(1) + t1 <= T(1));
+    if (o.callback) { c.sync(); stats.niter = iter; ex.user_exit = o.callback(&ws, o.callback_user) != 0; }
+    ex.tired = iter >= itmax;
+    ex.ill_cond_lim = (test3 <= ctol);
+    const bool solved_lim = (test2 <= axtol);
+    const bool solved_opt = ArNorm <= atol + rtol * ArNorm0;
+    const bool zero_resid_lim = (test1 <= rNormtol);
+    if (iter >= window) ex.fwd_err = err_lbnd <= etol * std::sqrt(xENorm2);
+    ex.ill_cond = ex.ill_cond_mach || ex.ill_cond_lim;
+    ex.zero_resid = zero_resid_mach || zero_resid_lim;
+    ex.solved = solved_mach || solved_lim || solved_opt || ex.zero_resid || ex.fwd_err || ex.on_boundary;
+    ex.overtimed = (now_seconds() - start_time) > o.timemax;
+  }
+  if (o.verbose > 0) printf("\n");
+  c.sync();
+  stats.Anorm = Anorm;
+  stats.niter = iter; stats.solved = ex.solved; stats.inconsistent = !ex.zero_resid;
+  stats.timer = now_seconds() - start_time;
+  stats.status = ex.status();
+}
+
+#define INST(T)                                                                                                         \
+  template void lsqr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
+                              const SolveOpts&);                                                                        \
+  template void lsmr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
+                              const SolveOpts&);
+INST(double)
+INST(float)
+#undef INST
+
+}  // namespace kb

@@ -33,7 +33,7 @@ void coo_to_csr(int n, const std::vector<int>& I, const std::vector<int>& J, con
     std::vector<long long> pos(cnt.begin(), cnt.end() - 1);
     for (size_t k = 0; k < nz; k++) { const long long q = pos[I[k]]++; cj[q] = J[k]; cv[q] = V[k]; }
   }
-  out.n = n;
+  out.n = n; out.ncols = n;
   out.rowptr.assign((size_t)n + 1, 0);
   out.colind.clear(); out.val.clear();
   out.colind.reserve(nz); out.val.reserve(nz);
@@ -96,17 +96,20 @@ void read_matrix_market(const char* path, HostCsr& out) {
   coo_to_csr((int)M, I, J, V, out);
 }
 
-// out = A^T (columns ascending by construction)
+// out = A^T, m x n -> n x m.  Rows of A are scattered in ascending order, so every row of A^T lists its columns (the
+// rows of A) in ascending order and A^T u sums in ascending row order of A, as a sequential A' * u does.
 void transpose_csr(const HostCsr& A, HostCsr& out) {
-  const int n = A.n;
+  const int m = A.n, n = A.ncols;
   const size_t nz = A.colind.size();
-  out.n = n;
+  for (size_t k = 0; k < nz; k++)
+    if (A.colind[k] < 0 || A.colind[k] >= n) throw std::runtime_error("transpose: column index outside the operator's columns");
+  out.n = n; out.ncols = m;
   out.rowptr.assign((size_t)n + 1, 0);
   for (size_t k = 0; k < nz; k++) out.rowptr[(size_t)A.colind[k] + 1]++;
   for (int i = 0; i < n; i++) out.rowptr[(size_t)i + 1] += out.rowptr[i];
   out.colind.resize(nz); out.val.resize(nz);
   std::vector<long long> pos(out.rowptr.begin(), out.rowptr.end() - 1);
-  for (int i = 0; i < n; i++)
+  for (int i = 0; i < m; i++)
     for (long long k = A.rowptr[i]; k < A.rowptr[(size_t)i + 1]; k++) {
       const long long q = pos[A.colind[k]]++;
       out.colind[q] = i; out.val[q] = A.val[k];
@@ -115,11 +118,11 @@ void transpose_csr(const HostCsr& A, HostCsr& out) {
 
 template <class T> void csr_from_host(Ctx& c, Csr<T>& dst, const HostCsr& h) {
   std::vector<T> v(h.val.begin(), h.val.end());
-  csr_upload<T>(c, dst, h.n, (long long)h.colind.size(), h.rowptr.data(), h.colind.data(), v.data(), 0, 8, false);
+  csr_upload<T>(c, dst, h.n, (long long)h.colind.size(), h.rowptr.data(), h.colind.data(), v.data(), 0, 8, false, h.ncols);
 }
 
 template <class T> void csr_to_host(Ctx& c, const Csr<T>& A, HostCsr& h) {
-  h.n = A.n;
+  h.n = A.n; h.ncols = A.ncols;
   std::vector<int> rp((size_t)A.n + 1), ci((size_t)A.nnz);
   std::vector<T> v((size_t)A.nnz);
   KB_CUDA(cudaMemcpyAsync(rp.data(), A.rowptr, sizeof(int) * rp.size(), cudaMemcpyDeviceToHost, c.stream));

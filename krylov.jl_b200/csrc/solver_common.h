@@ -79,4 +79,27 @@ template <class T> static inline int roots_quadratic(T q2, T q1, T q0, int nitre
   return 0;
 }
 
+// to_boundary (src/krylov_utils.jl:375-402)
+template <class T>
+static inline int to_boundary(Ctx& c, int n, const T* x, const T* d, T* z, T radius, T dNorm2, const LinOp<T>& M, bool ldiv, T* s1, T* s2) {
+  if (!(radius > 0)) return 1;
+  T rxd, xNorm2 = 0;
+  if (M.is_identity()) {
+    rxd = k_dot<T>(c, n, x, d);
+    if (dNorm2 == T(0)) dNorm2 = k_dot<T>(c, n, d, d);
+    xNorm2 = k_dot<T>(c, n, x, x);
+  } else {
+    op_apply(c, M, x, z, ldiv);
+    rxd = k_dot<T>(c, n, z, d);
+    xNorm2 = k_dot<T>(c, n, z, x);
+    op_apply(c, M, d, z, ldiv);
+    dNorm2 = k_dot<T>(c, n, z, d);
+  }
+  if (dNorm2 == T(0)) return 2;
+  const T radius2 = radius * radius;
+  if (!(xNorm2 <= radius2)) return 3;
+  if (roots_quadratic<T>(dNorm2, 2 * rxd, xNorm2 - radius2, 1, s1, s2)) return 4;
+  return 0;
+}
+
 }  // namespace kb

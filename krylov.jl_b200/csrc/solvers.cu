@@ -17,7 +17,7 @@ namespace kb {
 // ---------------------------------------------------------------------------
 template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int memory, int window, int device) {
   const double t0 = now_seconds();
-  if (m != n) throw std::runtime_error("System must be square");
+  if (m != n && !is_ls_kind(kind)) throw std::runtime_error("System must be square");
   Workspace<T>* ws = new Workspace<T>();
   try {
     ws->kind = kind; ws->m = m; ws->n = n;
@@ -61,6 +61,12 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         break;
       }
       case S_CG_LANCZOS: ws->Mv = A(); ws->Mv_prev = A(); ws->p = A(); ws->Mv_next = A(); break;    // CgLanczosWorkspace :575-591
+      case S_LSQR: case S_LSMR:                     // LsqrWorkspace / LsmrWorkspace: Av, Aᴴu, u, v are allocated by the solve
+        ws->Nv = A(); ws->Mu = dev_alloc<T>((size_t)m);
+        if (kind == S_LSQR) ws->w = A(); else { ws->h = A(); ws->hbar = A(); }
+        ws->window = window > 0 ? window : 5;
+        ws->err_vec.assign(ws->window, T(0));
+        break;
       default: throw std::runtime_error("unsupported solver");
     }
   } catch (...) {
@@ -76,7 +82,7 @@ template <class T> void ws_destroy(Workspace<T>* ws) {
   if (ws->ctx.stream) cudaStreamSynchronize(ws->ctx.stream);
   T* vecs[] = {ws->x, ws->dx, ws->r, ws->p, ws->Ap, ws->z, ws->npc_dir, ws->p2, ws->v, ws->s, ws->qd, ws->t, ws->yz,
                ws->r1, ws->r2, ws->w1, ws->w2, ws->y, ws->vv, ws->w, ws->q, ws->pp, ws->bbuf, ws->cbuf,
-               ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next};
+               ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next, ws->Nv, ws->Mu, ws->Av, ws->Atu, ws->h, ws->hbar};
   for (T* p : vecs) dev_free(p);
   for (T* p : ws->V) dev_free(p);
   for (T* p : ws->Z) dev_free(p);
@@ -110,9 +116,6 @@ template <class T> void ws_warm_start(Workspace<T>* ws, const T* x0_dev) {
 // ===========================================================================
 // cg!  (src/cg.jl:120-291)
 // ===========================================================================
-template <class T>
-static int to_boundary(Ctx& c, int n, const T* x, const T* d, T* z, T radius, T dNorm2, const LinOp<T>& M, bool ldiv, T* s1, T* s2);
-
 template <class T>
 void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
   const double start_time = now_seconds();
@@ -250,29 +253,6 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   stats.niter = iter; stats.solved = solved; stats.inconsistent = inconsistent;
   stats.timer = now_seconds() - start_time;
   stats.status = status;
-}
-
-// to_boundary (src/krylov_utils.jl:375-402)
-template <class T>
-static int to_boundary(Ctx& c, int n, const T* x, const T* d, T* z, T radius, T dNorm2, const LinOp<T>& M, bool ldiv, T* s1, T* s2) {
-  if (!(radius > 0)) return 1;
-  T rxd, xNorm2 = 0;
-  if (M.is_identity()) {
-    rxd = k_dot<T>(c, n, x, d);
-    if (dNorm2 == T(0)) dNorm2 = k_dot<T>(c, n, d, d);
-    xNorm2 = k_dot<T>(c, n, x, x);
-  } else {
-    op_apply(c, M, x, z, ldiv);
-    rxd = k_dot<T>(c, n, z, d);
-    xNorm2 = k_dot<T>(c, n, z, x);
-    op_apply(c, M, d, z, ldiv);
-    dNorm2 = k_dot<T>(c, n, z, d);
-  }
-  if (dNorm2 == T(0)) return 2;
-  const T radius2 = radius * radius;
-  if (!(xNorm2 <= radius2)) return 3;
-  if (roots_quadratic<T>(dNorm2, 2 * rxd, xNorm2 - radius2, 1, s1, s2)) return 4;
-  return 0;
 }
 
 // ===========================================================================

@@ -33,12 +33,13 @@ __global__ void fill_int_kernel(int cnt, int* out, int v) {
 
 template <class T>
 void csr_upload(Ctx& c, Csr<T>& A, int n, long long nnz, const void* rowptr, const void* colind, const T* val,
-                int index_base, int index_bytes, bool on_device) {
+                int index_base, int index_bytes, bool on_device, int ncols) {
+  if (ncols < 0) ncols = n;
   if (n < 0 || nnz < 0 || nnz > 2147483647LL - 64) throw std::runtime_error("CSR operator: n/nnz out of int32 range");
   if (index_bytes != 4 && index_bytes != 8) throw std::runtime_error("CSR operator: index_bytes must be 4 or 8");
   if (index_base != 0 && index_base != 1) throw std::runtime_error("CSR operator: index_base must be 0 or 1");
   csr_free(A);
-  A.n = n; A.nnz = nnz;
+  A.n = n; A.ncols = ncols; A.nnz = nnz;
   const size_t rp_len = (size_t)n + 1, rp_pad = kTileRows + 16;
   A.rowptr = dev_alloc<int>(rp_len + rp_pad);
   A.colind = dev_alloc<int>((size_t)nnz + 16);
@@ -95,7 +96,7 @@ template <class T> void csr_free(Csr<T>& A) {
 // Staging plan: largest tile (nnz of kTileRows consecutive rows) and longest
 // row decide whether the TMA ring fits, how deep it is, and the grid.
 // ---------------------------------------------------------------------------
-__global__ void plan_kernel(int n, int ntiles, const int* __restrict__ rowptr,
+__global__ void plan_kernel(int n, int ncols, int ntiles, const int* __restrict__ rowptr,
                             int* out /* [0]=tile_cap [1]=max_row [2]=unsorted [3]=rowptr not monotone [4]=max col [5]=negative col */,
                             const int* __restrict__ colind, long long nnz) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -108,8 +109,8 @@ __global__ void plan_kernel(int n, int ntiles, const int* __restrict__ rowptr,
     if (kb > ke || kb < 0 || (long long)ke > nnz) { bad = 1; continue; }
     mr = max(mr, ke - kb);
     for (int k = kb; k < ke; k++) { const int cj = colind[k]; mc = max(mc, cj); neg |= cj < 0; }
-    // halo columns (index >= n, row-partitioned operators) keep their global position in the row: skip them
-    for (int k = kb + 1; k < ke; k++) uns |= (colind[k] <= colind[k - 1]) && colind[k] < n && colind[k - 1] < n;
+    // halo columns (index >= ncols, row-partitioned operators) keep their global position in the row: skip them
+    for (int k = kb + 1; k < ke; k++) uns |= (colind[k] <= colind[k - 1]) && colind[k] < ncols && colind[k - 1] < ncols;
   }
   if (bad) atomicExch(&out[3], 1);
   __syncthreads();
@@ -133,7 +134,7 @@ template <class T> void csr_plan(Ctx& c, Csr<T>& A) {
   int ends[2] = {0, (int)A.nnz};
   if (A.n > 0) {
     KB_CUDA(cudaMemcpyAsync(dout + 4, &h[4], sizeof(int), cudaMemcpyHostToDevice, c.stream));
-    plan_kernel<<<sm_count() * 4, 256, 0, c.stream>>>(A.n, A.ntiles, A.rowptr, dout, A.colind, A.nnz);
+    plan_kernel<<<sm_count() * 4, 256, 0, c.stream>>>(A.n, A.ncols, A.ntiles, A.rowptr, dout, A.colind, A.nnz);
     KB_CUDA(cudaGetLastError());
     KB_CUDA(cudaMemcpyAsync(&ends[0], A.rowptr, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     KB_CUDA(cudaMemcpyAsync(&ends[1], A.rowptr + A.n, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
@@ -313,7 +314,7 @@ template <class T> void op_apply(Ctx& c, const LinOp<T>& op, const T* x, T* y, b
     case LinOp<T>::HOST_CB:
       // reference: ccall(op.fptr, ..., x, y, userdata) on host pointers
       // (interfaces/src/c_operator.jl:35-42); here x/y live in HBM, so stage.
-      KB_CUDA(cudaMemcpyAsync(op.hx, x, sizeof(T) * (size_t)op.n, cudaMemcpyDeviceToHost, c.stream));
+      KB_CUDA(cudaMemcpyAsync(op.hx, x, sizeof(T) * (size_t)(op.nin ? op.nin : op.n), cudaMemcpyDeviceToHost, c.stream));
       c.sync();
       op.fn(op.hx, op.hy, op.userdata);
       KB_CUDA(cudaMemcpyAsync(y, op.hy, sizeof(T) * (size_t)op.n, cudaMemcpyHostToDevice, c.stream));
@@ -323,7 +324,7 @@ template <class T> void op_apply(Ctx& c, const LinOp<T>& op, const T* x, T* y, b
 }
 
 #define INST(T)                                                                                                  \
-  template void csr_upload<T>(Ctx&, Csr<T>&, int, long long, const void*, const void*, const T*, int, int, bool); \
+  template void csr_upload<T>(Ctx&, Csr<T>&, int, long long, const void*, const void*, const T*, int, int, bool, int); \
   template void csr_free<T>(Csr<T>&);                                                                            \
   template void csr_plan<T>(Ctx&, Csr<T>&);                                                                      \
   template void k_spmv<T>(Ctx&, const Csr<T>&, const T*, T*, int);                                               \

@@ -69,6 +69,27 @@ struct XPlain {
   __device__ __forceinline__ T operator()(int j) const { return __ldg(&x[j]); }
 };
 
+// x gather with a pending scale (LSQR / LSMR: u = Mu / beta is never written back, every read applies the factor).
+// The factor is produced on the device by the previous kernel; gather_for_cta() loads it once per CTA, and each
+// gathered value is x[j] * scale rounded once -- the product kscal! would have stored.
+template <class T>
+struct XScaled {
+  const T* __restrict__ x;
+  const T* scale_src;
+  T scale;
+  __device__ __forceinline__ T operator()(int j) const { return mul_rn(__ldg(&x[j]), scale); }
+};
+
+// Per-CTA set-up of a gather functor before the tile loop (identity for the plain and halo gathers).
+template <class G>
+__device__ __forceinline__ G gather_for_cta(const G& g) { return g; }
+template <class T>
+__device__ __forceinline__ XScaled<T> gather_for_cta(const XScaled<T>& g) {
+  XScaled<T> out = g;
+  out.scale = *g.scale_src;
+  return out;
+}
+
 // Row-partitioned operators: column j >= nloc is halo entry j - nloc of the local halo buffer (filled by
 // k_halo_exchange); the source is chosen by a pointer select, not a branch, so the batch of gathers stays a
 // straight line of loads.

@@ -104,12 +104,23 @@ mutable struct B200CSR{T<:BlasT}
 end
 # SparseMatrixCSC{T,Int64} is CSC, 1-based, Int64.  CSR(A) == CSC(A'): for the (symmetric) CG/MINRES
 # operators the arrays can be passed as they are; for a general A pass the CSC arrays of copy(A').
-function B200CSR(A::SparseMatrixCSC{T,Int64}; symmetric::Bool = issymmetric(A)) where T<:BlasT
+function B200CSR(A::SparseMatrixCSC{T,Int64}; symmetric::Bool = size(A, 1) == size(A, 2) && issymmetric(A)) where T<:BlasT
+  size(A, 1) == size(A, 2) || return rect_csr(A)
   At = symmetric ? A : SparseMatrixCSC(transpose(A))
   h = ccall((:kb200_csr_create, lib), Ptr{Cvoid},
             (Ptr{Cvoid}, Cint, Cint, Clonglong, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Cint),
             ctx(), dtype_id(T), size(A, 1), nnz(A), At.colptr, At.rowval, At.nzval, 1, 8, 0)
   B200CSR{T}(h, size(A)...)
+end
+# Rectangular A (LSQR / LSMR): the CSC arrays of A are the CSR arrays of A^T (n x m), so upload those as they are and
+# let the library form A from them -- one transpose instead of one here and one in the library.
+function rect_csr(A::SparseMatrixCSC{T,Int64}) where T<:BlasT
+  m, n = size(A)
+  ht = ccall((:kb200_csr_create_rect, lib), Ptr{Cvoid},
+             (Ptr{Cvoid}, Cint, Cint, Cint, Clonglong, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Cint),
+             ctx(), dtype_id(T), n, m, nnz(A), A.colptr, A.rowval, A.nzval, 1, 8, 0)
+  At = B200CSR{T}(ht, n, m)
+  adjoint(At)
 end
 # Matrix Market ingestion on the library side (benchmark/benchmarks.jl:23-33 reads SuiteSparse .mtx files)
 function B200CSR(path::AbstractString, ::Type{T} = Float64) where T<:BlasT
@@ -119,8 +130,10 @@ function B200CSR(path::AbstractString, ::Type{T} = Float64) where T<:BlasT
   check(ccall((:kb200_csr_info, lib), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Clonglong}), h, n, nz))
   B200CSR{T}(h, n[], n[])
 end
-# A' : a new device-resident operator holding the transpose (= adjoint for the real types of this path);
-# opens the LSQR / LSMR / BiLQ / QMR family through the primitive overloads (docs/src/matrix_free.md:36-44)
+# A' : a new device-resident operator holding the transpose (= adjoint for the real types of this path), square or
+# rectangular.  lsqr! / lsmr! on a B200CSR run natively (ls_solve! below; the library forms and caches A^T itself);
+# the other methods of the family (BiLQ, QMR, CGLS, CRAIG, ...) reach A' through the primitive overloads, one `ccall`
+# per k* operation (docs/src/matrix_free.md:36-44)
 function Base.adjoint(A::B200CSR{T}) where T
   h = ccall((:kb200_csr_transpose, lib), Ptr{Cvoid}, (Ptr{Cvoid}, Ptr{Cvoid}), ctx(), A.handle)
   B200CSR{T}(h, A.n, A.m)
@@ -182,7 +195,7 @@ end
 # created ONCE per Krylov.jl workspace and kept in HANDLES, so an in-place solve allocates nothing
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
-                       :bicgstab => 10, :cgs => 11, :cg_lanczos => 100)
+                       :bicgstab => 10, :cgs => 11, :lsqr => 21, :lsmr => 22, :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -190,6 +203,7 @@ end
 struct CExt    # KrylovB200Options (include/krylov_b200.h)
   history::Cint; ldiv::Cint; etol::Cdouble; conlim::Cdouble; fused::Cint; batch::Cint
   callback::Ptr{Cvoid}; callback_user::Ptr{Cvoid}; time_kernels::Cint; check_curvature::Cint; cr_gamma::Cdouble
+  axtol::Cdouble; btol::Cdouble
 end
 struct CStats  # KrylovB200Stats (include/krylov_b200.h)
   niter::Cint; solved::Cint; inconsistent::Cint; indefinite::Cint; npcCount::Cint
@@ -282,7 +296,7 @@ function fused_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; c::Un
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, NaN, NaN))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, restart, reorthogonalization, linesearch))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -328,6 +342,39 @@ Krylov.minres!(ws::Krylov.MinresWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::
 Krylov.minres!(ws::Krylov.MinresWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}, x0::B200Vector{T}; kw...) where T =
   fused_solve!(:minres, ws, A, b, x0; window = length(ws.err_vec), kw...)
 
+# ---- lsqr! / lsmr! (src/lsqr.jl:142-162, src/lsmr.jl:146-166) on a rectangular B200CSR: one krylov_solve per solve ----
+# The fused Golub-Kahan passes run when M = N = I and radius = 0; B200Diagonal M (m entries) / N (n entries) and the
+# trust region run the library's primitive path.
+function ls_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N = I, ldiv::Bool = false, sqd::Bool = false,
+                   λ::T = zero(T), radius::T = zero(T), etol::T = √eps(T), axtol::T = √eps(T), btol::T = √eps(T),
+                   conlim::T = 1 / √eps(T), atol::T = zero(T), rtol::T = zero(T), itmax::Int = 0, timemax::Float64 = Inf,
+                   verbose::Int = 0, history::Bool = false, callback = workspace -> false, iostream::IO = stdout) where T
+  length(b) == A.m || error("Inconsistent problem size")
+  sqd && (λ ≠ 0) && error("sqd cannot be set to true if λ ≠ 0 !")
+  sqd && (λ = one(T))
+  h = handle_for(method, ws, A, 0, length(ws.err_vec))
+  set_precond!(h, 0, M)
+  set_precond!(h, 1, N)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, axtol, btol))
+  o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, C_NULL, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.lsqr!(ws::Krylov.LsqrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  ls_solve!(:lsqr, ws, A, b; kw...)
+Krylov.lsmr!(ws::Krylov.LsmrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  ls_solve!(:lsmr, ws, A, b; kw...)
+
 # ---- block_gmres! (src/block_gmres.jl:78-110; C ABI krylov.h:250-285): one krylov_block_solve per solve ------------------
 # B, X, X0 are column-major n x p device matrices; the library keeps row-major panels internally and runs the
 # tall-skinny products of Float64 p = 8 / 16 / 32 on the FP64 tensor cores.
@@ -362,7 +409,7 @@ function Krylov.block_gmres!(ws::Krylov.BlockGmresWorkspace{T,T,B200Vector{T},B2
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN))
   o = Ref(COpts(atol, rtol, itmax, verbose, 0.0, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, restart, reorthogonalization, false))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))

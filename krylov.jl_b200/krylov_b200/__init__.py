@@ -36,7 +36,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "elapsed_time", "Aprod_count", "warm_start_", "device_count", "B200Error",
            "FomWorkspace", "FgmresWorkspace", "CgsWorkspace", "CgLanczosWorkspace", "fom", "fom_", "fgmres", "fgmres_",
            "cgs", "cgs_", "cg_lanczos", "cg_lanczos_", "CrWorkspace", "DiomWorkspace", "DqgmresWorkspace", "cr", "cr_", "diom",
-           "diom_", "dqgmres", "dqgmres_", "BlockGmresWorkspace", "block_gmres", "block_gmres_", "CsrOperator"]
+           "diom_", "dqgmres", "dqgmres_", "BlockGmresWorkspace", "block_gmres", "block_gmres_", "CsrOperator",
+           "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_"]
 
 
 class B200Error(RuntimeError):
@@ -93,13 +94,14 @@ class CsrOperator:
         A = CsrOperator.read_mtx("bcsstk01.mtx")     # Matrix Market ingestion (benchmark/benchmarks.jl:23-33)
         At = A.transpose()                           # A^T = A^H for the real types of this path
         kb.cg(A, b)                                  # solvers accept it like a SciPy matrix
+        G = CsrOperator.from_scipy(G_mn)             # rectangular (m, n): kb.lsqr(G, b), kb.lsmr(G, b)
     """
 
     def __init__(self, csr_handle, ctx, dtype, owns_ctx=True):
         self._csr, self._ctx, self.dtype, self._owns_ctx = csr_handle, ctx, np.dtype(dtype), owns_ctx
-        n, nnz = C.c_int(), C.c_longlong()
-        lib().kb200_csr_info(self._csr, C.byref(n), C.byref(nnz))
-        self.shape, self.nnz = (n.value, n.value), nnz.value
+        m, n, nnz = C.c_int(), C.c_int(), C.c_longlong()
+        lib().kb200_csr_shape(self._csr, C.byref(m), C.byref(n), C.byref(nnz))
+        self.shape, self.nnz = (m.value, n.value), nnz.value
 
     @classmethod
     def read_mtx(cls, path, dtype=np.float64, device: int = -1):
@@ -120,8 +122,13 @@ class CsrOperator:
         dtype = np.dtype(dtype or M.dtype)
         ctx = lib().kb200_ctx_create(device)
         rp, ci, va = np.ascontiguousarray(M.indptr), np.ascontiguousarray(M.indices), np.ascontiguousarray(M.data, dtype=dtype)
-        h = lib().kb200_csr_create(ctx, _dtype_id(dtype), M.shape[0], int(M.nnz), rp.ctypes.data_as(C.c_void_p),
-                                   ci.astype(rp.dtype).ctypes.data_as(C.c_void_p), va.ctypes.data_as(C.c_void_p), 0, rp.dtype.itemsize, 0)
+        ci = ci.astype(rp.dtype)
+        args = (int(M.nnz), rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p), va.ctypes.data_as(C.c_void_p), 0,
+                rp.dtype.itemsize, 0)
+        if M.shape[0] == M.shape[1]:
+            h = lib().kb200_csr_create(ctx, _dtype_id(dtype), M.shape[0], *args)
+        else:
+            h = lib().kb200_csr_create_rect(ctx, _dtype_id(dtype), M.shape[0], M.shape[1], *args)
         if not h:
             lib().kb200_ctx_destroy(ctx)
             raise B200Error(_lib.last_error())
@@ -149,9 +156,11 @@ class CsrOperator:
     def matvec(self, x):
         """y = A x on the GPU (host arrays in and out)."""
         x = np.ascontiguousarray(x, dtype=self.dtype)
+        if x.shape[0] != self.shape[1]:
+            raise B200Error(f"x has {x.shape[0]} entries, the operator {self.shape[1]} columns")
         n = self.shape[0]
         L = lib()
-        dx, dy = L.kb200_alloc(x.nbytes), L.kb200_alloc(x.nbytes)
+        dx, dy = L.kb200_alloc(x.nbytes), L.kb200_alloc(n * self.dtype.itemsize)
         try:
             L.kb200_h2d(dx, x.ctypes.data_as(C.c_void_p), x.nbytes)
             if L.kb200_spmv_csr(self._ctx, self._csr, dx, dy, 0) != 0 or L.kb200_sync(self._ctx) != 0:
@@ -699,9 +708,135 @@ def block_gmres_(ws: BlockGmresWorkspace, A, B, X0=None, **kw):
     return ws.solve(A, B, **kw)
 
 
+class _LeastSquaresWorkspace(KrylovWorkspace):
+    """Workspace of lsqr! / lsmr! on an m x n operator (src/krylov_workspaces.jl LsqrWorkspace / LsmrWorkspace):
+    b has m entries, x has n.  `window` (default 5) sizes the forward-error window."""
+
+    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, window: int = 0, device: str = "host", memory: int = 0):
+        super().__init__(m_or_A, n_or_b, dtype, memory=memory, window=window, device=device)
+
+    def _wrap_rect(self, f, nin, nout):
+        """Host callback y = f(x) with len(x) = nin and len(y) = nout (staged through pinned memory)."""
+        if self.device == "cuda":
+            raise B200Error("Python callables are host operators; create the workspace with device='host'")
+        dt = self.dtype
+
+        def tramp(xp, yp, _ud):
+            x = np.ctypeslib.as_array(C.cast(xp, C.POINTER(C.c_byte)), shape=(nin * dt.itemsize,)).view(dt)
+            y = np.ctypeslib.as_array(C.cast(yp, C.POINTER(C.c_byte)), shape=(nout * dt.itemsize,)).view(dt)
+            y[:] = f(x)
+        return _lib.MATVEC(tramp)
+
+    def solve(self, A, b, *, M=None, N=None, ldiv=False, sqd=False, lambda_=0.0, radius=0.0, etol=None, axtol=None,
+              btol=None, conlim=None, atol=0.0, rtol=0.0, itmax=0, timemax=math.inf, verbose=0, history=False,
+              callback=None, fused=True):
+        """lsqr!(ws, A, b; kwargs...) / lsmr!(ws, A, b; kwargs...)  -- kwargs as in lsqr.jl:145-162 (atol and rtol
+        default to 0 as in Julia; etol, axtol, btol default to sqrt(eps), conlim to 1/sqrt(eps)).
+
+        A: a SciPy matrix, a CsrOperator or a (rowptr, colind, values) tuple (uploaded as a CSR operator), or a
+        scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables.  M (m entries) and N (n entries):
+        None, the diagonal of a Diagonal preconditioner, or a host callable."""
+        if sqd and lambda_ != 0:
+            raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
+        if sqd:
+            lambda_ = 1.0
+        m, n = self.m, self.n
+        o = lib().krylov_default_options()
+        o.atol, o.rtol = float(atol), float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        o.radius, o.lambda_ = float(radius), float(lambda_)
+        e = lib().krylov_b200_default_options()
+        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        for name, val in (("etol", etol), ("axtol", axtol), ("btol", btol), ("conlim", conlim)):
+            if val is not None:
+                setattr(e, name, float(val))
+        keep = []
+        if callback is not None:
+            wsref = self
+
+            def cb_tramp(_ws, _user):
+                r = callback(wsref)
+                if not isinstance(r, (bool, np.bool_)):
+                    wsref._cb_error = TypeError(f"callback must return Bool, got {type(r).__name__}")
+                    return 1
+                return int(r)
+            e.callback = _lib.CALLBACK(cb_tramp)
+            keep.append(e.callback)
+        self._cb_error = None
+        lib().krylov_b200_set_options(self._h, C.byref(e))
+
+        null = _lib.MATVEC()
+        fA = fAt = null
+        if hasattr(A, "matvec") and hasattr(A, "rmatvec") and not isinstance(A, CsrOperator):   # LinearOperator
+            fA, fAt = self._wrap_rect(A.matvec, n, m), self._wrap_rect(A.rmatvec, m, n)
+        elif isinstance(A, tuple) and len(A) == 2 and all(callable(f) for f in A):
+            fA, fAt = self._wrap_rect(A[0], n, m), self._wrap_rect(A[1], m, n)
+        elif A is not None:
+            self.set_operator(A)
+        keep += [fA, fAt]
+        fP = [null, null]
+        for which, (P, ln) in enumerate(((M, m), (N, n))):
+            if P is not None and callable(P) and not hasattr(P, "shape"):
+                fP[which] = self._wrap_rect(P, ln, ln)
+                keep.append(fP[which])
+                self._set_diag(which, None)
+            else:
+                if P is not None and getattr(P, "ndim", 1) != 1:
+                    raise B200Error("LSQR / LSMR take diagonal preconditioners (1-D arrays) or host callables")
+                self._set_diag(which, P)
+        if not _is_torch(b):
+            b = np.ascontiguousarray(b, dtype=self.dtype)
+            if self.device == "cuda":
+                raise B200Error("ktypeof(b) must be a device vector for a device workspace")
+        elif self.device != "cuda":
+            raise B200Error("ktypeof(b) must be a host vector for a host workspace")
+        if b.shape[0] != m:
+            raise B200Error("Inconsistent problem size")
+        pb, kb_ = _ptr(b)
+        self._order_after(kb_)
+        rc = lib().krylov_solve(self._h, fA, fAt, fP[0], fP[1], pb, None, None, C.byref(o))
+        del keep
+        if self._cb_error is not None:
+            raise self._cb_error
+        if rc != 0:
+            raise B200Error(_lib.last_error())
+        return self
+
+
+class LsqrWorkspace(_LeastSquaresWorkspace):
+    solver = "lsqr"
+
+
+class LsmrWorkspace(_LeastSquaresWorkspace):
+    solver = "lsmr"
+
+
+def _make_least_squares(name):
+    def f(A, b, *, n=None, window=0, **kw):
+        m = b.shape[0]
+        if n is None:
+            if not hasattr(A, "shape"):
+                raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
+            n = A.shape[1]
+        dt = b.cpu().numpy().dtype if _is_torch(b) else np.asarray(b).dtype
+        if dt not in (np.float32, np.float64):
+            dt = np.float64
+        ws = _WS[name](m, int(n), dt, window=window, device="cuda" if _is_torch(b) else "host")
+        try:
+            ws.solve(A, b, **kw)
+            return ws.x, ws.stats
+        finally:
+            ws.free()
+    f.__name__ = name
+    f.__doc__ = f"(x, stats) = {name}(A, b; window=5, kwargs...)  (src/{name}.jl); A is m x n, b has m entries"
+    return f
+
+
 _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "bicgstab": BicgstabWorkspace,
        "fom": FomWorkspace, "fgmres": FgmresWorkspace, "cgs": CgsWorkspace, "cg_lanczos": CgLanczosWorkspace,
-       "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace}
+       "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
+       "lsmr": LsmrWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -751,6 +886,8 @@ fom_, fgmres_, cgs_, cg_lanczos_ = (_make_inplace(s) for s in ("fom", "fgmres", 
 fom, fgmres, cgs, cg_lanczos = (_make_outofplace(s) for s in ("fom", "fgmres", "cgs", "cg_lanczos"))
 cr_, diom_, dqgmres_ = (_make_inplace(s) for s in ("cr", "diom", "dqgmres"))
 cr, diom, dqgmres = (_make_outofplace(s) for s in ("cr", "diom", "dqgmres"))
+lsqr_, lsmr_ = (_make_inplace(s) for s in ("lsqr", "lsmr"))
+lsqr, lsmr = (_make_least_squares(s) for s in ("lsqr", "lsmr"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):

@@ -19,7 +19,8 @@ KRYLOV_CPU, KRYLOV_CUDA = 0, 1
 KRYLOV_CG, KRYLOV_MINRES, KRYLOV_GMRES, KRYLOV_BICGSTAB = 0, 3, 8, 10
 KRYLOV_FOM, KRYLOV_FGMRES, KRYLOV_CGS, KRYLOV_B200_CG_LANCZOS = 7, 9, 11, 100
 KRYLOV_CR, KRYLOV_DIOM, KRYLOV_DQGMRES = 1, 5, 6
-SOLVER_IDS = {"cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
+KRYLOV_LSQR, KRYLOV_LSMR = 21, 22
+SOLVER_IDS = {"lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
               "fom": KRYLOV_FOM, "fgmres": KRYLOV_FGMRES, "cgs": KRYLOV_CGS, "cg_lanczos": KRYLOV_B200_CG_LANCZOS,
               "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES}
 
@@ -42,7 +43,8 @@ class KrylovOptions(C.Structure):
 class KrylovB200Options(C.Structure):
     _fields_ = [("history", C.c_int), ("ldiv", C.c_int), ("etol", C.c_double), ("conlim", C.c_double),
                 ("fused", C.c_int), ("batch", C.c_int), ("callback", CALLBACK), ("callback_user", C.c_void_p),
-                ("time_kernels", C.c_int), ("check_curvature", C.c_int), ("cr_gamma", C.c_double)]
+                ("time_kernels", C.c_int), ("check_curvature", C.c_int), ("cr_gamma", C.c_double),
+                ("axtol", C.c_double), ("btol", C.c_double)]
 
 
 class KrylovB200Stats(C.Structure):
@@ -117,10 +119,12 @@ SIGNATURES = {
     "kb200_divcopy": (_I, [_P, _I, _I, _P, _P, _D]),
     "kb200_fill": (_I, [_P, _I, _I, _P, _D]),
     "kb200_csr_create": (_P, [_P, _I, _I, _LL, _P, _P, _P, _I, _I, _I]),
+    "kb200_csr_create_rect": (_P, [_P, _I, _I, _I, _LL, _P, _P, _P, _I, _I, _I]),
     "kb200_csr_destroy": (None, [_P]),
     "kb200_csr_read_mtx": (_P, [_P, C.c_char_p, _I]),
     "kb200_csr_transpose": (_P, [_P, _P]),
     "kb200_csr_info": (_I, [_P, C.POINTER(_I), C.POINTER(_LL)]),
+    "kb200_csr_shape": (_I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_LL)]),
     "kb200_csr_download": (_I, [_P, _P, _P, _P, _P]),
     "kb200_mtx_read": (_I, [C.c_char_p, C.POINTER(_I), C.POINTER(_LL), _P, _P, _P]),
     "kb200_host_householder": (_I, [_I, _I, _P, _P, _P, _I]),

@@ -94,3 +94,30 @@ def csr_matvec_ones(rowptr, colind, values):
     rows = torch.repeat_interleave(torch.arange(n, device=values.device), (rowptr[1:] - rowptr[:-1]).long())
     out.index_add_(0, rows, values)
     return out
+
+
+def grad_csr(N, dtype=np.float64, xp=np, device=None):
+    """Forward-difference gradient G = [Dx; Dy; Dz] of an N x N x N grid (unknown (i,j,k) -> i + N*(j + N*k)), the
+    rectangular operator of the least-squares benchmark: m = 3 N^2 (N-1) rows, n = N^3 columns, two nonzeros per row
+    (-1 at the point, +1 at its neighbour along the axis), columns ascending.  Rows of Dx come first (point order,
+    i < N-1), then Dy (j < N-1), then Dz (k < N-1).  Its null space is the constant vector.  Returns
+    (rowptr, colind, values) as int32 / 0-based CSR."""
+    is_t = xp is not np
+    kw = dict(device=device) if is_t else {}
+    i64 = xp.int64
+    pts = xp.arange(N ** 3, dtype=i64, **kw)
+    i, j, k = pts % N, (pts // N) % N, pts // (N * N)
+    cols = []
+    for stride, coord in ((1, i), (N, j), (N * N, k)):
+        base = pts[coord < N - 1]
+        cols.append(xp.stack([base, base + stride], 1).reshape(-1))
+    colind = xp.cat(cols) if is_t else np.concatenate(cols)
+    m = colind.shape[0] // 2
+    rowptr = xp.arange(0, 2 * m + 1, 2, dtype=i64, **kw)
+    if is_t:
+        import torch
+        tdt = torch.float64 if np.dtype(dtype) == np.float64 else torch.float32
+        values = torch.tensor([-1.0, 1.0], dtype=tdt, **kw).repeat(m)
+        return rowptr.to(torch.int32), colind.to(torch.int32), values
+    values = np.tile(np.asarray([-1.0, 1.0], dtype=dtype), m)
+    return rowptr.astype(np.int32), colind.astype(np.int32), values
