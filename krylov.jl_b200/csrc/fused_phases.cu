@@ -410,8 +410,6 @@ void fused_multi_axpy(Workspace<T>& ws, T* xr, int k, const T* y, T* const* vecs
     launch_stream<T, 0>(ws.ctx, ws.n, body, NoFin(), 5);
   }
 }
-template <class T>
-void gmres_fused_update_x(Workspace<T>& ws, T* xr, int k, const T* y) { fused_multi_axpy<T>(ws, xr, k, y, ws.V.data()); }
 
 // ===========================================================================
 // Sibling solvers (SURVEY.md 8f-3), M = N = I, CSR operator: the vector operations of one iteration are grouped into
@@ -724,7 +722,6 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void cr_fused_step<T>(Workspace<T>&, const Csr<T>&, T, T*, T*, T*, T*);                                   \
   template T cr_fused_directions<T>(Workspace<T>&, T);                                                               \
   template void fused_multi_axpy<T>(Workspace<T>&, T*, int, const T*, T* const*);                                    \
-  template void gmres_fused_update_x<T>(Workspace<T>&, T*, int, const T*);                                          \
   template void lsq_fused_bidiag<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, bool, T*, T*, T*);        \
   template T lsq_fused_update<T>(Workspace<T>&, bool, bool, T, T, T, T);
 INST(double)

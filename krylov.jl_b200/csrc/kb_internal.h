@@ -5,9 +5,10 @@
 //   blas1.cu      k* primitives on device vectors   (src/krylov_utils.jl:309-349)
 //   spmv.cu       CSR operator: plain and TMA-staged SpMV (kmul!, krylov_utils.jl:305)
 //   cg_fused.cu   two-launch CG iteration               (src/cg.jl:195-268)
-//   fused_phases.cu  fused iteration phases of bicgstab!/minres!/gmres! (+ the Arnoldi step fom!/fgmres! share)
-//   solvers.cu    host control flow of cg!/gmres!/bicgstab!/minres! on the primitives
-//   siblings.cu   cgs!, cg_lanczos!, fom!, fgmres!, dqgmres!, diom!, cr! on the same kernels (SURVEY.md 8f-3)
+//   fused_phases.cu  fused iteration phases of bicgstab!/minres! and the Arnoldi step of gmres!/fom!/fgmres!
+//   solvers.cu    host control flow of cg!/bicgstab!/minres! and the one Arnoldi driver of gmres!/fom!/fgmres!
+//   siblings.cu   cgs!, cg_lanczos!, dqgmres!, diom!, cr! on the same kernels (SURVEY.md 8f-3)
+//   solver_common.h  host helpers of the drivers, among them SolveRun: the callback / clock / exit protocol
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
 //   lsq.cu        host control flow of lsqr!/lsmr! on rectangular operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
@@ -252,14 +253,15 @@ template <class T> void ws_warm_start(Workspace<T>* ws, const T* x0_dev);
 // Solver drivers (device pointers for b, c).  Throw std::runtime_error where
 // the reference calls error(...).
 template <class T> void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
-template <class T> void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void bicgstab_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
+// one Arnoldi driver (solvers.cu)
+template <class T> void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
+template <class T> void fom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
+template <class T> void fgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 // Sibling solvers on the same kernels (siblings.cu; SURVEY.md 8f-3)
 template <class T> void cgs_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
-template <class T> void fom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
-template <class T> void fgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void dqgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void diom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
@@ -300,7 +302,6 @@ template <class T> T lanczos_fused_recur(Workspace<T>& ws, T delta, T beta, bool
 template <class T> void lanczos_fused_update(Workspace<T>& ws, T beta, T gamma, T sigma, T omega);
 template <class T> void cr_fused_step(Workspace<T>& ws, const Csr<T>& A, T alpha, T* xx, T* rr, T* ArAr, T* rAr);
 template <class T> T cr_fused_directions(Workspace<T>& ws, T beta);
-template <class T> void gmres_fused_update_x(Workspace<T>& ws, T* xr, int k, const T* y);
 int gmres_fused_max();
 // LSQR / LSMR (fused_phases.cu), M = N = I, A and A^T CSR operators, no trust region.  Golub-Kahan step: P1 (SpMV on A
 // with Mu <- A v - alpha Mu and ||Mu||^2) and P2 (SpMV on A^T with Nv <- A^T u - beta Nv, ||Nv||^2 and, for LSQR,

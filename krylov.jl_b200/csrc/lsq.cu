@@ -15,13 +15,6 @@ namespace kb {
 
 namespace {
 
-// allocate_if for a vector of length len (u, Mu and Av have m entries)
-template <class T> void allocate_len(Workspace<T>& ws, T*& v, int len) {
-  const double t0 = now_seconds();
-  if (!v) v = dev_alloc<T>((size_t)len);
-  ws.stats.allocation_timer += now_seconds() - t0;
-}
-
 // knorm_elliptic(n, x, y) (src/krylov_utils.jl:319)
 template <class T> T knorm_elliptic(Ctx& c, int n, const T* x, const T* y) {
   return x == y ? k_nrm2<T>(c, n, x) : std::sqrt(k_dot<T>(c, n, x, y));
@@ -59,11 +52,12 @@ Setup lsq_prologue(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, cons
   Setup s;
   s.MisI = M.is_identity(); s.NisI = N.is_identity();
   s.fused = o.fused && A.kind == LinOp<T>::CSR && At.kind == LinOp<T>::CSR && s.MisI && s.NisI && !(o.radius > 0);
-  allocate_len(ws, ws.Mu, m);
-  allocate_len(ws, ws.Nv, n);
-  if (!s.MisI) allocate_len(ws, ws.u, m);
-  if (!s.NisI) allocate_len(ws, ws.v, n);
-  if (!s.fused) { allocate_len(ws, ws.Av, m); allocate_len(ws, ws.Atu, n); }
+  allocate_if(true, ws, ws.Mu, m);                // u, Mu and Av have m entries
+  allocate_if(true, ws, ws.Nv);
+  allocate_if(!s.MisI, ws, ws.u, m);
+  allocate_if(!s.NisI, ws, ws.v);
+  allocate_if(!s.fused, ws, ws.Av, m);
+  allocate_if(!s.fused, ws, ws.Atu);
   ws.stats.reset();
   ws.stats.Anorm = NAN;
   k_fill<T>(c, n, ws.x, T(0));
@@ -137,13 +131,6 @@ struct Exit {
   }
 };
 
-template <class T> void early_exit(Workspace<T>& ws, double start_time, const char* status) {
-  ws.ctx.sync();
-  ws.stats.niter = 0; ws.stats.solved = true; ws.stats.inconsistent = false;
-  ws.stats.timer = now_seconds() - start_time;
-  ws.stats.status = status;
-}
-
 template <class T> int ls_itmax(const Workspace<T>& ws, int itmax) {
   if (itmax != 0) return itmax;
   const long long mn = (long long)ws.m + ws.n;
@@ -158,7 +145,9 @@ template <class T> int ls_itmax(const Workspace<T>& ws, int itmax) {
 template <class T>
 void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
                 const SolveOpts& o) {
-  const double start_time = now_seconds();
+  // LSQR / LSMR workspaces refuse warm starts and row partitioning, so run.finish never adds dx and the cross-rank
+  // OR in run.poll is a no-op for them; they share the protocol for its callback / clock / sync order.
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int m = ws.m, n = ws.n;
   const bool history = o.history, ldiv = o.ldiv;
@@ -174,7 +163,7 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   T beta1;
   const Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta1);
   if (beta1 == 0) {
-    early_exit(ws, start_time, "x is a zero-residual solution");
+    run.finish(0, true, false, "x is a zero-residual solution");
     if (history) { stats.residuals.push_back(0); stats.Aresiduals.push_back(0); }
     return;
   }
@@ -193,7 +182,7 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   if (o.verbose > 0) {
     printf("%5s  %7s  %7s  %7s  %7s  %7s  %7s  %7s  %7s  %5s\n", "k", "α", "β", "‖r‖", "‖Aᴴr‖", "compat", "backwrd", "‖A‖", "κ(A)", "timer");
     printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)beta1, (double)alpha, (double)beta1,
-           (double)alpha, 0.0, 1.0, (double)Anorm, (double)Acond, now_seconds() - start_time);
+           (double)alpha, 0.0, 1.0, (double)Anorm, (double)Acond, run.elapsed());
   }
   T rNorm = beta1, r1Norm = rNorm, r2Norm = rNorm, res2 = 0;
   (void)r1Norm;
@@ -202,7 +191,7 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   const T ArNorm0 = ArNorm;
   if (history) stats.Aresiduals.push_back(ArNorm);
   if (alpha == 0) {                                          // Aᴴb = 0: x = 0 is a minimum least-squares solution
-    early_exit(ws, start_time, "x is a minimum least-squares solution");
+    run.finish(0, true, false, "x is a minimum least-squares solution");
     return;
   }
   k_scal<T>(c, n, T(1) / alpha, v);
@@ -302,12 +291,12 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
     const T rNormtol = btol + axtol * Anorm * xNorm / beta1;
     if (kdisplay(iter, o.verbose))
       printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)alpha, (double)beta, (double)rNorm,
-             (double)ArNorm, (double)test1, (double)test2, (double)Anorm, (double)Acond, now_seconds() - start_time);
+             (double)ArNorm, (double)test1, (double)test2, (double)Anorm, (double)Acond, run.elapsed());
 
     ex.ill_cond_mach = (T(1) + test3 <= T(1));
     const bool solved_mach = (T(1) + test2 <= T(1));
     const bool zero_resid_mach = (T(1) + t1 <= T(1));
-    if (o.callback) { c.sync(); stats.niter = iter; ex.user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, ex.user_exit, ex.overtimed);
     ex.tired = iter >= itmax;
     ex.ill_cond_lim = (test3 <= ctol);
     const bool solved_lim = (test2 <= axtol);
@@ -317,13 +306,9 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
     ex.ill_cond = ex.ill_cond_mach || ex.ill_cond_lim;
     ex.zero_resid = zero_resid_mach || zero_resid_lim;
     ex.solved = solved_mach || solved_lim || solved_opt || ex.zero_resid || ex.fwd_err || ex.on_boundary;
-    ex.overtimed = (now_seconds() - start_time) > o.timemax;
   }
   if (o.verbose > 0) printf("\n");
-  c.sync();
-  stats.niter = iter; stats.solved = ex.solved; stats.inconsistent = !ex.zero_resid;
-  stats.timer = now_seconds() - start_time;
-  stats.status = ex.status();
+  run.finish(iter, ex.solved, !ex.zero_resid, ex.status());
 }
 
 // ===========================================================================
@@ -332,7 +317,7 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
 template <class T>
 void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
                 const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int m = ws.m, n = ws.n;
   const bool history = o.history, ldiv = o.ldiv;
@@ -348,7 +333,7 @@ void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   T beta1;
   const Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta1);
   if (beta1 == 0) {
-    early_exit(ws, start_time, "x is a zero-residual solution");
+    run.finish(0, true, false, "x is a zero-residual solution");
     if (history) { stats.residuals.push_back(0); stats.Aresiduals.push_back(0); }
     return;
   }
@@ -375,10 +360,10 @@ void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   if (o.verbose > 0) {
     printf("%5s  %7s  %7s  %7s  %7s  %8s  %8s  %7s  %5s\n", "k", "‖r‖", "‖Aᴴr‖", "β", "α", "cos", "sin", "‖A‖²", "timer");
     printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %.2fs\n", iter, (double)beta1, (double)alpha, (double)beta1,
-           (double)alpha, 0.0, 1.0, (double)Anorm2, now_seconds() - start_time);
+           (double)alpha, 0.0, 1.0, (double)Anorm2, run.elapsed());
   }
   if (alpha == 0) {                                          // Aᴴb = 0: x = 0 is a minimum least-squares solution
-    early_exit(ws, start_time, "x is a minimum least-squares solution");
+    run.finish(0, true, false, "x is a minimum least-squares solution");
     stats.Anorm = Anorm;
     return;
   }
@@ -474,12 +459,12 @@ void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
     const T rNormtol = btol + axtol * Anorm * xNorm / beta1;
     if (kdisplay(iter, o.verbose))
       printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm, (double)beta,
-             (double)alpha, (double)cs, (double)sn, (double)Anorm2, now_seconds() - start_time);
+             (double)alpha, (double)cs, (double)sn, (double)Anorm2, run.elapsed());
 
     ex.ill_cond_mach = (T(1) + test3 <= T(1));
     const bool solved_mach = (T(1) + test2 <= T(1));
     const bool zero_resid_mach = (T(1) + t1 <= T(1));
-    if (o.callback) { c.sync(); stats.niter = iter; ex.user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, ex.user_exit, ex.overtimed);
     ex.tired = iter >= itmax;
     ex.ill_cond_lim = (test3 <= ctol);
     const bool solved_lim = (test2 <= axtol);
@@ -489,14 +474,10 @@ void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
     ex.ill_cond = ex.ill_cond_mach || ex.ill_cond_lim;
     ex.zero_resid = zero_resid_mach || zero_resid_lim;
     ex.solved = solved_mach || solved_lim || solved_opt || ex.zero_resid || ex.fwd_err || ex.on_boundary;
-    ex.overtimed = (now_seconds() - start_time) > o.timemax;
   }
   if (o.verbose > 0) printf("\n");
-  c.sync();
   stats.Anorm = Anorm;
-  stats.niter = iter; stats.solved = ex.solved; stats.inconsistent = !ex.zero_resid;
-  stats.timer = now_seconds() - start_time;
-  stats.status = ex.status();
+  run.finish(iter, ex.solved, !ex.zero_resid, ex.status());
 }
 
 #define INST(T)                                                                                                         \

@@ -1,8 +1,8 @@
 // siblings.cu -- sibling solvers that run on the hot-path kernels unchanged
-// (SURVEY.md section 8f-3): cgs!, cg_lanczos!, fom!, fgmres!.  Same rules as
-// solvers.cu: the reference's host control flow statement by statement (files
+// (SURVEY.md section 8f-3): cgs!, cg_lanczos!, dqgmres!, diom!, cr!.  Same rules
+// as solvers.cu: the reference's host control flow statement by statement (files
 // cited per function), every vector operation a kernel from blas1.cu / spmv.cu
-// / fused_phases.cu.  FOM and FGMRES share GMRES's fused Arnoldi step.
+// / fused_phases.cu.  fom! and fgmres! run on GMRES's Arnoldi driver in solvers.cu.
 #include <cstring>
 
 #include "solver_common.h"
@@ -15,7 +15,7 @@ namespace kb {
 template <class T>
 void cgs_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_in, const LinOp<T>& M, const LinOp<T>& N,
                const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv;
@@ -41,21 +41,14 @@ void cgs_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_in, c
   if (!MisI) op_apply(c, M, r0, r, ldiv);
   T rNorm = k_nrm2<T>(c, n, r);
   if (history) stats.residuals.push_back(rNorm);
-  auto finish_early = [&](bool solved, const char* status) {
-    stats.niter = 0; stats.solved = solved; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time; stats.status = status;
-    if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-    ws.warm_start = false;
-    c.sync();
-  };
-  if (rNorm == 0) { finish_early(true, "x is a zero-residual solution"); return; }
+  if (rNorm == 0) { run.finish(0, true, false, "x is a zero-residual solution"); return; }
   T rho = k_dot<T>(c, n, cvec, r);
-  if (rho == 0) { finish_early(false, "Breakdown bᴴc = 0"); return; }
+  if (rho == 0) { run.finish(0, false, false, "Breakdown bᴴc = 0"); return; }
   int iter = 0;
   const int itmax = default_itmax(ws, o.itmax);
   const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
   if (o.verbose > 0) printf("%5s  %7s  %5s\n", "k", "‖rₖ‖", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, now_seconds() - start_time);
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, run.elapsed());
   k_copy<T>(c, n, u, r);
   k_copy<T>(c, n, p, r);
   k_fill<T>(c, n, q, T(0));
@@ -102,13 +95,11 @@ void cgs_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_in, c
     }
     if (history) stats.residuals.push_back(rNorm);
     const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-    if (o.callback) { c.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, user_exit, overtimed);
     solved = (rNorm <= eps_tol) || resid_decrease_mach;
     tired = iter >= itmax;
     breakdown = (alpha == 0 || std::isnan(alpha));
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
-    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, now_seconds() - start_time);
+    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, run.elapsed());
   }
   if (o.verbose > 0) printf("\n");
   if (tired) status = "maximum number of iterations exceeded";
@@ -116,12 +107,7 @@ void cgs_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_in, c
   if (solved) status = "solution good enough given atol and rtol";
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-  ws.warm_start = false;
-  c.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = false;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, false, status);
 }
 
 // ===========================================================================
@@ -129,7 +115,7 @@ void cgs_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_in, c
 // ===========================================================================
 template <class T>
 void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv, check_curvature = o.check_curvature;
@@ -154,12 +140,8 @@ void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const Lin
   T rNorm = sigma;
   if (history) stats.residuals.push_back(rNorm);
   if (beta == 0) {
-    stats.niter = 0; stats.solved = true; stats.Anorm = 0; stats.indefinite = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
-    if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-    ws.warm_start = false;
-    c.sync();
+    stats.Anorm = 0; stats.indefinite = false;
+    run.finish(0, true, false, "x is a zero-residual solution");
     return;
   }
   k_copy<T>(c, n, p, v);
@@ -171,7 +153,7 @@ void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const Lin
   T omega = 0, gamma = 1, Anorm2 = 0, beta_prev = 0;
   const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
   if (o.verbose > 0) printf("%5s  %7s  %5s\n", "k", "‖rₖ‖", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, now_seconds() - start_time);
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, run.elapsed());
   bool indefinite = false, solved = rNorm <= eps_tol, tired = iter >= itmax, user_exit = false, overtimed = false;
   std::string status = "unknown";
 
@@ -207,13 +189,11 @@ void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const Lin
     rNorm = std::fabs(sigma);
     if (history) stats.residuals.push_back(rNorm);
     iter = iter + 1;
-    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, now_seconds() - start_time);
+    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, run.elapsed());
     const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-    if (o.callback) { c.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, user_exit, overtimed);
     solved = (rNorm <= eps_tol) || resid_decrease_mach;
     tired = iter >= itmax;
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
   }
   if (o.verbose > 0) printf("\n");
   if (tired) status = "maximum number of iterations exceeded";
@@ -221,234 +201,8 @@ void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const Lin
   if (solved) status = "solution good enough given atol and rtol";
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-  ws.warm_start = false;
-  c.sync();
-  stats.niter = iter; stats.solved = solved; stats.Anorm = std::sqrt(Anorm2); stats.indefinite = indefinite;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
-}
-
-// ---------------------------------------------------------------------------
-// fom! and fgmres! share everything but the small factorization kept on the
-// host (LU vs Givens QR) and where the right preconditioner lives (FGMRES
-// stores Z[k] = N V[k]); one driver, the differences are marked.
-//   fom!     src/fom.jl:121-368
-//   fgmres!  src/fgmres.jl:128-388
-// ---------------------------------------------------------------------------
-template <class T, bool FLEX>
-static void arnoldi_family_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N,
-                                 const SolveOpts& o) {
-  const double start_time = now_seconds();
-  Ctx& cx = ws.ctx;
-  const int n = ws.n;
-  const bool history = o.history, ldiv = o.ldiv, restart = o.restart, reorth = o.reorthogonalization;
-  if (o.verbose > 0) printf("%s: system of size %d\n", FLEX ? "FGMRES" : "FOM", n);
-  const bool MisI = M.is_identity(), NisI = N.is_identity();
-  allocate_if(!MisI, ws, ws.q);
-  if (!FLEX) allocate_if(!NisI, ws, ws.pp);
-  allocate_if(restart, ws, ws.dx);
-  T *dx = ws.dx, *x = ws.x, *w = ws.w;
-  std::vector<T*>& V = ws.V;
-  std::vector<T*>& Z = ws.Z;
-  // FGMRES: c, s (sgiv), z (zg), R.   FOM: l (sgiv), z (zg), U (R); c is unused.
-  std::vector<T>&c = ws.c, &s = ws.sgiv, &z = ws.zg, &R = ws.R;
-  std::vector<T>& l = ws.sgiv;
-  Stats& stats = ws.stats;
-  const bool warm_start = ws.warm_start;
-  stats.reset();
-  T* q = MisI ? w : ws.q;
-  T* r0 = MisI ? w : ws.q;
-  T* xr = restart ? dx : x;
-
-  k_fill<T>(cx, n, x, T(0));
-  if (warm_start) {
-    op_apply(cx, A, dx, w);
-    k_axpby<T>(cx, n, T(1), b, T(-1), w);
-    if (restart) k_axpy<T>(cx, n, T(1), dx, x);
-  } else {
-    k_copy<T>(cx, n, w, b);
-  }
-  if (!MisI) op_apply(cx, M, w, r0, ldiv);
-  T beta = k_nrm2<T>(cx, n, r0);
-  T rNorm = beta;
-  if (history) stats.residuals.push_back(beta);
-  const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
-  if (beta == 0) {
-    stats.niter = 0; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
-    if (warm_start) k_axpy<T>(cx, n, T(1), dx, x);
-    ws.warm_start = false;
-    cx.sync();
-    return;
-  }
-  const int mem = (int)s.size();                              // length(c) / length(l)
-  int npass = 0, iter = 0, inner_iter = 0;
-  const int itmax = default_itmax(ws, o.itmax);
-  int inner_itmax = itmax;
-  if (o.verbose > 0) printf("%5s  %5s  %7s  %7s  %5s\n", "pass", "k", "‖rₖ‖", "hₖ₊₁.ₖ", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %5d  %7.1e  %7s  %.2fs\n", npass, iter, (double)rNorm, "✗ ✗ ✗ ✗", now_seconds() - start_time);
-  const T btol = std::pow(eps_of<T>(), T(0.75));
-  // the fused Arnoldi step folds a left diagonal M into the SpMV epilogue; FOM needs N = I (FGMRES materialises Z[k])
-  const bool fusedA = o.fused && A.kind == LinOp<T>::CSR && !reorth && (FLEX || NisI) &&
-                      (MisI || (M.kind == LinOp<T>::DIAG && !ldiv));
-  ws.mdiag_fused = (fusedA && !MisI) ? M.diag : nullptr;
-  bool breakdown = false, inconsistent = false, solved = rNorm <= eps_tol, tired = iter >= itmax;
-  bool inner_tired = inner_iter >= inner_itmax, user_exit = false, overtimed = false;
-  std::string status = "unknown";
-
-  while (!(solved || tired || breakdown || user_exit || overtimed)) {
-    int nr = 0;
-    // The reference zero-fills V (and Z) every cycle.  FGMRES reads only entries it wrote first, so (as in
-    // gmres_solve) the fill is kept only where callbacks could see unused columns.  FOM does read a zero V[k+1]
-    // after a user exit or timeout (its inner loop does not test them, fom.jl:237), so FOM always fills.
-    if (!restart || !FLEX) for (int i = 0; i < mem; i++) { k_fill<T>(cx, n, V[i], T(0)); if (FLEX) k_fill<T>(cx, n, Z[i], T(0)); }
-    std::fill(s.begin(), s.end(), T(0));
-    if (FLEX) std::fill(c.begin(), c.end(), T(0));
-    std::fill(R.begin(), R.end(), T(0));
-    std::fill(z.begin(), z.end(), T(0));
-    if (restart) {
-      k_fill<T>(cx, n, xr, T(0));
-      if (npass >= 1) {
-        op_apply(cx, A, x, w);
-        k_axpby<T>(cx, n, T(1), b, T(-1), w);
-        if (!MisI) op_apply(cx, M, w, r0, ldiv);
-      }
-    }
-    beta = k_nrm2<T>(cx, n, r0);
-    z[0] = beta;
-    k_divcopy<T>(cx, n, V[0], r0, rNorm);
-    npass = npass + 1;
-    ws.inner_iter = 0;
-    inner_tired = false;
-
-    // fom.jl:237 tests only solved/inner_tired/breakdown; fgmres.jl:243 also the user exit and the timer
-    while (!(solved || inner_tired || breakdown || (FLEX && (user_exit || overtimed)))) {
-      ws.inner_iter = ws.inner_iter + 1;
-      inner_iter = ws.inner_iter;
-      if (!restart && (inner_iter > mem)) {
-        const double t0 = now_seconds();
-        for (int i = 0; i < inner_iter; i++) R.push_back(T(0));
-        s.push_back(T(0));                                    // FGMRES s / FOM l
-        if (FLEX) { c.push_back(T(0)); Z.push_back(dev_alloc<T>((size_t)n)); }
-        else z.push_back(T(0));                               // fom.jl:249 grows z here, fgmres.jl:329 with V
-        stats.allocation_timer += now_seconds() - t0;
-      }
-      T* vk = V[inner_iter - 1];
-      T* p;
-      if (FLEX) {                                             // z_k <- N_k v_k, unconditional (fgmres.jl:262)
-        p = Z[inner_iter - 1];
-        if (NisI) k_copy<T>(cx, n, p, vk); else op_apply(cx, N, vk, p, ldiv);
-      } else {
-        p = NisI ? vk : ws.pp;
-        if (!NisI) op_apply(cx, N, vk, p, ldiv);
-      }
-      T Hbis;
-      if (fusedA && inner_iter <= gmres_fused_max()) {
-        gmres_fused_arnoldi<T>(ws, *A.csr, inner_iter, &R[nr], &Hbis, p);
-      } else {
-        op_apply(cx, A, p, w);
-        if (!MisI) op_apply(cx, M, w, q, ldiv);
-        for (int i = 0; i < inner_iter; i++) {
-          R[nr + i] = k_dot<T>(cx, n, V[i], q);
-          k_axpy<T>(cx, n, -R[nr + i], V[i], q);
-        }
-        if (reorth) {
-          for (int i = 0; i < inner_iter; i++) {
-            const T Htmp = k_dot<T>(cx, n, V[i], q);
-            R[nr + i] += Htmp;
-            k_axpy<T>(cx, n, -Htmp, V[i], q);
-          }
-        }
-        Hbis = k_nrm2<T>(cx, n, q);
-      }
-      T zeta_next = 0;
-      if (FLEX) {                                             // Givens QR of H, fgmres.jl:285-303
-        for (int i = 0; i < inner_iter - 1; i++) {
-          const T Rtmp = c[i] * R[nr + i] + s[i] * R[nr + i + 1];
-          R[nr + i + 1] = s[i] * R[nr + i] - c[i] * R[nr + i + 1];
-          R[nr + i] = Rtmp;
-        }
-        sym_givens<T>(R[nr + inner_iter - 1], Hbis, &c[inner_iter - 1], &s[inner_iter - 1], &R[nr + inner_iter - 1]);
-        zeta_next = s[inner_iter - 1] * z[inner_iter - 1];
-        z[inner_iter - 1] = c[inner_iter - 1] * z[inner_iter - 1];
-        rNorm = std::fabs(zeta_next);
-      } else {                                                // LU of H without pivoting, fom.jl:274-288
-        if (inner_iter >= 2) {
-          for (int i = 2; i <= inner_iter; i++) R[nr + i - 1] = R[nr + i - 1] - l[i - 2] * R[nr + i - 2];
-          z[inner_iter - 1] = -l[inner_iter - 2] * z[inner_iter - 2];
-        }
-        l[inner_iter - 1] = Hbis / R[nr + inner_iter - 1];
-        rNorm = Hbis * std::fabs(z[inner_iter - 1] / R[nr + inner_iter - 1]);
-      }
-      if (history) stats.residuals.push_back(rNorm);
-      nr = nr + inner_iter;
-      const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-      if (o.callback) { cx.sync(); stats.niter = iter + inner_iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
-      const bool resid_decrease_lim = rNorm <= eps_tol;
-      breakdown = Hbis <= btol;
-      solved = resid_decrease_lim || resid_decrease_mach;
-      inner_tired = restart ? inner_iter >= std::min(mem, inner_itmax) : inner_iter >= inner_itmax;
-      overtimed = (now_seconds() - start_time) > o.timemax;
-      agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
-      if (kdisplay(iter + inner_iter, o.verbose))
-        printf("%5d  %5d  %7.1e  %7.1e  %.2fs\n", npass, iter + inner_iter, (double)rNorm, (double)Hbis, now_seconds() - start_time);
-      if (!(solved || inner_tired || breakdown || user_exit || overtimed)) {
-        if (!restart && (inner_iter >= mem)) {
-          const double t0 = now_seconds();
-          V.push_back(dev_alloc<T>((size_t)n));
-          if (FLEX) z.push_back(T(0));
-          stats.allocation_timer += now_seconds() - t0;
-        }
-        k_divcopy<T>(cx, n, V[inner_iter], q, Hbis);
-        if (FLEX) z[inner_iter] = zeta_next;
-      }
-    }
-    std::vector<T>& y = z;                                    // back substitution, fom.jl:322-331 / fgmres.jl:335-350
-    for (int i = inner_iter; i >= 1; i--) {
-      int pos = nr + i - inner_iter;
-      for (int j = inner_iter; j >= i + 1; j--) {
-        y[i - 1] = y[i - 1] - R[pos - 1] * y[j - 1];
-        pos = pos - j + 1;
-      }
-      if (FLEX && std::fabs(R[pos - 1]) <= btol) { y[i - 1] = T(0); inconsistent = true; }
-      else y[i - 1] = y[i - 1] / R[pos - 1];
-    }
-    T* const* basis = FLEX ? Z.data() : V.data();             // x_k = Z_k y_k (FGMRES) or N V_k y_k (FOM)
-    if (fusedA) fused_multi_axpy<T>(ws, xr, inner_iter, y.data(), basis);
-    else for (int i = 0; i < inner_iter; i++) k_axpy<T>(cx, n, y[i], basis[i], xr);
-    if (!FLEX && !NisI) { k_copy<T>(cx, n, ws.pp, xr); op_apply(cx, N, ws.pp, xr, ldiv); }
-    if (restart) k_axpy<T>(cx, n, T(1), xr, x);
-    inner_itmax = inner_itmax - inner_iter;
-    iter = iter + inner_iter;
-    tired = iter >= itmax;
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
-  }
-  if (o.verbose > 0) printf("\n");
-  if (tired) status = "maximum number of iterations exceeded";
-  if (!FLEX && breakdown) status = "inconsistent linear system";
-  if (solved) status = "solution good enough given atol and rtol";
-  if (FLEX && inconsistent) status = "found approximate least-squares solution";
-  if (user_exit) status = "user-requested exit";
-  if (overtimed) status = "time limit exceeded";
-  if (warm_start && !restart) k_axpy<T>(cx, n, T(1), dx, x);
-  ws.warm_start = false;
-  cx.sync();
-  stats.niter = iter; stats.solved = solved;
-  stats.inconsistent = FLEX ? inconsistent : (!solved && breakdown);
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
-}
-
-template <class T>
-void fom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
-  arnoldi_family_solve<T, false>(ws, A, b, M, N, o);
-}
-template <class T>
-void fgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
-  arnoldi_family_solve<T, true>(ws, A, b, M, N, o);
+  stats.Anorm = std::sqrt(Anorm2); stats.indefinite = indefinite;
+  run.finish(iter, solved, false, status);
 }
 
 // ---------------------------------------------------------------------------
@@ -460,7 +214,7 @@ void fgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
 // ---------------------------------------------------------------------------
 template <class T, bool QR>
 static void truncated_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& cx = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv, reorth = o.reorthogonalization;
@@ -484,20 +238,12 @@ static void truncated_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, con
   if (!MisI) op_apply(cx, M, t, r0, ldiv);
   T rNorm = k_nrm2<T>(cx, n, r0);
   if (history) stats.residuals.push_back(rNorm);
-  if (rNorm == 0) {
-    stats.niter = 0; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
-    if (warm_start) k_axpy<T>(cx, n, T(1), dx, x);
-    ws.warm_start = false;
-    cx.sync();
-    return;
-  }
+  if (rNorm == 0) { run.finish(0, true, false, "x is a zero-residual solution"); return; }
   int iter = 0;
   const int itmax = default_itmax(ws, o.itmax);
   const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
   if (o.verbose > 0) printf("%5s  %7s  %5s\n", "k", "‖rₖ‖", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, now_seconds() - start_time);
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, run.elapsed());
   const int mem = (int)V.size();
   for (int i = 0; i < mem; i++) k_fill<T>(cx, n, V[i], T(0));
   for (size_t i = 0; i < P.size(); i++) k_fill<T>(cx, n, P[i], T(0));
@@ -603,12 +349,10 @@ static void truncated_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, con
     }
     if (history) stats.residuals.push_back(rNorm);
     const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-    if (o.callback) { cx.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, user_exit, overtimed);
     solved = (rNorm <= eps_tol) || resid_decrease_mach;
     tired = iter >= itmax;
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
-    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, now_seconds() - start_time);
+    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm, run.elapsed());
   }
   if (o.verbose > 0) printf("\n");
   if (QR) {                                     // dqgmres.jl:319-322 assigns in this order (tired overrides solved)
@@ -620,12 +364,7 @@ static void truncated_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, con
   }
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start) k_axpy<T>(cx, n, T(1), dx, x);
-  ws.warm_start = false;
-  cx.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = false;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, false, status);
 }
 
 template <class T>
@@ -658,7 +397,7 @@ static void cr_to_boundary(Ctx& c, int n, const T* x, const T* d, T radius, T xN
 
 template <class T>
 void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv, linesearch = o.linesearch;
@@ -684,29 +423,20 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   T rNorm = std::sqrt(k_dot<T>(c, n, r, p));                  // knorm_elliptic(n, r, p)
   if (history) stats.residuals.push_back(rNorm);
   if (rNorm == 0) {
-    stats.niter = 0; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
     if (history) stats.Aresiduals.push_back(0);
-    if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-    ws.warm_start = false;
-    c.sync();
+    run.finish(0, true, false, "x is a zero-residual solution");
     return;
   }
   op_apply(c, A, r, Ar);
   T rho = k_dot<T>(c, n, r, Ar);
   if (rho == 0) {
-    stats.niter = 0; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "b is a zero-curvature direction";
     if (history) stats.Aresiduals.push_back(0);
-    ws.warm_start = false;
     if (linesearch || radius > 0) {
       k_copy<T>(c, n, x, p);
       k_copy<T>(c, n, npc_dir, p);
       stats.npcCount = 1; stats.indefinite = true;
     }
-    c.sync();
+    run.finish(0, true, false, "b is a zero-curvature direction", false);
     return;
   }
   k_copy<T>(c, n, p, r);
@@ -720,7 +450,7 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   if (history) stats.Aresiduals.push_back(ArNorm);
   const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
   if (o.verbose > 0) printf("%5s  %8s  %8s  %8s  %5s\n", "k", "‖x‖", "‖r‖", "quad", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %8.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)xNorm, (double)rNorm, (double)mquad, now_seconds() - start_time);
+  if (kdisplay(iter, o.verbose)) printf("%5d  %8.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)xNorm, (double)rNorm, (double)mquad, run.elapsed());
   bool descent = pr > 0, solved = rNorm <= eps_tol, tired = iter >= itmax, on_boundary = false, npcurv = false;
   bool user_exit = false, overtimed = false;
   // grouped passes (no trust region, no linesearch, M = I): 3 launches and 2 read-backs per iteration instead of 9 and 5
@@ -737,10 +467,6 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
       if (p_curv || r_curv) {                                 // cr.jl:233-262
         npcurv = true;
         if (o.verbose > 0) printf("nonpositive curvature detected: pᴴAp = %8.1e and rᴴAr = %8.1e\n", (double)pAp, (double)rho);
-        stats.solved = true; stats.niter = iter; stats.inconsistent = false;
-        stats.timer = now_seconds() - start_time;
-        stats.status = "nonpositive curvature";
-        ws.warm_start = false;
         stats.indefinite = true;
         if (iter == 0) {
           k_copy<T>(c, n, npc_dir, p);
@@ -750,7 +476,7 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
           if (r_curv) { k_copy<T>(c, n, npc_dir, r); stats.npcCount += 1; }
           if (p_curv) { stats.npcCount += 1; if (!r_curv) k_copy<T>(c, n, npc_dir, p); }
         }
-        c.sync();
+        run.finish(iter, true, false, "nonpositive curvature", false);
         return;
       }
     } else if (pAp <= 0 && radius == 0) {
@@ -829,15 +555,13 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
     iter = iter + 1;
     if (kdisplay(iter, o.verbose)) {
       mquad = mquad - alpha * pr + alpha * alpha * pAp / 2;
-      printf("%5d  %8.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)xNorm, (double)rNorm, (double)mquad, now_seconds() - start_time);
+      printf("%5d  %8.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)xNorm, (double)rNorm, (double)mquad, run.elapsed());
     }
     const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-    if (o.callback) { c.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, user_exit, overtimed);
     const bool resid_decrease = (rNorm <= eps_tol) || resid_decrease_mach;
     solved = resid_decrease || npcurv || on_boundary;
     tired = iter >= itmax;
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
     if (solved || tired || user_exit || overtimed) continue;
     const T rhobar = rho;
     rho = fusedC ? rAr_fused : k_dot<T>(c, n, r, Ar);
@@ -850,15 +574,7 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
     pNorm2 = rNorm2 + 2 * beta * pr - 2 * beta * alpha * pAp + beta * beta * pNorm2;
     if (pNorm2 > sqeps) pNorm = std::sqrt(pNorm2);
     else if (std::fabs(pNorm2) <= sqeps) pNorm = T(0);
-    else {
-      stats.niter = iter; stats.solved = solved; stats.inconsistent = false;
-      stats.timer = now_seconds() - start_time;
-      stats.status = "solver encountered numerical issues";
-      if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-      ws.warm_start = false;
-      c.sync();
-      return;
-    }
+    else { run.finish(iter, solved, false, "solver encountered numerical issues"); return; }
     pr = rNorm2 + beta * pr - beta * alpha * pAp;
     abspr = std::fabs(pr);
     pAp = rho + beta * beta * pAp;
@@ -872,19 +588,12 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   if (overtimed) status = "time limit exceeded";
   if (npcurv) status = "nonpositive curvature";
   if (on_boundary) status = "on trust-region boundary";
-  if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-  ws.warm_start = false;
-  c.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = false;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, false, status);
 }
 
 #define INST(T)                                                                                                          \
   template void cgs_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void cg_lanczos_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);        \
-  template void fom_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
-  template void fgmres_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void dqgmres_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void diom_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void cr_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);

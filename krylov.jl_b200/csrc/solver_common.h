@@ -1,7 +1,8 @@
-// solver_common.h -- small host helpers shared by the solver drivers (solvers.cu, siblings.cu).
+// solver_common.h -- small host helpers shared by the solver drivers (solvers.cu, siblings.cu, lsq.cu).
 #pragma once
 #include <cmath>
 #include <limits>
+#include <string>
 
 #include "kb_internal.h"
 
@@ -10,10 +11,10 @@ namespace kb {
 template <class T> static inline T eps_of() { return std::numeric_limits<T>::epsilon(); }
 template <class T> static inline T tol_of(double t) { return t < 0 ? std::sqrt(eps_of<T>()) : (T)t; }
 
-// allocate_if (src/krylov_utils.jl:281-288)
-template <class T> static inline void allocate_if(bool cond, Workspace<T>& ws, T*& v) {
+// allocate_if (src/krylov_utils.jl:281-288); len < 0: ws.n entries (LSQR / LSMR also hold vectors of m entries)
+template <class T> static inline void allocate_if(bool cond, Workspace<T>& ws, T*& v, int len = -1) {
   const double t0 = now_seconds();
-  if (cond && !v) v = dev_alloc<T>((size_t)ws.n);
+  if (cond && !v) v = dev_alloc<T>((size_t)(len < 0 ? ws.n : len));
   ws.stats.allocation_timer += now_seconds() - t0;
 }
 
@@ -22,6 +23,34 @@ template <class T> static inline void allocate_if(bool cond, Workspace<T>& ws, T
 template <class T> static inline void agree_exit(Workspace<T>& ws, const SolveOpts& o, bool& user_exit, bool& overtimed) {
   if (ws.dist.world > 1 && (o.callback != nullptr || o.timemax < 1e300)) dist_agree_on_exit(ws.ctx, user_exit, overtimed);
 }
+
+// The library's exit protocol, shared by every single right-hand-side driver.  Constructed at driver entry: it takes
+// the start time and the warm-start flag there.
+template <class T> struct SolveRun {
+  Workspace<T>& ws;
+  const SolveOpts& o;
+  const double start;
+  const bool warm_start;
+  SolveRun(Workspace<T>& ws_, const SolveOpts& o_) : ws(ws_), o(o_), start(now_seconds()), warm_start(ws_.warm_start) {}
+  double elapsed() const { return now_seconds() - start; }
+  // End of an iteration: the callback (when one is set and `callback` is true) sees a synchronized stream and
+  // stats.niter = niter; the clock is read after it; a row-partitioned solve ORs both flags over the ranks.
+  void poll(int niter, bool& user_exit, bool& overtimed, bool callback = true) {
+    if (callback && o.callback) { ws.ctx.sync(); ws.stats.niter = niter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    overtimed = elapsed() > o.timemax;
+    agree_exit(ws, o, user_exit, overtimed);
+  }
+  // End of the solve: x += dx when warm-started (unless add_dx is false), one sync, then the statistics.
+  void finish(int niter, bool solved, bool inconsistent, const std::string& status, bool add_dx = true) {
+    if (warm_start && add_dx) k_axpy<T>(ws.ctx, ws.n, T(1), ws.dx, ws.x);
+    ws.warm_start = false;
+    ws.ctx.sync();
+    Stats& st = ws.stats;
+    st.niter = niter; st.solved = solved; st.inconsistent = inconsistent;
+    st.timer = elapsed();
+    st.status = status;
+  }
+};
 
 static inline bool kdisplay(int iter, int verbose) { return verbose > 0 && iter % verbose == 0; }
 

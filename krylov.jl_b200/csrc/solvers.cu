@@ -1,7 +1,8 @@
-// solvers.cu -- host control flow of cg!, bicgstab!, gmres!, minres! on device
-// vectors.  Each driver keeps the reference's scalar recurrences, stopping
-// tests, status strings and aliasing rules (files cited per function); every
-// vector operation is a kernel from blas1.cu / spmv.cu, nothing is computed on
+// solvers.cu -- host control flow of cg!, bicgstab!, minres! and of the one
+// Arnoldi driver behind gmres!, fom! and fgmres!, on device vectors.  Each
+// driver keeps the reference's scalar recurrences, stopping tests, status
+// strings and aliasing rules (files cited per function); every vector operation
+// is a kernel from blas1.cu / spmv.cu / fused_phases.cu, nothing is computed on
 // the host except O(1)/O(k^2) scalar work the reference also does on the host.
 #include <cmath>
 #include <cstring>
@@ -118,7 +119,7 @@ template <class T> void ws_warm_start(Workspace<T>* ws, const T* x0_dev) {
 // ===========================================================================
 template <class T>
 void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int n = ws.n;
   const T radius = (T)o.radius;
@@ -155,15 +156,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   if (!(gamma >= 0)) throw std::runtime_error("The linear operator `A` or the preconditioner `M` is not symmetric positive definite.");
   T rNorm = std::sqrt(gamma);
   if (history) stats.residuals.push_back(rNorm);
-  if (gamma == 0) {
-    stats.niter = 0; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
-    if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-    ws.warm_start = false;
-    c.sync();
-    return;
-  }
+  if (gamma == 0) { run.finish(0, true, false, "x is a zero-residual solution"); return; }
   int iter = 0;
   int itmax = default_itmax(ws, o.itmax);
   T pAp = 0, pNorm2 = gamma;
@@ -180,7 +173,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
     ws.mdiag_fused = (MisI || M.kind != LinOp<T>::DIAG) ? nullptr : M.diag;   // Diagonal M: applied inside K1/K2 (z is not materialised)
     ws.mblocks_fused = M.kind == LinOp<T>::BDIAG ? M.blocks : nullptr;        // block-Jacobi M: z = M r materialised in phase B
     ws.mbs_fused = M.kind == LinOp<T>::BDIAG ? M.bs : 0;
-    cg_fused_loop<T>(ws, *A.csr, o, gamma, eps_tol, itmax, start_time, solved, tired, zero_curvature, inconsistent,
+    cg_fused_loop<T>(ws, *A.csr, o, gamma, eps_tol, itmax, run.start, solved, tired, zero_curvature, inconsistent,
                      user_exit, overtimed, iter);
   } else {
     T* p = ws.p;
@@ -209,7 +202,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
         sigma = s1 > s2 ? s1 : s2;
       }
       if (kdisplay(iter, o.verbose))
-        printf("  %8.1e  %8.1e  %8.1e  %.2fs\n", (double)pAp, (double)alpha, (double)sigma, now_seconds() - start_time);
+        printf("  %8.1e  %8.1e  %8.1e  %.2fs\n", (double)pAp, (double)alpha, (double)sigma, run.elapsed());
       if ((radius > 0) && ((pAp <= 0) || (alpha > sigma))) {
         alpha = sigma;
         if (pAp <= 0) { k_copy<T>(c, n, ws.npc_dir, p); stats.npcCount = 1; stats.indefinite = true; }
@@ -233,9 +226,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
       }
       iter = iter + 1;
       tired = iter >= itmax;
-      if (o.callback) { c.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
-      overtimed = (now_seconds() - start_time) > o.timemax;
-      agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
+      run.poll(iter, user_exit, overtimed);
       if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e", iter, (double)rNorm);
     }
   }
@@ -247,12 +238,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   if (tired) status = "maximum number of iterations exceeded";
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-  ws.warm_start = false;
-  c.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = inconsistent;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, inconsistent, status);
 }
 
 // ===========================================================================
@@ -261,7 +247,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
 template <class T>
 void bicgstab_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_in, const LinOp<T>& M, const LinOp<T>& N,
                     const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv;
@@ -288,21 +274,14 @@ void bicgstab_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_
   T alpha = 1, omega = 1, rho = 1;
   T rNorm = k_nrm2<T>(c, n, r);
   if (history) stats.residuals.push_back(rNorm);
-  auto finish_early = [&](bool solved, const char* status) {
-    stats.niter = 0; stats.solved = solved; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time; stats.status = status;
-    if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-    ws.warm_start = false;
-    c.sync();
-  };
-  if (rNorm == 0) { finish_early(true, "x is a zero-residual solution"); return; }
+  if (rNorm == 0) { run.finish(0, true, false, "x is a zero-residual solution"); return; }
   int iter = 0;
   const int itmax = default_itmax(ws, o.itmax);
   const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
   if (o.verbose > 0) printf("%5s  %7s  %8s  %8s  %5s\n", "k", "‖rₖ‖", "|αₖ|", "|ωₖ|", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)rNorm, 1.0, 1.0, now_seconds() - start_time);
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)rNorm, 1.0, 1.0, run.elapsed());
   T next_rho = k_dot<T>(c, n, cvec, r);
-  if (next_rho == 0) { finish_early(false, "Breakdown bᴴc = 0"); return; }
+  if (next_rho == 0) { run.finish(0, false, false, "Breakdown bᴴc = 0"); return; }
   bool solved = rNorm <= eps_tol, tired = iter >= itmax, breakdown = false, user_exit = false, overtimed = false;
   std::string status = "unknown";
   const bool fusedB = o.fused && A.kind == LinOp<T>::CSR && NisI && (MisI || (M.kind == LinOp<T>::DIAG && !ldiv));
@@ -337,14 +316,12 @@ void bicgstab_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_
     }
     if (history) stats.residuals.push_back(rNorm);
     const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-    if (o.callback) { c.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, user_exit, overtimed);
     solved = (rNorm <= eps_tol) || resid_decrease_mach;
     tired = iter >= itmax;
     breakdown = (alpha == 0 || std::isnan(alpha));
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
     if (kdisplay(iter, o.verbose))
-      printf("%5d  %7.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)rNorm, (double)std::fabs(alpha), (double)std::fabs(omega), now_seconds() - start_time);
+      printf("%5d  %7.1e  %8.1e  %8.1e  %.2fs\n", iter, (double)rNorm, (double)std::fabs(alpha), (double)std::fabs(omega), run.elapsed());
   }
   if (o.verbose > 0) printf("\n");
   if (tired) status = "maximum number of iterations exceeded";
@@ -352,31 +329,39 @@ void bicgstab_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* c_
   if (solved) status = "solution good enough given atol and rtol";
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-  ws.warm_start = false;
-  c.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = false;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, false, status);
 }
 
-// ===========================================================================
-// gmres!  (src/gmres.jl:121-384)
-// ===========================================================================
-template <class T>
-void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
-  const double start_time = now_seconds();
+// ---------------------------------------------------------------------------
+// gmres!, fom! and fgmres! are one driver: the restart cycle, MGS with optional reorthogonalization, the fused
+// Arnoldi step, memory growth, the back substitution and the x update are shared.  They differ in the small
+// factorization of H kept on the host (Givens QR: GMRES, FGMRES; LU without pivoting: FOM) and in where the right
+// preconditioner lives (FGMRES stores Z[k] = N_k V[k]; GMRES and FOM apply N through pp).  The differences are marked.
+//   gmres!   src/gmres.jl:121-384
+//   fom!     src/fom.jl:121-368
+//   fgmres!  src/fgmres.jl:128-388
+// ---------------------------------------------------------------------------
+enum class Arnoldi { GMRES, FOM, FGMRES };
+
+template <class T, Arnoldi K>
+static void arnoldi_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
+  constexpr bool QR = K != Arnoldi::FOM;          // Givens QR of H (else LU)
+  constexpr bool FLEX = K == Arnoldi::FGMRES;     // right preconditioner kept in Z[k]
+  SolveRun<T> run(ws, o);
   Ctx& cx = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv, restart = o.restart, reorth = o.reorthogonalization;
-  if (o.verbose > 0) printf("GMRES: system of size %d\n", n);
+  if (o.verbose > 0) printf("%s: system of size %d\n", K == Arnoldi::GMRES ? "GMRES" : FLEX ? "FGMRES" : "FOM", n);
   const bool MisI = M.is_identity(), NisI = N.is_identity();
   allocate_if(!MisI, ws, ws.q);
-  allocate_if(!NisI, ws, ws.pp);
+  if (!FLEX) allocate_if(!NisI, ws, ws.pp);
   allocate_if(restart, ws, ws.dx);
   T *dx = ws.dx, *x = ws.x, *w = ws.w;
   std::vector<T*>& V = ws.V;
+  std::vector<T*>& Z = ws.Z;
+  // QR: c, s (sgiv), z (zg), R.   FOM: l (sgiv), z (zg), U (R); c is unused.
   std::vector<T>&c = ws.c, &s = ws.sgiv, &z = ws.zg, &R = ws.R;
+  std::vector<T>& l = ws.sgiv;
   Stats& stats = ws.stats;
   const bool warm_start = ws.warm_start;
   stats.reset();
@@ -397,37 +382,32 @@ void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>
   T rNorm = beta;
   if (history) stats.residuals.push_back(beta);
   const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
-  if (beta == 0) {
-    stats.niter = 0; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
-    if (warm_start) k_axpy<T>(cx, n, T(1), dx, x);
-    ws.warm_start = false;
-    cx.sync();
-    return;
-  }
-  const int mem = (int)c.size();                              // gmres.jl:181
+  if (beta == 0) { run.finish(0, true, false, "x is a zero-residual solution"); return; }
+  const int mem = (int)s.size();                              // length(c) / length(l)
   int npass = 0, iter = 0, inner_iter = 0;
   const int itmax = default_itmax(ws, o.itmax);
   int inner_itmax = itmax;
   if (o.verbose > 0) printf("%5s  %5s  %7s  %7s  %5s\n", "pass", "k", "‖rₖ‖", "hₖ₊₁.ₖ", "timer");
-  if (kdisplay(iter, o.verbose)) printf("%5d  %5d  %7.1e  %7s  %.2fs\n", npass, iter, (double)rNorm, "✗ ✗ ✗ ✗", now_seconds() - start_time);
+  if (kdisplay(iter, o.verbose)) printf("%5d  %5d  %7.1e  %7s  %.2fs\n", npass, iter, (double)rNorm, "✗ ✗ ✗ ✗", run.elapsed());
   const T btol = std::pow(eps_of<T>(), T(0.75));              // gmres.jl:195
-  const bool fusedG = o.fused && A.kind == LinOp<T>::CSR && NisI && !reorth && (MisI || (M.kind == LinOp<T>::DIAG && !ldiv));
-  ws.mdiag_fused = (fusedG && !MisI) ? M.diag : nullptr;
+  // the fused Arnoldi step folds a left diagonal M into the SpMV epilogue; GMRES and FOM need N = I (FGMRES
+  // materialises Z[k])
+  const bool fusedA = o.fused && A.kind == LinOp<T>::CSR && !reorth && (FLEX || NisI) &&
+                      (MisI || (M.kind == LinOp<T>::DIAG && !ldiv));
+  ws.mdiag_fused = (fusedA && !MisI) ? M.diag : nullptr;
   bool breakdown = false, inconsistent = false, solved = rNorm <= eps_tol, tired = iter >= itmax;
   bool inner_tired = inner_iter >= inner_itmax, user_exit = false, overtimed = false;
   std::string status = "unknown";
 
   while (!(solved || tired || breakdown || user_exit || overtimed)) {
     int nr = 0;
-    // gmres.jl:211-213 zero-fills V[1..mem] every cycle.  Every V[i] read below
-    // is written first (V[1] by kdivcopy!, V[k+1] at the end of step k), so the
-    // fill is dead for the results; it is kept only for the non-restart case
-    // where user callbacks may look at unused columns.
-    if (!restart) for (int i = 0; i < mem; i++) k_fill<T>(cx, n, V[i], T(0));
+    // The reference zero-fills V (and Z) every cycle.  GMRES and FGMRES read only entries they wrote first (V[1] by
+    // kdivcopy!, V[k+1] at the end of step k), so the fill is kept only where callbacks could see unused columns.
+    // FOM does read a zero V[k+1] after a user exit or timeout (its inner loop does not test them, fom.jl:237), so
+    // FOM always fills.
+    if (!restart || !QR) for (int i = 0; i < mem; i++) { k_fill<T>(cx, n, V[i], T(0)); if (FLEX) k_fill<T>(cx, n, Z[i], T(0)); }
     std::fill(s.begin(), s.end(), T(0));
-    std::fill(c.begin(), c.end(), T(0));
+    if (QR) std::fill(c.begin(), c.end(), T(0));
     std::fill(R.begin(), R.end(), T(0));
     std::fill(z.begin(), z.end(), T(0));
     if (restart) {
@@ -445,103 +425,136 @@ void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>
     ws.inner_iter = 0;
     inner_tired = false;
 
-    while (!(solved || inner_tired || breakdown || user_exit || overtimed)) {
+    // fom.jl:237 tests only solved/inner_tired/breakdown; gmres! and fgmres! (fgmres.jl:243) also the user exit and the timer
+    while (!(solved || inner_tired || breakdown || (QR && (user_exit || overtimed)))) {
       ws.inner_iter = ws.inner_iter + 1;
       inner_iter = ws.inner_iter;
       if (!restart && (inner_iter > mem)) {                   // gmres.jl:244-252
         const double t0 = now_seconds();
         for (int i = 0; i < inner_iter; i++) R.push_back(T(0));
-        s.push_back(T(0)); c.push_back(T(0));
+        s.push_back(T(0));                                    // s / FOM l
+        if (QR) c.push_back(T(0));
+        if (FLEX) Z.push_back(dev_alloc<T>((size_t)n));
+        if (!QR) z.push_back(T(0));                           // fom.jl:249 grows z here, gmres.jl / fgmres.jl with V
         stats.allocation_timer += now_seconds() - t0;
       }
+      if (!QR && inner_iter > (int)V.size()) {
+        // FOM past `memory` after a user exit or timeout: its inner loop runs one more step (fom.jl:237), on a
+        // V[k] the previous step did not form.  Give it the zero column it has within `memory`.
+        V.push_back(dev_alloc<T>((size_t)n));
+        k_fill<T>(cx, n, V.back(), T(0));
+      }
+      T* vk = V[inner_iter - 1];
+      T* p;
+      if (FLEX) {                                             // z_k <- N_k v_k, unconditional (fgmres.jl:262)
+        p = Z[inner_iter - 1];
+        if (NisI) k_copy<T>(cx, n, p, vk); else op_apply(cx, N, vk, p, ldiv);
+      } else {
+        p = NisI ? vk : ws.pp;
+        if (!NisI) op_apply(cx, N, vk, p, ldiv);
+      }
       T Hbis;
-      if (fusedG && inner_iter <= gmres_fused_max()) {
+      if (fusedA && inner_iter <= gmres_fused_max()) {
         // 1 + k launches: SpMV fused with the first MGS dot, then one launch per MGS step that applies
         // q -= h_i v_i and accumulates the next dot (or ||q||^2); one read-back of the whole R column.
-        gmres_fused_arnoldi<T>(ws, *A.csr, inner_iter, &R[nr], &Hbis);
+        gmres_fused_arnoldi<T>(ws, *A.csr, inner_iter, &R[nr], &Hbis, p);
       } else {
-      T* vk = V[inner_iter - 1];
-      T* p = NisI ? vk : ws.pp;
-      if (!NisI) op_apply(cx, N, vk, p, ldiv);
-      op_apply(cx, A, p, w);
-      if (!MisI) op_apply(cx, M, w, q, ldiv);
-      for (int i = 0; i < inner_iter; i++) {                  // MGS, gmres.jl:259-262
-        R[nr + i] = k_dot<T>(cx, n, V[i], q);
-        k_axpy<T>(cx, n, -R[nr + i], V[i], q);
-      }
-      if (reorth) {
-        for (int i = 0; i < inner_iter; i++) {
-          const T Htmp = k_dot<T>(cx, n, V[i], q);
-          R[nr + i] += Htmp;
-          k_axpy<T>(cx, n, -Htmp, V[i], q);
+        op_apply(cx, A, p, w);
+        if (!MisI) op_apply(cx, M, w, q, ldiv);
+        for (int i = 0; i < inner_iter; i++) {                // MGS, gmres.jl:259-262
+          R[nr + i] = k_dot<T>(cx, n, V[i], q);
+          k_axpy<T>(cx, n, -R[nr + i], V[i], q);
         }
+        if (reorth) {
+          for (int i = 0; i < inner_iter; i++) {
+            const T Htmp = k_dot<T>(cx, n, V[i], q);
+            R[nr + i] += Htmp;
+            k_axpy<T>(cx, n, -Htmp, V[i], q);
+          }
+        }
+        Hbis = k_nrm2<T>(cx, n, q);
       }
-      Hbis = k_nrm2<T>(cx, n, q);
+      T zeta_next = 0;
+      if (QR) {                                               // Givens QR of H, gmres.jl:280-284 / fgmres.jl:285-303
+        for (int i = 0; i < inner_iter - 1; i++) {
+          const T Rtmp = c[i] * R[nr + i] + s[i] * R[nr + i + 1];
+          R[nr + i + 1] = s[i] * R[nr + i] - c[i] * R[nr + i + 1];
+          R[nr + i] = Rtmp;
+        }
+        sym_givens<T>(R[nr + inner_iter - 1], Hbis, &c[inner_iter - 1], &s[inner_iter - 1], &R[nr + inner_iter - 1]);
+        zeta_next = s[inner_iter - 1] * z[inner_iter - 1];
+        z[inner_iter - 1] = c[inner_iter - 1] * z[inner_iter - 1];
+        rNorm = std::fabs(zeta_next);
+      } else {                                                // LU of H without pivoting, fom.jl:274-288
+        if (inner_iter >= 2) {
+          for (int i = 2; i <= inner_iter; i++) R[nr + i - 1] = R[nr + i - 1] - l[i - 2] * R[nr + i - 2];
+          z[inner_iter - 1] = -l[inner_iter - 2] * z[inner_iter - 2];
+        }
+        l[inner_iter - 1] = Hbis / R[nr + inner_iter - 1];
+        rNorm = Hbis * std::fabs(z[inner_iter - 1] / R[nr + inner_iter - 1]);
       }
-      for (int i = 0; i < inner_iter - 1; i++) {              // gmres.jl:280-284
-        const T Rtmp = c[i] * R[nr + i] + s[i] * R[nr + i + 1];
-        R[nr + i + 1] = s[i] * R[nr + i] - c[i] * R[nr + i + 1];
-        R[nr + i] = Rtmp;
-      }
-      sym_givens<T>(R[nr + inner_iter - 1], Hbis, &c[inner_iter - 1], &s[inner_iter - 1], &R[nr + inner_iter - 1]);
-      const T zeta_next = s[inner_iter - 1] * z[inner_iter - 1];
-      z[inner_iter - 1] = c[inner_iter - 1] * z[inner_iter - 1];
-      rNorm = std::fabs(zeta_next);
       if (history) stats.residuals.push_back(rNorm);
       nr = nr + inner_iter;
       const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
-      if (o.callback) { cx.sync(); stats.niter = iter + inner_iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+      run.poll(iter + inner_iter, user_exit, overtimed);
       const bool resid_decrease_lim = rNorm <= eps_tol;
       breakdown = Hbis <= btol;
       solved = resid_decrease_lim || resid_decrease_mach;
       inner_tired = restart ? inner_iter >= std::min(mem, inner_itmax) : inner_iter >= inner_itmax;
-      overtimed = (now_seconds() - start_time) > o.timemax;
-      agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
       if (kdisplay(iter + inner_iter, o.verbose))
-        printf("%5d  %5d  %7.1e  %7.1e  %.2fs\n", npass, iter + inner_iter, (double)rNorm, (double)Hbis, now_seconds() - start_time);
+        printf("%5d  %5d  %7.1e  %7.1e  %.2fs\n", npass, iter + inner_iter, (double)rNorm, (double)Hbis, run.elapsed());
       if (!(solved || inner_tired || breakdown || user_exit || overtimed)) {   // gmres.jl:318-327
         if (!restart && (inner_iter >= mem)) {
           const double t0 = now_seconds();
           V.push_back(dev_alloc<T>((size_t)n));
-          z.push_back(T(0));
+          if (QR) z.push_back(T(0));
           stats.allocation_timer += now_seconds() - t0;
         }
         k_divcopy<T>(cx, n, V[inner_iter], q, Hbis);
-        z[inner_iter] = zeta_next;
+        if (QR) z[inner_iter] = zeta_next;
       }
     }
-    std::vector<T>& y = z;                                    // gmres.jl:331-345
+    std::vector<T>& y = z;                                    // back substitution, gmres.jl:331-345 / fom.jl:322-331
     for (int i = inner_iter; i >= 1; i--) {
       int pos = nr + i - inner_iter;                          // 1-based
       for (int j = inner_iter; j >= i + 1; j--) {
         y[i - 1] = y[i - 1] - R[pos - 1] * y[j - 1];
         pos = pos - j + 1;
       }
-      if (std::fabs(R[pos - 1]) <= btol) { y[i - 1] = T(0); inconsistent = true; }
+      if (QR && std::fabs(R[pos - 1]) <= btol) { y[i - 1] = T(0); inconsistent = true; }
       else y[i - 1] = y[i - 1] / R[pos - 1];
     }
-    if (fusedG) gmres_fused_update_x<T>(ws, xr, inner_iter, y.data());      // same sums, same order, one pass per 8 vectors
-    else for (int i = 0; i < inner_iter; i++) k_axpy<T>(cx, n, y[i], V[i], xr);
-    if (!NisI) { k_copy<T>(cx, n, ws.pp, xr); op_apply(cx, N, ws.pp, xr, ldiv); }
+    T* const* basis = FLEX ? Z.data() : V.data();             // x_k = Z_k y_k (FGMRES) or N V_k y_k (GMRES, FOM)
+    if (fusedA) fused_multi_axpy<T>(ws, xr, inner_iter, y.data(), basis);   // same sums, same order, one pass per 8 vectors
+    else for (int i = 0; i < inner_iter; i++) k_axpy<T>(cx, n, y[i], basis[i], xr);
+    if (!FLEX && !NisI) { k_copy<T>(cx, n, ws.pp, xr); op_apply(cx, N, ws.pp, xr, ldiv); }
     if (restart) k_axpy<T>(cx, n, T(1), xr, x);
     inner_itmax = inner_itmax - inner_iter;
     iter = iter + inner_iter;
     tired = iter >= itmax;
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
+    run.poll(iter, user_exit, overtimed, false);             // the clock only: the callback ran in the inner loop
   }
   if (o.verbose > 0) printf("\n");
   if (tired) status = "maximum number of iterations exceeded";
+  if (!QR && breakdown) status = "inconsistent linear system";
   if (solved) status = "solution good enough given atol and rtol";
-  if (inconsistent) status = "found approximate least-squares solution";
+  if (QR && inconsistent) status = "found approximate least-squares solution";
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start && !restart) k_axpy<T>(cx, n, T(1), dx, x);
-  ws.warm_start = false;
-  cx.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = inconsistent;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, QR ? inconsistent : (!solved && breakdown), status, !restart);
+}
+
+template <class T>
+void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
+  arnoldi_solve<T, Arnoldi::GMRES>(ws, A, b, M, N, o);
+}
+template <class T>
+void fom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
+  arnoldi_solve<T, Arnoldi::FOM>(ws, A, b, M, N, o);
+}
+template <class T>
+void fgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o) {
+  arnoldi_solve<T, Arnoldi::FGMRES>(ws, A, b, M, N, o);
 }
 
 // ===========================================================================
@@ -549,7 +562,7 @@ void gmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>
 // ===========================================================================
 template <class T>
 void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
-  const double start_time = now_seconds();
+  SolveRun<T> run(ws, o);
   Ctx& c = ws.ctx;
   const int n = ws.n;
   const bool history = o.history, ldiv = o.ldiv, linesearch = o.linesearch;
@@ -586,13 +599,8 @@ void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
   T beta1 = k_dot<T>(c, n, r1, v);
   if (beta1 < 0) throw std::runtime_error("Preconditioner is not positive definite");
   if (beta1 == 0) {                                           // minres.jl:220-231
-    stats.niter = 1; stats.solved = true; stats.inconsistent = false;
-    stats.timer = now_seconds() - start_time;
-    stats.status = "x is a zero-residual solution";
     if (history) { stats.residuals.push_back(beta1); stats.Aresiduals.push_back(0); stats.Acond.push_back(0); }
-    if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-    ws.warm_start = false;
-    c.sync();
+    run.finish(1, true, false, "x is a zero-residual solution");
     return;
   }
   beta1 = std::sqrt(beta1);
@@ -682,16 +690,12 @@ void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
       }
       if (cg_ >= 0) {
         if (o.verbose > 0) printf("nonpositive curvature detected:  cs * γbar = %e\n", (double)cg_);
-        stats.solved = true; stats.npcCount = 1;
+        stats.npcCount = 1;
         // (the reference's `w1 = w` only rebinds a local name)
         if (iter == 1) k_copy<T>(c, n, x, b);
         else if (delta_w < 0) stats.npcCount = 2;
-        stats.niter = iter; stats.inconsistent = false;
-        stats.timer = now_seconds() - start_time;
-        stats.status = "nonpositive curvature";
-        ws.warm_start = false;
         stats.indefinite = true;
-        c.sync();
+        run.finish(iter, true, false, "nonpositive curvature", false);
         return;
       }
     }
@@ -729,14 +733,9 @@ void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
     if (history) stats.Acond.push_back(Acond);
     if (kdisplay(iter, o.verbose))
       printf("%5d  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm,
-             (double)beta, (double)cs, (double)sn, (double)ANorm, (double)Acond, (double)test1, (double)test2, now_seconds() - start_time);
+             (double)beta, (double)cs, (double)sn, (double)ANorm, (double)Acond, (double)test1, (double)test2, run.elapsed());
     if (iter == 1 && beta / beta1 <= 10 * epsM) {             // minres.jl:425-435
-      stats.niter = 1; stats.solved = true; stats.inconsistent = true;
-      stats.timer = now_seconds() - start_time;
-      stats.status = "x is a minimum least-squares solution";
-      if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-      ws.warm_start = false;
-      c.sync();
+      run.finish(1, true, true, "x is a minimum least-squares solution");
       return;
     }
     ill_cond_mach = (T(1) + T(1) / Acond <= T(1));
@@ -749,13 +748,11 @@ void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
     zero_resid_lim = MisI && (test1 <= eps_of<T>());
     const bool resid_decrease_lim = (rNorm <= eps_tol);
     if (iter >= window) fwd_err = err_lbnd <= etol * std::sqrt(xENorm2);
-    if (o.callback) { c.sync(); stats.niter = iter; user_exit = o.callback(&ws, o.callback_user) != 0; }
+    run.poll(iter, user_exit, overtimed);
     zero_resid = zero_resid_mach || zero_resid_lim;
     const bool resid_decrease = resid_decrease_mach || resid_decrease_lim;
     ill_cond = ill_cond_mach || ill_cond_lim;
     solved = solved_mach || solved_lim || zero_resid || fwd_err || resid_decrease;
-    overtimed = (now_seconds() - start_time) > o.timemax;
-    agree_exit(ws, o, user_exit, overtimed);      // row-partitioned: same decision on every rank
   }
   if (o.verbose > 0) printf("\n");
   if (tired) status = "maximum number of iterations exceeded";
@@ -766,12 +763,7 @@ void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
   if (fwd_err) status = "truncated forward error small enough";
   if (user_exit) status = "user-requested exit";
   if (overtimed) status = "time limit exceeded";
-  if (warm_start) k_axpy<T>(c, n, T(1), dx, x);
-  ws.warm_start = false;
-  c.sync();
-  stats.niter = iter; stats.solved = solved; stats.inconsistent = !zero_resid;
-  stats.timer = now_seconds() - start_time;
-  stats.status = status;
+  run.finish(iter, solved, !zero_resid, status);
 }
 
 #define INST(T)                                                                                                   \
@@ -780,6 +772,8 @@ void minres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T
   template void ws_warm_start<T>(Workspace<T>*, const T*);                                                        \
   template void cg_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);          \
   template void gmres_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
+  template void fom_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
+  template void fgmres_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void bicgstab_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void minres_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);
 INST(double)

@@ -79,7 +79,7 @@ def test_cg_lanczos_negative_curvature(kb, O):
     assert np.allclose(x, xo, rtol=1e-10, atol=1e-14)
 
 
-@pytest.mark.parametrize("name", ["fom", "fgmres"])
+@pytest.mark.parametrize("name", ["fom", "fgmres", "gmres"])
 @pytest.mark.parametrize("kw", [dict(), dict(restart=True), dict(M=True), dict(N=True), dict(M=True, N=True, restart=True),
                                 dict(reorthogonalization=True), dict(x0=True), dict(x0=True, restart=True)])
 def test_fom_fgmres_match_oracle(kb, O, name, kw):
@@ -105,12 +105,12 @@ def test_fom_fgmres_match_oracle(kb, O, name, kw):
     tol = 1e-5 if name == "fom" else 1e-6
     for fused in (True, False):
         _check(out[fused][1], out[fused][0], so, xo, tol=tol)
-    eligible = not kw.get("reorthogonalization") and not (name == "fom" and kw.get("N"))
+    eligible = not kw.get("reorthogonalization") and not (name in ("fom", "gmres") and kw.get("N"))
     if eligible:
         assert out[True][2] < out[False][2]
 
 
-@pytest.mark.parametrize("name", ["fom", "fgmres"])
+@pytest.mark.parametrize("name", ["fom", "fgmres", "gmres"])
 def test_fom_fgmres_memory_growth_and_special_cases(kb, O, name):
     f, fo = getattr(kb, name), getattr(O, name)
     A, b = O.kron_unsymmetric(7)
@@ -155,6 +155,10 @@ def test_sibling_float32_and_callback(kb, O):
         assert st.status == "user-requested exit" and st.niter == (4 if name == "fom" else 3), name
         with pytest.raises(TypeError):
             getattr(kb, name)(A, b, callback=lambda w: "string")
+    # the same extra FOM step past `memory` (no restart), where V[k] was never allocated: a zero column as within it
+    cnt = []
+    x, st = kb.fom(Ak, bk, memory=5, atol=0.0, rtol=0.0, callback=lambda w: (cnt.append(1), len(cnt) >= 7)[1])
+    assert st.status == "user-requested exit" and st.niter == 8
 
 
 def test_sibling_solvers_through_the_reference_c_abi(kb, O):
