@@ -43,9 +43,9 @@ typedef enum { KRYLOV_FLOAT32 = 0, KRYLOV_FLOAT64 = 1, KRYLOV_COMPLEX32 = 2, KRY
 typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
 
 /* positional, frozen (krylov.h:48-83).  Implemented here: CG, MINRES, GMRES, BICGSTAB (the hot path), the
- * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, and the least-squares solvers LSQR and
- * LSMR on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a CSR operator of
- * m rows and n columns is attached); every other value returns -2. */
+ * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, and the least-squares solvers LSQR,
+ * LSMR, LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a
+ * CSR operator of m rows and n columns is attached); every other value returns -2. */
 typedef enum {
   KRYLOV_CG = 0, KRYLOV_CR = 1, KRYLOV_SYMMLQ = 2, KRYLOV_MINRES = 3, KRYLOV_MINRES_QLP = 4, KRYLOV_DIOM = 5,
   KRYLOV_DQGMRES = 6, KRYLOV_FOM = 7, KRYLOV_GMRES = 8, KRYLOV_FGMRES = 9, KRYLOV_BICGSTAB = 10, KRYLOV_CGS = 11,
@@ -134,7 +134,7 @@ const char *krylov_b200_last_error(void);
 /* Attach a CSR matrix as the operator A of `ws`: replaces mul!(y, A, x) at
  * cg.jl:196, gmres.jl:257, bicgstab.jl:221,228, minres.jl:289.
  *   rowptr[n+1], colind[nnz], values[nnz] (element type = workspace dtype);
- *   LSQR / LSMR workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
+ *   least-squares workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
  *   the library forms A^T once (host-side) on the first solve and keeps it until the operator changes;
  *   index_base 0|1, index_bytes 4|8 (Julia's SparseMatrixCSC{T,Int64} passes
  *   1 and 8 -- for a symmetric matrix its CSC arrays ARE the CSR arrays);
@@ -148,7 +148,8 @@ int krylov_b200_share_operator(void *ws, void *src);
 int krylov_b200_attach_csr(void *ws, void *csr);
 /* Diagonal preconditioner: which = 0 -> M, 1 -> N; d[n] holds the diagonal of
  * the operator the solver applies (P^-1 with the default ldiv=false). NULL detaches.
- * LSQR / LSMR: M acts on the data space (d[m]), N on the solution space (d[n]). */
+ * LSQR / LSMR / LSLQ: M acts on the data space (d[m]), N on the solution space (d[n]).  CGLS / CRLS: M acts on the
+ * residual space (d[m]); they take no N (a solve with N attached or matvec_N given is refused). */
 int krylov_b200_set_preconditioner_diag(void *ws, int which, const void *d, int location);
 /* Block-Jacobi preconditioner (docs/src/preconditioners.md:33,159): which = 0 -> M, 1 -> N; blocks[ceil(n/bs)][bs][bs]
  * (row-major dense diagonal blocks, 2 <= bs <= 8, element type = workspace dtype; a last block of n % bs rows uses
@@ -177,7 +178,10 @@ typedef struct {
   int check_curvature; /* CG-Lanczos: kwarg `check_curvature` (src/cg_lanczos.jl:94)                            */
   double cr_gamma;     /* CR: kwarg `γ` (src/cr.jl:112); NaN -> sqrt(eps)                                        */
   double axtol;        /* LSQR, LSMR: kwarg `axtol` (src/lsqr.jl:152); NaN -> sqrt(eps)                          */
-  double btol;         /* LSQR, LSMR: kwarg `btol`; NaN -> sqrt(eps)                                              */
+  double btol;         /* LSQR, LSMR, LSLQ: kwarg `btol`; NaN -> sqrt(eps)                                        */
+  double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0                       */
+  double utol;         /* LSLQ: kwarg `utol`; NaN -> sqrt(eps)                                                       */
+  int transfer_to_lsqr; /* LSLQ: 1 -> return the LSQR point (kwarg `transfer_to_lsqr`)                                */
 } KrylovB200Options;
 KrylovB200Options krylov_b200_default_options(void);
 int krylov_b200_set_options(void *ws, const KrylovB200Options *opts);
@@ -196,9 +200,14 @@ typedef struct {
   double timer;
   char status[96];
   double Anorm;       /* LanczosStats.Anorm (cg_lanczos!); NaN for the other solvers */
+  int error_with_bnd;  /* LSLQStats (src/krylov_stats.jl:352-365): the error bounds became complex              */
+  int nerr_lbnds;      /* LSLQ history lengths (krylov_b200_get_history which = 3, 4, 5)                        */
+  int nerr_ubnds_lq;
+  int nerr_ubnds_cg;
 } KrylovB200Stats;
 int krylov_b200_get_stats(void *ws, KrylovB200Stats *out);
-/* which: 0 residuals, 1 Aresiduals, 2 Acond.  Returns the number copied (<= cap) or -1. */
+/* which: 0 residuals, 1 Aresiduals, 2 Acond; LSLQ: 3 err_lbnds, 4 err_ubnds_lq, 5 err_ubnds_cg.
+ * Returns the number copied (<= cap) or -1. */
 int krylov_b200_get_history(void *ws, int which, double *out, int cap);
 /* Device pointer of a workspace vector by its reference field name
  * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"). */

@@ -40,7 +40,7 @@ struct Handle {
   int p = 0;
   void* ws = nullptr;
   std::shared_ptr<CsrAny> csr;
-  std::shared_ptr<CsrAny> csrT;        // LSQR / LSMR: A^T of the attached operator, built on first use ...
+  std::shared_ptr<CsrAny> csrT;        // least squares: A^T of the attached operator, built on first use ...
   const CsrAny* csrT_for = nullptr;    // ... for this operator
   void* Mdiag = nullptr;
   void* Ndiag = nullptr;
@@ -76,7 +76,8 @@ int fail(const char* where, const char* msg) {
 
 bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
-         s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR;
+         s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
+         s == S_LSLQ || s == S_CGLS || s == S_CRLS;
 }
 
 int pick_device() {
@@ -111,6 +112,7 @@ int m_of(Handle* h) {
   return h->dtype == KRYLOV_FLOAT64 ? W<double>(h)->m : W<float>(h)->m;
 }
 bool is_ls(const Handle* h) { return !h->block && is_ls_kind(h->solver); }
+bool is_cg_ls(int s) { return s == S_CGLS || s == S_CRLS; }     // CGLS / CRLS: M on the residual space, no N
 template <class T> Csr<T>& csr_of(CsrAny& a);
 template <> Csr<double>& csr_of<double>(CsrAny& a) { return a.d; }
 template <> Csr<float>& csr_of<float>(CsrAny& a) { return a.f; }
@@ -172,6 +174,10 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   s.cr_gamma = std::isnan(h->ext.cr_gamma) ? -1 : h->ext.cr_gamma;
   if (h->solver == S_MINRES) { s.lambda = o->lambda; s.linesearch = o->linesearch != 0; }
   if (is_ls_kind(h->solver)) { s.lambda = o->lambda; s.radius = o->radius; }   // _typed_solve_ls_mn_radius! (c_stores.jl:403-423)
+  if (h->solver == S_LSLQ) s.radius = 0;            // _typed_solve_ls_mn!: λ and no trust region
+  s.sigma = std::isnan(h->ext.sigma) ? 0 : h->ext.sigma;
+  s.utol = std::isnan(h->ext.utol) ? -1 : h->ext.utol;
+  s.transfer_to_lsqr = h->ext.transfer_to_lsqr != 0;
   // _typed_solve_gmres! serves GMRES, FGMRES and FOM (c_stores.jl:376-398)
   if (h->solver == S_GMRES || h->solver == S_FGMRES || h->solver == S_FOM) {
     s.restart = o->restart != 0; s.reorthogonalization = o->reorthogonalization != 0;
@@ -203,7 +209,8 @@ std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src) {
   return a;
 }
 
-// lsqr! / lsmr! (c_stores.jl:403-423): b has m entries, x has n; A maps n -> m and needs its adjoint
+// lsqr! / lsmr! (c_stores.jl:403-423), cgls! / crls! (_typed_solve_ls_m_radius!): b has m entries, x has n; A maps
+// n -> m and needs its adjoint
 template <class T>
 int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, void* ud,
                 const KrylovOptions* opts) {
@@ -213,7 +220,10 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
   const int m = ws->m, n = ws->n;
   LinOp<T> A, At;
   if (fA) {
-    if (!fAt) throw std::runtime_error("lsqr and lsmr apply the adjoint of A: matvec_At must be given with matvec_A");
+    if (!fAt)
+      throw std::runtime_error(is_cg_ls(h->solver)      ? "cgls and crls apply the adjoint of A: matvec_At must be given with matvec_A"
+                             : h->solver == S_LSLQ ? "lslq applies the adjoint of A: matvec_At must be given with matvec_A"
+                                                   : "lsqr and lsmr apply the adjoint of A: matvec_At must be given with matvec_A");
     A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
     At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
   } else if (h->csr) {
@@ -236,10 +246,18 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
   M.n = m; N.n = n;                      // M acts on the m-dimensional data space, N on the n-dimensional solution space
   if (!fM && h->Mdiag) { M.kind = LinOp<T>::DIAG; M.diag = (const T*)h->Mdiag; }
   if (!fN && h->Ndiag) { N.kind = LinOp<T>::DIAG; N.diag = (const T*)h->Ndiag; }
+  // The reference's C layer drops N for CGLS / CRLS; a caller passing one expects it to act, so it is refused.
+  if (is_cg_ls(h->solver) && !N.is_identity())
+    throw std::runtime_error("cgls and crls take no right preconditioner N (M acts on the m-dimensional residual space)");
   if (!b) throw std::runtime_error("b is NULL");
   const T* bd = stage_in<T>(h, ws, b, ws->bbuf);
-  if (h->solver == S_LSQR) lsqr_solve<T>(*ws, A, At, bd, M, N, so);
-  else lsmr_solve<T>(*ws, A, At, bd, M, N, so);
+  switch (h->solver) {
+    case S_LSQR: lsqr_solve<T>(*ws, A, At, bd, M, N, so); break;
+    case S_LSMR: lsmr_solve<T>(*ws, A, At, bd, M, N, so); break;
+    case S_LSLQ: lslq_solve<T>(*ws, A, At, bd, M, N, so); break;
+    case S_CGLS: cgls_solve<T>(*ws, A, At, bd, M, so); break;
+    case S_CRLS: crls_solve<T>(*ws, A, At, bd, M, so); break;
+  }
   return 0;
 }
 
@@ -307,7 +325,10 @@ template <class T> int do_get_x(Handle* h, void* x, int n) {
 
 template <class T> int do_warm_start(Handle* h, const void* x0, int n) {
   Workspace<T>* ws = W<T>(h);
-  if (is_ls_kind(h->solver)) throw std::runtime_error("lsqr and lsmr do not support warm-start (they take no x0)");
+  if (is_ls_kind(h->solver))
+    throw std::runtime_error(is_cg_ls(h->solver)      ? "cgls and crls do not support warm-start (they take no x0)"
+                             : h->solver == S_LSLQ ? "lslq does not support warm-start (it takes no x0)"
+                                                 : "lsqr and lsmr do not support warm-start (they take no x0)");
   if (n != ws->n) throw std::runtime_error("x0 should have size n");
   KB_CUDA(cudaSetDevice(ws->ctx.device));
   // c_stores.jl:218-229: allocate dx if empty, copy, set the flag
@@ -334,8 +355,10 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
       {"Nv", ws->Nv}, {"Mu", ws->Mu}, {"Av", ws->Av}, {"Atu", ws->Atu}, {"h", ws->h}, {"hbar", ws->hbar}};
   for (auto& e : tab) if (!strcmp(e.n, nm)) return e.p;
   if (nm[0] == 'P' && nm[1]) { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->Z.size()) return ws->Z[i - 1]; return nullptr; }
-  if (!strcmp(nm, "Ar")) return ws->Ap;
-  if (!strcmp(nm, "Mq")) return ws->z;
+  if (!strcmp(nm, "Ar")) return ws->Ar ? ws->Ar : ws->Ap;   // CRLS has its own Ar; CR's Ar is Ap
+  if (!strcmp(nm, "Mr") || !strcmp(nm, "Ms")) return ws->Mr;
+  if (!strcmp(nm, "Mq")) return ws->kind == S_CGLS ? ws->Mr : ws->z;   // CGLS: Mq aliases Mr (cgls.jl:156)
+  if (!strcmp(nm, "w̄") || !strcmp(nm, "wbar")) return ws->kind == S_LSLQ ? ws->w : nullptr;
   if (nm[0] == 'Z') { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->Z.size()) return ws->Z[i - 1]; return nullptr; }
   if (nm[0] == 'V') { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->V.size()) return ws->V[i - 1]; }
   return nullptr;
@@ -620,7 +643,7 @@ int krylov_b200_set_operator_csr(void* ws, int n, long long nnz, const void* row
     a->dtype = h->dtype;
     Ctx& cx = ctx_of(h);
     KB_CUDA(cudaSetDevice(cx.device));
-    // n: number of rows (m of an LSQR / LSMR workspace, whose operator has the workspace's n columns)
+    // n: number of rows (m of a least-squares workspace, whose operator has the workspace's n columns)
     if (n != m_of(h)) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
     const int ncols = is_ls(h) ? n_of(h) : -1;
     if (h->dtype == KRYLOV_FLOAT64)
@@ -659,7 +682,7 @@ int krylov_b200_set_preconditioner_diag(void* ws, int which, const void* d, int 
     void*& slot = which == 0 ? h->Mdiag : h->Ndiag;
     if (!d) { dev_free(slot); slot = nullptr; return 0; }
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
-    const int n = which == 0 ? m_of(h) : n_of(h);     // LSQR / LSMR: M has m entries, N has n
+    const int n = which == 0 ? m_of(h) : n_of(h);     // least squares: M has m entries, N has n
     KB_CUDA(cudaSetDevice(ctx_of(h).device));
     if (!slot) slot = dev_alloc<char>(esz * (size_t)n);
     KB_CUDA(cudaMemcpy(slot, d, esz * (size_t)n, location ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
@@ -677,7 +700,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
     h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0;
     if (!blocks) return 0;
-    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on LSQR / LSMR workspaces");
+    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on least-squares (LSQR, LSMR, CGLS, CRLS) workspaces");
     if (bs < 2 || bs > 8) return fail("krylov_b200_set_preconditioner_blockdiag", "block size must be in 2..8");
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
     const int n = n_of(h);
@@ -706,6 +729,7 @@ KrylovB200Options krylov_b200_default_options(void) {
   KrylovB200Options o;
   memset(&o, 0, sizeof(o));
   o.etol = NAN; o.conlim = NAN; o.fused = 1; o.cr_gamma = NAN; o.axtol = NAN; o.btol = NAN;
+  o.sigma = 0.0; o.utol = NAN; o.transfer_to_lsqr = 0;
   return o;
 }
 
@@ -726,6 +750,9 @@ int krylov_b200_get_stats(void* ws, KrylovB200Stats* out) {
   out->nAcond = (int)s.Acond.size(); out->allocation_timer = s.allocation_timer; out->timer = s.timer;
   strncpy(out->status, s.status.c_str(), sizeof(out->status) - 1);
   out->Anorm = s.Anorm;
+  out->error_with_bnd = s.error_with_bnd;
+  out->nerr_lbnds = (int)s.err_lbnds.size(); out->nerr_ubnds_lq = (int)s.err_ubnds_lq.size();
+  out->nerr_ubnds_cg = (int)s.err_ubnds_cg.size();
   return 0;
 }
 
@@ -734,7 +761,8 @@ int krylov_b200_get_history(void* ws, int which, double* out, int cap) {
   if (!h) return fail("krylov_b200_get_history", "unknown workspace handle");
   if (!out || cap < 0) return fail("krylov_b200_get_history", "bad arguments (out is NULL or cap < 0)");
   const Stats& s = stats_any(h);
-  const std::vector<double>& v = which == 0 ? s.residuals : which == 1 ? s.Aresiduals : s.Acond;
+  const std::vector<double>& v = which == 0 ? s.residuals : which == 1 ? s.Aresiduals : which == 3 ? s.err_lbnds
+                                : which == 4 ? s.err_ubnds_lq : which == 5 ? s.err_ubnds_cg : s.Acond;
   int k = (int)v.size() < cap ? (int)v.size() : cap;
   for (int i = 0; i < k; i++) out[i] = v[i];
   return k;
@@ -896,7 +924,7 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_b200_dist_init", "unknown workspace handle");
-    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned LSQR / LSMR solves are not available");
+    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) solves are not available");
     return h->dtype == KRYLOV_FLOAT64 ? dist_init_t<double>(h, rank, world, nhalo, halo_rank, halo_off)
                                       : dist_init_t<float>(h, rank, world, nhalo, halo_rank, halo_off);
   } catch (const std::exception& e) { return fail("krylov_b200_dist_init", e); }

@@ -1,4 +1,4 @@
-// fused_phases.cu -- fused iteration phases of bicgstab!, minres! and gmres!
+// fused_phases.cu -- fused iteration phases of bicgstab!, minres!, gmres!, the siblings and the least-squares solvers
 // (SURVEY.md section 8a phase structures).  Each phase is ONE launch: an SpMV
 // or a streaming pass whose epilogue applies the adjacent axpy/axpby/scal
 // updates and accumulates the dot products the next scalar needs; the CTA that
@@ -704,6 +704,184 @@ template <class T> T lsq_fused_update(Workspace<T>& ws, bool lsmr, bool scale_v,
   return std::sqrt(xx[0]);
 }
 
+// LSLQ (src/lslq.jl:302-320,411-416): after LSQR's P1 / P2 (want_ww = false), one pass over n:
+//   v = Nv / alpha ; x += (c zeta) w̄ ; x += (s zeta) v ; w̄ = -c v + s w̄
+template <class T> struct LslqUpdateBody {
+  T* v; T* x; T* wbar; T inv_alpha, czeta, szeta, c, s; int scale_v;
+  __device__ __forceinline__ void operator()(int i, T*) const {
+    T vi = v[i];
+    if (scale_v) { vi = mul_rn(inv_alpha, vi); v[i] = vi; }
+    const T wi = wbar[i];
+    x[i] = add_rn(add_rn(x[i], mul_rn(czeta, wi)), mul_rn(szeta, vi));
+    wbar[i] = add_rn(mul_rn(-c, vi), mul_rn(s, wi));
+  }
+};
+template <class T> void lslq_fused_update(Workspace<T>& ws, bool scale_v, T inv_alpha, T czeta, T szeta, T c, T s) {
+  launch_stream<T, 0>(ws.ctx, ws.n, LslqUpdateBody<T>{ws.Nv, ws.x, ws.w, inv_alpha, czeta, szeta, c, s, scale_v ? 1 : 0},
+                      NoFin(), 5);
+}
+
+// ===========================================================================
+// CGLS  (src/cgls.jl:192-219, M = I, no trust region)
+// The scalars chain through the device block: K1's Fin derives alpha, K3's Fin gamma and beta, K4's Fin <p, p> (the
+// next delta's lambda term).  The host reads {<r, r>, gamma} once, after K3; K4 is already queued behind the copy.
+// ===========================================================================
+template <class T> struct CglsState { T gamma, alpha, beta, pp, rr; };
+
+template <class T> struct CglsK1Epi {     // q = A p ; <q, q>                       (cgls.jl:193,195)
+  T* q;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const { q[row] = acc; d[0] += acc * acc; }
+};
+template <class T> struct CglsK1Fin {     // delta (+ lambda <p, p>) ; alpha = gamma / delta   (cgls.jl:195-197)
+  CglsState<T>* s; T lambda;
+  __device__ void operator()(const T* tot) const {
+    T delta = tot[0];
+    if (lambda > T(0)) delta = add_rn(delta, mul_rn(lambda, s->pp));
+    s->alpha = div_rn(s->gamma, delta);
+  }
+};
+template <class T> struct CglsK2Body {    // r -= alpha q ; <r, r>                  (cgls.jl:207,215)
+  T* r; const T* q; const CglsState<T>* s;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    const T rn = add_rn(r[i], mul_rn(-s->alpha, q[i]));
+    r[i] = rn;
+    d[0] += rn * rn;
+  }
+};
+template <class T> struct CglsK2Fin {
+  CglsState<T>* s;
+  __device__ void operator()(const T* tot) const { s->rr = tot[0]; }
+};
+template <class T> struct CglsK3Epi {     // x += alpha p ; s = A^T r (- lambda x) ; <s, s>   (cgls.jl:206,209-211)
+  T* x; const T* p; T* sv; const CglsState<T>* s; T lambda;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T xn = add_rn(x[row], mul_rn(s->alpha, p[row]));
+    x[row] = xn;
+    T sn = acc;
+    if (lambda > T(0)) sn = add_rn(sn, mul_rn(-lambda, xn));
+    sv[row] = sn;
+    d[0] += sn * sn;
+  }
+};
+template <class T> struct CglsK3Fin {     // beta = gamma_next / gamma ; gamma = gamma_next   (cgls.jl:212,214)
+  CglsState<T>* s;
+  __device__ void operator()(const T* tot) const { s->beta = div_rn(tot[0], s->gamma); s->gamma = tot[0]; }
+};
+template <class T> struct CglsK4Body {    // p = s + beta p ; <p, p>                (cgls.jl:213)
+  T* p; const T* sv; const CglsState<T>* s;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    const T pn = add_rn(mul_rn(T(1), sv[i]), mul_rn(s->beta, p[i]));
+    p[i] = pn;
+    d[0] += pn * pn;
+  }
+};
+template <class T> struct CglsK4Fin {
+  CglsState<T>* s;
+  __device__ void operator()(const T* tot) const { s->pp = tot[0]; }
+};
+
+template <class T>
+void cgls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T lambda, T* rr, T* gamma_out) {
+  Ctx& c = ws.ctx;
+  typedef CglsState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  if (init) {                     // p = s, so <p, p> is the gamma the host computed
+    memset(H, 0, sizeof(St));
+    H->gamma = gamma; H->pp = gamma;
+    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+  }
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.p}, CglsK1Epi<T>{ws.q}, CglsK1Fin<T>{S, lambda}, 4);
+  launch_stream<T, 1>(c, ws.m, CglsK2Body<T>{ws.r, ws.q, S}, CglsK2Fin<T>{S}, 5);
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.r}, CglsK3Epi<T>{ws.x, ws.p, ws.s, S, lambda}, CglsK3Fin<T>{S}, 4);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  launch_stream<T, 1>(c, ws.n, CglsK4Body<T>{ws.p, ws.s, S}, CglsK4Fin<T>{S}, 5);
+  c.sync();
+  *rr = H[1].rr; *gamma_out = H[1].gamma;
+}
+
+// ===========================================================================
+// CRLS  (src/crls.jl:194-240, M = I, no trust region)
+// L4's Fin derives the next alpha, L2's Fin gamma and beta; the host reads {<Ar, Ar>, <x, x>, <r, r>, gamma} once,
+// after L2; L3 and L4 are already queued behind the copy.
+// ===========================================================================
+template <class T> struct CrlsState { T gamma, alpha, beta, ArAr, xx, rr; };
+
+template <class T> struct CrlsL1Body {    // x += alpha p ; Ar -= alpha q ; <Ar, Ar>, <x, x>   (crls.jl:217-219,237)
+  T* x; T* Ar; const T* p; const T* q; const CrlsState<T>* s;
+  __device__ __forceinline__ void operator()(int j, T* d) const {
+    const T alpha = s->alpha;
+    const T xn = add_rn(x[j], mul_rn(alpha, p[j]));
+    x[j] = xn;
+    const T an = add_rn(Ar[j], mul_rn(-alpha, q[j]));
+    Ar[j] = an;
+    d[0] += an * an; d[1] += xn * xn;
+  }
+};
+template <class T> struct CrlsL1Fin {
+  CrlsState<T>* s;
+  __device__ void operator()(const T* tot) const { s->ArAr = tot[0]; s->xx = tot[1]; }
+};
+template <class T> struct CrlsL2Epi {     // r -= alpha Ap ; s = A Ar ; <s, s>, <r, r>   (crls.jl:222-225)
+  T* r; const T* Ap; T* sv; const CrlsState<T>* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T rn = add_rn(r[row], mul_rn(-s->alpha, Ap[row]));
+    r[row] = rn;
+    sv[row] = acc;
+    d[0] += acc * acc; d[1] += rn * rn;
+  }
+};
+template <class T> struct CrlsL2Fin {     // gamma_next (+ lambda ||Ar||^2) ; beta = gamma_next / gamma   (crls.jl:225-227,235)
+  CrlsState<T>* s; T lambda;
+  __device__ void operator()(const T* tot) const {
+    T g = tot[0];
+    if (lambda > T(0)) { const T an = sqrt_rn(s->ArAr); g = add_rn(g, mul_rn(mul_rn(lambda, an), an)); }
+    s->beta = div_rn(g, s->gamma);
+    s->gamma = g;
+    s->rr = tot[1];
+  }
+};
+template <class T> struct CrlsL3Body {    // Ap = s + beta Ap                       (crls.jl:230)
+  T* Ap; const T* sv; const CrlsState<T>* s;
+  __device__ __forceinline__ void operator()(int i, T*) const { Ap[i] = add_rn(mul_rn(T(1), sv[i]), mul_rn(s->beta, Ap[i])); }
+};
+template <class T> struct CrlsL4Epi {     // p = Ar + beta p ; q = A^T Ap (+ lambda p) ; <q, q>   (crls.jl:229,232-233,194)
+  T* p; const T* Ar; T* q; const CrlsState<T>* s; T lambda;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T pn = add_rn(mul_rn(T(1), Ar[row]), mul_rn(s->beta, p[row]));
+    p[row] = pn;
+    T qn = acc;
+    if (lambda > T(0)) qn = add_rn(qn, mul_rn(lambda, pn));
+    q[row] = qn;
+    d[0] += qn * qn;
+  }
+};
+template <class T> struct CrlsL4Fin {     // alpha = gamma / <q, q>                 (crls.jl:195)
+  CrlsState<T>* s;
+  __device__ void operator()(const T* tot) const { s->alpha = div_rn(s->gamma, tot[0]); }
+};
+
+template <class T>
+void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, T gamma, T lambda, T* ArAr,
+                          T* xx, T* rr, T* gamma_out) {
+  Ctx& c = ws.ctx;
+  typedef CrlsState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  if (init) {
+    memset(H, 0, sizeof(St));
+    H->alpha = alpha; H->gamma = gamma;
+    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+  }
+  launch_stream<T, 2>(c, ws.n, CrlsL1Body<T>{ws.x, ws.Ar, ws.p, ws.q, S}, CrlsL1Fin<T>{S}, 5);
+  launch_spmv_epi_g<T, 2>(c, A, XPlain<T>{ws.Ar}, CrlsL2Epi<T>{ws.r, ws.Ap, ws.s, S}, CrlsL2Fin<T>{S, lambda}, 4);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  launch_stream<T, 0>(c, ws.m, CrlsL3Body<T>{ws.Ap, ws.s, S}, NoFin(), 5);
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.Ap}, CrlsL4Epi<T>{ws.p, ws.Ar, ws.q, S, lambda}, CrlsL4Fin<T>{S}, 4);
+  c.sync();
+  *ArAr = H[1].ArAr; *xx = H[1].xx; *rr = H[1].rr; *gamma_out = H[1].gamma;
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -723,7 +901,10 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template T cr_fused_directions<T>(Workspace<T>&, T);                                                               \
   template void fused_multi_axpy<T>(Workspace<T>&, T*, int, const T*, T* const*);                                    \
   template void lsq_fused_bidiag<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, bool, T*, T*, T*);        \
-  template T lsq_fused_update<T>(Workspace<T>&, bool, bool, T, T, T, T);
+  template T lsq_fused_update<T>(Workspace<T>&, bool, bool, T, T, T, T);                                             \
+  template void lslq_fused_update<T>(Workspace<T>&, bool, T, T, T, T, T);                                          \
+  template void cgls_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T*, T*);            \
+  template void crls_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T, T*, T*, T*, T*);
 INST(double)
 INST(float)
 #undef INST

@@ -10,7 +10,7 @@
 //   siblings.cu   cgs!, cg_lanczos!, dqgmres!, diom!, cr! on the same kernels (SURVEY.md 8f-3)
 //   solver_common.h  host helpers of the drivers, among them SolveRun: the callback / clock / exit protocol
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
-//   lsq.cu        host control flow of lsqr!/lsmr! on rectangular operators (primitive and fused paths)
+//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! on rectangular operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
 #pragma once
@@ -150,7 +150,9 @@ struct SolveOpts {
   bool linesearch = false;          // CG, MINRES
   double lambda = 0;                // MINRES, LSQR, LSMR
   double etol = -1, conlim = -1;    // MINRES, LSQR, LSMR (<0 => defaults)
-  double axtol = -1, btol = -1;     // LSQR, LSMR (<0 => sqrt(eps(T)))
+  double axtol = -1, btol = -1;     // LSQR, LSMR (<0 => sqrt(eps(T))); btol: LSLQ too
+  double sigma = 0, utol = -1;      // LSLQ: σ (Gauss-Radau bounds when > 0), utol (<0 => sqrt(eps(T)))
+  bool transfer_to_lsqr = false;    // LSLQ
   bool restart = false;             // GMRES, FOM, FGMRES
   bool reorthogonalization = false; // GMRES, FOM, FGMRES
   bool check_curvature = false;     // CG-Lanczos
@@ -171,15 +173,20 @@ struct Stats {
   std::vector<double> residuals, Aresiduals, Acond;
   double allocation_timer = 0, timer = 0;
   double Anorm = NAN;                  // LanczosStats (cg_lanczos!)
+  bool error_with_bnd = false;         // LSLQStats (lslq!)
+  std::vector<double> err_lbnds, err_ubnds_lq, err_ubnds_cg;
   std::string status = "unknown";
-  void reset() { residuals.clear(); Aresiduals.clear(); Acond.clear(); indefinite = false; npcCount = 0; }
+  void reset() {
+    residuals.clear(); Aresiduals.clear(); Acond.clear(); indefinite = false; npcCount = 0;
+    err_lbnds.clear(); err_ubnds_lq.clear(); err_ubnds_cg.clear(); error_with_bnd = false;
+  }
 };
 
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
-                  S_CGS = 11, S_LSQR = 21, S_LSMR = 22, S_CG_LANCZOS = 100 };
+                  S_CGS = 11, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25, S_CG_LANCZOS = 100 };
 // the least-squares solvers: A is m x n, b has m entries and x has n
-inline bool is_ls_kind(int k) { return k == S_LSQR || k == S_LSMR; }
+inline bool is_ls_kind(int k) { return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS; }
 
 // One workspace per (solver, dtype): owns every device vector of the solver
 // (src/krylov_workspaces.jl; SURVEY.md appendix B for fields and aliasing).
@@ -201,6 +208,8 @@ struct Workspace {
   T *Mv = nullptr, *Mv_prev = nullptr, *Mv_next = nullptr;                            // CG-Lanczos (+ p, vv)
   T *Nv = nullptr, *Mu = nullptr, *Av = nullptr, *Atu = nullptr;                     // LSQR / LSMR (+ w, u, v; Mu, Av, u: m)
   T *h = nullptr, *hbar = nullptr;                                                   // LSMR
+  T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
+                                       // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
   std::vector<T*> V;
   std::vector<T*> Z;                   // FGMRES: Z[k] = N_k V[k];  DQGMRES / DIOM: the direction stack P
   std::vector<T> c, sgiv, zg, R;       // GMRES host-side Givens data
@@ -270,6 +279,13 @@ template <class T> void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const Li
                                    const LinOp<T>& N, const SolveOpts& o);
 template <class T> void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const LinOp<T>& N, const SolveOpts& o);
+template <class T> void lslq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                   const LinOp<T>& N, const SolveOpts& o);
+// CGLS / CRLS: M (m x m) acts on the residual space; they take no N.
+template <class T> void cgls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                   const SolveOpts& o);
+template <class T> void crls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                   const SolveOpts& o);
 
 // Fused CG (cg_fused.cu).  Returns false if the configuration is not eligible
 // (caller falls back to the generic primitive path, still on the GPU).
@@ -311,6 +327,18 @@ template <class T> void lsq_fused_bidiag(Workspace<T>& ws, const Csr<T>& A, cons
 // P3.  LSQR: v = Nv / alpha (scale_v), x += sigma w, w = v - tau w.  LSMR (lsmr = true, w = h):
 // v = Nv / alpha (scale_v), hbar = h - delta hbar, x += sigma hbar, h = v - tau h; returns ||x|| (LSMR only).
 template <class T> T lsq_fused_update(Workspace<T>& ws, bool lsmr, bool scale_v, T inv_alpha, T sigma, T tau, T delta);
+// LSLQ's update after P1 / P2 (w = w̄): v = Nv / alpha (scale_v), x += (c zeta) w̄, x += (s zeta) v, w̄ = -c v + s w̄.
+template <class T> void lslq_fused_update(Workspace<T>& ws, bool scale_v, T inv_alpha, T czeta, T szeta, T c, T s);
+// One CGLS iteration, M = I, no trust region, 4 launches: K1 q = A p (alpha on the device), K2 r -= alpha q, K3 s = A^T r
+// with x += alpha p and s -= lambda x, K4 p = s + beta p.  One read-back: <r, r> and gamma = <s, s>.
+// `init`: first iteration, sets gamma (and <p, p> = gamma) on the device from the host.
+template <class T> void cgls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T lambda,
+                                             T* rr, T* gamma_out);
+// One CRLS iteration, M = I, no trust region, 4 launches: L1 x += alpha p, Ar -= alpha q; L2 s = A Ar with r -= alpha Ap
+// (gamma, beta on the device); L3 Ap = s + beta Ap; L4 q = A^T Ap with p = Ar + beta p, q += lambda p (next alpha).
+// One read-back: <Ar, Ar>, <x, x>, <r, r> and gamma.  `init`: first iteration, sets alpha and gamma from the host.
+template <class T> void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, T gamma,
+                                             T lambda, T* ArAr, T* xx, T* rr, T* gamma_out);
 
 double now_seconds();
 

@@ -4,6 +4,10 @@
 // A is a CSR operator, M = N = I and there is no trust region, the fused path runs the same iteration as 3 launches
 // (fused_phases.cu: P1 on A, P2 on A^T, P3 over n) and one read-back (LSMR: two, its tests need ||x|| after P3).  The
 // scalar recurrences, stopping tests and status strings run on the host, unchanged.
+// lslq! (src/lslq.jl:201-520) runs the same Golub-Kahan step (fused: LSQR's P1 / P2 and its own update pass).
+// cgls! (src/cgls.jl:129-243) and crls! (src/crls.jl:120-268) run the normal-equations recurrences on the same operator
+// pair: 8 / 11 launches per iteration on the primitives, 4 fused ones (fused_phases.cu) and one read-back when A is a
+// CSR operator, M = I and there is no trust region.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -26,14 +30,19 @@ template <class T> T err_window_norm(const std::vector<T>& e) {   // knorm(windo
   return std::sqrt(ssq);
 }
 
-// Step to the trust-region boundary along d (lsqr.jl:355-358, lsmr.jl:358-361): returns the clipped sigma.
-template <class T> T clip_to_boundary(Ctx& c, int n, const T* x, const T* d, T* z, T radius, T sigma, bool& on_boundary) {
+// to_boundary(n, x, d, z, radius; dNorm2) with M = I, raising where the reference raises
+template <class T> void boundary_roots(Ctx& c, int n, const T* x, const T* d, T radius, T dNorm2, T* t1, T* t2) {
   LinOp<T> I;
-  T t1, t2;
-  const int e = to_boundary<T>(c, n, x, d, z, radius, T(0), I, false, &t1, &t2);
+  const int e = to_boundary<T>(c, n, x, d, nullptr, radius, dNorm2, I, false, t1, t2);
   if (e == 2) throw std::runtime_error("zero direction");
   if (e == 3) throw std::runtime_error("outside of the trust region");
   if (e) throw std::runtime_error("The quadratic `q` doesn't have real roots.");
+}
+
+// Step to the trust-region boundary along d (lsqr.jl:355-358, lsmr.jl:358-361): returns the clipped sigma.
+template <class T> T clip_to_boundary(Ctx& c, int n, const T* x, const T* d, T radius, T sigma, bool& on_boundary) {
+  T t1, t2;
+  boundary_roots<T>(c, n, x, d, radius, T(0), &t1, &t2);
   const T tmax = std::max(t1, t2), tmin = std::min(t1, t2);
   on_boundary = sigma > tmax || sigma < tmin;
   return sigma > 0 ? std::min(sigma, tmax) : std::max(sigma, tmin);
@@ -249,7 +258,7 @@ void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
     dNorm2 += ww / (rho * rho);
 
     T sigma = phi / rho;
-    if (radius > 0) sigma = clip_to_boundary<T>(c, n, ws.x, ws.w, v, radius, sigma, ex.on_boundary);
+    if (radius > 0) sigma = clip_to_boundary<T>(c, n, ws.x, ws.w, radius, sigma, ex.on_boundary);
 
     if (s.fused) {
       lsq_fused_update<T>(ws, false, scale_v, T(1) / alpha, sigma, theta / rho, T(0));
@@ -415,7 +424,7 @@ void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
       xNorm = lsq_fused_update<T>(ws, true, scale_v, T(1) / alpha, sigma, thetanew / rho, delta);
     } else {
       k_axpby<T>(c, n, T(1), ws.h, -delta, ws.hbar);            // ĥₖ = hₖ - δₖ * ĥₖ₋₁
-      if (radius > 0) sigma = clip_to_boundary<T>(c, n, ws.x, ws.hbar, v, radius, sigma, ex.on_boundary);
+      if (radius > 0) sigma = clip_to_boundary<T>(c, n, ws.x, ws.hbar, radius, sigma, ex.on_boundary);
       k_axpy<T>(c, n, sigma, ws.hbar, ws.x);                    // xₖ = xₖ₋₁ + σₖ * ĥₖ
       k_axpby<T>(c, n, T(1), v, -thetanew / rho, ws.h);         // hₖ₊₁ = vₖ₊₁ - (θₖ₊₁/ρₖ) * hₖ
     }
@@ -480,7 +489,428 @@ void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   run.finish(iter, ex.solved, !ex.zero_resid, ex.status());
 }
 
+// ===========================================================================
+// lslq!  (src/lslq.jl:201-520).  Unlike LSQR, `iter` is incremented at the END of the body, so the forward-error
+// window, the `tired` test and the CG-bound guard see the count from before the increment; λ is overwritten by the
+// regularization rotation while λ² keeps its initial value.
+// ===========================================================================
+template <class T>
+void lslq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("LSLQ: system of %d equations in %d variables\n", m, n);
+  T lambda = (T)o.lambda;
+  const T lambda2 = lambda * lambda;
+  const T sigma = (T)o.sigma;
+  const T conlim = o.conlim < 0 ? T(1) / std::sqrt(eps_of<T>()) : (T)o.conlim;
+  const T ctol = conlim > 0 ? T(1) / conlim : T(0);
+  const T etol = tol_of<T>(o.etol), utol = tol_of<T>(o.utol), btol = tol_of<T>(o.btol);
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  Stats& stats = ws.stats;
+  std::vector<T>& err_vec = ws.err_vec;
+  (void)btol;                                                   // lslq.jl computes `tol` from btol and never reads it
+
+  T beta1;
+  const Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta1);
+  if (beta1 == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    stats.error_with_bnd = false;
+    if (history) { stats.residuals.push_back(0); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  T beta = beta1;
+  lsq_start<T>(ws, s, At, N, ldiv, beta1);
+  T* v = s.NisI ? ws.Nv : ws.v;
+  T alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+  if (alpha == 0) {                                             // Aᴴb = 0: x = 0 is a minimum least-squares solution
+    run.finish(0, true, false, "x is a minimum least-squares solution");
+    stats.error_with_bnd = false;
+    if (history) { stats.residuals.push_back(beta1); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  k_scal<T>(c, n, T(1) / alpha, v);
+  if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+
+  T Anorm2 = alpha * alpha, Anorm = alpha;
+  T sigmax = 0, sigmin = std::numeric_limits<T>::infinity(), Acond = 0;
+  T xlqNorm = 0, xlqNorm2 = 0, xcgNorm2 = 0;
+  k_copy<T>(c, n, ws.w, v);                                     // w̄₁ = v₁
+  T err_lbnd = 0;
+  const int window = (int)err_vec.size();
+  std::fill(err_vec.begin(), err_vec.end(), T(0));
+  bool complex_error_bnd = false;
+
+  T alphaL = alpha, betaL = beta, rhobar = -sigma, gammabar = alpha, psi = beta1;
+  T cc = -1, ss = 0, delta = -1, tau = alpha * beta1, zeta = 0, zetabar = 0, zetatilde = 0, csig = -1;
+  T rNorm = beta1;
+  if (history) stats.residuals.push_back(rNorm);
+  T ArNorm = alpha * beta;
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+  if (o.verbose > 0) {
+    printf("%5s  %7s  %7s  %7s  %7s  %8s  %8s  %7s  %7s  %7s  %5s\n", "k", "‖r‖", "‖Aᴴr‖", "β", "α", "cos", "sin", "‖A‖²", "κ(A)",
+           "‖xL‖", "timer");
+    printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm,
+           (double)beta, (double)alpha, (double)cc, (double)ss, (double)Anorm2, (double)Acond, (double)xlqNorm, run.elapsed());
+  }
+
+  const T eps = atol + rtol * beta1;
+  bool solved = rNorm <= eps, tired = iter >= itmax, ill_cond = false, ill_cond_mach = false, ill_cond_lim = false;
+  bool zero_resid = false, fwd_err_lbnd = false, fwd_err_ubnd = false, user_exit = false, overtimed = false;
+
+  while (!(solved || tired || ill_cond || user_exit || overtimed)) {
+    // Golub-Kahan step: βₖ₊₁Muₖ₊₁ = Avₖ - αₖMuₖ, αₖ₊₁Nvₖ₊₁ = Aᴴuₖ₊₁ - βₖ₊₁Nvₖ
+    bool scale_v = false;
+    if (s.fused) {                                              // P1 + P2 and one read-back; v /= alpha is applied below
+      T alpha_new, unused;
+      lsq_fused_bidiag<T>(ws, *A.csr, *At.csr, iter == 0, alpha, false, &beta, &alpha_new, &unused);
+      if (beta != 0) { alpha = alpha_new; scale_v = alpha != 0; }
+    } else {
+      beta = lsq_bidiag_step<T>(ws, s, A, At, M, N, ldiv, alpha, [](T) {});
+    }
+    if (beta != 0) {
+      alphaL = alpha;                                           // rotate out the regularization term if present
+      betaL = beta;
+      if (lambda != 0) {
+        T cL, sL;
+        sym_givens<T>(beta, lambda, &cL, &sL, &betaL);
+        alphaL = cL * alpha;
+        lambda = std::sqrt(lambda2 + (sL * alpha) * (sL * alpha));   // the rotation updates the next λ
+      }
+      Anorm2 = Anorm2 + alphaL * alphaL + betaL * betaL;      // = ‖Lₖ‖²
+      Anorm = std::sqrt(Anorm2);
+    }
+
+    // Continue the QR factorization of Bₖ
+    T cp, sp, gamma;
+    sym_givens<T>(gammabar, betaL, &cp, &sp, &gamma);
+    tau = -tau * delta / gamma;
+    delta = sp * alphaL;
+    gammabar = -cp * alphaL;
+
+    T omega = 0;
+    if (sigma > 0 && !complex_error_bnd) {                      // QR factorization for the error estimate
+      T mubar = -csig * gamma, ssig, rho;
+      sym_givens<T>(rhobar, gamma, &csig, &ssig, &rho);
+      rhobar = ssig * mubar + csig * sigma;
+      mubar = -csig * delta;
+      const T h = delta * csig / rhobar;                        // eigenvector component and Gauss-Radau parameter
+      const T disc = sigma * (sigma - delta * h);
+      if (disc < 0) complex_error_bnd = true; else omega = std::sqrt(disc);
+      sym_givens<T>(rhobar, delta, &csig, &ssig, &rho);
+      rhobar = ssig * mubar + csig * sigma;
+    }
+
+    // Continue the LQ factorization of Rₖ
+    const T epsbar = -gamma * cc;
+    const T eta = gamma * ss;
+    T epsl;
+    sym_givens<T>(epsbar, delta, &cc, &ss, &epsl);
+    sigmax = std::max(sigmax, std::max(epsl, std::fabs(epsbar)));
+    sigmin = std::min(sigmin, std::min(epsl, std::fabs(epsbar)));
+    Acond = sigmax / sigmin;
+
+    const T zetaold = zeta;
+    zeta = (tau - zeta * eta) / epsl;
+    zetabar = zeta / cc;
+
+    const T ra = psi * cp - zetaold * eta, rb = psi * sp;
+    rNorm = std::sqrt(ra * ra + rb * rb);
+    if (history) stats.residuals.push_back(rNorm);
+    const T aa = gamma * epsl * zeta, ab = delta * eta * zetaold;
+    ArNorm = std::sqrt(aa * aa + ab * ab);
+    if (history) stats.Aresiduals.push_back(ArNorm);
+    psi = psi * sp;
+    xcgNorm2 = xlqNorm2 + zetabar * zetabar;
+
+    if (sigma > 0 && iter > 0 && !complex_error_bnd) {
+      const T disc = zetatilde * zetatilde - zetabar * zetabar;
+      if (disc < 0) {
+        complex_error_bnd = true;
+      } else {
+        const T err_ubnd_cg = std::sqrt(disc);
+        if (history) stats.err_ubnds_cg.push_back(err_ubnd_cg);
+        fwd_err_ubnd = err_ubnd_cg <= utol * std::sqrt(xcgNorm2);
+      }
+    }
+
+    const T test1 = rNorm;
+    const T test2 = ArNorm / (Anorm * rNorm);
+    const T test3 = T(1) / Acond;
+    const T t1 = test1 / (T(1) + Anorm * xlqNorm);
+
+    // update the LSLQ point and w̄
+    if (s.fused) {
+      lslq_fused_update<T>(ws, scale_v, T(1) / alpha, cc * zeta, ss * zeta, cc, ss);
+    } else {
+      k_axpy<T>(c, n, cc * zeta, ws.w, ws.x);
+      k_axpy<T>(c, n, ss * zeta, v, ws.x);
+      k_axpby<T>(c, n, -cc, v, ss, ws.w);
+    }
+    xlqNorm2 += zeta * zeta;
+    xlqNorm = std::sqrt(xlqNorm2);
+
+    err_vec[iter % window] = zeta;                              // iter: the count before this iteration
+    if (iter >= window) {
+      err_lbnd = err_window_norm(err_vec);
+      if (history) stats.err_lbnds.push_back(err_lbnd);
+      fwd_err_lbnd = err_lbnd <= etol * xlqNorm;
+    }
+
+    if (sigma > 0 && !complex_error_bnd) {                      // LQ forward-error upper bound
+      const T etatilde = omega * ss;
+      const T epstilde = -omega * cc;
+      const T tautilde = -tau * delta / omega;
+      zetatilde = (tautilde - zeta * etatilde) / epstilde;
+      if (history) stats.err_ubnds_lq.push_back(std::fabs(zetatilde));
+    }
+
+    ill_cond_mach = (T(1) + test3 <= T(1));
+    const bool solved_mach = (T(1) + test2 <= T(1));
+    const bool zero_resid_mach = (T(1) + t1 <= T(1));
+    run.poll(iter + 1, user_exit, overtimed);                    // callback, then the clock
+    tired = iter >= itmax;
+    ill_cond_lim = (test3 <= ctol);
+    const bool solved_lim = (test2 <= atol);                    // atol, as lslq.jl has it
+    const bool zero_resid_lim = (test1 <= eps);
+    ill_cond = ill_cond_mach || ill_cond_lim;
+    zero_resid = zero_resid_mach || zero_resid_lim;
+    solved = solved_mach || solved_lim || zero_resid || fwd_err_lbnd || fwd_err_ubnd;
+    iter = iter + 1;
+    if (kdisplay(iter, o.verbose))
+      printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm,
+             (double)beta, (double)alpha, (double)cc, (double)ss, (double)Anorm, (double)Acond, (double)xlqNorm, run.elapsed());
+  }
+  if (o.verbose > 0) printf("\n");
+  if (o.transfer_to_lsqr) k_axpy<T>(c, n, zetabar, ws.w, ws.x);   // the LSQR point
+
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (ill_cond_mach) st = "condition number seems too large for this machine";
+  if (ill_cond_lim) st = "condition number exceeds tolerance";
+  if (solved) st = "found approximate minimum least-squares solution";
+  if (zero_resid) st = "found approximate zero-residual solution";
+  if (fwd_err_lbnd) st = "forward error lower bound small enough";
+  if (fwd_err_ubnd) st = "forward error upper bound small enough";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  stats.error_with_bnd = complex_error_bnd;
+  run.finish(iter, solved, !zero_resid, st);
+}
+
+// ===========================================================================
+// cgls!  (src/cgls.jl:129-243).  M acts on the m-dimensional residual space; Mq aliases the Mr buffer when M != I.
+// ===========================================================================
+template <class T>
+void cgls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CGLS: system of %d equations in %d variables\n", m, n);
+  const bool MisI = M.is_identity();
+  const T lambda = (T)o.lambda, radius = (T)o.radius;
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  const bool fused = o.fused && A.kind == LinOp<T>::CSR && At.kind == LinOp<T>::CSR && MisI && !(radius > 0);
+  Stats& stats = ws.stats;
+  allocate_if(!MisI, ws, ws.Mr, m);
+  stats.reset();
+  T* Mr = MisI ? ws.r : ws.Mr;
+  T* Mq = MisI ? ws.q : ws.Mr;
+
+  k_fill<T>(c, n, ws.x, T(0));
+  k_copy<T>(c, m, ws.r, b);
+  const T bNorm = k_nrm2<T>(c, m, ws.r);
+  if (bNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    if (history) { stats.residuals.push_back(0); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  if (!MisI) op_apply(c, M, ws.r, Mr, ldiv);
+  op_apply(c, At, Mr, ws.s);
+  k_copy<T>(c, n, ws.p, ws.s);
+  T gamma = k_dot<T>(c, n, ws.s, ws.s);
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+
+  T rNorm = bNorm, ArNorm = std::sqrt(gamma);
+  if (history) { stats.residuals.push_back(rNorm); stats.Aresiduals.push_back(ArNorm); }
+  const T eps = atol + rtol * ArNorm;
+  if (o.verbose > 0) printf("%5s  %8s  %8s  %5s\n", "k", "‖Aᴴr‖", "‖r‖", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %8.2e  %.2fs\n", iter, (double)ArNorm, (double)rNorm, run.elapsed());
+
+  bool on_boundary = false, solved = ArNorm <= eps, tired = iter >= itmax, user_exit = false, overtimed = false;
+  while (!(solved || tired || user_exit || overtimed)) {
+    if (fused) {
+      T rr;
+      cgls_fused_iteration<T>(ws, *A.csr, *At.csr, iter == 0, gamma, lambda, &rr, &gamma);
+      rNorm = std::sqrt(rr);
+    } else {
+      op_apply(c, A, ws.p, ws.q);
+      if (!MisI) op_apply(c, M, ws.q, Mq, ldiv);
+      T delta = k_dot<T>(c, m, ws.q, Mq);                       // δ = qᴴMq
+      if (lambda > 0) delta += lambda * k_dot<T>(c, n, ws.p, ws.p);
+      T alpha = gamma / delta;
+      if (radius > 0) {                                         // step to the boundary (in the Euclidean norm)
+        T t1, t2;
+        boundary_roots<T>(c, n, ws.x, ws.p, radius, T(0), &t1, &t2);
+        const T sigma = std::max(t1, t2);
+        if (alpha > sigma) { alpha = sigma; on_boundary = true; }
+      }
+      k_axpy<T>(c, n, alpha, ws.p, ws.x);
+      k_axpy<T>(c, m, -alpha, ws.q, ws.r);
+      if (!MisI) op_apply(c, M, ws.r, Mr, ldiv);
+      op_apply(c, At, Mr, ws.s);
+      if (lambda > 0) k_axpy<T>(c, n, -lambda, ws.x, ws.s);    // s = Aᴴr - λx, with the updated x
+      const T gamma_next = k_dot<T>(c, n, ws.s, ws.s);
+      const T beta = gamma_next / gamma;
+      k_axpby<T>(c, n, T(1), ws.s, beta, ws.p);
+      gamma = gamma_next;
+      rNorm = k_nrm2<T>(c, m, ws.r);
+    }
+    ArNorm = std::sqrt(gamma);
+    if (history) { stats.residuals.push_back(rNorm); stats.Aresiduals.push_back(ArNorm); }
+    iter = iter + 1;
+    if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %8.2e  %.2fs\n", iter, (double)ArNorm, (double)rNorm, run.elapsed());
+    run.poll(iter, user_exit, overtimed);
+    solved = (ArNorm <= eps) || on_boundary;
+    tired = iter >= itmax;
+  }
+  if (o.verbose > 0) printf("\n");
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (solved) st = "solution good enough given atol and rtol";
+  if (on_boundary) st = "on trust-region boundary";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  run.finish(iter, solved, false, st);
+}
+
+// ===========================================================================
+// crls!  (src/crls.jl:120-268).  M acts on the m-dimensional residual space: Ms, Mr and MAp share one buffer.
+// ===========================================================================
+template <class T>
+void crls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CRLS: system of %d equations in %d variables\n", m, n);
+  const bool MisI = M.is_identity();
+  const T lambda = (T)o.lambda, radius = (T)o.radius;
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  const bool fused = o.fused && A.kind == LinOp<T>::CSR && At.kind == LinOp<T>::CSR && MisI && !(radius > 0);
+  Stats& stats = ws.stats;
+  allocate_if(!MisI, ws, ws.Mr, m);
+  stats.reset();
+  T* Ms = MisI ? ws.s : ws.Mr;
+  T* Mr = MisI ? ws.r : ws.Mr;
+  T* MAp = MisI ? ws.Ap : ws.Mr;
+
+  k_fill<T>(c, n, ws.x, T(0));
+  k_copy<T>(c, m, ws.r, b);
+  const T bNorm = k_nrm2<T>(c, m, ws.r);
+  T rNorm = bNorm;
+  if (history) stats.residuals.push_back(rNorm);
+  if (bNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    if (history) stats.Aresiduals.push_back(0);
+    return;
+  }
+  if (!MisI) op_apply(c, M, ws.r, Mr, ldiv);
+  op_apply(c, At, Mr, ws.Ar);
+  op_apply(c, A, ws.Ar, ws.s);
+  if (!MisI) op_apply(c, M, ws.s, Ms, ldiv);
+  k_copy<T>(c, n, ws.p, ws.Ar);
+  k_copy<T>(c, m, ws.Ap, ws.s);
+  op_apply(c, At, Ms, ws.q);
+  if (lambda > 0) k_axpy<T>(c, n, lambda, ws.p, ws.q);        // q = q + λ p
+  T gamma = k_dot<T>(c, m, ws.s, Ms);
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+
+  T ArNorm = k_nrm2<T>(c, n, ws.Ar);
+  if (lambda > 0) gamma += lambda * ArNorm * ArNorm;
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  const T eps = atol + rtol * ArNorm;
+  if (o.verbose > 0) printf("%5s  %8s  %8s  %5s\n", "k", "‖Aᴴr‖", "‖r‖", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %8.2e  %.2fs\n", iter, (double)ArNorm, (double)rNorm, run.elapsed());
+
+  bool on_boundary = false, solved = ArNorm <= eps, tired = iter >= itmax, psd = false, user_exit = false, overtimed = false;
+  T* p = ws.p;                                                  // rebound to Ar by the zero-curvature branch
+  while (!(solved || tired || user_exit || overtimed)) {
+    if (fused) {
+      T ArAr, xx, rr;
+      const T alpha0 = iter == 0 ? gamma / k_dot<T>(c, n, ws.q, ws.q) : T(0);   // later alphas stay on the device
+      crls_fused_iteration<T>(ws, *A.csr, *At.csr, iter == 0, alpha0, gamma, lambda, &ArAr, &xx, &rr, &gamma);
+      ArNorm = std::sqrt(ArAr);
+      rNorm = lambda > 0 ? std::sqrt(rr + lambda * xx) : std::sqrt(rr);
+    } else {
+      const T qNorm2 = k_dot<T>(c, n, ws.q, ws.q);
+      T alpha = gamma / qNorm2;
+      if (radius > 0) {                                         // α > 0 in CRLS
+        const T pNorm = k_nrm2<T>(c, n, p);
+        T t1, t2;
+        if (k_dot<T>(c, m, ws.Ap, ws.Ap) <= eps * std::sqrt(qNorm2) * pNorm) {   // the quadratic is constant along p
+          psd = true;
+          p = ws.Ar;                                            // p = Aᴴr
+          const T pNorm2 = ArNorm * ArNorm;
+          op_apply(c, At, ws.s, ws.q);
+          boundary_roots<T>(c, n, ws.x, p, radius, pNorm2, &t1, &t2);
+          alpha = std::min(ArNorm * ArNorm / gamma, std::max(t1, t2));
+        } else {
+          const T pNorm2 = pNorm * pNorm;
+          boundary_roots<T>(c, n, ws.x, p, radius, pNorm2, &t1, &t2);
+          const T sigma = std::max(t1, t2);
+          if (alpha >= sigma) { alpha = sigma; on_boundary = true; }
+        }
+      }
+      k_axpy<T>(c, n, alpha, p, ws.x);
+      k_axpy<T>(c, n, -alpha, ws.q, ws.Ar);
+      ArNorm = k_nrm2<T>(c, n, ws.Ar);
+      solved = psd || on_boundary;
+      if (solved) continue;                                     // leaves the loop: no iteration count, history or callback
+      k_axpy<T>(c, m, -alpha, ws.Ap, ws.r);
+      op_apply(c, A, ws.Ar, ws.s);
+      if (!MisI) op_apply(c, M, ws.s, Ms, ldiv);
+      T gamma_next = k_dot<T>(c, m, ws.s, Ms);
+      if (lambda > 0) gamma_next += lambda * ArNorm * ArNorm;
+      const T beta = gamma_next / gamma;
+      k_axpby<T>(c, n, T(1), ws.Ar, beta, p);
+      k_axpby<T>(c, m, T(1), ws.s, beta, ws.Ap);
+      if (!MisI) op_apply(c, M, ws.Ap, MAp, ldiv);
+      op_apply(c, At, MAp, ws.q);
+      if (lambda > 0) k_axpy<T>(c, n, lambda, p, ws.q);
+      gamma = gamma_next;
+      rNorm = lambda > 0 ? std::sqrt(k_dot<T>(c, m, ws.r, ws.r) + lambda * k_dot<T>(c, n, ws.x, ws.x)) : k_nrm2<T>(c, m, ws.r);
+    }
+    if (history) { stats.residuals.push_back(rNorm); stats.Aresiduals.push_back(ArNorm); }
+    iter = iter + 1;
+    if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %8.2e  %.2fs\n", iter, (double)ArNorm, (double)rNorm, run.elapsed());
+    run.poll(iter, user_exit, overtimed);
+    solved = (ArNorm <= eps) || on_boundary;
+    tired = iter >= itmax;
+  }
+  if (o.verbose > 0) printf("\n");
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (solved) st = "solution good enough given atol and rtol";
+  if (psd) st = "zero-curvature encountered";
+  if (on_boundary) st = "on trust-region boundary";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  run.finish(iter, solved, false, st);
+}
+
 #define INST(T)                                                                                                         \
+  template void lslq_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
+                              const SolveOpts&);                                                                        \
+  template void cgls_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&); \
+  template void crls_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&); \
   template void lsqr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
                               const SolveOpts&);                                                                        \
   template void lsmr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \

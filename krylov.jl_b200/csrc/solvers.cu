@@ -62,11 +62,18 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         break;
       }
       case S_CG_LANCZOS: ws->Mv = A(); ws->Mv_prev = A(); ws->p = A(); ws->Mv_next = A(); break;    // CgLanczosWorkspace :575-591
-      case S_LSQR: case S_LSMR:                     // LsqrWorkspace / LsmrWorkspace: Av, Aᴴu, u, v are allocated by the solve
+      case S_LSQR: case S_LSMR: case S_LSLQ:        // Lsqr / Lsmr / LslqWorkspace: Av, Aᴴu, u, v are allocated by the solve
         ws->Nv = A(); ws->Mu = dev_alloc<T>((size_t)m);
-        if (kind == S_LSQR) ws->w = A(); else { ws->h = A(); ws->hbar = A(); }
+        if (kind != S_LSMR) ws->w = A(); else { ws->h = A(); ws->hbar = A(); }     // LSLQ: w̄ in w
         ws->window = window > 0 ? window : 5;
         ws->err_vec.assign(ws->window, T(0));
+        break;
+      case S_CGLS:                                  // CglsWorkspace :1916-1944 (Mr is allocated by the solve)
+        ws->p = A(); ws->s = A(); ws->r = dev_alloc<T>((size_t)m); ws->q = dev_alloc<T>((size_t)m);
+        break;
+      case S_CRLS:                                  // CrlsWorkspace :2100-2131 (Ms is allocated by the solve)
+        ws->p = A(); ws->Ar = A(); ws->q = A();
+        ws->r = dev_alloc<T>((size_t)m); ws->Ap = dev_alloc<T>((size_t)m); ws->s = dev_alloc<T>((size_t)m);
         break;
       default: throw std::runtime_error("unsupported solver");
     }
@@ -83,7 +90,8 @@ template <class T> void ws_destroy(Workspace<T>* ws) {
   if (ws->ctx.stream) cudaStreamSynchronize(ws->ctx.stream);
   T* vecs[] = {ws->x, ws->dx, ws->r, ws->p, ws->Ap, ws->z, ws->npc_dir, ws->p2, ws->v, ws->s, ws->qd, ws->t, ws->yz,
                ws->r1, ws->r2, ws->w1, ws->w2, ws->y, ws->vv, ws->w, ws->q, ws->pp, ws->bbuf, ws->cbuf,
-               ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next, ws->Nv, ws->Mu, ws->Av, ws->Atu, ws->h, ws->hbar};
+               ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next, ws->Nv, ws->Mu, ws->Av, ws->Atu, ws->h, ws->hbar,
+               ws->Ar, ws->Mr};
   for (T* p : vecs) dev_free(p);
   for (T* p : ws->V) dev_free(p);
   for (T* p : ws->Z) dev_free(p);

@@ -195,7 +195,8 @@ end
 # created ONCE per Krylov.jl workspace and kept in HANDLES, so an in-place solve allocates nothing
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
-                       :bicgstab => 10, :cgs => 11, :lsqr => 21, :lsmr => 22, :cg_lanczos => 100)
+                       :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25,
+                       :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -203,12 +204,13 @@ end
 struct CExt    # KrylovB200Options (include/krylov_b200.h)
   history::Cint; ldiv::Cint; etol::Cdouble; conlim::Cdouble; fused::Cint; batch::Cint
   callback::Ptr{Cvoid}; callback_user::Ptr{Cvoid}; time_kernels::Cint; check_curvature::Cint; cr_gamma::Cdouble
-  axtol::Cdouble; btol::Cdouble
+  axtol::Cdouble; btol::Cdouble; sigma::Cdouble; utol::Cdouble; transfer_to_lsqr::Cint
 end
 struct CStats  # KrylovB200Stats (include/krylov_b200.h)
   niter::Cint; solved::Cint; inconsistent::Cint; indefinite::Cint; npcCount::Cint
   nresiduals::Cint; nAresiduals::Cint; nAcond::Cint
   allocation_timer::Cdouble; timer::Cdouble; status::NTuple{96,UInt8}; Anorm::Cdouble
+  error_with_bnd::Cint; nerr_lbnds::Cint; nerr_ubnds_lq::Cint; nerr_ubnds_cg::Cint
 end
 
 mutable struct Handle
@@ -269,9 +271,11 @@ function fill_stats!(ws, h::Handle, ::Type{T}) where T
   hasproperty(st, :indefinite) && (st.indefinite = s.indefinite != 0)
   hasproperty(st, :npcCount) && (st.npcCount = s.npcCount)
   hasproperty(st, :Anorm) && (st.Anorm = T(s.Anorm))            # LanczosStats (cg_lanczos!)
+  hasproperty(st, :error_with_bnd) && (st.error_with_bnd = s.error_with_bnd != 0)   # LSLQStats (lslq!)
   bytes = collect(s.status); z = findfirst(==(0x00), bytes)
   st.status = String(bytes[1:(z === nothing ? length(bytes) : z - 1)])
-  for (which, field, cnt) in ((0, :residuals, s.nresiduals), (1, :Aresiduals, s.nAresiduals), (2, :Acond, s.nAcond))
+  for (which, field, cnt) in ((0, :residuals, s.nresiduals), (1, :Aresiduals, s.nAresiduals), (2, :Acond, s.nAcond),
+                              (3, :err_lbnds, s.nerr_lbnds), (4, :err_ubnds_lq, s.nerr_ubnds_lq), (5, :err_ubnds_cg, s.nerr_ubnds_cg))
     hasproperty(st, field) || continue
     buf = Vector{Cdouble}(undef, cnt)
     got = cnt == 0 ? 0 : ccall((:krylov_b200_get_history, lib), Cint, (Ptr{Cvoid}, Cint, Ptr{Cdouble}, Cint), h.ptr, which, buf, cnt)
@@ -296,7 +300,7 @@ function fused_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; c::Un
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, NaN, NaN))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, NaN, NaN, 0.0, NaN, 0))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, restart, reorthogonalization, linesearch))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -357,7 +361,7 @@ function ls_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, axtol, btol))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, axtol, btol, 0.0, NaN, 0))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, 0, 0, 0))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -374,6 +378,70 @@ Krylov.lsqr!(ws::Krylov.LsqrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200C
   ls_solve!(:lsqr, ws, A, b; kw...)
 Krylov.lsmr!(ws::Krylov.LsmrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
   ls_solve!(:lsmr, ws, A, b; kw...)
+
+# ---- lslq! (src/lslq.jl:178-196) on a rectangular B200CSR: one krylov_solve per solve ----
+# Its own kwargs and defaults (atol = rtol = √eps(T), σ, utol, transfer_to_lsqr, no radius); B200Diagonal M (m entries)
+# and N (n entries).  The fused Golub-Kahan passes run when M = N = I.
+function lslq_solve!(ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N = I, ldiv::Bool = false, transfer_to_lsqr::Bool = false,
+                     sqd::Bool = false, λ::T = zero(T), σ::T = zero(T), etol::T = √eps(T), utol::T = √eps(T),
+                     btol::T = √eps(T), conlim::T = 1/√eps(T), atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0,
+                     timemax::Float64 = Inf, verbose::Int = 0, history::Bool = false, callback = workspace -> false,
+                     iostream::IO = stdout) where T
+  length(b) == A.m || error("Inconsistent problem size")
+  sqd && (λ ≠ 0) && error("sqd cannot be set to true if λ ≠ 0 !")
+  sqd && (λ = one(T))
+  h = handle_for(:lslq, ws, A, 0, length(ws.err_vec))
+  set_precond!(h, 0, M)
+  set_precond!(h, 1, N)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, btol, σ, utol,
+                 transfer_to_lsqr))
+  o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, 0, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, C_NULL, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.lslq!(ws::Krylov.LslqWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  lslq_solve!(ws, A, b; kw...)
+
+# ---- cgls! / crls! (src/cgls.jl:110-121, src/crls.jl:101-112) on a rectangular B200CSR: one krylov_solve per solve ----
+# Their own kwargs and defaults (atol = rtol = √eps(T)); M acts on the m-dimensional residual space (a B200Diagonal of
+# m entries) and there is no N.  The fused passes run when M = I and radius = 0.
+function normal_ls_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; M = I, ldiv::Bool = false,
+                          radius::T = zero(T), λ::T = zero(T), atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0,
+                          timemax::Float64 = Inf, verbose::Int = 0, history::Bool = false, callback = workspace -> false,
+                          iostream::IO = stdout) where T
+  length(b) == A.m || error("Inconsistent problem size")
+  h = handle_for(method, ws, A, 0, 0)
+  set_precond!(h, 0, M)
+  set_precond!(h, 1, I)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0))
+  o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, C_NULL, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.cgls!(ws::Krylov.CglsWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  normal_ls_solve!(:cgls, ws, A, b; kw...)
+Krylov.crls!(ws::Krylov.CrlsWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  normal_ls_solve!(:crls, ws, A, b; kw...)
 
 # ---- block_gmres! (src/block_gmres.jl:78-110; C ABI krylov.h:250-285): one krylov_block_solve per solve ------------------
 # B, X, X0 are column-major n x p device matrices; the library keeps row-major panels internally and runs the
@@ -409,7 +477,7 @@ function Krylov.block_gmres!(ws::Krylov.BlockGmresWorkspace{T,T,B200Vector{T},B2
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0))
   o = Ref(COpts(atol, rtol, itmax, verbose, 0.0, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, restart, reorthogonalization, false))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))

@@ -37,7 +37,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "FomWorkspace", "FgmresWorkspace", "CgsWorkspace", "CgLanczosWorkspace", "fom", "fom_", "fgmres", "fgmres_",
            "cgs", "cgs_", "cg_lanczos", "cg_lanczos_", "CrWorkspace", "DiomWorkspace", "DqgmresWorkspace", "cr", "cr_", "diom",
            "diom_", "dqgmres", "dqgmres_", "BlockGmresWorkspace", "block_gmres", "block_gmres_", "CsrOperator",
-           "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_"]
+           "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_",
+           "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_"]
 
 
 class B200Error(RuntimeError):
@@ -479,6 +480,9 @@ class KrylovWorkspace:
                           hist(0, s.nresiduals), hist(1, s.nAresiduals), hist(2, s.nAcond), s.allocation_timer, s.timer,
                           s.status.decode("utf-8"))
         out.Anorm = s.Anorm          # LanczosStats.Anorm (cg_lanczos!), NaN otherwise
+        if self.solver == "lslq":    # LSLQStats (src/krylov_stats.jl:352-365)
+            out.err_lbnds, out.err_ubnds_lq = hist(3, s.nerr_lbnds), hist(4, s.nerr_ubnds_lq)
+            out.err_ubnds_cg, out.error_with_bnd = hist(5, s.nerr_ubnds_cg), bool(s.error_with_bnd)
         return out
 
     @property
@@ -740,7 +744,6 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
             raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
         if sqd:
             lambda_ = 1.0
-        m, n = self.m, self.n
         o = lib().krylov_default_options()
         o.atol, o.rtol = float(atol), float(rtol)
         o.itmax, o.verbose = int(itmax), int(verbose)
@@ -751,6 +754,11 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
         for name, val in (("etol", etol), ("axtol", axtol), ("btol", btol), ("conlim", conlim)):
             if val is not None:
                 setattr(e, name, float(val))
+        return self._run(A, b, M, N, o, e, callback)
+
+    def _run(self, A, b, M, N, o, e, callback):
+        """Set the options, the operator pair and the preconditioners, stage b and call krylov_solve."""
+        m, n = self.m, self.n
         keep = []
         if callback is not None:
             wsref = self
@@ -783,7 +791,7 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
                 self._set_diag(which, None)
             else:
                 if P is not None and getattr(P, "ndim", 1) != 1:
-                    raise B200Error("LSQR / LSMR take diagonal preconditioners (1-D arrays) or host callables")
+                    raise B200Error(f"{self.solver} takes diagonal preconditioners (1-D arrays) or host callables")
                 self._set_diag(which, P)
         if not _is_torch(b):
             b = np.ascontiguousarray(b, dtype=self.dtype)
@@ -812,6 +820,72 @@ class LsmrWorkspace(_LeastSquaresWorkspace):
     solver = "lsmr"
 
 
+class LslqWorkspace(_LeastSquaresWorkspace):
+    """Workspace of lslq! on an m x n operator (src/krylov_workspaces.jl LslqWorkspace): b has m entries, x has n;
+    `window` (default 5) sizes the forward-error window."""
+    solver = "lslq"
+
+    def solve(self, A, b, *, M=None, N=None, ldiv=False, transfer_to_lsqr=False, sqd=False, lambda_=0.0, sigma=0.0,
+              etol=None, utol=None, btol=None, conlim=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
+              history=False, callback=None, fused=True, **unknown):
+        """lslq!(ws, A, b; kwargs...)  -- kwargs as in lslq.jl:178-196: etol, utol, btol, atol and rtol default to
+        sqrt(eps), conlim to 1/sqrt(eps); σ (`sigma`) > 0 turns on the Gauss-Radau error bounds.  M (m entries) and N
+        (n entries): None, the diagonal of a Diagonal preconditioner, or a host callable."""
+        if unknown:
+            raise B200Error(f"lslq!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        if sqd and lambda_ != 0:
+            raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
+        if sqd:
+            lambda_ = 1.0
+        o = lib().krylov_default_options()
+        if atol is not None:
+            o.atol = float(atol)
+        if rtol is not None:
+            o.rtol = float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        o.lambda_ = float(lambda_)
+        e = lib().krylov_b200_default_options()
+        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        e.sigma, e.transfer_to_lsqr = float(sigma), int(transfer_to_lsqr)
+        for name, val in (("etol", etol), ("utol", utol), ("btol", btol), ("conlim", conlim)):
+            if val is not None:
+                setattr(e, name, float(val))
+        return self._run(A, b, M, N, o, e, callback)
+
+
+class _NormalEquationsWorkspace(_LeastSquaresWorkspace):
+    """Workspace of cgls! / crls! on an m x n operator (src/krylov_workspaces.jl CglsWorkspace / CrlsWorkspace):
+    b has m entries, x has n."""
+
+    def solve(self, A, b, *, M=None, ldiv=False, radius=0.0, lambda_=0.0, atol=None, rtol=None, itmax=0,
+              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
+        """cgls!(ws, A, b; kwargs...) / crls!(ws, A, b; kwargs...)  -- kwargs as in cgls.jl:110-121 and
+        crls.jl:101-112: atol and rtol default to sqrt(eps), itmax = 0 means m + n.  M (m entries) acts on the residual
+        space: None, the diagonal of a Diagonal preconditioner, or a host callable.  There is no N."""
+        if unknown:
+            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        o = lib().krylov_default_options()
+        if atol is not None:
+            o.atol = float(atol)
+        if rtol is not None:
+            o.rtol = float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        o.radius, o.lambda_ = float(radius), float(lambda_)
+        e = lib().krylov_b200_default_options()
+        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        return self._run(A, b, M, None, o, e, callback)
+
+
+class CglsWorkspace(_NormalEquationsWorkspace):
+    solver = "cgls"
+
+
+class CrlsWorkspace(_NormalEquationsWorkspace):
+    solver = "crls"
+
+
 def _make_least_squares(name):
     def f(A, b, *, n=None, window=0, **kw):
         m = b.shape[0]
@@ -836,7 +910,8 @@ def _make_least_squares(name):
 _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "bicgstab": BicgstabWorkspace,
        "fom": FomWorkspace, "fgmres": FgmresWorkspace, "cgs": CgsWorkspace, "cg_lanczos": CgLanczosWorkspace,
        "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
-       "lsmr": LsmrWorkspace}
+       "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
+       "lslq": LslqWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -888,6 +963,8 @@ cr_, diom_, dqgmres_ = (_make_inplace(s) for s in ("cr", "diom", "dqgmres"))
 cr, diom, dqgmres = (_make_outofplace(s) for s in ("cr", "diom", "dqgmres"))
 lsqr_, lsmr_ = (_make_inplace(s) for s in ("lsqr", "lsmr"))
 lsqr, lsmr = (_make_least_squares(s) for s in ("lsqr", "lsmr"))
+cgls_, crls_, lslq_ = (_make_inplace(s) for s in ("cgls", "crls", "lslq"))
+cgls, crls, lslq = (_make_least_squares(s) for s in ("cgls", "crls", "lslq"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):

@@ -19,8 +19,8 @@ KRYLOV_CPU, KRYLOV_CUDA = 0, 1
 KRYLOV_CG, KRYLOV_MINRES, KRYLOV_GMRES, KRYLOV_BICGSTAB = 0, 3, 8, 10
 KRYLOV_FOM, KRYLOV_FGMRES, KRYLOV_CGS, KRYLOV_B200_CG_LANCZOS = 7, 9, 11, 100
 KRYLOV_CR, KRYLOV_DIOM, KRYLOV_DQGMRES = 1, 5, 6
-KRYLOV_LSQR, KRYLOV_LSMR = 21, 22
-SOLVER_IDS = {"lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
+KRYLOV_LSLQ, KRYLOV_LSQR, KRYLOV_LSMR, KRYLOV_CGLS, KRYLOV_CRLS = 20, 21, 22, 24, 25
+SOLVER_IDS = {"lslq": KRYLOV_LSLQ, "lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cgls": KRYLOV_CGLS, "crls": KRYLOV_CRLS, "cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
               "fom": KRYLOV_FOM, "fgmres": KRYLOV_FGMRES, "cgs": KRYLOV_CGS, "cg_lanczos": KRYLOV_B200_CG_LANCZOS,
               "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES}
 
@@ -44,14 +44,16 @@ class KrylovB200Options(C.Structure):
     _fields_ = [("history", C.c_int), ("ldiv", C.c_int), ("etol", C.c_double), ("conlim", C.c_double),
                 ("fused", C.c_int), ("batch", C.c_int), ("callback", CALLBACK), ("callback_user", C.c_void_p),
                 ("time_kernels", C.c_int), ("check_curvature", C.c_int), ("cr_gamma", C.c_double),
-                ("axtol", C.c_double), ("btol", C.c_double)]
+                ("axtol", C.c_double), ("btol", C.c_double), ("sigma", C.c_double), ("utol", C.c_double),
+                ("transfer_to_lsqr", C.c_int)]
 
 
 class KrylovB200Stats(C.Structure):
     _fields_ = [("niter", C.c_int), ("solved", C.c_int), ("inconsistent", C.c_int), ("indefinite", C.c_int),
                 ("npcCount", C.c_int), ("nresiduals", C.c_int), ("nAresiduals", C.c_int), ("nAcond", C.c_int),
                 ("allocation_timer", C.c_double), ("timer", C.c_double), ("status", C.c_char * 96),
-                ("Anorm", C.c_double)]
+                ("Anorm", C.c_double), ("error_with_bnd", C.c_int), ("nerr_lbnds", C.c_int), ("nerr_ubnds_lq", C.c_int),
+                ("nerr_ubnds_cg", C.c_int)]
 
 
 # every symbol include/krylov_b200.h declares: name -> (restype, argtypes)
