@@ -302,7 +302,8 @@ int kb200_mtx_read(const char *path, int *n, long long *nnz, int *rowptr, int *c
 int kb200_host_householder(int m, int k, double *Q, double *R, double *tau, int compact);
 int kb200_host_cholqr_factors(int p, const double *G, double *R, double *Rinv);
 int kb200_host_householder_signs(int p, const double *top, double *s);
-/* y = A x (x has the object's n columns, y its m rows).  variant: 0 auto, 1 row-per-thread LDG kernel, 2 TMA-staged kernel. */
+/* y = A x (x has the object's n columns, y its m rows).  variant: 0 auto, 1 row-per-thread LDG kernel, 2 TMA-staged kernel,
+ * 3 the constant-coefficient encoding (forced only; -1 and last_error when the operator is not encoded, see kb200_csr_dict). */
 int kb200_spmv_csr(void *ctx, void *csr, const void *x, void *y, int variant);
 /* W = A X on row-major n x p device panels (the SpMM of block_gmres).  variant: 0 auto (what block_gmres runs),
  * 1 p-threads-per-row kernel, 2 TMA-staged (p in {2,4,8,16,32} and a fitting tile plan, else -1 and last_error).
@@ -318,6 +319,10 @@ int krylov_b200_block_panel_op(void *ws, int op, int path, int rows, double alph
                                double beta, void *Out, const void *Next, void *G);
 /* staging plan of a CSR object: out[0]=ntiles out[1]=tile_cap out[2]=max_row out[3]=tma_ok out[4]=stages out[5]=grid out[6]=smem_bytes */
 int kb200_csr_plan(void *csr, long long *out7);
+/* constant-coefficient encoding of a square CSR object (every entry one of <= 8 (column - row, value) pairs, stored as one
+ * mask byte per row; built when the operator is created unless KB200_CSR_DICT=0): 1 if encoded (*npairs = number of
+ * pairs), 0 if not (*npairs = 0), -1 on a NULL object.  Fused CG runs its persistent kernel on the encoding. */
+int kb200_csr_dict(void *csr, int *npairs);
 
 #ifdef __cplusplus
 }

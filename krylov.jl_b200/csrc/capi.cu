@@ -30,8 +30,10 @@ struct CsrAny {
   int dtype = 1;
   Csr<double> d;
   Csr<float> f;
+  CsrDict<double> dd;                  // constant-coefficient encoding of a square operator (npairs == 0: none)
+  CsrDict<float> df;
   Ctx* owner_ctx = nullptr;
-  ~CsrAny() { csr_free(d); csr_free(f); }
+  ~CsrAny() { csr_free(d); csr_free(f); csr_dict_free(dd); csr_dict_free(df); }
 };
 
 struct Handle {
@@ -116,6 +118,9 @@ bool is_cg_ls(int s) { return s == S_CGLS || s == S_CRLS; }     // CGLS / CRLS: 
 template <class T> Csr<T>& csr_of(CsrAny& a);
 template <> Csr<double>& csr_of<double>(CsrAny& a) { return a.d; }
 template <> Csr<float>& csr_of<float>(CsrAny& a) { return a.f; }
+template <class T> CsrDict<T>& dict_of(CsrAny& a);
+template <> CsrDict<double>& dict_of<double>(CsrAny& a) { return a.dd; }
+template <> CsrDict<float>& dict_of<float>(CsrAny& a) { return a.df; }
 
 template <class T> void destroy_handle(Handle* h) {
   Workspace<T>* ws = W<T>(h);
@@ -270,7 +275,7 @@ int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fM, KrylovMatvec fN, const
   LinOp<T> A;
   if (fA) A = make_cb_op<T>(h, ws, fA, ud);
   else if (h->csr) {
-    A.kind = LinOp<T>::CSR; A.csr = &csr_of<T>(*h->csr); A.n = ws->n;
+    A.kind = LinOp<T>::CSR; A.csr = &csr_of<T>(*h->csr); A.dict = &dict_of<T>(*h->csr); A.n = ws->n;
     // columns: n local ones plus, row-partitioned, the halo entries -- anything beyond is an out-of-bounds gather
     const long long ncols = (long long)ws->n + (ws->dist.world > 1 ? ws->dist.halo.nhalo : 0);
     if (A.csr->n != ws->n || A.csr->max_col >= ncols)
@@ -647,9 +652,9 @@ int krylov_b200_set_operator_csr(void* ws, int n, long long nnz, const void* row
     if (n != m_of(h)) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
     const int ncols = is_ls(h) ? n_of(h) : -1;
     if (h->dtype == KRYLOV_FLOAT64)
-      csr_upload<double>(cx, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, ncols);
+      csr_upload<double>(cx, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, ncols, &a->dd);
     else
-      csr_upload<float>(cx, a->f, n, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0, ncols);
+      csr_upload<float>(cx, a->f, n, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0, ncols, &a->df);
     h->csr = a;
     h->csrT.reset();
     return 0;
@@ -1061,8 +1066,8 @@ void* kb200_csr_create(void* ctx, int dtype, int n, long long nnz, const void* r
     CsrAny* a = new CsrAny();
     a->dtype = dtype; a->owner_ctx = &c;
     try {
-      if (dtype == KRYLOV_FLOAT64) csr_upload<double>(c, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0);
-      else if (dtype == KRYLOV_FLOAT32) csr_upload<float>(c, a->f, n, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0);
+      if (dtype == KRYLOV_FLOAT64) csr_upload<double>(c, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, -1, &a->dd);
+      else if (dtype == KRYLOV_FLOAT32) csr_upload<float>(c, a->f, n, nnz, rowptr, colind, (const float*)values, index_base, index_bytes, location != 0, -1, &a->df);
       else throw std::runtime_error("unsupported dtype");
     } catch (...) { delete a; throw; }
     return a;
@@ -1200,6 +1205,11 @@ int kb200_spmv_csr(void* ctx, void* csr, const void* x, void* y, int variant) {
     const int max_col = a->dtype == KRYLOV_FLOAT64 ? a->d.max_col : a->f.max_col;
     const int ncols = a->dtype == KRYLOV_FLOAT64 ? a->d.ncols : a->f.ncols;
     if (max_col >= ncols) throw std::runtime_error("column index outside the operator's columns");
+    if (variant == 3) {                // the constant-coefficient encoding (forced only)
+      if (a->dtype == KRYLOV_FLOAT64) k_spmv_dict<double>(c, a->dd, (const double*)x, (double*)y);
+      else k_spmv_dict<float>(c, a->df, (const float*)x, (float*)y);
+      return 0;
+    }
     if (a->dtype == KRYLOV_FLOAT64) k_spmv<double>(c, a->d, (const double*)x, (double*)y, variant);
     else k_spmv<float>(c, a->f, (const float*)x, (float*)y, variant);
     return 0;
@@ -1244,6 +1254,14 @@ int kb200_csr_plan(void* csr, long long* out) {
     out[0] = A.ntiles; out[1] = A.tile_cap; out[2] = A.max_row; out[3] = A.tma_ok; out[4] = A.stages; out[5] = A.grid; out[6] = (long long)A.smem_bytes;
   }
   return 0;
+}
+
+int kb200_csr_dict(void* csr, int* npairs) {
+  CsrAny* a = (CsrAny*)csr;
+  if (!a) return -1;
+  const int np = a->dtype == KRYLOV_FLOAT64 ? a->dd.npairs : a->df.npairs;
+  if (npairs) *npairs = np;
+  return np > 0 ? 1 : 0;
 }
 
 }  // extern "C"

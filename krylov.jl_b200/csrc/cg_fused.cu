@@ -419,6 +419,30 @@ __device__ __forceinline__ T cg_phase_b_block(int n, int bs_rt, T nalpha, T* r, 
   return acc;
 }
 
+// Phase B element loops (cg.jl:240-242): r -= alpha Ap and <r, z> over elements i, i + stride, ... (4 per trip),
+// exactly as cg_persist runs them inline.
+template <class T, int MODE>
+__device__ __forceinline__ T cg_phase_b_elems(int n, T nalpha, T* r, const T* Ap, const T* mdiag, int i, int stride, T acc) {
+  for (; i + 3 * stride < n; i += 4 * stride) {
+    T rv[4], av[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) { rv[u] = r[i + u * stride]; av[u] = Ap[i + u * stride]; }
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int j = i + u * stride;
+      const T rn = add_rn(rv[u], mul_rn(nalpha, av[u]));
+      r[j] = rn;
+      acc += rn * (MODE == kJacobi ? mul_rn(__ldg(&mdiag[j]), rn) : rn);
+    }
+  }
+  for (; i < n; i += stride) {
+    const T rn = add_rn(r[i], mul_rn(nalpha, Ap[i]));
+    r[i] = rn;
+    acc += rn * (MODE == kJacobi ? mul_rn(__ldg(&mdiag[i]), rn) : rn);
+  }
+  return acc;
+}
+
 // Halo staging of the row-partitioned persistent kernel (one warp per CTA): this CTA's share of the halo list, all
 // loads in flight at once.  The halo entries of r and of the old direction land in the TAILS of the local vectors
 // (r and the p buffers of a row-partitioned workspace hold nloc + nhalo entries), so the gather of phase A is
@@ -549,6 +573,7 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPer
         else acc = cg_phase_b_block<T, 0>(n, a.mbs, nalpha, r, Ap, a.z, a.mblocks, i, stride);
         i = n;                                  // the element loops below are skipped
       }
+      // (the loops of cg_phase_b_elems, kept inline here: calling the helper changes this kernel's register allocation)
       for (; i + 3 * stride < n; i += 4 * stride) {
         T rv[4], av[4];
 #pragma unroll
@@ -585,6 +610,89 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPer
   }
   if (warp == kConsumerWarps && lane == 0) tile_drain<T>(P, (unsigned)passes * (unsigned)cnt, ppos);
   cg_report_to_host<T>(a, st);                 // st is final: every CTA left the loop after the same barrier
+}
+
+// cg_persist on a constant-coefficient operator (CsrDict): phase A reads one mask byte per row instead of the CSR
+// row (DESIGN.md §3: B_cg,dict = n + 9nv), so there is no tile ring and no producer work.  Single GPU, M = I or
+// Jacobi.  Everything else is cg_persist's: the same grid, 288 threads per CTA, tile t on CTA t mod G in the same
+// order, row = tile * 256 + thread, the same phase B and barriers -- hence the same rounding of every row sum and
+// every dot-product partial, and bit-identical iterates.
+template <class T> struct SlotLoads { T r, p, d; };   // r_j, p_old_j and (Jacobi) the diagonal of M at j
+
+template <class T, int MODE, int MINB>
+__global__ void __launch_bounds__(kTileThreads, MINB) cg_persist_dict(CsrDict<T> D, CgPersistArgs<T> a, CgState<T>* st, T* part,
+                                                                     GridBar* gb) {
+  __shared__ T sm[32];
+  __shared__ unsigned sflag[2];
+  __shared__ CgScal<T> sc;
+  volatile CgState<T>* vst = st;
+  if (vst->done) { cg_report_to_host<T>(a, st); return; }
+  if (threadIdx.x == 0) cg_load_scal<T>(st, &sc);
+  __syncthreads();
+  const int G = gridDim.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int n = D.n, ntiles = (n + kTileRows - 1) / kTileRows;
+  const int row0 = (int)blockIdx.x * kTileRows + tid, rstep = G * kTileRows;
+  // the masks do not change: this CTA's first one is loaded once, the next tile's while the current one is summed,
+  // so no gather waits for its mask
+  const unsigned m0 = (warp < kConsumerWarps && row0 < n) ? __ldg(&D.mask[row0]) : 0u;
+  for (int k = 0; k < a.max_iters; k++) {
+    const int iter = sc.iter;
+    const T beta = sc.beta, alpha_prev = sc.alpha;
+    const bool xup = iter > 0;
+    const T* p_old = (iter & 1) ? a.P1 : a.P0;
+    T* p_new = (iter & 1) ? a.P0 : a.P1;
+    T dacc = T(0);
+    const bool timing = a.timed && blockIdx.x == 0 && tid == 0;
+    unsigned long long t0 = 0, t1 = 0;
+    if (timing) t0 = globaltimer_ns();
+    // ------------------------------ phase A (= K1) ------------------------------
+    if (warp < kConsumerWarps) {
+      const T* r = a.r;
+      const T* mdiag = a.mdiag;
+      // p_j = z_j + beta p_j (cg.jl:259 applied on the fly): the loads of a slot, then its value
+      auto load = [&](int j) -> SlotLoads<T> {
+        return SlotLoads<T>{r[j], p_old[j], MODE == kJacobi ? __ldg(&mdiag[j]) : T(0)};
+      };
+      auto value = [&](const SlotLoads<T>& l) -> T {
+        const T z = MODE == kJacobi ? mul_rn(l.d, l.r) : l.r;
+        return add_rn(z, mul_rn(beta, l.p));
+      };
+      unsigned m = m0;
+      for (int t = blockIdx.x, row = row0; t < ntiles; t += G, row += rstep) {
+        const unsigned mnext = (t + G < ntiles && row + rstep < n) ? __ldg(&D.mask[row + rstep]) : 0u;
+        if (row < n) {
+          const T po = p_old[row];
+          T z = r[row];
+          if (MODE == kJacobi) z = mul_rn(__ldg(&mdiag[row]), z);
+          const T pn = add_rn(z, mul_rn(beta, po));
+          const T xr = xup ? a.x[row] : T(0);
+          const T acc = dict_row_sum<T>(D, row, m, load, value);
+          p_new[row] = pn;
+          a.Ap[row] = acc;
+          if (xup) a.x[row] = add_rn(xr, mul_rn(alpha_prev, po));
+          dacc += pn * acc;
+        }
+        m = mnext;
+      }
+    }
+    bool ok = grid_reduce_barrier<T>(gb, dacc, part, sm, sflag, st, &sc, [&](T tot) {
+      if (lane == 0) cg_k1_finalize(st, tot);
+    });
+    if (!ok || sc.done) break;
+    if (timing) t1 = globaltimer_ns();
+    // ------------------------------ phase B (= K2) ------------------------------
+    const T nalpha = -sc.alpha;
+    const T acc = cg_phase_b_elems<T, MODE>(n, nalpha, a.r, a.Ap, a.mdiag, (int)blockIdx.x * kTileThreads + tid, G * kTileThreads, T(0));
+    ok = grid_reduce_barrier<T>(gb, acc, part, sm, sflag, st, &sc, [&](T tot) {
+      if (lane == 0) cg_k2_finalize(st, tot);
+    });
+    if (timing) {
+      const unsigned long long t2 = globaltimer_ns();
+      gb->ns_a += t1 - t0; gb->ns_b += t2 - t1; gb->timed_iters += 1;
+    }
+    if (!ok || sc.done) break;
+  }
+  cg_report_to_host<T>(a, st);
 }
 
 // Prologue of a row-partitioned solve in push mode: send the boundary entries of r_0 to the neighbours' halo
@@ -679,9 +787,9 @@ template <class T> bool cg_fused_eligible(const LinOp<T>& A, const LinOp<T>& M, 
 }
 
 template <class T>
-void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const SolveOpts& o, T gamma0, T eps_tol, int itmax, double start_time,
-                   bool& solved, bool& tired, bool& zero_curvature, bool& inconsistent, bool& user_exit, bool& overtimed,
-                   int& iter) {
+void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, const SolveOpts& o, T gamma0, T eps_tol, int itmax,
+                   double start_time, bool& solved, bool& tired, bool& zero_curvature, bool& inconsistent, bool& user_exit,
+                   bool& overtimed, int& iter) {
   Ctx& c = ws.ctx;
   const int n = ws.n;
   typedef CgState<T> St;
@@ -787,6 +895,8 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const SolveOpts& o, T gamm
   if (bjac && !persist) throw std::runtime_error("block-Jacobi M reached the fused CG loop without the persistent kernel");
   typedef void (*KpFn)(Csr<T>, CgPersistArgs<T>, CgState<T>*, T*, GridBar*, DistComm*);
   KpFn kp = nullptr;
+  typedef void (*KdFn)(CsrDict<T>, CgPersistArgs<T>, CgState<T>*, T*, GridBar*);
+  KdFn kdict = nullptr;
   int pgrid = 0;
   CgPersistArgs<T> pa;
   memset(&pa, 0, sizeof(pa));
@@ -811,6 +921,15 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const SolveOpts& o, T gamm
     KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kp, kTileThreads, A.smem_bytes));
     if (occ < 1) throw std::runtime_error("cg_persist does not fit on an SM with the planned shared-memory ring");
     pgrid = std::min(std::min(occ, A.ctas_per_sm) * sm_count(), std::max(1, A.ntiles));
+    // constant-coefficient operator (single GPU, M = I or Jacobi): the encoded kernel on the SAME grid, whose rows,
+    // tiles and partials are then those of cg_persist (bit-identical iterates)
+    if (dict && dict->npairs > 0 && dict->n == n && !dist && !bjac) {
+      KdFn kd = A.ctas_per_sm >= 3 ? (jac ? cg_persist_dict<T, kJacobi, 3> : cg_persist_dict<T, kPlain, 3>)
+                                   : (jac ? cg_persist_dict<T, kJacobi, 2> : cg_persist_dict<T, kPlain, 2>);
+      int occd = 0;
+      KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occd, kd, kTileThreads, 0));
+      if (occd * sm_count() >= pgrid) kdict = kd;
+    }
     pa.r = ws.r; pa.P0 = ws.p; pa.P1 = ws.p2; pa.Ap = ws.Ap; pa.x = ws.x;
     pa.mdiag = md;
     pa.z = ws.z; pa.mblocks = ws.mblocks_fused; pa.mbs = ws.mbs_fused;
@@ -871,8 +990,14 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const SolveOpts& o, T gamm
       pa.hsnap = hslot(slot);
       pa.hseq = hseq + slot;
       pa.seq = expect[slot] = ++ws.fused_seq;
-      void* args[] = {(void*)&Acopy, (void*)&pa, (void*)&dst, (void*)&partp, (void*)&gbar, (void*)&dcm};
-      KB_CUDA(cudaLaunchCooperativeKernel((const void*)kp, dim3(pgrid), dim3(kTileThreads), args, A.smem_bytes, c.stream));
+      if (kdict) {
+        CsrDict<T> Dcopy = *dict;
+        void* args[] = {(void*)&Dcopy, (void*)&pa, (void*)&dst, (void*)&partp, (void*)&gbar};
+        KB_CUDA(cudaLaunchCooperativeKernel((const void*)kdict, dim3(pgrid), dim3(kTileThreads), args, 0, c.stream));
+      } else {
+        void* args[] = {(void*)&Acopy, (void*)&pa, (void*)&dst, (void*)&partp, (void*)&gbar, (void*)&dcm};
+        KB_CUDA(cudaLaunchCooperativeKernel((const void*)kp, dim3(pgrid), dim3(kTileThreads), args, A.smem_bytes, c.stream));
+      }
       c.launches += 1;
       enq += batch;
       return;                                   // the kernel reports into pinned host memory itself
@@ -978,8 +1103,8 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const SolveOpts& o, T gamm
   template bool cg_fused_eligible<T>(const LinOp<T>&, const LinOp<T>&, const SolveOpts&);                    \
   template void cg_fused_prepare<T>(Workspace<T>&);                                                          \
   template void cg_dist_push_r<T>(Workspace<T>&);                                                            \
-  template void cg_fused_loop<T>(Workspace<T>&, const Csr<T>&, const SolveOpts&, T, T, int, double, bool&, bool&, \
-                                 bool&, bool&, bool&, bool&, int&);
+  template void cg_fused_loop<T>(Workspace<T>&, const Csr<T>&, const CsrDict<T>*, const SolveOpts&, T, T, int, double, \
+                                 bool&, bool&, bool&, bool&, bool&, bool&, int&);
 INST(double)
 INST(float)
 #undef INST

@@ -102,13 +102,34 @@ struct Csr {
   int ctas_per_sm = 0;      // resident CTAs per SM the ring was sized for
 };
 
-// ncols < 0: square (ncols = n)
+// Constant-coefficient encoding of a square CSR operator (DESIGN.md §2).  When every stored entry is one of at most
+// kDictSlots (column - row, value) pairs, the pairs form an operator-wide dictionary sorted by offset (then by the
+// value's bits) and each row is one byte: bit u set <=> the row holds pair u.  Because the columns of a row ascend,
+// so do its offsets: the bit order is the summation order and the encoded row sums are bit-identical to the CSR ones.
+// Kept OUT of Csr<T> (whose parameter block the existing kernels share) and passed by value to the kernels that
+// read it, so offsets and values sit in the parameter bank.
+constexpr int kDictSlots = 8;
+template <class T>
+struct CsrDict {
+  int n = 0;
+  int npairs = 0;                       // 0: not encoded (the operator keeps the CSR path only)
+  int off[kDictSlots] = {};             // column - row of pair u, ascending
+  T val[kDictSlots] = {};
+  unsigned char* mask = nullptr;        // n bytes (device), allocated with the operator
+};
+
+// ncols < 0: square (ncols = n).  dict != nullptr: try to encode the operator (csr_plan).
 template <class T> void csr_upload(Ctx& c, Csr<T>& A, int n, long long nnz, const void* rowptr, const void* colind,
-                                   const T* val, int index_base, int index_bytes, bool on_device, int ncols = -1);
+                                   const T* val, int index_base, int index_bytes, bool on_device, int ncols = -1,
+                                   CsrDict<T>* dict = nullptr);
 template <class T> void csr_free(Csr<T>& A);
-template <class T> void csr_plan(Ctx& c, Csr<T>& A);
+template <class T> void csr_dict_free(CsrDict<T>& D);
+// dict != nullptr: also build the encoding when the operator qualifies (KB200_CSR_DICT=0 disables it)
+template <class T> void csr_plan(Ctx& c, Csr<T>& A, CsrDict<T>* dict = nullptr);
 // y = A x.  variant: 0 auto (TMA-staged when the plan allows), 1 force row-per-thread LDG, 2 force TMA-staged
 template <class T> void k_spmv(Ctx& c, const Csr<T>& A, const T* x, T* y, int variant = 0);
+// y = A x through the encoded rows (kb200_spmv_csr variant 3); throws when the operator is not encoded
+template <class T> void k_spmv_dict(Ctx& c, const CsrDict<T>& D, const T* x, T* y);
 // Row-partitioned operators: send this rank's boundary entries of x to the peers' halo buffers and meet in the
 // in-kernel barrier (no-op on a single GPU).  Every y = A x on a distributed workspace is preceded by one.
 template <class T> void k_halo_exchange(Ctx& c, const T* x);
@@ -122,7 +143,8 @@ template <class T>
 struct LinOp {
   enum Kind { NONE, CSR, DIAG, BDIAG, HOST_CB, DEV_CB } kind = NONE;
   const Csr<T>* csr = nullptr;
-  const T* diag = nullptr;       // DIAG: y = diag .* x (or x ./ diag with ldiv)
+  const CsrDict<T>* dict = nullptr;   // CSR: its constant-coefficient encoding, if any (the persistent CG kernel reads it)
+  const T* diag = nullptr;      // DIAG: y = diag .* x (or x ./ diag with ldiv)
   const T* blocks = nullptr;     // BDIAG: dense bs x bs diagonal blocks, row-major, ceil(n / bs) of them (block-Jacobi)
   const T* blocks_inv = nullptr; //        their inverses (ldiv = true applies these)
   int bs = 0;
@@ -293,8 +315,9 @@ template <class T> bool cg_fused_eligible(const LinOp<T>& A, const LinOp<T>& M, 
 template <class T> void cg_dist_push_r(Workspace<T>& ws);
 template <class T> void cg_fused_prepare(Workspace<T>& ws);   // device/pinned scalar blocks, p2, events (ws_create)
 constexpr size_t kFusedBlockBytes = 4096;
-template <class T> void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const SolveOpts& o, T gamma0, T eps_tol, int itmax,
-                                      double start_time, bool& solved, bool& tired, bool& zero_curvature,
+// dict: the operator's encoding (nullptr or npairs == 0: CSR only); the single-GPU persistent kernel runs on it
+template <class T> void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, const SolveOpts& o, T gamma0,
+                                      T eps_tol, int itmax, double start_time, bool& solved, bool& tired, bool& zero_curvature,
                                       bool& inconsistent, bool& user_exit, bool& overtimed, int& iter);
 
 // Fused iteration phases of BiCGSTAB / MINRES / GMRES (fused_phases.cu); eligible when A is a CSR operator,

@@ -181,7 +181,7 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
     ws.mdiag_fused = (MisI || M.kind != LinOp<T>::DIAG) ? nullptr : M.diag;   // Diagonal M: applied inside K1/K2 (z is not materialised)
     ws.mblocks_fused = M.kind == LinOp<T>::BDIAG ? M.blocks : nullptr;        // block-Jacobi M: z = M r materialised in phase B
     ws.mbs_fused = M.kind == LinOp<T>::BDIAG ? M.bs : 0;
-    cg_fused_loop<T>(ws, *A.csr, o, gamma, eps_tol, itmax, run.start, solved, tired, zero_curvature, inconsistent,
+    cg_fused_loop<T>(ws, *A.csr, A.dict, o, gamma, eps_tol, itmax, run.start, solved, tired, zero_curvature, inconsistent,
                      user_exit, overtimed, iter);
   } else {
     T* p = ws.p;

@@ -366,4 +366,25 @@ __device__ __forceinline__ void tile_consume_pass(const Csr<T>& A, const TilePip
   }
 }
 
+// Row sum of an ENCODED row (CsrDict, kb_internal.h): mask m, one bit per dictionary pair.  The kDictSlots gathers
+// are one straight-line batch; an unused slot reads the row itself (always a valid address -- row + off may fall
+// outside [0, n)) and its product is not added (the select of tile_consume_pass).  The pairs are sorted by offset,
+// so the set bits come in column order: same operands, same order and same rounding as the CSR row.
+// `load(j)` only issues the loads of column j; `value(l)` forms x_j from them afterwards, so that all loads of the
+// row are in flight before the first arithmetic waits on one (a gather that computes as it loads gets 4-6 in flight).
+template <class T, class Load, class Value>
+__device__ __forceinline__ T dict_row_sum(const CsrDict<T>& D, int row, unsigned m, Load load, Value value) {
+  decltype(load(0)) lv[kDictSlots];
+#pragma unroll
+  for (int u = 0; u < kDictSlots; u++) lv[u] = load(((m >> u) & 1u) ? row + D.off[u] : row);
+  asm volatile("" ::: "memory");          // keep the loads above the sums
+  T acc = T(0);
+#pragma unroll
+  for (int u = 0; u < kDictSlots; u++) {
+    const T nx = add_rn(acc, mul_rn(D.val[u], value(lv[u])));
+    acc = ((m >> u) & 1u) ? nx : acc;
+  }
+  return acc;
+}
+
 }  // namespace kb

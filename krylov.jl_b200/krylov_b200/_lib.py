@@ -134,6 +134,7 @@ SIGNATURES = {
     "kb200_host_householder_signs": (_I, [_I, _P, _P]),
     "kb200_spmv_csr": (_I, [_P, _P, _P, _P, _I]),
     "kb200_csr_plan": (_I, [_P, C.POINTER(_LL)]),
+    "kb200_csr_dict": (_I, [_P, C.POINTER(_I)]),
     "kb200_spmm_csr": (_I, [_P, _P, _I, _P, _P, _I]),
     "krylov_b200_block_panel_op": (_I, [_P, _I, _I, _I, _D, _P, _P, _D, _P, _P, _P]),
 }

@@ -8,7 +8,8 @@ tree's build), the libraries alternating chunk by chunk.
 
 Prints the differences and exits 1 when any configuration differs.  The configurations cover the 13 single
 right-hand-side solvers with the fused paths on and off: diagonal M and N, ldiv, warm starts, restart and growth past
-`memory`, reorthogonalization, b = 0, itmax = 3, a callback exit, timemax = 0, the solver-specific exits and Float32.
+`memory`, reorthogonalization, b = 0, itmax = 3, a callback exit, timemax = 0, the solver-specific exits and Float32,
+and CG on a constant-coefficient operator (the path of the CsrDict encoding, M = I and a diagonal M, both types).
 """
 import json
 import os
@@ -35,6 +36,7 @@ def problems():
         rp, ci, va = t
         return sp.csr_matrix((va, ci, rp), shape=(n, m or n))
     lap = csr(div_grad_csr(6), 216) + sp.diags(np.linspace(0.0, 4.0, 216))        # non-constant diagonal
+    dg = csr(div_grad_csr(30, 20, 10), 6000)                                       # constant coefficients: 7 pairs (CsrDict)
     kron = csr(kron_unsymmetric_csr(6), 216) + sp.diags(np.linspace(0.0, 3.0, 216))
     N = 5
     grad = csr(grad_csr(N), 3 * N * N * (N - 1), N ** 3)
@@ -47,6 +49,7 @@ def problems():
     rng = np.random.default_rng(7)
     P = {
         "lap": (lap, np.ones(216)),
+        "dg": (dg, rng.standard_normal(6000)),
         "kron": (kron, kron @ np.ones(216)),
         "grad": (grad, rng.standard_normal(grad.shape[0])),
         "indef": (indef, indef @ np.arange(1.0, 11.0)),
@@ -97,6 +100,10 @@ def configs():
             add(s, p, memory=3)
         if s in ("bicgstab", "cgs"):
             add(s, "bc0", c="e1")
+    for dtype in ("float64", "float32"):            # the persistent kernel on the constant-coefficient encoding
+        add("cg", "dg", dtype=dtype)
+        add("cg", "dg", dtype=dtype, M="pos")
+        add("cg", "dg", dtype=dtype, itmax=40, atol=0.0, rtol=0.0)
     add("cg", "indef", linesearch=True)
     add("cg", "lap", radius=0.5)
     add("cg", "indef12", radius=5.0)
