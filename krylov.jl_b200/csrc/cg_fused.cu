@@ -16,7 +16,7 @@
 //     (dist.cuh).  Block-Jacobi M (MODE = kBlockJac): z = M r is formed block by block in phase B.
 //   * cg_k1_tma / cg_k1_rows + cg_k2: two launches per iteration, used when x must be current after every
 //     iteration (callbacks, verbose, timemax), when the operator has no TMA tile plan, and as the A/B reference
-//     (fused = 2, KB200_PERSIST=0).  Their row-partitioned variant pulls halo entries nonzero by nonzero.
+//     (fused = 2).  Their row-partitioned variant pulls halo entries nonzero by nonzero.
 //
 // The host only enqueues launches and polls the scalar block (one read-back per batch of iterations); launches
 // enqueued past the stopping point see `done` and return immediately, so niter, x, r, p at exit are those of the
@@ -419,10 +419,10 @@ __device__ __forceinline__ T cg_phase_b_block(int n, int bs_rt, T nalpha, T* r, 
   return acc;
 }
 
-// Phase B element loops (cg.jl:240-242): r -= alpha Ap and <r, z> over elements i, i + stride, ... (4 per trip),
-// exactly as cg_persist runs them inline.
+// Phase B element loops (cg.jl:240-242): r -= alpha Ap and <r, z> over elements i, i + stride, ... (4 per trip).
 template <class T, int MODE>
-__device__ __forceinline__ T cg_phase_b_elems(int n, T nalpha, T* r, const T* Ap, const T* mdiag, int i, int stride, T acc) {
+__device__ __forceinline__ T cg_phase_b_elems(int n, T nalpha, T* r, const T* Ap, const T* mdiag, int i, int stride) {
+  T acc = T(0);
   for (; i + 3 * stride < n; i += 4 * stride) {
     T rv[4], av[4];
 #pragma unroll
@@ -466,7 +466,71 @@ __device__ __forceinline__ void cg_stage_halo(HaloMap halo, const CgPeerTab<T>* 
   }
 }
 
-template <class T, int MODE, int MINB, int DEPTH>
+// The iterations of one persistent launch (at most a.max_iters), shared by cg_persist and cg_persist_dict, which
+// differ only in phase A.  `phase_a(k, iter, beta, alpha_prev, p_old, p_new)` runs phase A (= K1) of the launch's
+// k-th iteration: p_new = z + beta p_old, Ap = A p_new and the pending x += alpha_prev p_old over this thread's rows;
+// it returns the thread's share of <p, Ap>.  Everything else is here: the scalars broadcast through `sc`, the parity
+// of the direction buffers, the phase timing, both barriers with their reductions and phase B (= K2).  Returns the
+// number of iterations whose phase A ran.
+template <class T, int MODE, class PhaseA>
+__device__ __forceinline__ int cg_persist_iterations(int n, const CgPersistArgs<T>& a, CgState<T>* st, T* part, GridBar* gb,
+                                                     DistComm* dc, T* sm, unsigned* sflag, CgScal<T>& sc, PhaseA phase_a) {
+  const int G = gridDim.x, tid = threadIdx.x, lane = tid & 31;
+  int passes = 0;
+  for (int k = 0; k < a.max_iters; k++) {
+    const int iter = sc.iter;
+    const T beta = sc.beta, alpha_prev = sc.alpha;
+    T* p_old = (iter & 1) ? a.P1 : a.P0;
+    T* p_new = (iter & 1) ? a.P0 : a.P1;
+    const bool timing = a.timed && blockIdx.x == 0 && tid == 0;
+    unsigned long long t0 = 0, t1 = 0;
+    if (timing) t0 = globaltimer_ns();
+    // ------------------------------ phase A (= K1) ------------------------------
+    const T dacc = phase_a(k, iter, beta, alpha_prev, p_old, p_new);
+    passes = k + 1;
+    bool ok = grid_reduce_barrier<T>(gb, dacc, part, sm, sflag, st, &sc, [&](T tot) {
+      if (MODE == kDist) {
+        tot = (T)dist_allreduce_sum_warp<T>(dc, (double)tot);
+        if (*(volatile int*)&dc->error) { if (lane == 0) { st->comm_error = 1; st->done = 1; } return; }
+      }
+      if (lane == 0) cg_k1_finalize(st, tot);
+    });
+    if (!ok || sc.done) break;
+    if (timing) t1 = globaltimer_ns();
+    // ------------------------------ phase B (= K2) ------------------------------
+    const T nalpha = -sc.alpha;
+    const int i = (int)blockIdx.x * kTileThreads + tid, stride = G * kTileThreads;
+    T acc;
+    if (MODE == kBlockJac) {
+      if (a.mbs == 4) acc = cg_phase_b_block<T, 4>(n, 4, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
+      else if (a.mbs == 2) acc = cg_phase_b_block<T, 2>(n, 2, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
+      else if (a.mbs == 8) acc = cg_phase_b_block<T, 8>(n, 8, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
+      else acc = cg_phase_b_block<T, 0>(n, a.mbs, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
+    } else {
+      acc = cg_phase_b_elems<T, MODE>(n, nalpha, a.r, a.Ap, a.mdiag, i, stride);
+    }
+    ok = grid_reduce_barrier<T>(gb, acc, part, sm, sflag, st, &sc, [&](T tot) {
+      if (MODE == kDist) {
+        tot = (T)dist_allreduce_sum_warp<T>(dc, (double)tot);
+        if (*(volatile int*)&dc->error) { if (lane == 0) { st->comm_error = 1; st->done = 1; } return; }
+      }
+      if (lane == 0) {
+        cg_k2_finalize(st, tot);
+        if (MODE == kDist) gb->halo_ready = 0u;    // every consumer is past phase A: re-arm the staging counter
+      }
+    });
+    if (timing) {
+      const unsigned long long t2 = globaltimer_ns();
+      gb->ns_a += t1 - t0; gb->ns_b += t2 - t1; gb->timed_iters += 1;
+    }
+    if (!ok || sc.done) break;
+  }
+  return passes;
+}
+
+// Phase A from the TMA tile ring: the producer warp streams this CTA's tiles (running ahead into the next
+// iteration's first tiles), the consumer warps gather p_j = z_j + beta p_j on the fly.
+template <class T, int MODE, int MINB>
 __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPersistArgs<T> a, CgState<T>* st, T* part,
                                                                 GridBar* gb, DistComm* dc) {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -474,7 +538,7 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPer
   __shared__ unsigned sflag[2];
   __shared__ CgScal<T> sc;
   volatile CgState<T>* vst = st;
-  if (vst->done) { cg_report_to_host<T>(a, st); return; }    // uniform: st only changes inside the barriers below
+  if (vst->done) { cg_report_to_host<T>(a, st); return; }    // uniform: st only changes inside the barriers
   if (threadIdx.x == 0) cg_load_scal<T>(st, &sc);            // published by the __syncthreads of P.init below
   TilePipe<T> P;
   P.init(A, smem);
@@ -489,19 +553,10 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPer
   const unsigned pre = (unsigned)min(P.S, cnt);
   const uint64_t pol = l2_evict_first_policy();
   unsigned ppos = 0, cpos = 0;
-  int passes = 0;
-  const int n = A.n;
-  for (int k = 0; k < a.max_iters; k++) {
-    const int iter = sc.iter;
-    const T beta = sc.beta, alpha_prev = sc.alpha;
+  const int passes = cg_persist_iterations<T, MODE>(A.n, a, st, part, gb, dc, sm, sflag, sc,
+                                                    [&](int k, int iter, T beta, T alpha_prev, T* p_old, T* p_new) -> T {
     const bool xup = iter > 0;                 // x += alpha_{k-1} p_{k-1} rides in phase A (cg.jl:239)
-    T* p_old = (iter & 1) ? a.P1 : a.P0;
-    T* p_new = (iter & 1) ? a.P0 : a.P1;
     T dacc = T(0);
-    const bool timing = a.timed && blockIdx.x == 0 && tid == 0;
-    unsigned long long t0 = 0, t1 = 0;
-    if (timing) t0 = globaltimer_ns();
-    // ------------------------------ phase A (= K1) ------------------------------
     if (warp == kConsumerWarps) {
       if (lane == 0) {
         const unsigned target = (unsigned)(k + 1) * (unsigned)cnt + (k + 1 < a.max_iters ? pre : 0u);
@@ -537,86 +592,26 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPer
         if (lane == 0) atomicAdd(&gb->halo_ready, 1u);       // 8 consumer warps per CTA report
         // interior tiles first; the tiles with halo columns (last in this CTA's sequence) only after every CTA's
         // producer warp has staged its share of the halo
-        tile_consume_pass<T, DEPTH>(A, P, cpos, 0, cnt_int, tile_at, gather, row_begin, row_done);
+        tile_consume_pass<T>(A, P, cpos, 0, cnt_int, tile_at, gather, row_begin, row_done);
         if (cnt_int < cnt) {
           if (lane == 0) { while (ld_acquire_gpu_u32(&gb->halo_ready) < (unsigned)(G * kConsumerWarps)) { } }
           __syncwarp();
-          tile_consume_pass<T, DEPTH>(A, P, cpos, cnt_int, cnt, tile_at, gather, row_begin, row_done);
+          tile_consume_pass<T>(A, P, cpos, cnt_int, cnt, tile_at, gather, row_begin, row_done);
         }
       } else {
-        tile_consume_pass<T, DEPTH>(A, P, cpos, 0, cnt, tile_at, gather, row_begin, row_done);
+        tile_consume_pass<T>(A, P, cpos, 0, cnt, tile_at, gather, row_begin, row_done);
       }
     }
-    passes = k + 1;
-    bool ok = grid_reduce_barrier<T>(gb, dacc, part, sm, sflag, st, &sc, [&](T tot) {
-      if (MODE == kDist) {
-        tot = (T)dist_allreduce_sum_warp<T>(dc, (double)tot);
-        if (*(volatile int*)&dc->error) { if (lane == 0) { st->comm_error = 1; st->done = 1; } return; }
-      }
-      if (lane == 0) cg_k1_finalize(st, tot);
-    });
-    if (!ok || sc.done) break;
-    if (timing) t1 = globaltimer_ns();
-    // ------------------------------ phase B (= K2) ------------------------------
-    {
-      const T alpha = sc.alpha, nalpha = -alpha;
-      T* r = a.r;
-      const T* Ap = a.Ap;
-      const T* mdiag = a.mdiag;
-      T acc = T(0);
-      const int stride = G * kTileThreads;
-      int i = (int)blockIdx.x * kTileThreads + tid;
-      if (MODE == kBlockJac) {
-        if (a.mbs == 4) acc = cg_phase_b_block<T, 4>(n, 4, nalpha, r, Ap, a.z, a.mblocks, i, stride);
-        else if (a.mbs == 2) acc = cg_phase_b_block<T, 2>(n, 2, nalpha, r, Ap, a.z, a.mblocks, i, stride);
-        else if (a.mbs == 8) acc = cg_phase_b_block<T, 8>(n, 8, nalpha, r, Ap, a.z, a.mblocks, i, stride);
-        else acc = cg_phase_b_block<T, 0>(n, a.mbs, nalpha, r, Ap, a.z, a.mblocks, i, stride);
-        i = n;                                  // the element loops below are skipped
-      }
-      // (the loops of cg_phase_b_elems, kept inline here: calling the helper changes this kernel's register allocation)
-      for (; i + 3 * stride < n; i += 4 * stride) {
-        T rv[4], av[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) { rv[u] = r[i + u * stride]; av[u] = Ap[i + u * stride]; }
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-          const int j = i + u * stride;
-          const T rn = add_rn(rv[u], mul_rn(nalpha, av[u]));
-          r[j] = rn;
-          acc += rn * (MODE == kJacobi ? mul_rn(__ldg(&mdiag[j]), rn) : rn);
-        }
-      }
-      for (; i < n; i += stride) {
-        const T rn = add_rn(r[i], mul_rn(nalpha, Ap[i]));
-        r[i] = rn;
-        acc += rn * (MODE == kJacobi ? mul_rn(__ldg(&mdiag[i]), rn) : rn);
-      }
-      ok = grid_reduce_barrier<T>(gb, acc, part, sm, sflag, st, &sc, [&](T tot) {
-        if (MODE == kDist) {
-          tot = (T)dist_allreduce_sum_warp<T>(dc, (double)tot);
-          if (*(volatile int*)&dc->error) { if (lane == 0) { st->comm_error = 1; st->done = 1; } return; }
-        }
-        if (lane == 0) {
-          cg_k2_finalize(st, tot);
-          gb->halo_ready = 0u;                 // every consumer is past phase A: re-arm the staging counter
-        }
-      });
-      if (timing) {
-        const unsigned long long t2 = globaltimer_ns();
-        gb->ns_a += t1 - t0; gb->ns_b += t2 - t1; gb->timed_iters += 1;
-      }
-      if (!ok || sc.done) break;
-    }
-  }
+    return dacc;
+  });
   if (warp == kConsumerWarps && lane == 0) tile_drain<T>(P, (unsigned)passes * (unsigned)cnt, ppos);
   cg_report_to_host<T>(a, st);                 // st is final: every CTA left the loop after the same barrier
 }
 
-// cg_persist on a constant-coefficient operator (CsrDict): phase A reads one mask byte per row instead of the CSR
-// row (DESIGN.md §3: B_cg,dict = n + 9nv), so there is no tile ring and no producer work.  Single GPU, M = I or
-// Jacobi.  Everything else is cg_persist's: the same grid, 288 threads per CTA, tile t on CTA t mod G in the same
-// order, row = tile * 256 + thread, the same phase B and barriers -- hence the same rounding of every row sum and
-// every dot-product partial, and bit-identical iterates.
+// Phase A from a constant-coefficient operator (CsrDict): one mask byte per row instead of the CSR row (DESIGN.md §3:
+// B_cg,dict = n + 9nv), so there is no tile ring and no producer work.  Single GPU, M = I or Jacobi.  The launch
+// shape is cg_persist's: the same grid, 288 threads per CTA, tile t on CTA t mod G in the same order, row = tile * 256
+// + thread -- hence the same rounding of every row sum and every dot-product partial, and bit-identical iterates.
 template <class T> struct SlotLoads { T r, p, d; };   // r_j, p_old_j and (Jacobi) the diagonal of M at j
 
 template <class T, int MODE, int MINB>
@@ -629,23 +624,16 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist_dict(CsrDict<T>
   if (vst->done) { cg_report_to_host<T>(a, st); return; }
   if (threadIdx.x == 0) cg_load_scal<T>(st, &sc);
   __syncthreads();
-  const int G = gridDim.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int G = gridDim.x, tid = threadIdx.x, warp = tid >> 5;
   const int n = D.n, ntiles = (n + kTileRows - 1) / kTileRows;
   const int row0 = (int)blockIdx.x * kTileRows + tid, rstep = G * kTileRows;
   // the masks do not change: this CTA's first one is loaded once, the next tile's while the current one is summed,
   // so no gather waits for its mask
   const unsigned m0 = (warp < kConsumerWarps && row0 < n) ? __ldg(&D.mask[row0]) : 0u;
-  for (int k = 0; k < a.max_iters; k++) {
-    const int iter = sc.iter;
-    const T beta = sc.beta, alpha_prev = sc.alpha;
+  cg_persist_iterations<T, MODE>(n, a, st, part, gb, nullptr, sm, sflag, sc,
+                                 [&](int, int iter, T beta, T alpha_prev, const T* p_old, T* p_new) -> T {
     const bool xup = iter > 0;
-    const T* p_old = (iter & 1) ? a.P1 : a.P0;
-    T* p_new = (iter & 1) ? a.P0 : a.P1;
     T dacc = T(0);
-    const bool timing = a.timed && blockIdx.x == 0 && tid == 0;
-    unsigned long long t0 = 0, t1 = 0;
-    if (timing) t0 = globaltimer_ns();
-    // ------------------------------ phase A (= K1) ------------------------------
     if (warp < kConsumerWarps) {
       const T* r = a.r;
       const T* mdiag = a.mdiag;
@@ -675,23 +663,8 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist_dict(CsrDict<T>
         m = mnext;
       }
     }
-    bool ok = grid_reduce_barrier<T>(gb, dacc, part, sm, sflag, st, &sc, [&](T tot) {
-      if (lane == 0) cg_k1_finalize(st, tot);
-    });
-    if (!ok || sc.done) break;
-    if (timing) t1 = globaltimer_ns();
-    // ------------------------------ phase B (= K2) ------------------------------
-    const T nalpha = -sc.alpha;
-    const T acc = cg_phase_b_elems<T, MODE>(n, nalpha, a.r, a.Ap, a.mdiag, (int)blockIdx.x * kTileThreads + tid, G * kTileThreads, T(0));
-    ok = grid_reduce_barrier<T>(gb, acc, part, sm, sflag, st, &sc, [&](T tot) {
-      if (lane == 0) cg_k2_finalize(st, tot);
-    });
-    if (timing) {
-      const unsigned long long t2 = globaltimer_ns();
-      gb->ns_a += t1 - t0; gb->ns_b += t2 - t1; gb->timed_iters += 1;
-    }
-    if (!ok || sc.done) break;
-  }
+    return dacc;
+  });
   cg_report_to_host<T>(a, st);
 }
 
@@ -774,26 +747,99 @@ template <class T> void cg_dist_tile_order(Workspace<T>& ws, const Csr<T>& A) {
 }
 
 // ---------------------------------------------------------------------------
-template <class T> bool cg_fused_eligible(const LinOp<T>& A, const LinOp<T>& M, const SolveOpts& o) {
-  // M = I, or a Diagonal M applied with mul! (the Jacobi case of SURVEY.md 8f-1), folded into the two kernels
-  const bool m_ok = M.is_identity() || (M.kind == LinOp<T>::DIAG && !o.ldiv);
-  if (o.fused && A.kind == LinOp<T>::CSR && M.kind == LinOp<T>::BDIAG && !o.ldiv && o.radius == 0) {
-    // block-Jacobi M: only the persistent kernel carries it (phase B forms z = M r block by block)
-    const char* epers = getenv("KB200_PERSIST");
-    const bool single_step = (o.callback != nullptr) || (o.timemax < 1e300) || o.verbose > 0;
-    return A.csr->tma_ok && o.persist != 0 && !single_step && !(epers && atoi(epers) == 0);
+// The one decision of the fused path.  Fused CG needs a CSR operator and no trust region.  M = I and a Diagonal M
+// applied with mul! (the Jacobi case of SURVEY.md 8f-1) are folded into every fused kernel; a block-Jacobi M only into
+// the persistent one (phase B forms z = M r block by block), so it gets "not fused" wherever that kernel cannot run.
+// Row-partitioned solves are fused with M = I only: everything else runs the primitive path, whose SpMV is preceded
+// by the general halo exchange and whose dots end in the in-kernel all-reduce.
+template <class T>
+CgFusedPlan<T> cg_fused_plan(const Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& M, const SolveOpts& o) {
+  CgFusedPlan<T> pl;
+  const bool dist = ws.dist.world > 1;
+  const bool jac = M.kind == LinOp<T>::DIAG && !o.ldiv, bjac = M.kind == LinOp<T>::BDIAG && !o.ldiv;
+  if (!o.fused || A.kind != LinOp<T>::CSR || o.radius != 0 || !(M.is_identity() || jac || bjac) || (dist && !M.is_identity()))
+    return pl;
+  const Csr<T>& C = *A.csr;
+  const int n = ws.n;
+  pl.single_step = (o.callback != nullptr) || (o.timemax < 1e300) || o.verbose > 0;
+  // x += alpha p moves from K2 into the next K1 (one vector pass less) unless x must be current after every
+  // iteration (callbacks, verbose, time limits) -- KB200_XUP=0 keeps the update in K2 for A/B measurements.
+  const char* exu = getenv("KB200_XUP");
+  pl.xup = !pl.single_step && !(exu && atoi(exu) == 0);
+  // Persistent cooperative kernel (one launch per batch of iterations) whenever the tile plan is staged and x need
+  // not be current after every iteration; fused = 2 (o.persist = 0) keeps the two-launch kernels.
+  pl.persist = C.tma_ok && pl.xup && o.persist != 0;
+  if (bjac && !pl.persist) return pl;
+  pl.fused = true;
+  pl.A = &C;
+  pl.mdiag = jac ? M.diag : nullptr;
+  pl.mblocks = bjac ? M.blocks : nullptr;
+  pl.mbs = bjac ? M.bs : 0;
+  pl.batch = pl.single_step ? 1 : (o.batch > 0 ? std::min(o.batch, kHist / 2) : 32);   // iterations per launch / host poll
+  if (pl.persist) {
+    // register budget follows the plan's CTAs per SM: 3 (72 registers, the default plan) or 2 (112 registers: all 16
+    // loads of an 8-nonzero gather batch in flight per thread; selected with KB200_CTAS_PER_SM=2 / large tiles).
+    // The block code of phase B needs the 2-CTA budget.
+    if (bjac) pl.kp = cg_persist<T, kBlockJac, 2>;
+    else if (C.ctas_per_sm >= 3) pl.kp = dist ? cg_persist<T, kDist, 3> : (jac ? cg_persist<T, kJacobi, 3> : cg_persist<T, kPlain, 3>);
+    else pl.kp = dist ? cg_persist<T, kDist, 2> : (jac ? cg_persist<T, kJacobi, 2> : cg_persist<T, kPlain, 2>);
+    ensure_dyn_smem((const void*)pl.kp, 220 * 1024);
+    int occ = 0;
+    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pl.kp, kTileThreads, C.smem_bytes));
+    if (occ < 1) throw std::runtime_error("cg_persist does not fit on an SM with the planned shared-memory ring");
+    pl.pgrid = std::min(std::min(occ, C.ctas_per_sm) * sm_count(), std::max(1, C.ntiles));
+    // constant-coefficient operator (single GPU, M = I or Jacobi): the encoded kernel on the SAME grid, whose rows,
+    // tiles and partials are then those of cg_persist (bit-identical iterates)
+    const CsrDict<T>* dict = A.dict;
+    if (dict && dict->npairs > 0 && dict->n == n && !dist && !bjac) {
+      const typename CgFusedPlan<T>::KdFn kd =
+          C.ctas_per_sm >= 3 ? (jac ? cg_persist_dict<T, kJacobi, 3> : cg_persist_dict<T, kPlain, 3>)
+                             : (jac ? cg_persist_dict<T, kJacobi, 2> : cg_persist_dict<T, kPlain, 2>);
+      int occd = 0;
+      KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occd, kd, kTileThreads, 0));
+      if (occd * sm_count() >= pl.pgrid) { pl.kd = kd; pl.dict = dict; }
+    }
+    return pl;
   }
-  return o.fused && A.kind == LinOp<T>::CSR && m_ok && o.radius == 0;
+  const bool xup = pl.xup;
+  if (C.tma_ok) {
+    if (dist) pl.k1 = xup ? cg_k1_tma<T, kDist, 3, true> : cg_k1_tma<T, kDist, 3, false>;
+    else if (jac) pl.k1 = xup ? cg_k1_tma<T, kJacobi, 3, true> : cg_k1_tma<T, kJacobi, 3, false>;
+    else if (C.ctas_per_sm >= 4) pl.k1 = xup ? cg_k1_tma<T, kPlain, 4, true> : cg_k1_tma<T, kPlain, 4, false>;
+    else if (C.ctas_per_sm == 3) pl.k1 = xup ? cg_k1_tma<T, kPlain, 3, true> : cg_k1_tma<T, kPlain, 3, false>;
+    else pl.k1 = xup ? cg_k1_tma<T, kPlain, 1, true> : cg_k1_tma<T, kPlain, 1, false>;
+    // The grid must equal what is actually co-resident: a register count that silently drops the occupancy below
+    // the plan's CTAs/SM would otherwise run the tiles in 1.5 waves (K1 then takes about twice as long).
+    ensure_dyn_smem((const void*)pl.k1, 220 * 1024);
+    int occ = 0;
+    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pl.k1, kTileThreads, C.smem_bytes));
+    if (occ < 1) throw std::runtime_error("cg_k1_tma does not fit on an SM with the planned shared-memory ring");
+    pl.k1_grid = std::min(std::min(occ, C.ctas_per_sm) * sm_count(), std::max(1, C.ntiles));
+    pl.k1_block = kTileThreads;
+    pl.k1_smem = C.smem_bytes;
+  } else {
+    if (dist) pl.k1 = xup ? cg_k1_rows<T, kDist, true> : cg_k1_rows<T, kDist, false>;
+    else if (jac) pl.k1 = xup ? cg_k1_rows<T, kJacobi, true> : cg_k1_rows<T, kJacobi, false>;
+    else pl.k1 = xup ? cg_k1_rows<T, kPlain, true> : cg_k1_rows<T, kPlain, false>;
+    pl.k1_grid = stream_grid(n, 1, 8);
+    pl.k1_block = kBlock;
+    pl.k1_smem = 0;
+  }
+  if (dist) pl.k2 = xup ? cg_k2<T, kDist, false> : cg_k2<T, kDist, true>;
+  else if (jac) pl.k2 = xup ? cg_k2<T, kJacobi, false> : cg_k2<T, kJacobi, true>;
+  else pl.k2 = xup ? cg_k2<T, kPlain, false> : cg_k2<T, kPlain, true>;
+  pl.k2_grid = stream_grid(n, 4, 8);
+  return pl;
 }
 
 template <class T>
-void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, const SolveOpts& o, T gamma0, T eps_tol, int itmax,
-                   double start_time, bool& solved, bool& tired, bool& zero_curvature, bool& inconsistent, bool& user_exit,
-                   bool& overtimed, int& iter) {
+CgFusedExit cg_fused_loop(Workspace<T>& ws, const CgFusedPlan<T>& pl, const SolveOpts& o, T gamma0, T eps_tol, int itmax,
+                          double start_time) {
   Ctx& c = ws.ctx;
   const int n = ws.n;
   typedef CgState<T> St;
   const bool dist = ws.dist.world > 1;
+  const Csr<T>& A = *pl.A;
   cg_fused_prepare<T>(ws);                      // no-op: done at workspace creation
   St* dst = (St*)ws.fused_state;
   St* hst = (St*)ws.fused_host;                 // two read-back slots, kOffGridBar apart
@@ -808,50 +854,14 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, co
   KB_CUDA(cudaMemsetAsync((char*)ws.fused_state + kOffGridBar, 0, sizeof(GridBar), c.stream));
   // (no sync: the copy reads slot 0 in stream order before any kernel or read-back of this solve writes it)
 
-  const bool jac = ws.mdiag_fused != nullptr;
-  const bool single_step = (o.callback != nullptr) || (o.timemax < 1e300) || o.verbose > 0;
-  // x += alpha p moves from K2 into the next K1 (one vector pass less) unless x must be current after every
-  // iteration (callbacks, verbose, time limits) -- KB200_XUP=0 keeps the update in K2 for A/B measurements.
-  const char* exu = getenv("KB200_XUP");
-  const bool xup = !single_step && !(exu && atoi(exu) == 0);
-  // All variants share one signature: pick the kernel once.
-  typedef void (*K1Fn)(Csr<T>, const T*, const T*, T*, T*, CgState<T>*, T*, unsigned*, DistComm*, CgPeers<T>, T*);
-  typedef void (*K2Fn)(int, T*, T*, const T*, const T*, CgState<T>*, T*, unsigned*, DistComm*, const T*, PushPlan<T>);
-  K1Fn k1 = nullptr;
-  K2Fn k2 = nullptr;
-  if (A.tma_ok) {
-    if (dist) k1 = xup ? cg_k1_tma<T, kDist, 3, true> : cg_k1_tma<T, kDist, 3, false>;
-    else if (jac) k1 = xup ? cg_k1_tma<T, kJacobi, 3, true> : cg_k1_tma<T, kJacobi, 3, false>;
-    else if (A.ctas_per_sm >= 4) k1 = xup ? cg_k1_tma<T, kPlain, 4, true> : cg_k1_tma<T, kPlain, 4, false>;
-    else if (A.ctas_per_sm == 3) k1 = xup ? cg_k1_tma<T, kPlain, 3, true> : cg_k1_tma<T, kPlain, 3, false>;
-    else k1 = xup ? cg_k1_tma<T, kPlain, 1, true> : cg_k1_tma<T, kPlain, 1, false>;
-  } else {
-    if (dist) k1 = xup ? cg_k1_rows<T, kDist, true> : cg_k1_rows<T, kDist, false>;
-    else if (jac) k1 = xup ? cg_k1_rows<T, kJacobi, true> : cg_k1_rows<T, kJacobi, false>;
-    else k1 = xup ? cg_k1_rows<T, kPlain, true> : cg_k1_rows<T, kPlain, false>;
-  }
-  if (dist) k2 = xup ? cg_k2<T, kDist, false> : cg_k2<T, kDist, true>;
-  else if (jac) k2 = xup ? cg_k2<T, kJacobi, false> : cg_k2<T, kJacobi, true>;
-  else k2 = xup ? cg_k2<T, kPlain, false> : cg_k2<T, kPlain, true>;
-  // The persistent grid must equal what is actually co-resident: a register count that silently drops the
-  // occupancy below the plan's CTAs/SM would otherwise run the tiles in 1.5 waves (K1 then takes about twice as long).
-  int k1_grid = A.grid;
-  if (A.tma_ok) {
-    ensure_dyn_smem((const void*)k1, 220 * 1024);
-    int occ = 0;
-    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k1, kTileThreads, A.smem_bytes));
-    if (occ < 1) throw std::runtime_error("cg_k1_tma does not fit on an SM with the planned shared-memory ring");
-    const int resident = std::min(occ, A.ctas_per_sm) * sm_count();
-    k1_grid = std::min(resident, std::max(1, A.ntiles));
-  }
-  const int g2 = stream_grid(n, 4, 8);
-  const int g1r = stream_grid(n, 1, 8);
+  const bool persist = pl.persist, single_step = pl.single_step;
+  const int batch = pl.batch;
   T* P[2] = {ws.p, ws.p2};   // ws.p holds z (= r) from the prologue: with beta = 0, K1 forms p = r + 0*p
   T* part = (T*)c.partials;
   // peers' direction buffers in the same order as P[]
   CgPeers<T> peersP[2];
   memset(peersP, 0, sizeof(peersP));
-  const T* md = ws.mdiag_fused;
+  const T* md = pl.mdiag;
   peersP[0].mdiag = md; peersP[1].mdiag = md;
   PushPlan<T> push_r;
   memset(&push_r, 0, sizeof(push_r));
@@ -882,57 +892,13 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, co
     }
   }
 
-  static const char* ebatch = getenv("KB200_BATCH");            // A/B measurements of the per-launch fixed cost
-  int batch = o.batch > 0 ? o.batch : (single_step ? 1 : (ebatch && atoi(ebatch) > 0 ? atoi(ebatch) : 32));   // iterations per launch / host poll
-  if (batch > kHist / 2) batch = kHist / 2;
-  if (single_step) batch = 1;
-
-  // Persistent cooperative variant (one launch per batch of iterations): whenever the tile plan is staged and x
-  // need not be current after every iteration.  KB200_PERSIST=0 keeps the two-launch kernels (A/B measurements).
-  const char* epers = getenv("KB200_PERSIST");
-  const bool persist = A.tma_ok && xup && !(epers && atoi(epers) == 0) && o.persist != 0;
-  const bool bjac = ws.mblocks_fused != nullptr;
-  if (bjac && !persist) throw std::runtime_error("block-Jacobi M reached the fused CG loop without the persistent kernel");
-  typedef void (*KpFn)(Csr<T>, CgPersistArgs<T>, CgState<T>*, T*, GridBar*, DistComm*);
-  KpFn kp = nullptr;
-  typedef void (*KdFn)(CsrDict<T>, CgPersistArgs<T>, CgState<T>*, T*, GridBar*);
-  KdFn kdict = nullptr;
-  int pgrid = 0;
   CgPersistArgs<T> pa;
   memset(&pa, 0, sizeof(pa));
   GridBar* gbar = (GridBar*)((char*)ws.fused_state + kOffGridBar);
   if (persist) {
-    // register budget follows the plan's CTAs per SM: 3 (72 registers, the default plan) or 2 (112 registers: all 16
-    // loads of an 8-nonzero gather batch in flight per thread; selected with KB200_CTAS_PER_SM=2 / large tiles)
-    static const char* edep = getenv("KB200_GATHER_DEPTH");
-    const int depth = edep ? atoi(edep) : 0;
-    if (A.ctas_per_sm >= 3) {
-      // 8-deep gather batches by default; KB200_GATHER_DEPTH=4 selects 4-deep ones (sweeps)
-      if (bjac) kp = cg_persist<T, kBlockJac, 2, 8>;   // the block code of phase B needs the 96-register budget (2 CTAs per SM)
-      else if (depth == 4) kp = dist ? cg_persist<T, kDist, 3, 4> : (jac ? cg_persist<T, kJacobi, 3, 4> : cg_persist<T, kPlain, 3, 4>);
-      else kp = dist ? cg_persist<T, kDist, 3, 8> : (jac ? cg_persist<T, kJacobi, 3, 8> : cg_persist<T, kPlain, 3, 8>);
-    } else {
-      if (bjac) kp = cg_persist<T, kBlockJac, 2, 8>;
-      else if (depth == 4) kp = dist ? cg_persist<T, kDist, 2, 4> : (jac ? cg_persist<T, kJacobi, 2, 4> : cg_persist<T, kPlain, 2, 4>);
-      else kp = dist ? cg_persist<T, kDist, 2, 8> : (jac ? cg_persist<T, kJacobi, 2, 8> : cg_persist<T, kPlain, 2, 8>);
-    }
-    ensure_dyn_smem((const void*)kp, 220 * 1024);
-    int occ = 0;
-    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kp, kTileThreads, A.smem_bytes));
-    if (occ < 1) throw std::runtime_error("cg_persist does not fit on an SM with the planned shared-memory ring");
-    pgrid = std::min(std::min(occ, A.ctas_per_sm) * sm_count(), std::max(1, A.ntiles));
-    // constant-coefficient operator (single GPU, M = I or Jacobi): the encoded kernel on the SAME grid, whose rows,
-    // tiles and partials are then those of cg_persist (bit-identical iterates)
-    if (dict && dict->npairs > 0 && dict->n == n && !dist && !bjac) {
-      KdFn kd = A.ctas_per_sm >= 3 ? (jac ? cg_persist_dict<T, kJacobi, 3> : cg_persist_dict<T, kPlain, 3>)
-                                   : (jac ? cg_persist_dict<T, kJacobi, 2> : cg_persist_dict<T, kPlain, 2>);
-      int occd = 0;
-      KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occd, kd, kTileThreads, 0));
-      if (occd * sm_count() >= pgrid) kdict = kd;
-    }
     pa.r = ws.r; pa.P0 = ws.p; pa.P1 = ws.p2; pa.Ap = ws.Ap; pa.x = ws.x;
     pa.mdiag = md;
-    pa.z = ws.z; pa.mblocks = ws.mblocks_fused; pa.mbs = ws.mbs_fused;
+    pa.z = ws.z; pa.mblocks = pl.mblocks; pa.mbs = pl.mbs;
     pa.max_iters = batch;
     pa.timed = o.time_kernels ? 1 : 0;
     if (dist) {
@@ -990,19 +956,19 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, co
       pa.hsnap = hslot(slot);
       pa.hseq = hseq + slot;
       pa.seq = expect[slot] = ++ws.fused_seq;
-      if (kdict) {
-        CsrDict<T> Dcopy = *dict;
+      if (pl.kd) {
+        CsrDict<T> Dcopy = *pl.dict;
         void* args[] = {(void*)&Dcopy, (void*)&pa, (void*)&dst, (void*)&partp, (void*)&gbar};
-        KB_CUDA(cudaLaunchCooperativeKernel((const void*)kdict, dim3(pgrid), dim3(kTileThreads), args, 0, c.stream));
+        KB_CUDA(cudaLaunchCooperativeKernel((const void*)pl.kd, dim3(pl.pgrid), dim3(kTileThreads), args, 0, c.stream));
       } else {
         void* args[] = {(void*)&Acopy, (void*)&pa, (void*)&dst, (void*)&partp, (void*)&gbar, (void*)&dcm};
-        KB_CUDA(cudaLaunchCooperativeKernel((const void*)kp, dim3(pgrid), dim3(kTileThreads), args, A.smem_bytes, c.stream));
+        KB_CUDA(cudaLaunchCooperativeKernel((const void*)pl.kp, dim3(pl.pgrid), dim3(kTileThreads), args, A.smem_bytes, c.stream));
       }
       c.launches += 1;
       enq += batch;
       return;                                   // the kernel reports into pinned host memory itself
     }
-    for (int b = 0; !persist && b < batch; b++, enq++) {
+    for (int b = 0; b < batch; b++, enq++) {
       T* p_old = P[enq & 1];
       T* p_new = P[(enq + 1) & 1];
       const CgPeers<T>& pe = peersP[enq & 1];
@@ -1010,10 +976,9 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, co
       const bool timed = o.time_kernels && ti >= 0 && ti < kTimedCount;
       if (timed) KB_CUDA(cudaEventRecord(tev[3 * ti], c.stream));
       DistComm* dcm = dist ? c.dcomm : nullptr;
-      if (A.tma_ok) k1<<<k1_grid, kTileThreads, A.smem_bytes, c.stream>>>(A, ws.r, p_old, p_new, ws.Ap, dst, part, c.tickets + 2, dcm, pe, ws.x);
-      else k1<<<g1r, kBlock, 0, c.stream>>>(A, ws.r, p_old, p_new, ws.Ap, dst, part, c.tickets + 2, dcm, pe, ws.x);
+      pl.k1<<<pl.k1_grid, pl.k1_block, pl.k1_smem, c.stream>>>(A, ws.r, p_old, p_new, ws.Ap, dst, part, c.tickets + 2, dcm, pe, ws.x);
       if (timed) KB_CUDA(cudaEventRecord(tev[3 * ti + 1], c.stream));
-      k2<<<g2, kBlock, 0, c.stream>>>(n, ws.x, ws.r, p_new, ws.Ap, dst, part, c.tickets + 3, dcm, md, push_r);
+      pl.k2<<<pl.k2_grid, kBlock, 0, c.stream>>>(n, ws.x, ws.r, p_new, ws.Ap, dst, part, c.tickets + 3, dcm, md, push_r);
       if (timed) KB_CUDA(cudaEventRecord(tev[3 * ti + 2], c.stream));
       c.launches += 2;
     }
@@ -1024,6 +989,7 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, co
 
   int cur = 0, seen = 0;   // seen: iterations whose rNorm has been pushed to the history
   St last;
+  bool user_exit = false, overtimed = false;
   enqueue(0);
   for (;;) {
     if (!single_step) enqueue(cur ^ 1);           // keep the GPU busy while the host inspects `cur`
@@ -1077,34 +1043,30 @@ void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, co
   if (last.comm_error) throw std::runtime_error("cross-GPU all-reduce timed out: a peer rank is not participating");
   if (last.not_spd) throw std::runtime_error("The linear operator `A` or the preconditioner `M` is not symmetric positive definite.");
 
-  iter = last.iter;
-  solved = last.solved != 0;
-  tired = last.tired != 0;
-  zero_curvature = last.zero_curvature != 0;
-  inconsistent = last.inconsistent != 0;
+  const int iter = last.iter;
   // Which buffer holds the current direction?  K1 of iteration k writes P[(k+1)&1].
   // Normal exit after K2 of iteration iter-1: p = P[iter & 1].  Exit from K1's
   // curvature test at iteration `iter` (iter not incremented): p = P[(iter+1) & 1].
-  const bool k1_exit = zero_curvature || last.npc;
+  const bool k1_exit = last.zero_curvature || last.npc;
   T* pcur = k1_exit ? P[(iter + 1) & 1] : P[iter & 1];
   if (pcur != ws.p) { T* tmp = ws.p; ws.p = ws.p2; ws.p2 = tmp; ws.dist.swapped = !ws.dist.swapped; }
   // XUP: the x update of the last completed iteration has not been applied yet (the K1 that would have done it
   // saw `done`).  A K1 exit applied its predecessor's update during its own pass, so nothing is pending then.
-  if (xup && !k1_exit && iter > 0) k_axpy<T>(c, n, last.alpha, ws.p, ws.x);
+  if (pl.xup && !k1_exit && iter > 0) k_axpy<T>(c, n, last.alpha, ws.p, ws.x);
   if (last.npc) {                                   // linesearch branch, cg.jl:203-209
     if (iter == 0) k_copy<T>(c, n, ws.x, ws.p);
     k_copy<T>(c, n, ws.npc_dir, ws.p);
     ws.stats.npcCount = 1;
     ws.stats.indefinite = true;
   }
+  return CgFusedExit{iter, last.solved != 0, last.tired != 0, last.zero_curvature != 0, last.inconsistent != 0, user_exit, overtimed};
 }
 
 #define INST(T)                                                                                              \
-  template bool cg_fused_eligible<T>(const LinOp<T>&, const LinOp<T>&, const SolveOpts&);                    \
+  template CgFusedPlan<T> cg_fused_plan<T>(const Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void cg_fused_prepare<T>(Workspace<T>&);                                                          \
   template void cg_dist_push_r<T>(Workspace<T>&);                                                            \
-  template void cg_fused_loop<T>(Workspace<T>&, const Csr<T>&, const CsrDict<T>*, const SolveOpts&, T, T, int, double, \
-                                 bool&, bool&, bool&, bool&, bool&, bool&, int&);
+  template CgFusedExit cg_fused_loop<T>(Workspace<T>&, const CgFusedPlan<T>&, const SolveOpts&, T, T, int, double);
 INST(double)
 INST(float)
 #undef INST

@@ -238,9 +238,7 @@ struct Workspace {
   std::vector<T> err_vec;              // MINRES, LSQR, LSMR window
   int memory = 20, window = 5;
   int inner_iter = 0;
-  const T* mdiag_fused = nullptr;      // diagonal of M for the fused CG kernels (set per solve; nullptr: M = I)
-  const T* mblocks_fused = nullptr;    // block-Jacobi M for the persistent CG kernel (set per solve; nullptr: none)
-  int mbs_fused = 0;
+  const T* mdiag_fused = nullptr;      // diagonal of M for the fused phases (set per solve; nullptr: M = I)
   double k1_ms = 0, k2_ms = 0;         // average event-timed duration of the fused kernels (time_kernels)
   int timed_pairs = 0;
   void* fused_state = nullptr;         // device scalar block of the fused paths
@@ -309,16 +307,43 @@ template <class T> void cgls_solve(Workspace<T>& ws, const LinOp<T>& A, const Li
 template <class T> void crls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const SolveOpts& o);
 
-// Fused CG (cg_fused.cu).  Returns false if the configuration is not eligible
-// (caller falls back to the generic primitive path, still on the GPU).
-template <class T> bool cg_fused_eligible(const LinOp<T>& A, const LinOp<T>& M, const SolveOpts& o);
+// Fused CG (cg_fused.cu).  cg_fused_plan decides once whether and how a solve runs fused: fused == false sends it
+// to the generic primitive path (still on the GPU); otherwise the plan holds everything cg_fused_loop launches.
+template <class T> struct CgState;
+template <class T> struct CgPeers;
+template <class T> struct CgPersistArgs;
+struct GridBar;
+template <class T>
+struct CgFusedPlan {
+  typedef void (*K1Fn)(Csr<T>, const T*, const T*, T*, T*, CgState<T>*, T*, unsigned*, DistComm*, CgPeers<T>, T*);
+  typedef void (*K2Fn)(int, T*, T*, const T*, const T*, CgState<T>*, T*, unsigned*, DistComm*, const T*, PushPlan<T>);
+  typedef void (*KpFn)(Csr<T>, CgPersistArgs<T>, CgState<T>*, T*, GridBar*, DistComm*);
+  typedef void (*KdFn)(CsrDict<T>, CgPersistArgs<T>, CgState<T>*, T*, GridBar*);
+  bool fused = false;
+  bool persist = false;         // one cooperative launch per batch of iterations; false: K1 + K2 per iteration
+  bool single_step = false;     // callback, verbose or timemax: x is current and the stream idle after every iteration
+  bool xup = false;             // x += alpha p rides in the next K1 / phase A (else in K2)
+  int batch = 1;                // iterations per launch / host poll
+  const Csr<T>* A = nullptr;
+  const T* mdiag = nullptr;     // Jacobi M (nullptr: none)
+  const T* mblocks = nullptr;   // block-Jacobi M: dense mbs x mbs diagonal blocks, row-major (nullptr: none)
+  int mbs = 0;
+  K1Fn k1 = nullptr;            // two-launch kernels and their launch shapes
+  K2Fn k2 = nullptr;
+  int k1_grid = 0, k1_block = 0, k2_grid = 0;
+  size_t k1_smem = 0;
+  KpFn kp = nullptr;            // persistent kernel on CSR ...
+  KdFn kd = nullptr;            // ... or on the operator's encoding `dict` (nullptr: CSR)
+  const CsrDict<T>* dict = nullptr;
+  int pgrid = 0;
+};
+struct CgFusedExit { int iter; bool solved, tired, zero_curvature, inconsistent, user_exit, overtimed; };
+template <class T> CgFusedPlan<T> cg_fused_plan(const Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& M, const SolveOpts& o);
+template <class T> CgFusedExit cg_fused_loop(Workspace<T>& ws, const CgFusedPlan<T>& plan, const SolveOpts& o, T gamma0, T eps_tol,
+                                             int itmax, double start_time);
 template <class T> void cg_dist_push_r(Workspace<T>& ws);
 template <class T> void cg_fused_prepare(Workspace<T>& ws);   // device/pinned scalar blocks, p2, events (ws_create)
 constexpr size_t kFusedBlockBytes = 4096;
-// dict: the operator's encoding (nullptr or npairs == 0: CSR only); the single-GPU persistent kernel runs on it
-template <class T> void cg_fused_loop(Workspace<T>& ws, const Csr<T>& A, const CsrDict<T>* dict, const SolveOpts& o, T gamma0,
-                                      T eps_tol, int itmax, double start_time, bool& solved, bool& tired, bool& zero_curvature,
-                                      bool& inconsistent, bool& user_exit, bool& overtimed, int& iter);
 
 // Fused iteration phases of BiCGSTAB / MINRES / GMRES (fused_phases.cu); eligible when A is a CSR operator,
 // M = N = I (and for GMRES no reorthogonalization).

@@ -136,7 +136,6 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   if (ws.warm_start && linesearch) throw std::runtime_error("warm_start and linesearch cannot be used together");
   if (o.verbose > 0) printf("CG: system of %d equations in %d variables\n", n, n);
   const bool MisI = M.is_identity();
-  const bool dist = ws.dist.world > 1;
   allocate_if(!MisI, ws, ws.z);
   allocate_if(linesearch || radius > 0, ws, ws.npc_dir);
   T *dx = ws.dx, *x = ws.x, *r = ws.r, *Ap = ws.Ap;
@@ -175,14 +174,12 @@ void cg_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   bool inconsistent = false, on_boundary = false, zero_curvature = false, user_exit = false, overtimed = false;
   std::string status = "unknown";
 
-  // row-partitioned: the fused kernels cover M = I; everything else runs the primitive path, whose SpMV is
-  // preceded by the general halo exchange and whose dots end in the in-kernel all-reduce
-  if (cg_fused_eligible(A, M, o) && !(dist && !MisI) && !(solved || tired)) {
-    ws.mdiag_fused = (MisI || M.kind != LinOp<T>::DIAG) ? nullptr : M.diag;   // Diagonal M: applied inside K1/K2 (z is not materialised)
-    ws.mblocks_fused = M.kind == LinOp<T>::BDIAG ? M.blocks : nullptr;        // block-Jacobi M: z = M r materialised in phase B
-    ws.mbs_fused = M.kind == LinOp<T>::BDIAG ? M.bs : 0;
-    cg_fused_loop<T>(ws, *A.csr, A.dict, o, gamma, eps_tol, itmax, run.start, solved, tired, zero_curvature, inconsistent,
-                     user_exit, overtimed, iter);
+  const CgFusedPlan<T> plan = (solved || tired) ? CgFusedPlan<T>() : cg_fused_plan<T>(ws, A, M, o);
+  if (plan.fused) {
+    const CgFusedExit e = cg_fused_loop<T>(ws, plan, o, gamma, eps_tol, itmax, run.start);
+    iter = e.iter;
+    solved = e.solved; tired = e.tired; zero_curvature = e.zero_curvature; inconsistent = e.inconsistent;
+    user_exit = e.user_exit; overtimed = e.overtimed;
   } else {
     T* p = ws.p;
     while (!(solved || tired || zero_curvature || user_exit || overtimed)) {

@@ -319,7 +319,7 @@ __device__ __forceinline__ void tile_drain(const TilePipe<T>& P, unsigned consum
 
 // Consumers (threads 0 .. kTileRows-1): tiles j0 <= j < j1 of this CTA's sequence (a pass is one call with
 // [0, cnt), or two calls when something must happen between the interior tiles and the halo tiles).
-template <class T, int DEPTH, class TileAt, class Gather, class RowBegin, class RowDone>
+template <class T, class TileAt, class Gather, class RowBegin, class RowDone>
 __device__ __forceinline__ void tile_consume_pass(const Csr<T>& A, const TilePipe<T>& P, unsigned& cpos, int j0, int j1, TileAt tile_at,
                                                   Gather gather, RowBegin row_begin, RowDone row_done) {
   constexpr int VA = 16 / sizeof(T);
@@ -343,18 +343,18 @@ __device__ __forceinline__ void tile_consume_pass(const Csr<T>& A, const TilePip
       // The gathers here are plain (coherent) loads, which the compiler will not speculate: guarded loads would
       // be chained load -> use -> load.  Clamp the index instead (every address is valid) and select the sum, so
       // the batch is straight-line code and all gathers of a row are issued together.
-      for (int k = kb; k < ke; k += DEPTH) {
-        T xv[DEPTH], av[DEPTH];
+      for (int k = kb; k < ke; k += kGatherDepth) {
+        T xv[kGatherDepth], av[kGatherDepth];
 #pragma unroll
-        for (int u = 0; u < DEPTH; u++) xv[u] = gather(crow[min(k + u, ke - 1)]);
+        for (int u = 0; u < kGatherDepth; u++) xv[u] = gather(crow[min(k + u, ke - 1)]);
         asm volatile("" ::: "memory");        // keep the gathers above everything else (the optimiser would sink them)
         // the matrix values come from shared memory (short latency): fetch them only now, so that the registers
         // of the batch hold gathered data instead -- at 72 registers per thread that is the difference between
         // 2 and 8 global loads in flight
 #pragma unroll
-        for (int u = 0; u < DEPTH; u++) av[u] = vrow[min(k + u, ke - 1)];
+        for (int u = 0; u < kGatherDepth; u++) av[u] = vrow[min(k + u, ke - 1)];
 #pragma unroll
-        for (int u = 0; u < DEPTH; u++) {
+        for (int u = 0; u < kGatherDepth; u++) {
           const T nx = add_rn(acc, mul_rn(av[u], xv[u]));
           acc = (k + u < ke) ? nx : acc;
         }

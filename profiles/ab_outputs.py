@@ -9,7 +9,8 @@ tree's build), the libraries alternating chunk by chunk.
 Prints the differences and exits 1 when any configuration differs.  The configurations cover the 13 single
 right-hand-side solvers with the fused paths on and off: diagonal M and N, ldiv, warm starts, restart and growth past
 `memory`, reorthogonalization, b = 0, itmax = 3, a callback exit, timemax = 0, the solver-specific exits and Float32,
-and CG on a constant-coefficient operator (the path of the CsrDict encoding, M = I and a diagonal M, both types).
+and CG on a constant-coefficient operator (the path of the CsrDict encoding, M = I and a diagonal M, both types), CG's
+two-launch kernels (fused = 2), a block-Jacobi M and the in-kernel phase timing (time_kernels).
 """
 import json
 import os
@@ -104,6 +105,10 @@ def configs():
         add("cg", "dg", dtype=dtype)
         add("cg", "dg", dtype=dtype, M="pos")
         add("cg", "dg", dtype=dtype, itmax=40, atol=0.0, rtol=0.0)
+        for prob in ("lap", "dg"):                  # the two-launch kernels
+            out.append(dict(solver="cg", prob=prob, kw=dict(dtype=dtype, fused=2)))
+    add("cg", "lap", M="bj4")                       # block-Jacobi M, (54, 4, 4) blocks
+    add("cg", "dg", time_kernels=True)
     add("cg", "indef", linesearch=True)
     add("cg", "lap", radius=0.5)
     add("cg", "indef12", radius=5.0)
@@ -155,7 +160,8 @@ def run_chunk(lo, hi, path):
             b = np.zeros_like(b)
         diag = A.diagonal()
         vec = {"d": lambda: 1.0 / diag, "sd": lambda: 1.0 / np.sqrt(diag),
-               "pos": lambda ln: np.linspace(0.5, 2.0, ln)}
+               "pos": lambda ln: np.linspace(0.5, 2.0, ln),
+               "bj4": lambda: np.linalg.inv(np.stack([A[k:k + 4, k:k + 4].toarray() for k in range(0, n, 4)]))}
         for which, ln in (("M", m), ("N", n)):
             if which in kw:
                 kw[which] = vec["pos"](ln) if kw[which] == "pos" else vec[kw[which]]()

@@ -103,12 +103,12 @@ def test_persistent_cg_register_budget_and_coherent_loads():
     appear for the matrix structure / tile order, which are 32-bit loads)."""
     ents = _entries("cg_fused")
     dm = _demangle([e[0] for e in ents])
-    hit = [(dm[n], r, s) for n, r, s in ents if re.search(r"cg_persist<double, \d, 3, ", dm[n])]      # the 3-CTA/SM variants
+    hit = [(dm[n], r, s) for n, r, s in ents if re.search(r"cg_persist<double, \d, 3>", dm[n])]      # the 3-CTA/SM variants
     assert len(hit) >= 3
     for name, regs, spill in hit:
         assert regs <= 72 and spill == 0, (name, regs, spill)
     for mode in (0, 1):
-        body = _sass_of("cg_fused", f"cg_persistIdLi{mode}ELi3ELi8")
+        body = _sass_of("cg_fused", f"cg_persistIdLi{mode}ELi3E")
         # row-partitioned variant: the communicator's constants (mailbox pointer, spin budget; dist.cuh) are 64-bit
         # read-only loads, two per barrier -- nothing else may be
         allowed = 0 if mode == 0 else 4
@@ -128,8 +128,8 @@ def test_gather_batches_keep_loads_in_flight():
             elif "DMUL" in l or "DADD" in l or "DFMA" in l:
                 cur = 0
         return best
-    assert longest_run(_sass_of("cg_fused", "cg_persistIdLi0ELi3ELi8")) >= 6
-    assert longest_run(_sass_of("cg_fused", "cg_persistIdLi1ELi3ELi8")) >= 6       # row-partitioned variant
+    assert longest_run(_sass_of("cg_fused", "cg_persistIdLi0ELi3E")) >= 6
+    assert longest_run(_sass_of("cg_fused", "cg_persistIdLi1ELi3E")) >= 6       # row-partitioned variant
     assert longest_run(_sass_of("cg_fused", "cg_k1_tmaIdLi0ELi3ELb1")) >= 6
     assert longest_run(_sass_of("spmv", "spmv_tma_kernelIdLb0ENS_6XPlain")) >= 6
 

@@ -49,6 +49,23 @@ def test_cg_block_jacobi_fused_matches_oracle(kb, O, bs):
     ws.free()
 
 
+def test_cg_block_jacobi_without_x_update_in_k1_falls_back(kb, O, monkeypatch):
+    """KB200_XUP=0 rules out the persistent kernel, the only fused kernel that carries a block-Jacobi M: the solve
+    must take the primitive path (same iterations, status and x as fused=False) instead of failing."""
+    A, b = O.sparse_laplacian(12)
+    A = sp.csr_matrix(A + sp.diags(np.linspace(0.0, 2.0, A.shape[0])))
+    n = A.shape[0]
+    Minv = np.linalg.inv(_diag_blocks(A, 4))
+    ws = kb.CgWorkspace(n, n, np.float64)
+    ws.solve(A, b, M=Minv, atol=0.0, rtol=1e-10, fused=False)
+    ref = (ws.stats.niter, ws.stats.status, np.array(ws.x))
+    monkeypatch.setenv("KB200_XUP", "0")
+    ws.solve(A, b, M=Minv, atol=0.0, rtol=1e-10, fused=True)
+    assert (ws.stats.niter, ws.stats.status) == ref[:2]
+    assert np.array_equal(ws.x, ref[2])
+    ws.free()
+
+
 def test_block_jacobi_ldiv_and_other_solvers(kb, O):
     Ak, bk = O.kron_unsymmetric(9)                       # n = 729 = 3^6: ragged last block for bs = 4, 8
     Ak = sp.csr_matrix(Ak + sp.diags(np.linspace(0.0, 3.0, Ak.shape[0])))
