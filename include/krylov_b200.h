@@ -43,9 +43,11 @@ typedef enum { KRYLOV_FLOAT32 = 0, KRYLOV_FLOAT64 = 1, KRYLOV_COMPLEX32 = 2, KRY
 typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
 
 /* positional, frozen (krylov.h:48-83).  Implemented here: CG, MINRES, GMRES, BICGSTAB (the hot path), the
- * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, and the least-squares solvers LSQR,
- * LSMR, LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a
- * CSR operator of m rows and n columns is attached); every other value returns -2. */
+ * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, BILQ and QMR on a square operator and
+ * its adjoint (matvec_At with matvec_A, or the transpose of an attached CSR operator; `c` is accepted, default b), and
+ * the least-squares solvers LSQR, LSMR, LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A
+ * maps n -> m and matvec_At m -> n, or a CSR operator of m rows and n columns is attached); every other value returns
+ * -2. */
 typedef enum {
   KRYLOV_CG = 0, KRYLOV_CR = 1, KRYLOV_SYMMLQ = 2, KRYLOV_MINRES = 3, KRYLOV_MINRES_QLP = 4, KRYLOV_DIOM = 5,
   KRYLOV_DQGMRES = 6, KRYLOV_FOM = 7, KRYLOV_GMRES = 8, KRYLOV_FGMRES = 9, KRYLOV_BICGSTAB = 10, KRYLOV_CGS = 11,
@@ -135,7 +137,8 @@ const char *krylov_b200_last_error(void);
  * cg.jl:196, gmres.jl:257, bicgstab.jl:221,228, minres.jl:289.
  *   rowptr[n+1], colind[nnz], values[nnz] (element type = workspace dtype);
  *   least-squares workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
- *   the library forms A^T once (host-side) on the first solve and keeps it until the operator changes;
+ *   least-squares, BiLQ and QMR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
+ *   until the operator changes;
  *   index_base 0|1, index_bytes 4|8 (Julia's SparseMatrixCSC{T,Int64} passes
  *   1 and 8 -- for a symmetric matrix its CSC arrays ARE the CSR arrays);
  *   location 0 = host arrays, 1 = device arrays.
@@ -182,6 +185,7 @@ typedef struct {
   double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0                       */
   double utol;         /* LSLQ: kwarg `utol`; NaN -> sqrt(eps)                                                       */
   int transfer_to_lsqr; /* LSLQ: 1 -> return the LSQR point (kwarg `transfer_to_lsqr`)                                */
+  int transfer_to_bicg; /* BiLQ: 1 (default) -> return the BiCG point when it converges first (kwarg `transfer_to_bicg`) */
 } KrylovB200Options;
 KrylovB200Options krylov_b200_default_options(void);
 int krylov_b200_set_options(void *ws, const KrylovB200Options *opts);

@@ -42,7 +42,7 @@ struct Handle {
   int p = 0;
   void* ws = nullptr;
   std::shared_ptr<CsrAny> csr;
-  std::shared_ptr<CsrAny> csrT;        // least squares: A^T of the attached operator, built on first use ...
+  std::shared_ptr<CsrAny> csrT;        // least squares, BiLQ, QMR: A^T of the attached operator, built on first use ...
   const CsrAny* csrT_for = nullptr;    // ... for this operator
   void* Mdiag = nullptr;
   void* Ndiag = nullptr;
@@ -79,7 +79,7 @@ int fail(const char* where, const char* msg) {
 bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
          s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
-         s == S_LSLQ || s == S_CGLS || s == S_CRLS;
+         s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR;
 }
 
 int pick_device() {
@@ -115,6 +115,7 @@ int m_of(Handle* h) {
 }
 bool is_ls(const Handle* h) { return !h->block && is_ls_kind(h->solver); }
 bool is_cg_ls(int s) { return s == S_CGLS || s == S_CRLS; }     // CGLS / CRLS: M on the residual space, no N
+bool is_biorth(int s) { return s == S_BILQ || s == S_QMR; }      // BiLQ / QMR: square, apply A and its adjoint
 template <class T> Csr<T>& csr_of(CsrAny& a);
 template <> Csr<double>& csr_of<double>(CsrAny& a) { return a.d; }
 template <> Csr<float>& csr_of<float>(CsrAny& a) { return a.f; }
@@ -183,6 +184,7 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   s.sigma = std::isnan(h->ext.sigma) ? 0 : h->ext.sigma;
   s.utol = std::isnan(h->ext.utol) ? -1 : h->ext.utol;
   s.transfer_to_lsqr = h->ext.transfer_to_lsqr != 0;
+  s.transfer_to_bicg = h->ext.transfer_to_bicg != 0;
   // _typed_solve_gmres! serves GMRES, FGMRES and FOM (c_stores.jl:376-398)
   if (h->solver == S_GMRES || h->solver == S_FGMRES || h->solver == S_FOM) {
     s.restart = o->restart != 0; s.reorthogonalization = o->reorthogonalization != 0;
@@ -214,6 +216,16 @@ std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src) {
   return a;
 }
 
+// A^T of the handle's CSR operator, formed once per attached operator and kept on the handle until it changes
+template <class T> const Csr<T>* adjoint_csr(Handle* h, Workspace<T>* ws) {
+  if (!h->csrT || h->csrT_for != h->csr.get()) {
+    h->csrT.reset();
+    h->csrT = transpose_any(ws->ctx, *h->csr);
+    h->csrT_for = h->csr.get();
+  }
+  return &csr_of<T>(*h->csrT);
+}
+
 // lsqr! / lsmr! (c_stores.jl:403-423), cgls! / crls! (_typed_solve_ls_m_radius!): b has m entries, x has n; A maps
 // n -> m and needs its adjoint
 template <class T>
@@ -237,13 +249,8 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
       throw std::runtime_error("CSR operator: size inconsistent with the workspace ((m, n) = (" + std::to_string(m) + ", " +
                                std::to_string(n) + "), operator rows = " + std::to_string(C.n) + ", largest column = " +
                                std::to_string(C.max_col) + ")");
-    if (!h->csrT || h->csrT_for != h->csr.get()) {
-      h->csrT.reset();
-      h->csrT = transpose_any(ws->ctx, *h->csr);
-      h->csrT_for = h->csr.get();
-    }
     A.kind = LinOp<T>::CSR; A.csr = &C; A.n = m;
-    At.kind = LinOp<T>::CSR; At.csr = &csr_of<T>(*h->csrT); At.n = n;
+    At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = n;
   } else {
     throw std::runtime_error("no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr");
   }
@@ -267,8 +274,8 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
 }
 
 template <class T>
-int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fM, KrylovMatvec fN, const void* b, const void* c, void* ud,
-             const KrylovOptions* opts) {
+int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, const void* c,
+             void* ud, const KrylovOptions* opts) {
   Workspace<T>* ws = W<T>(h);
   KB_CUDA(cudaSetDevice(ws->ctx.device));
   SolveOpts so = map_opts(h, opts);
@@ -311,6 +318,23 @@ int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fM, KrylovMatvec fN, const
       // the reference's C layer never forwards `c` for BiCGSTAB (c = b); we accept it when given
       const T* cd = stage_in<T>(h, ws, c, ws->cbuf);
       bicgstab_solve<T>(*ws, A, bd, cd, M, N, so);
+      break;
+    }
+    case S_BILQ: case S_QMR: {
+      // the adjoint: matvec_At with matvec_A, else the cached transpose of the CSR operator
+      LinOp<T> At;
+      if (fA) {
+        if (!fAt) throw std::runtime_error("bilq and qmr apply the adjoint of A: matvec_At must be given with matvec_A");
+        At = make_cb_op<T>(h, ws, fAt, ud);
+      } else {
+        At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = ws->n;
+      }
+      if (M.kind == LinOp<T>::BDIAG || N.kind == LinOp<T>::BDIAG)
+        throw std::runtime_error("bilq and qmr apply M^H and N^H: block-Jacobi preconditioners are not available for them");
+      // like BiCGSTAB's, `c` is accepted when given (the reference's C layer never forwards it: c = b)
+      const T* cd = stage_in<T>(h, ws, c, ws->cbuf);
+      if (h->solver == S_BILQ) bilq_solve<T>(*ws, A, At, bd, cd, M, N, so);
+      else qmr_solve<T>(*ws, A, At, bd, cd, M, N, so);
       break;
     }
   }
@@ -364,6 +388,11 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
   if (!strcmp(nm, "Mr") || !strcmp(nm, "Ms")) return ws->Mr;
   if (!strcmp(nm, "Mq")) return ws->kind == S_CGLS ? ws->Mr : ws->z;   // CGLS: Mq aliases Mr (cgls.jl:156)
   if (!strcmp(nm, "w̄") || !strcmp(nm, "wbar")) return ws->kind == S_LSLQ ? ws->w : nullptr;
+  if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ ? ws->w : nullptr;
+  if (!strcmp(nm, "uₖ₋₁") || !strcmp(nm, "u_prev")) return ws->u_prev;      // BiLQ / QMR (rotated by pointer)
+  if (!strcmp(nm, "vₖ₋₁") || !strcmp(nm, "v_prev")) return ws->v_prev;
+  if (!strcmp(nm, "uₖ")) return ws->u;
+  if (!strcmp(nm, "vₖ")) return ws->v;
   if (nm[0] == 'Z') { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->Z.size()) return ws->Z[i - 1]; return nullptr; }
   if (nm[0] == 'V') { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->V.size()) return ws->V[i - 1]; }
   return nullptr;
@@ -422,8 +451,8 @@ int krylov_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, Krylov
     if (is_ls(h))                    // the square solvers never apply the adjoint
       return h->dtype == KRYLOV_FLOAT64 ? do_solve_ls<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts)
                                         : do_solve_ls<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts);
-    return h->dtype == KRYLOV_FLOAT64 ? do_solve<double>(h, matvec_A, matvec_M, matvec_N, b, c, userdata, opts)
-                                      : do_solve<float>(h, matvec_A, matvec_M, matvec_N, b, c, userdata, opts);
+    return h->dtype == KRYLOV_FLOAT64 ? do_solve<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts)
+                                      : do_solve<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts);
   } catch (const std::exception& e) { return fail("krylov_solve", e); }
 }
 
@@ -734,7 +763,7 @@ KrylovB200Options krylov_b200_default_options(void) {
   KrylovB200Options o;
   memset(&o, 0, sizeof(o));
   o.etol = NAN; o.conlim = NAN; o.fused = 1; o.cr_gamma = NAN; o.axtol = NAN; o.btol = NAN;
-  o.sigma = 0.0; o.utol = NAN; o.transfer_to_lsqr = 0;
+  o.sigma = 0.0; o.utol = NAN; o.transfer_to_lsqr = 0; o.transfer_to_bicg = 1;
   return o;
 }
 
@@ -930,6 +959,8 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_b200_dist_init", "unknown workspace handle");
     if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) solves are not available");
+    if (is_biorth(h->solver))        // A^T of a row block needs the column halo of A, not its row halo
+      return fail("krylov_b200_dist_init", "row-partitioned BiLQ / QMR solves are not available");
     return h->dtype == KRYLOV_FLOAT64 ? dist_init_t<double>(h, rank, world, nhalo, halo_rank, halo_off)
                                       : dist_init_t<float>(h, rank, world, nhalo, halo_rank, halo_off);
   } catch (const std::exception& e) { return fail("krylov_b200_dist_init", e); }

@@ -882,6 +882,131 @@ void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, b
   *ArAr = H[1].ArAr; *xx = H[1].xx; *rr = H[1].rr; *gamma_out = H[1].gamma;
 }
 
+// ===========================================================================
+// BiLQ / QMR  (src/bilq.jl:234-254,310-335, src/qmr.jl:238-258,314-350, M = N = I)
+// One Lanczos biorthogonalization step is two SpMV launches: B1's Fin leaves alpha in the device block, B2 reads it and
+// its Fin stores <p, q>; the host reads {alpha, <p, q>} once, runs the factorization, and one streaming pass U applies
+// the direction / solution update and forms v_{k+1}, u_{k+1} in the buffers of v_{k-1}, u_{k-1} (the caller rotates
+// the pointers).  When <p, q> = 0 the reference keeps v_k and u_k: U then copies them instead of dividing.
+// ===========================================================================
+template <class T> struct BiorthState { T alpha, pq; };
+
+template <class T> struct BiorthB1Epi {   // q = A v - gamma v_{k-1} ; <u, q>          (bilq.jl:236,244,247)
+  T* q; const T* vprev; const T* u; T gamma;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T qn = add_rn(acc, mul_rn(-gamma, vprev[row]));
+    q[row] = qn;
+    d[0] += u[row] * qn;
+  }
+};
+template <class T> struct BiorthB1Fin {
+  BiorthState<T>* s;
+  __device__ void operator()(const T* tot) const { s->alpha = tot[0]; }
+};
+template <class T> struct BiorthB2Epi {   // p = A^T u - beta u_{k-1} - alpha u ; q -= alpha v ; <p, q>   (:241,245,249-252)
+  T* p; T* q; const T* uprev; const T* u; const T* v; const BiorthState<T>* s; T beta;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T alpha = s->alpha;
+    const T pn = add_rn(add_rn(acc, mul_rn(-beta, uprev[row])), mul_rn(-alpha, u[row]));
+    const T qn = add_rn(q[row], mul_rn(-alpha, v[row]));
+    p[row] = pn;
+    q[row] = qn;
+    d[0] += pn * qn;
+  }
+};
+template <class T> struct BiorthB2Fin {
+  BiorthState<T>* s;
+  __device__ void operator()(const T* tot) const { s->pq = tot[0]; }
+};
+// v_{k+1} = q / beta_{k+1}, u_{k+1} = p / gamma_{k+1} into the rotated buffers (kdivcopy!: true divisions)
+template <class T> struct BiorthNext {
+  T* vnext; T* unext; const T* q; const T* p; const T* v; const T* u; T beta1, gamma1; int keep;
+  __device__ __forceinline__ T operator()(int i) const {
+    if (keep) { unext[i] = u[i]; return vnext[i] = v[i]; }
+    unext[i] = div_rn(p[i], gamma1);
+    return vnext[i] = div_rn(q[i], beta1);
+  }
+};
+// QMR (qmr.jl:316-350): w_k = (v - lambda w_{k-1} - eps w_{k-2}) / delta in the kscal!/kaxpy!/kdiv! order (first
+// iteration: w_1 = v / delta into w_{k-1}); x += zeta w_k; the next v, u; ||v_{k+1}||^2 (tau).
+template <class T, bool FIRST> struct BiorthQmrBody {   // FIRST: iteration 1 (its own instantiation: no spill)
+  T* wk; const T* w1; T* x; const T* v; BiorthNext<T> nx; T eps2, lambda, inv_delta, delta, zeta; int iter;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    const T vi = v[i];
+    T w;
+    if (FIRST) {
+      w = div_rn(vi, delta);
+    } else {
+      w = wk[i];
+      if (iter >= 3) w = mul_rn(-eps2, w);
+      w = add_rn(w, mul_rn(-lambda, w1[i]));
+      w = add_rn(w, mul_rn(T(1), vi));
+      w = mul_rn(inv_delta, w);
+    }
+    wk[i] = w;
+    x[i] = add_rn(x[i], mul_rn(zeta, w));
+    const T vn = nx(i);
+    d[0] += vn * vn;
+  }
+};
+// BiLQ (bilq.jl:310-335): d̅ = v on the first iteration, else x += (zeta c) d̅, x += (zeta s) v, d̅ = -c v + s d̅;
+// the next v, u; <v_k, v_{k+1}> and ||v_{k+1}||^2.
+template <class T> struct BiorthBilqBody {
+  T* dbar; T* x; const T* v; BiorthNext<T> nx; T czeta, szeta, c, s; int first;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    const T vi = v[i];
+    if (first) {
+      dbar[i] = vi;
+    } else {
+      const T di = dbar[i];
+      x[i] = add_rn(add_rn(x[i], mul_rn(czeta, di)), mul_rn(szeta, vi));
+      dbar[i] = add_rn(mul_rn(-c, vi), mul_rn(s, di));
+    }
+    const T vn = nx(i);
+    d[0] += vi * vn; d[1] += vn * vn;
+  }
+};
+
+template <class T>
+void biorth_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, T beta, T gamma, T* alpha, T* pq) {
+  Ctx& c = ws.ctx;
+  typedef BiorthState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.v}, BiorthB1Epi<T>{ws.q, ws.v_prev, ws.u, gamma}, BiorthB1Fin<T>{S}, 4);
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.u}, BiorthB2Epi<T>{ws.p, ws.q, ws.u_prev, ws.u, ws.v, S, beta},
+                          BiorthB2Fin<T>{S}, 4);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  c.sync();
+  *alpha = H[1].alpha; *pq = H[1].pq;
+}
+
+template <class T>
+T qmr_fused_update(Workspace<T>& ws, T* wk, const T* w1, int iter, T eps2, T lambda, T delta, T zeta, T beta1, T gamma1,
+                   bool keep) {
+  Ctx& c = ws.ctx;
+  const BiorthNext<T> nx{ws.v_prev, ws.u_prev, ws.q, ws.p, ws.v, ws.u, beta1, gamma1, keep ? 1 : 0};
+  if (iter == 1)
+    launch_stream<T, 1>(c, ws.n, BiorthQmrBody<T, true>{wk, w1, ws.x, ws.v, nx, eps2, lambda, T(1) / delta, delta, zeta, iter},
+                        StoreFin<T, 1>{sib_slots<T>(c)}, 5);
+  else
+    launch_stream<T, 1>(c, ws.n, BiorthQmrBody<T, false>{wk, w1, ws.x, ws.v, nx, eps2, lambda, T(1) / delta, delta, zeta, iter},
+                        StoreFin<T, 1>{sib_slots<T>(c)}, 5);
+  T out[1]; sib_read<T, 1>(c, out);
+  return out[0];
+}
+
+template <class T>
+void bilq_fused_update(Workspace<T>& ws, bool first, T czeta, T szeta, T cs, T sn, T beta1, T gamma1, bool keep, T* vv1,
+                       T* v1v1) {
+  Ctx& c = ws.ctx;
+  const BiorthNext<T> nx{ws.v_prev, ws.u_prev, ws.q, ws.p, ws.v, ws.u, beta1, gamma1, keep ? 1 : 0};
+  launch_stream<T, 2>(c, ws.n, BiorthBilqBody<T>{ws.w, ws.x, ws.v, nx, czeta, szeta, cs, sn, first ? 1 : 0},
+                      StoreFin<T, 2>{sib_slots<T>(c)}, 5);
+  T out[2]; sib_read<T, 2>(c, out);
+  *vv1 = out[0]; *v1v1 = out[1];
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -904,7 +1029,10 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template T lsq_fused_update<T>(Workspace<T>&, bool, bool, T, T, T, T);                                             \
   template void lslq_fused_update<T>(Workspace<T>&, bool, T, T, T, T, T);                                          \
   template void cgls_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T*, T*);            \
-  template void crls_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T, T*, T*, T*, T*);
+  template void crls_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T, T*, T*, T*, T*);   \
+  template void biorth_fused_lanczos<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, T, T, T*, T*);                  \
+  template T qmr_fused_update<T>(Workspace<T>&, T*, const T*, int, T, T, T, T, T, T, bool);                          \
+  template void bilq_fused_update<T>(Workspace<T>&, bool, T, T, T, T, T, T, bool, T*, T*);
 INST(double)
 INST(float)
 #undef INST

@@ -10,6 +10,7 @@
 //   siblings.cu   cgs!, cg_lanczos!, dqgmres!, diom!, cr! on the same kernels (SURVEY.md 8f-3)
 //   solver_common.h  host helpers of the drivers, among them SolveRun: the callback / clock / exit protocol
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
+//   biorth.cu     host control flow of bilq!/qmr! (one Lanczos biorthogonalization driver; A and A^T)
 //   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! on rectangular operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
@@ -175,6 +176,7 @@ struct SolveOpts {
   double axtol = -1, btol = -1;     // LSQR, LSMR (<0 => sqrt(eps(T))); btol: LSLQ too
   double sigma = 0, utol = -1;      // LSLQ: σ (Gauss-Radau bounds when > 0), utol (<0 => sqrt(eps(T)))
   bool transfer_to_lsqr = false;    // LSLQ
+  bool transfer_to_bicg = true;     // BiLQ
   bool restart = false;             // GMRES, FOM, FGMRES
   bool reorthogonalization = false; // GMRES, FOM, FGMRES
   bool check_curvature = false;     // CG-Lanczos
@@ -206,7 +208,7 @@ struct Stats {
 
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
-                  S_CGS = 11, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25, S_CG_LANCZOS = 100 };
+                  S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25, S_CG_LANCZOS = 100 };
 // the least-squares solvers: A is m x n, b has m entries and x has n
 inline bool is_ls_kind(int k) { return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS; }
 
@@ -230,6 +232,7 @@ struct Workspace {
   T *Mv = nullptr, *Mv_prev = nullptr, *Mv_next = nullptr;                            // CG-Lanczos (+ p, vv)
   T *Nv = nullptr, *Mu = nullptr, *Av = nullptr, *Atu = nullptr;                     // LSQR / LSMR (+ w, u, v; Mu, Av, u: m)
   T *h = nullptr, *hbar = nullptr;                                                   // LSMR
+  T *u_prev = nullptr, *v_prev = nullptr;                                             // BiLQ / QMR (+ u, v, q, p; w1, w2 / w)
   T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
                                        // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
   std::vector<T*> V;
@@ -387,6 +390,23 @@ template <class T> void cgls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, 
 // One read-back: <Ar, Ar>, <x, x>, <r, r> and gamma.  `init`: first iteration, sets alpha and gamma from the host.
 template <class T> void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, T gamma,
                                              T lambda, T* ArAr, T* xx, T* rr, T* gamma_out);
+// BiLQ / QMR (fused_phases.cu), M = N = I, A and A^T CSR operators.  One Lanczos biorthogonalization step: B1 (SpMV on A
+// gathering v: q = A v - gamma v_prev, alpha = <u, q> on the device) and B2 (SpMV on A^T gathering u: p = A^T u -
+// beta u_prev - alpha u, q -= alpha v, <p, q>), then one read-back of {alpha, <p, q>}.
+template <class T> void biorth_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, T beta, T gamma, T* alpha, T* pq);
+// QMR's update pass: w_k (into wk; w1 = w_{k-1}), x += zeta w_k, v_prev = q / beta1 and u_prev = p / gamma1 (keep: copies of
+// v and u); returns ||v_prev||^2.  The caller then swaps v / v_prev and u / u_prev.
+template <class T> T qmr_fused_update(Workspace<T>& ws, T* wk, const T* w1, int iter, T eps2, T lambda, T delta, T zeta, T beta1,
+                                      T gamma1, bool keep);
+// BiLQ's update pass (d̅ in ws.w): d̅ = v when first, else x += czeta d̅ + szeta v, d̅ = -c v + s d̅; the next v, u as for QMR;
+// returns <v, v_next> and ||v_next||^2.
+template <class T> void bilq_fused_update(Workspace<T>& ws, bool first, T czeta, T szeta, T c, T s, T beta1, T gamma1, bool keep,
+                                          T* vv1, T* v1v1);
+// bilq! / qmr! (biorth.cu): square A with its adjoint At (a CSR operator holding A^T, or a callback); c = nullptr: c = b.
+template <class T> void bilq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const T* c,
+                                   const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
+template <class T> void qmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const T* c,
+                                  const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 
 double now_seconds();
 

@@ -75,6 +75,10 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         ws->p = A(); ws->Ar = A(); ws->q = A();
         ws->r = dev_alloc<T>((size_t)m); ws->Ap = dev_alloc<T>((size_t)m); ws->s = dev_alloc<T>((size_t)m);
         break;
+      case S_BILQ: case S_QMR:                      // BilqWorkspace / QmrWorkspace (t, s are allocated by the solve)
+        ws->u_prev = A(); ws->u = A(); ws->q = A(); ws->v_prev = A(); ws->v = A(); ws->p = A();
+        if (kind == S_QMR) { ws->w1 = A(); ws->w2 = A(); } else { ws->w = A(); }   // w_{k-2}, w_{k-1} / d̅
+        break;
       default: throw std::runtime_error("unsupported solver");
     }
   } catch (...) {
@@ -91,7 +95,7 @@ template <class T> void ws_destroy(Workspace<T>* ws) {
   T* vecs[] = {ws->x, ws->dx, ws->r, ws->p, ws->Ap, ws->z, ws->npc_dir, ws->p2, ws->v, ws->s, ws->qd, ws->t, ws->yz,
                ws->r1, ws->r2, ws->w1, ws->w2, ws->y, ws->vv, ws->w, ws->q, ws->pp, ws->bbuf, ws->cbuf,
                ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next, ws->Nv, ws->Mu, ws->Av, ws->Atu, ws->h, ws->hbar,
-               ws->Ar, ws->Mr};
+               ws->Ar, ws->Mr, ws->u_prev, ws->v_prev};
   for (T* p : vecs) dev_free(p);
   for (T* p : ws->V) dev_free(p);
   for (T* p : ws->Z) dev_free(p);

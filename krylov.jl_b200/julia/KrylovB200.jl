@@ -195,7 +195,7 @@ end
 # created ONCE per Krylov.jl workspace and kept in HANDLES, so an in-place solve allocates nothing
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
-                       :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25,
+                       :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25, :bilq => 12, :qmr => 13,
                        :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
@@ -204,7 +204,7 @@ end
 struct CExt    # KrylovB200Options (include/krylov_b200.h)
   history::Cint; ldiv::Cint; etol::Cdouble; conlim::Cdouble; fused::Cint; batch::Cint
   callback::Ptr{Cvoid}; callback_user::Ptr{Cvoid}; time_kernels::Cint; check_curvature::Cint; cr_gamma::Cdouble
-  axtol::Cdouble; btol::Cdouble; sigma::Cdouble; utol::Cdouble; transfer_to_lsqr::Cint
+  axtol::Cdouble; btol::Cdouble; sigma::Cdouble; utol::Cdouble; transfer_to_lsqr::Cint; transfer_to_bicg::Cint
 end
 struct CStats  # KrylovB200Stats (include/krylov_b200.h)
   niter::Cint; solved::Cint; inconsistent::Cint; indefinite::Cint; npcCount::Cint
@@ -300,7 +300,7 @@ function fused_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; c::Un
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, NaN, NaN, 0.0, NaN, 0))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, NaN, NaN, 0.0, NaN, 0, 1))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, restart, reorthogonalization, linesearch))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -361,7 +361,7 @@ function ls_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, axtol, btol, 0.0, NaN, 0))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, axtol, btol, 0.0, NaN, 0, 1))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, 0, 0, 0))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -396,7 +396,7 @@ function lslq_solve!(ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N = I, ldiv::Bo
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
   ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, btol, σ, utol,
-                 transfer_to_lsqr))
+                 transfer_to_lsqr, 1))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, 0, 0, 0, 0))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -425,7 +425,7 @@ function normal_ls_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; M
   set_precond!(h, 1, I)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0, 1))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, 0, 0, 0))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -442,6 +442,42 @@ Krylov.cgls!(ws::Krylov.CglsWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200C
   normal_ls_solve!(:cgls, ws, A, b; kw...)
 Krylov.crls!(ws::Krylov.CrlsWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
   normal_ls_solve!(:crls, ws, A, b; kw...)
+
+# ---- bilq! / qmr! (src/bilq.jl:97-115, src/qmr.jl:104-114) on a square B200CSR: one krylov_solve per solve ------------
+# The library forms Aᵀ once per operator and runs the fused Lanczos biorthogonalization when M = N = I; `c` defaults to b.
+function biorth_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; c::B200Vector{T} = b,
+                       transfer_to_bicg::Bool = true, M = I, N = I, ldiv::Bool = false, atol::T = √eps(T),
+                       rtol::T = √eps(T), itmax::Int = 0, timemax::Float64 = Inf, verbose::Int = 0, history::Bool = false,
+                       callback = workspace -> false, iostream::IO = stdout) where T
+  A.m == A.n || error("System must be square")
+  length(b) == A.m || error("Inconsistent problem size")
+  h = handle_for(method, ws, A, 0, 0)
+  set_precond!(h, 0, M)
+  set_precond!(h, 1, N)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0,
+                 transfer_to_bicg))
+  o = Ref(COpts(atol, rtol, itmax, verbose, 0.0, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    if ws.warm_start                      # warm_start!(ws, x0) stored x0 in ws.Δx
+      check(ccall((:krylov_warm_start, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.Δx.ptr, A.n))
+      ws.warm_start = false
+    end
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, c.ptr, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.bilq!(ws::Krylov.BilqWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  biorth_solve!(:bilq, ws, A, b; kw...)
+Krylov.qmr!(ws::Krylov.QmrWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  biorth_solve!(:qmr, ws, A, b; kw...)
 
 # ---- block_gmres! (src/block_gmres.jl:78-110; C ABI krylov.h:250-285): one krylov_block_solve per solve ------------------
 # B, X, X0 are column-major n x p device matrices; the library keeps row-major panels internally and runs the
@@ -477,7 +513,7 @@ function Krylov.block_gmres!(ws::Krylov.BlockGmresWorkspace{T,T,B200Vector{T},B2
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0, 1))
   o = Ref(COpts(atol, rtol, itmax, verbose, 0.0, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, restart, reorthogonalization, false))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))

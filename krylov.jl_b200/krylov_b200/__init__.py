@@ -38,7 +38,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "cgs", "cgs_", "cg_lanczos", "cg_lanczos_", "CrWorkspace", "DiomWorkspace", "DqgmresWorkspace", "cr", "cr_", "diom",
            "diom_", "dqgmres", "dqgmres_", "BlockGmresWorkspace", "block_gmres", "block_gmres_", "CsrOperator",
            "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_",
-           "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_"]
+           "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_",
+           "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_"]
 
 
 class B200Error(RuntimeError):
@@ -756,8 +757,8 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
                 setattr(e, name, float(val))
         return self._run(A, b, M, N, o, e, callback)
 
-    def _run(self, A, b, M, N, o, e, callback):
-        """Set the options, the operator pair and the preconditioners, stage b and call krylov_solve."""
+    def _run(self, A, b, M, N, o, e, callback, c=None):
+        """Set the options, the operator pair and the preconditioners, stage b (and c) and call krylov_solve."""
         m, n = self.m, self.n
         keep = []
         if callback is not None:
@@ -802,8 +803,14 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
         if b.shape[0] != m:
             raise B200Error("Inconsistent problem size")
         pb, kb_ = _ptr(b)
-        self._order_after(kb_)
-        rc = lib().krylov_solve(self._h, fA, fAt, fP[0], fP[1], pb, None, None, C.byref(o))
+        if c is not None:
+            if not _is_torch(c):
+                c = np.ascontiguousarray(c, dtype=self.dtype)
+            if c.shape[0] != m:
+                raise B200Error("Inconsistent problem size")
+        pc, kc = _ptr(c)
+        self._order_after(kb_, kc)
+        rc = lib().krylov_solve(self._h, fA, fAt, fP[0], fP[1], pb, pc, None, C.byref(o))
         del keep
         if self._cb_error is not None:
             raise self._cb_error
@@ -886,6 +893,52 @@ class CrlsWorkspace(_NormalEquationsWorkspace):
     solver = "crls"
 
 
+class _BiorthWorkspace(_LeastSquaresWorkspace):
+    """Workspace of bilq! / qmr! on a square operator (src/krylov_workspaces.jl BilqWorkspace / QmrWorkspace).  Both
+    apply A and its adjoint: a CSR operator (its transpose is formed once and cached), or a
+    scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables."""
+    nA = 2
+
+    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
+        super().__init__(m_or_A, n_or_b, dtype, device=device)
+
+    def _solve(self, A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown,
+               transfer_to_bicg=True):
+        if unknown:
+            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        o = lib().krylov_default_options()
+        if atol is not None:
+            o.atol = float(atol)
+        if rtol is not None:
+            o.rtol = float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        e = lib().krylov_b200_default_options()
+        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        e.transfer_to_bicg = int(transfer_to_bicg)
+        return self._run(A, b, M, N, o, e, callback, c)
+
+
+class BilqWorkspace(_BiorthWorkspace):
+    solver = "bilq"
+
+    def solve(self, A, b, *, c=None, transfer_to_bicg=True, M=None, N=None, ldiv=False, atol=None, rtol=None, itmax=0,
+              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
+        """bilq!(ws, A, b; kwargs...)  -- kwargs as in bilq.jl:97-109: c defaults to b, atol and rtol to sqrt(eps),
+        itmax = 0 means 2n.  M, N: None, the diagonal of a Diagonal preconditioner, or a self-adjoint host callable."""
+        return self._solve(A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown,
+                           transfer_to_bicg)
+
+
+class QmrWorkspace(_BiorthWorkspace):
+    solver = "qmr"
+
+    def solve(self, A, b, *, c=None, M=None, N=None, ldiv=False, atol=None, rtol=None, itmax=0, timemax=math.inf,
+              verbose=0, history=False, callback=None, fused=True, **unknown):
+        """qmr!(ws, A, b; kwargs...)  -- kwargs as in qmr.jl:104-115 (defaults as for bilq!)."""
+        return self._solve(A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown)
+
+
 def _make_least_squares(name):
     def f(A, b, *, n=None, window=0, **kw):
         m = b.shape[0]
@@ -911,7 +964,7 @@ _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "b
        "fom": FomWorkspace, "fgmres": FgmresWorkspace, "cgs": CgsWorkspace, "cg_lanczos": CgLanczosWorkspace,
        "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
        "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
-       "lslq": LslqWorkspace}
+       "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -965,11 +1018,14 @@ lsqr_, lsmr_ = (_make_inplace(s) for s in ("lsqr", "lsmr"))
 lsqr, lsmr = (_make_least_squares(s) for s in ("lsqr", "lsmr"))
 cgls_, crls_, lslq_ = (_make_inplace(s) for s in ("cgls", "crls", "lslq"))
 cgls, crls, lslq = (_make_least_squares(s) for s in ("cgls", "crls", "lslq"))
+bilq_, qmr_ = (_make_inplace(s) for s in ("bilq", "qmr"))
+bilq, qmr = (_make_outofplace(s) for s in ("bilq", "qmr"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):
     return {"cg": cg, "gmres": gmres, "bicgstab": bicgstab, "minres": minres, "fom": fom, "fgmres": fgmres, "cgs": cgs,
-            "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres}[method](A, b, x0, **kw)
+            "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres, "bilq": bilq,
+            "qmr": qmr}[method](A, b, x0, **kw)
 
 
 # workspace_accessors.jl:140-152

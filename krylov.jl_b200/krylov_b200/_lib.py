@@ -22,7 +22,7 @@ KRYLOV_CR, KRYLOV_DIOM, KRYLOV_DQGMRES = 1, 5, 6
 KRYLOV_LSLQ, KRYLOV_LSQR, KRYLOV_LSMR, KRYLOV_CGLS, KRYLOV_CRLS = 20, 21, 22, 24, 25
 SOLVER_IDS = {"lslq": KRYLOV_LSLQ, "lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cgls": KRYLOV_CGLS, "crls": KRYLOV_CRLS, "cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
               "fom": KRYLOV_FOM, "fgmres": KRYLOV_FGMRES, "cgs": KRYLOV_CGS, "cg_lanczos": KRYLOV_B200_CG_LANCZOS,
-              "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES}
+              "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES, "bilq": 12, "qmr": 13}
 
 MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p)
 BLOCK_MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p)
@@ -45,7 +45,7 @@ class KrylovB200Options(C.Structure):
                 ("fused", C.c_int), ("batch", C.c_int), ("callback", CALLBACK), ("callback_user", C.c_void_p),
                 ("time_kernels", C.c_int), ("check_curvature", C.c_int), ("cr_gamma", C.c_double),
                 ("axtol", C.c_double), ("btol", C.c_double), ("sigma", C.c_double), ("utol", C.c_double),
-                ("transfer_to_lsqr", C.c_int)]
+                ("transfer_to_lsqr", C.c_int), ("transfer_to_bicg", C.c_int)]
 
 
 class KrylovB200Stats(C.Structure):
