@@ -612,10 +612,13 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist(Csr<T> A, CgPer
 // B_cg,dict = n + 9nv), so there is no tile ring and no producer work.  Single GPU, M = I or Jacobi.  The launch
 // shape is cg_persist's: the same grid, 288 threads per CTA, tile t on CTA t mod G in the same order, row = tile * 256
 // + thread -- hence the same rounding of every row sum and every dot-product partial, and bit-identical iterates.
+// MINB names the plan the grid was sized for (the CTAs per SM of cg_persist's ring).  The encoded kernel has no ring,
+// so both instantiations are compiled for the 3-CTA register budget (72): with the 2-CTA budget ptxas gives the Float64
+// Jacobi kernel 89 registers for its row pipeline, and 3 CTAs of it no longer fit on an SM.
 template <class T> struct SlotLoads { T r, p, d; };   // r_j, p_old_j and (Jacobi) the diagonal of M at j
 
 template <class T, int MODE, int MINB>
-__global__ void __launch_bounds__(kTileThreads, MINB) cg_persist_dict(CsrDict<T> D, CgPersistArgs<T> a, CgState<T>* st, T* part,
+__global__ void __launch_bounds__(kTileThreads, 3) cg_persist_dict(CsrDict<T> D, CgPersistArgs<T> a, CgState<T>* st, T* part,
                                                                      GridBar* gb) {
   __shared__ T sm[32];
   __shared__ unsigned sflag[2];
@@ -645,15 +648,23 @@ __global__ void __launch_bounds__(kTileThreads, MINB) cg_persist_dict(CsrDict<T>
         const T z = MODE == kJacobi ? mul_rn(l.d, l.r) : l.r;
         return add_rn(z, mul_rn(beta, l.p));
       };
+      // Software pipeline of the rows (DESIGN.md §3): the first-touch loads of this thread's NEXT row (r, p_old,
+      // the Jacobi diagonal and x, 6-8 registers) are issued before the current row's gathers, so they are in flight
+      // during its sums instead of starting the next trip's latency chain.  r, p_old and the diagonal do not change
+      // in phase A, and x[row] is written only by this thread after it was read: the values, and every rounding, are
+      // those of loads issued in place.
       unsigned m = m0;
+      SlotLoads<T> nxt{};
+      T xnxt = T(0);
+      if (row0 < n) { nxt = load(row0); xnxt = xup ? a.x[row0] : T(0); }
       for (int t = blockIdx.x, row = row0; t < ntiles; t += G, row += rstep) {
         const unsigned mnext = (t + G < ntiles && row + rstep < n) ? __ldg(&D.mask[row + rstep]) : 0u;
         if (row < n) {
-          const T po = p_old[row];
-          T z = r[row];
-          if (MODE == kJacobi) z = mul_rn(__ldg(&mdiag[row]), z);
-          const T pn = add_rn(z, mul_rn(beta, po));
-          const T xr = xup ? a.x[row] : T(0);
+          const SlotLoads<T> here = nxt;
+          const T xr = xnxt;
+          if (t + G < ntiles && row + rstep < n) { nxt = load(row + rstep); xnxt = xup ? a.x[row + rstep] : T(0); }
+          const T po = here.p;
+          const T pn = value(here);                            // p_new[row] = z_row + beta p_old[row]
           const T acc = dict_row_sum<T>(D, row, m, load, value);
           p_new[row] = pn;
           a.Ap[row] = acc;
