@@ -43,7 +43,8 @@ typedef enum { KRYLOV_FLOAT32 = 0, KRYLOV_FLOAT64 = 1, KRYLOV_COMPLEX32 = 2, KRY
 typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
 
 /* positional, frozen (krylov.h:48-83).  Implemented here: CG, MINRES, GMRES, BICGSTAB (the hot path), the
- * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, BILQ and QMR on a square operator and
+ * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, CAR and MINARES on a symmetric operator
+ * (CAR takes M, MINARES the shift `lambda` and no preconditioner; neither takes N), BILQ and QMR on a square operator and
  * its adjoint (matvec_At with matvec_A, or the transpose of an attached CSR operator; `c` is accepted, default b), and
  * the least-squares solvers LSQR, LSMR, LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A
  * maps n -> m and matvec_At m -> n, or a CSR operator of m rows and n columns is attached); every other value returns
@@ -180,7 +181,8 @@ typedef struct {
   int time_kernels;   /* fused CG: time the two phases of the iteration (see krylov_b200_get_kernel_times) */
   int check_curvature; /* CG-Lanczos: kwarg `check_curvature` (src/cg_lanczos.jl:94)                            */
   double cr_gamma;     /* CR: kwarg `γ` (src/cr.jl:112); NaN -> sqrt(eps)                                        */
-  double axtol;        /* LSQR, LSMR: kwarg `axtol` (src/lsqr.jl:152); NaN -> sqrt(eps)                          */
+  double axtol;        /* LSQR, LSMR: kwarg `axtol` (src/lsqr.jl:152); MINARES: kwarg `Artol`, the relative
+                          tolerance on ||A r|| (src/minares.jl:99); NaN -> sqrt(eps)                                  */
   double btol;         /* LSQR, LSMR, LSLQ: kwarg `btol`; NaN -> sqrt(eps)                                        */
   double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0                       */
   double utol;         /* LSLQ: kwarg `utol`; NaN -> sqrt(eps)                                                       */

@@ -79,7 +79,7 @@ int fail(const char* where, const char* msg) {
 bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
          s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
-         s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR;
+         s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR || s == S_CAR || s == S_MINARES;
 }
 
 int pick_device() {
@@ -179,6 +179,7 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   if (h->solver == S_DIOM || h->solver == S_DQGMRES) s.reorthogonalization = o->reorthogonalization != 0;      // _typed_solve_mn_reorth!
   s.cr_gamma = std::isnan(h->ext.cr_gamma) ? -1 : h->ext.cr_gamma;
   if (h->solver == S_MINRES) { s.lambda = o->lambda; s.linesearch = o->linesearch != 0; }
+  if (h->solver == S_MINARES) s.lambda = o->lambda;   // _typed_solve_sym_lambda! (CAR: _typed_solve!, M only)
   if (is_ls_kind(h->solver)) { s.lambda = o->lambda; s.radius = o->radius; }   // _typed_solve_ls_mn_radius! (c_stores.jl:403-423)
   if (h->solver == S_LSLQ) s.radius = 0;            // _typed_solve_ls_mn!: λ and no trust region
   s.sigma = std::isnan(h->ext.sigma) ? 0 : h->ext.sigma;
@@ -307,6 +308,13 @@ int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, Kryl
     case S_FGMRES: fgmres_solve<T>(*ws, A, bd, M, N, so); break;
     case S_CG_LANCZOS: cg_lanczos_solve<T>(*ws, A, bd, M, so); break;
     case S_CR: cr_solve<T>(*ws, A, bd, M, so); break;
+    case S_CAR: case S_MINARES:
+      // the reference's C layer drops N for both; a caller passing one expects it to act, so it is refused
+      if (!N.is_identity())
+        throw std::runtime_error("car and minares take no right preconditioner N (matvec_N): only M, and for minares none");
+      if (h->solver == S_CAR) car_solve<T>(*ws, A, bd, M, so);
+      else minares_solve<T>(*ws, A, bd, M, so);
+      break;
     case S_DQGMRES: dqgmres_solve<T>(*ws, A, bd, M, N, so); break;
     case S_DIOM: diom_solve<T>(*ws, A, bd, M, N, so); break;
     case S_CGS: {
@@ -393,6 +401,11 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
   if (!strcmp(nm, "vₖ₋₁") || !strcmp(nm, "v_prev")) return ws->v_prev;
   if (!strcmp(nm, "uₖ")) return ws->u;
   if (!strcmp(nm, "vₖ")) return ws->v;
+  if (!strcmp(nm, "vₖ₊₁") || !strcmp(nm, "v_next")) return ws->kind == S_MINARES ? ws->vv : nullptr;   // MINARES
+  if (!strcmp(nm, "wₖ₋₁") || !strcmp(nm, "w_prev")) return ws->kind == S_MINARES ? ws->w1 : nullptr;
+  if (!strcmp(nm, "wₖ₋₂") || !strcmp(nm, "w_prev2")) return ws->kind == S_MINARES ? ws->w2 : nullptr;
+  if (!strcmp(nm, "dₖ₋₁") || !strcmp(nm, "d_prev")) return ws->d1;
+  if (!strcmp(nm, "dₖ₋₂") || !strcmp(nm, "d_prev2")) return ws->d2;
   if (nm[0] == 'Z') { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->Z.size()) return ws->Z[i - 1]; return nullptr; }
   if (nm[0] == 'V') { int i = atoi(nm + 1); if (i >= 1 && i <= (int)ws->V.size()) return ws->V[i - 1]; }
   return nullptr;
@@ -961,6 +974,8 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
     if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) solves are not available");
     if (is_biorth(h->solver))        // A^T of a row block needs the column halo of A, not its row halo
       return fail("krylov_b200_dist_init", "row-partitioned BiLQ / QMR solves are not available");
+    if (h->solver == S_CAR || h->solver == S_MINARES)
+      return fail("krylov_b200_dist_init", "row-partitioned CAR / MINARES solves are not available");
     return h->dtype == KRYLOV_FLOAT64 ? dist_init_t<double>(h, rank, world, nhalo, halo_rank, halo_off)
                                       : dist_init_t<float>(h, rank, world, nhalo, halo_rank, halo_off);
   } catch (const std::exception& e) { return fail("krylov_b200_dist_init", e); }

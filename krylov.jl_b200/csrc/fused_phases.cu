@@ -1007,6 +1007,174 @@ void bilq_fused_update(Workspace<T>& ws, bool first, T czeta, T szeta, T cs, T s
   *vv1 = out[0]; *v1v1 = out[1];
 }
 
+// ===========================================================================
+// CAR  (src/car.jl:187-214, M = I: Mu === u)
+// C1 updates x, r, s and returns ||r||^2, ||s||^2 (the host decides `solved` from ||r||); when not solved, C2 (SpMV on s)
+// leaves rho_next = <t, s> and beta = rho_next / rho in the device block, C3 reads beta and updates the directions,
+// and the host reads {rho_next, <u, u>} once and re-derives beta with the same division.
+// ===========================================================================
+template <class T> struct CarState { T rho_next, beta, uu; };
+
+template <class T> struct CarC1Body {     // x += alpha p ; r -= alpha q ; s -= alpha u ; ||r||^2, ||s||^2   (car.jl:189-191)
+  T* x; T* r; T* s; const T* p; const T* q; const T* u; T alpha;
+  __device__ __forceinline__ void operator()(int j, T* d) const {
+    x[j] = add_rn(x[j], mul_rn(alpha, p[j]));
+    const T rn = add_rn(r[j], mul_rn(-alpha, q[j]));
+    r[j] = rn;
+    const T sn = add_rn(s[j], mul_rn(-alpha, u[j]));
+    s[j] = sn;
+    d[0] += rn * rn; d[1] += sn * sn;
+  }
+};
+template <class T> struct CarC2Epi {      // t = A s ; <t, s>                       (car.jl:203-204)
+  T* t; const T* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const { t[row] = acc; d[0] += acc * __ldg(&s[row]); }
+};
+template <class T> struct CarC2Fin {      // rho_next ; beta = rho_next / rho        (car.jl:205)
+  CarState<T>* st; T rho;
+  __device__ void operator()(const T* tot) const { st->rho_next = tot[0]; st->beta = div_rn(tot[0], rho); }
+};
+template <class T> struct CarC3Body {     // p = r + beta p ; q = s + beta q ; u = t + beta u ; <u, u>   (car.jl:207-209)
+  T* p; T* q; T* u; const T* r; const T* s; const T* t; const CarState<T>* st;
+  __device__ __forceinline__ void operator()(int j, T* d) const {
+    const T beta = st->beta;
+    p[j] = add_rn(mul_rn(T(1), r[j]), mul_rn(beta, p[j]));
+    q[j] = add_rn(mul_rn(T(1), s[j]), mul_rn(beta, q[j]));
+    const T un = add_rn(mul_rn(T(1), t[j]), mul_rn(beta, u[j]));
+    u[j] = un;
+    d[0] += un * un;
+  }
+};
+template <class T> struct CarC3Fin {
+  CarState<T>* st;
+  __device__ void operator()(const T* tot) const { st->uu = tot[0]; }
+};
+
+template <class T> void car_fused_step(Workspace<T>& ws, T alpha, T* rr, T* ss) {
+  Ctx& c = ws.ctx;
+  launch_stream<T, 2>(c, ws.n, CarC1Body<T>{ws.x, ws.r, ws.s, ws.p, ws.q, ws.u, alpha}, StoreFin<T, 2>{sib_slots<T>(c)}, 5);
+  T out[2]; sib_read<T, 2>(c, out);
+  *rr = out[0]; *ss = out[1];
+}
+template <class T> void car_fused_directions(Workspace<T>& ws, const Csr<T>& A, T rho, T* rho_next, T* uu) {
+  Ctx& c = ws.ctx;
+  typedef CarState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  launch_spmv_epi<T, 1>(c, A, ws.s, CarC2Epi<T>{ws.t, ws.s}, CarC2Fin<T>{S, rho}, 4);
+  launch_stream<T, 1>(c, ws.n, CarC3Body<T>{ws.p, ws.q, ws.u, ws.r, ws.s, ws.t, S}, CarC3Fin<T>{S}, 5);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  c.sync();
+  *rho_next = H[1].rho_next; *uu = H[1].uu;
+}
+
+// ===========================================================================
+// MINARES  (src/minares.jl:283-321,450-471)
+// M1's Fin leaves alpha_{k+1} in the device block and M2 reads it; the host reads {alpha, ||v_k||^2} once, runs every
+// rotation unchanged, and M3 applies the scaling of v_k, the d recurrence and the solution update.  w_k and d_k are
+// formed in the buffers of w_{k-1} / d_{k-1} at iteration 1 and of w_{k-2} / d_{k-2} after (the caller rotates them).
+// ===========================================================================
+template <class T> struct MinaresState { T alpha, vv; };
+
+// w_k = v_k / lam (iteration 1, kdivcopy!), else (v_k - gamma1 w_{k-1} - eps2 w_{k-2}) / lam in the
+// kscal!/kaxpy!/kaxpy!/kdiv! order   (minares.jl:283-302)
+template <class T> struct MinaresW {
+  T* wk; const T* w1; T eps2, gamma1, lam, inv_lam; int iter;
+  __device__ __forceinline__ void operator()(int i, T vi) const {
+    T w;
+    if (iter == 1) {
+      w = div_rn(vi, lam);
+    } else {
+      w = wk[i];
+      if (iter >= 3) w = mul_rn(-eps2, w);
+      w = add_rn(w, mul_rn(-gamma1, w1[i]));
+      w = add_rn(w, mul_rn(T(1), vi));
+      w = mul_rn(inv_lam, w);
+    }
+    wk[i] = w;
+  }
+};
+template <class T> struct MinaresM1Epi {  // w_k ; v_k = A v_{k+1} - beta v_k (+ shift v_{k+1}) ; <v_k, v_{k+1}>   (:307-311)
+  MinaresW<T> w; T* vk; const T* vk1; T beta1, shift; int shifted;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T vi = vk[row];
+    w(row, vi);
+    T vn = add_rn(mul_rn(T(1), acc), mul_rn(-beta1, vi));
+    const T v1 = __ldg(&vk1[row]);
+    if (shifted) vn = add_rn(vn, mul_rn(shift, v1));
+    vk[row] = vn;
+    d[0] += vn * v1;
+  }
+};
+template <class T> struct MinaresM1Fin {
+  MinaresState<T>* st;
+  __device__ void operator()(const T* tot) const { st->alpha = tot[0]; }
+};
+template <class T> struct MinaresWBody {  // w_k only: no product once the Lanczos process has terminated
+  MinaresW<T> w; const T* vk;
+  __device__ __forceinline__ void operator()(int j, T*) const { w(j, vk[j]); }
+};
+template <class T> struct MinaresM2Body { // v_k -= alpha v_{k+1} ; ||v_k||^2        (minares.jl:312-313)
+  T* vk; const T* vk1; const MinaresState<T>* st;
+  __device__ __forceinline__ void operator()(int j, T* d) const {
+    const T vn = add_rn(vk[j], mul_rn(-st->alpha, vk1[j]));
+    vk[j] = vn;
+    d[0] += vn * vn;
+  }
+};
+template <class T> struct MinaresM2Fin {
+  MinaresState<T>* st;
+  __device__ void operator()(const T* tot) const { st->vv = tot[0]; }
+};
+// v_k /= beta (kdiv!) ; d_k = w_k / mu (iteration 1, kdivcopy!), else (w_k - phi1 d_{k-1} - rho2 d_{k-2}) / mu ;
+// x += zeta d_k   (minares.jl:319,450-471)
+template <class T> struct MinaresM3Body {
+  T* vk; T* dk; const T* d1; const T* wk; T* x; T inv_beta, rho2, phi1, mu, inv_mu, zeta; int scale, iter;
+  __device__ __forceinline__ void operator()(int j, T*) const {
+    if (scale) vk[j] = mul_rn(inv_beta, vk[j]);
+    T dd;
+    if (iter == 1) {
+      dd = div_rn(wk[j], mu);
+    } else {
+      dd = dk[j];
+      if (iter >= 3) dd = mul_rn(-rho2, dd);
+      dd = add_rn(dd, mul_rn(-phi1, d1[j]));
+      dd = add_rn(dd, mul_rn(T(1), wk[j]));
+      dd = mul_rn(inv_mu, dd);
+    }
+    dk[j] = dd;
+    x[j] = add_rn(x[j], mul_rn(zeta, dd));
+  }
+};
+
+template <class T>
+void minares_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, bool lanczos, int iter, T* vk, const T* vk1, T* wk, const T* w1,
+                           T eps2, T gamma1, T lam, T beta1, T shift, T* alpha, T* vv) {
+  Ctx& c = ws.ctx;
+  const MinaresW<T> w{wk, w1, eps2, gamma1, lam, T(1) / lam, iter};
+  if (!lanczos) {
+    launch_stream<T, 0>(c, ws.n, MinaresWBody<T>{w, vk}, NoFin(), 5);
+    return;
+  }
+  typedef MinaresState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  launch_spmv_epi<T, 1>(c, A, vk1, MinaresM1Epi<T>{w, vk, vk1, beta1, shift, shift != T(0) ? 1 : 0}, MinaresM1Fin<T>{S}, 4);
+  launch_stream<T, 1>(c, ws.n, MinaresM2Body<T>{vk, vk1, S}, MinaresM2Fin<T>{S}, 5);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  c.sync();
+  *alpha = H[1].alpha; *vv = H[1].vv;
+}
+
+template <class T>
+void minares_fused_update(Workspace<T>& ws, int iter, T* vk, bool scale, T beta, T* dk, const T* d1, const T* wk, T rho2,
+                          T phi1, T mu, T zeta) {
+  launch_stream<T, 0>(ws.ctx, ws.n,
+                      MinaresM3Body<T>{vk, dk, d1, wk, ws.x, scale ? T(1) / beta : T(1), rho2, phi1, mu, T(1) / mu, zeta,
+                                       scale ? 1 : 0, iter},
+                      NoFin(), 5);
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1032,7 +1200,12 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void crls_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T, T*, T*, T*, T*);   \
   template void biorth_fused_lanczos<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, T, T, T*, T*);                  \
   template T qmr_fused_update<T>(Workspace<T>&, T*, const T*, int, T, T, T, T, T, T, bool);                          \
-  template void bilq_fused_update<T>(Workspace<T>&, bool, T, T, T, T, T, T, bool, T*, T*);
+  template void bilq_fused_update<T>(Workspace<T>&, bool, T, T, T, T, T, T, bool, T*, T*);                           \
+  template void car_fused_step<T>(Workspace<T>&, T, T*, T*);                                                         \
+  template void car_fused_directions<T>(Workspace<T>&, const Csr<T>&, T, T*, T*);                                    \
+  template void minares_fused_lanczos<T>(Workspace<T>&, const Csr<T>&, bool, int, T*, const T*, T*, const T*, T, T, T, T, T, \
+                                         T*, T*);                                                                    \
+  template void minares_fused_update<T>(Workspace<T>&, int, T*, bool, T, T*, const T*, const T*, T, T, T, T);
 INST(double)
 INST(float)
 #undef INST

@@ -7,7 +7,7 @@
 //   cg_fused.cu   two-launch CG iteration               (src/cg.jl:195-268)
 //   fused_phases.cu  fused iteration phases of bicgstab!/minres! and the Arnoldi step of gmres!/fom!/fgmres!
 //   solvers.cu    host control flow of cg!/bicgstab!/minres! and the one Arnoldi driver of gmres!/fom!/fgmres!
-//   siblings.cu   cgs!, cg_lanczos!, dqgmres!, diom!, cr! on the same kernels (SURVEY.md 8f-3)
+//   siblings.cu   cgs!, cg_lanczos!, dqgmres!, diom!, cr!, car!, minares! on the same kernels (SURVEY.md 8f-3)
 //   solver_common.h  host helpers of the drivers, among them SolveRun: the callback / clock / exit protocol
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
 //   biorth.cu     host control flow of bilq!/qmr! (one Lanczos biorthogonalization driver; A and A^T)
@@ -208,7 +208,8 @@ struct Stats {
 
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
-                  S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25, S_CG_LANCZOS = 100 };
+                  S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
+                  S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
 // the least-squares solvers: A is m x n, b has m entries and x has n
 inline bool is_ls_kind(int k) { return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS; }
 
@@ -233,6 +234,8 @@ struct Workspace {
   T *Nv = nullptr, *Mu = nullptr, *Av = nullptr, *Atu = nullptr;                     // LSQR / LSMR (+ w, u, v; Mu, Av, u: m)
   T *h = nullptr, *hbar = nullptr;                                                   // LSMR
   T *u_prev = nullptr, *v_prev = nullptr;                                             // BiLQ / QMR (+ u, v, q, p; w1, w2 / w)
+  T *d1 = nullptr, *d2 = nullptr;      // MINARES: d_{k-1}, d_{k-2} (+ v = v_k, vv = v_{k+1}, w1 = w_{k-1}, w2 = w_{k-2}, q)
+                                       // CAR: r, p, s, q, t, u (+ Mu, lazy)
   T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
                                        // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
   std::vector<T*> V;
@@ -297,6 +300,9 @@ template <class T> void cg_lanczos_solve(Workspace<T>& ws, const LinOp<T>& A, co
 template <class T> void dqgmres_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void diom_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
+template <class T> void car_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
+// minares! takes no preconditioner (the reference refuses M != I); o.lambda shifts A, o.axtol holds its Artol
+template <class T> void minares_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
 // Least squares on an m x n operator (lsq.cu).  At: the adjoint (a CSR operator holding A^T, or a callback m -> n).
 template <class T> void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const LinOp<T>& N, const SolveOpts& o);
@@ -369,6 +375,20 @@ template <class T> T lanczos_fused_recur(Workspace<T>& ws, T delta, T beta, bool
 template <class T> void lanczos_fused_update(Workspace<T>& ws, T beta, T gamma, T sigma, T omega);
 template <class T> void cr_fused_step(Workspace<T>& ws, const Csr<T>& A, T alpha, T* xx, T* rr, T* ArAr, T* rAr);
 template <class T> T cr_fused_directions(Workspace<T>& ws, T beta);
+// CAR (fused_phases.cu), M = I.  C1: x += alpha p ; r -= alpha q ; s -= alpha u, one read-back of ||r||^2, ||s||^2.
+template <class T> void car_fused_step(Workspace<T>& ws, T alpha, T* rr, T* ss);
+// C2: t = A s, rho_next = <t, s> and beta = rho_next / rho on the device; C3: p = r + beta p ; q = s + beta q ;
+// u = t + beta u, <u, u>.  One read-back of {rho_next, <u, u>}.
+template <class T> void car_fused_directions(Workspace<T>& ws, const Csr<T>& A, T rho, T* rho_next, T* uu);
+// MINARES (fused_phases.cu).  M1: w_k from v_k, w_{k-1}, w_{k-2} (into wk: w_{k-1}'s buffer at iteration 1, w_{k-2}'s
+// after); with `lanczos`, M1 is the SpMV on v_{k+1} that also forms v_k = A v_{k+1} - beta v_k (+ shift v_{k+1}) and
+// alpha = <v_k, v_{k+1}> on the device, and M2 v_k -= alpha v_{k+1} with ||v_k||^2: one read-back of {alpha, ||v_k||^2}.
+// Without `lanczos` (past the early-termination point) M1 is a streaming pass with the w update only.
+template <class T> void minares_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, bool lanczos, int iter, T* vk, const T* vk1,
+                                              T* wk, const T* w1, T eps2, T gamma1, T lam, T beta1, T shift, T* alpha, T* vv);
+// M3: v_k /= beta (scale), d_k from w_k, d_{k-1}, d_{k-2} (into dk, as for w), x += zeta d_k.
+template <class T> void minares_fused_update(Workspace<T>& ws, int iter, T* vk, bool scale, T beta, T* dk, const T* d1,
+                                             const T* wk, T rho2, T phi1, T mu, T zeta);
 int gmres_fused_max();
 // LSQR / LSMR (fused_phases.cu), M = N = I, A and A^T CSR operators, no trust region.  Golub-Kahan step: P1 (SpMV on A
 // with Mu <- A v - alpha Mu and ||Mu||^2) and P2 (SpMV on A^T with Nv <- A^T u - beta Nv, ||Nv||^2 and, for LSQR,

@@ -591,7 +591,385 @@ void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M
   run.finish(iter, solved, false, status);
 }
 
+// ===========================================================================
+// car!  (src/car.jl:108-256)
+//   workspace fields: r, p, s, q, t, u, Mu (lazy; Mu === u when M = I)
+// ===========================================================================
+template <class T>
+void car_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CAR: system of %d equations in %d variables\n", n, n);
+  const bool MisI = M.is_identity();
+  allocate_if(!MisI, ws, ws.Mu);
+  T *dx = ws.dx, *x = ws.x, *r = ws.r, *p = ws.p, *s = ws.s, *q = ws.q, *t = ws.t, *u = ws.u;
+  T* Mu = MisI ? u : ws.Mu;
+  Stats& stats = ws.stats;
+  const bool warm_start = ws.warm_start;
+  stats.reset();
+
+  k_fill<T>(c, n, x, T(0));
+  if (warm_start) { op_apply(c, A, dx, r); k_axpby<T>(c, n, T(1), b, T(-1), r); }
+  else k_copy<T>(c, n, r, b);
+  if (MisI) k_copy<T>(c, n, p, r);                            // p₀ = r₀ = M(b - Ax₀)
+  else { op_apply(c, M, r, p, ldiv); k_copy<T>(c, n, r, p); }
+  op_apply(c, A, r, s);                                       // s₀ = Ar₀
+  if (MisI) k_copy<T>(c, n, q, s);                            // q₀ = MAp₀ and s₀ = MAr₀
+  else { op_apply(c, M, s, q, ldiv); k_copy<T>(c, n, s, q); }
+  op_apply(c, A, s, t);                                       // t₀ = As₀
+  k_copy<T>(c, n, u, t);                                      // u₀ = Aq₀
+  T rho = k_dot<T>(c, n, t, s);                               // ρ₀ = ⟨t₀ , s₀⟩
+  T rNorm = k_nrm2<T>(c, n, r);
+  if (history) stats.residuals.push_back(rNorm);
+  T ArNorm = MisI ? k_nrm2<T>(c, n, s) : std::sqrt(k_dot<T>(c, n, r, u));   // knorm_elliptic(n, r, u)
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  if (rNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    return;
+  }
+  int iter = 0;
+  const int itmax = default_itmax(ws, o.itmax);
+  const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
+  if (o.verbose > 0) printf("%5s  %7s  %7s  %7s  %7s  %5s\n", "k", "‖rₖ‖", "‖Arₖ‖", "α", "β", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %7.1e  %7s  %7s  %.2fs\n", iter, (double)rNorm, (double)ArNorm, "✗ ✗ ✗ ✗", "✗ ✗ ✗ ✗", run.elapsed());
+  bool solved = rNorm <= eps_tol, tired = iter >= itmax, user_exit = false, overtimed = false;
+  // grouped passes (M = I, CSR operator): 3 launches and 2 read-backs per iteration instead of 11 and 4
+  const bool fusedC = o.fused && A.kind == LinOp<T>::CSR && MisI;
+  T uu = 0;
+  bool have_uu = false;
+
+  while (!(solved || tired || user_exit || overtimed)) {
+    if (!MisI) op_apply(c, M, u, Mu, ldiv);
+    const T alpha = rho / (have_uu ? uu : k_dot<T>(c, n, u, Mu));   // αₖ = ρₖ / ⟨uₖ, Muₖ⟩
+    T beta = 0, ss = 0;
+    if (fusedC) {
+      T rr;
+      car_fused_step<T>(ws, alpha, &rr, &ss);
+      rNorm = std::sqrt(rr);
+    } else {
+      k_axpy<T>(c, n, alpha, p, x);                           // xₖ₊₁ = xₖ + αₖ * pₖ
+      k_axpy<T>(c, n, -alpha, q, r);                          // rₖ₊₁ = rₖ - αₖ * qₖ
+      k_axpy<T>(c, n, -alpha, Mu, s);                         // sₖ₊₁ = sₖ - αₖ * Muₖ
+      rNorm = k_nrm2<T>(c, n, r);
+    }
+    if (history) stats.residuals.push_back(rNorm);
+    const bool resid_decrease_mach = (rNorm + T(1) <= T(1));
+    solved = rNorm <= eps_tol || resid_decrease_mach;
+    if (!solved) {
+      if (fusedC) {                                           // C2 + C3; ‖Arₖ‖ = ‖sₖ₊₁‖ from C1
+        T rho_next;
+        car_fused_directions<T>(ws, *A.csr, rho, &rho_next, &uu);
+        have_uu = true;
+        beta = rho_next / rho;
+        rho = rho_next;
+        ArNorm = std::sqrt(ss);
+      } else {
+        op_apply(c, A, s, t);                                 // tₖ₊₁ = A * sₖ₊₁
+        const T rho_next = k_dot<T>(c, n, t, s);              // ρₖ₊₁ = ⟨tₖ₊₁ , sₖ₊₁⟩
+        beta = rho_next / rho;                                // βₖ = ρₖ₊₁ / ρₖ
+        rho = rho_next;
+        k_axpby<T>(c, n, T(1), r, beta, p);                   // pₖ₊₁ = rₖ₊₁ + βₖ * pₖ
+        k_axpby<T>(c, n, T(1), s, beta, q);                   // qₖ₊₁ = sₖ₊₁ + βₖ * qₖ
+        k_axpby<T>(c, n, T(1), t, beta, u);                   // uₖ₊₁ = tₖ₊₁ + βₖ * uₖ
+        ArNorm = MisI ? k_nrm2<T>(c, n, s) : std::sqrt(k_dot<T>(c, n, r, u));
+      }
+      if (history) stats.Aresiduals.push_back(ArNorm);
+    }
+    iter = iter + 1;
+    tired = iter >= itmax;
+    run.poll(iter, user_exit, overtimed);
+    if (kdisplay(iter, o.verbose) && !solved)
+      printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm, (double)alpha, (double)beta, run.elapsed());
+    if (kdisplay(iter, o.verbose) && solved)
+      printf("%5d  %7.1e  %7s  %7.1e  %7s  %.2fs\n", iter, (double)rNorm, "✗ ✗ ✗ ✗", (double)alpha, "✗ ✗ ✗ ✗", run.elapsed());
+  }
+  if (o.verbose > 0) printf("\n");
+  std::string status = "unknown";
+  if (solved) status = "solution good enough given atol and rtol";
+  if (tired) status = "maximum number of iterations exceeded";
+  if (user_exit) status = "user-requested exit";
+  if (overtimed) status = "time limit exceeded";
+  run.finish(iter, solved, false, status);
+}
+
+// ===========================================================================
+// minares!  (src/minares.jl:113-595), M = I (the reference refuses any other M)
+//   workspace fields: vₖ (v), vₖ₊₁ (vv), wₖ₋₂ (w2), wₖ₋₁ (w1), dₖ₋₂ (d2), dₖ₋₁ (d1), q; the pairs rotate by pointer
+//   (@kswap!).  Every rotation runs on the host; the fused path (CSR operator) groups the vector work of an
+//   iteration into M1 (the SpMV with the w update), M2 and M3, with one read-back.
+// ===========================================================================
+template <class T>
+void minares_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int n = ws.n;
+  const bool history = o.history;
+  const T lambda = (T)o.lambda;
+  if (o.verbose > 0) printf("MINARES: system of size %d\n", n);
+  if (!M.is_identity()) throw std::runtime_error("Preconditioners are not yet supported");
+  T *dx = ws.dx, *x = ws.x, *q = ws.q;
+  T *vk = ws.v, *vk1 = ws.vv, *wk2 = ws.w2, *wk1 = ws.w1, *dk2 = ws.d2, *dk1 = ws.d1;
+  Stats& stats = ws.stats;
+  const bool warm_start = ws.warm_start;
+  stats.reset();
+  int iter = 0;
+  const int itmax = default_itmax(ws, o.itmax);
+  const bool fusedM = o.fused && A.kind == LinOp<T>::CSR;
+
+  k_fill<T>(c, n, x, T(0));
+  if (warm_start) {                                           // β₁v₁ = r₀ = b - (A + λI)x₀
+    op_apply(c, A, dx, vk);
+    if (lambda != 0) k_axpy<T>(c, n, lambda, dx, vk);
+    k_axpby<T>(c, n, T(1), b, T(-1), vk);
+  } else {
+    k_copy<T>(c, n, vk, b);
+  }
+  T betak = k_nrm2<T>(c, n, vk);
+  if (betak != 0) k_scal<T>(c, n, T(1) / betak, vk);          // kdiv!
+  const T beta1 = betak;
+  op_apply(c, A, vk, vk1);                                    // β₂v₂ = (A + λI)v₁ - α₁v₁
+  if (lambda != 0) k_axpy<T>(c, n, lambda, vk, vk1);
+  T alphak = k_dot<T>(c, n, vk, vk1);
+  k_axpy<T>(c, n, -alphak, vk, vk1);
+  T betak1 = k_nrm2<T>(c, n, vk1);
+  if (betak1 != 0) k_scal<T>(c, n, T(1) / betak1, vk1);
+
+  T xik1 = 0;
+  T tauk2 = 0, tauk1 = 0, tauk = 0;
+  T thetabark2 = 0;
+  T psibisk2 = 0, psibark1 = 0;
+  T pik2 = 0, pik1 = 0, pik = 0;
+  T chibark = 0;
+  T zetabisk = 0, zetabark1 = 0, gammabark = 0;
+  T lambdabark = 0, gammak1 = 0;
+  T ct4 = 0, st4 = 0, ct3 = 0, st3 = 0, ct2 = 0, st2 = 0, ct1 = 0, st1 = 0, ct0 = 0, st0 = 0;   // c̃₂ₖ₋₄ ... c̃₂ₖ
+  k_fill<T>(c, n, wk2, T(0));
+  k_fill<T>(c, n, wk1, T(0));
+  k_fill<T>(c, n, dk2, T(0));
+  k_fill<T>(c, n, dk1, T(0));
+  const T b1a1 = betak * alphak;                              // β₁α₁, β₁β₂: zₖ's first entries
+  const T b1b2 = betak * betak1;
+  T epsk2 = 0, epsk1 = 0;
+  long long ell = (long long)itmax + 2;
+
+  T rNorm = beta1;
+  const T eps_tol = tol_of<T>(o.atol) + tol_of<T>(o.rtol) * rNorm;
+  if (history) stats.residuals.push_back(rNorm);
+  T ArNorm = std::sqrt(b1a1 * b1a1 + b1b2 * b1b2);
+  const T kappa = tol_of<T>(o.atol) + tol_of<T>(o.axtol) * ArNorm;
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  if (rNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    return;
+  }
+  if (o.verbose > 0) printf("%5s  %7s  %7s  %7s  %8s  %5s\n", "k", "‖rₖ‖", "‖Arₖ‖", "βₖ₊₁", "ζₖ", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %7.1e  %7.1e  %8s  %.2fs\n", iter, (double)rNorm, (double)ArNorm, (double)beta1, " ✗ ✗ ✗ ✗", run.elapsed());
+  const double btol = std::pow((double)eps_of<T>(), 3.0 / 4.0);   // eps(T)^(3/4) is a Float64 in the reference
+
+  bool solved = (rNorm <= eps_tol) || (ArNorm <= kappa), breakdown = false, tired = iter >= itmax;
+  bool user_exit = false, overtimed = false;
+  while (!(solved || tired || breakdown || user_exit || overtimed)) {
+    iter = iter + 1;
+    const long long k = iter;
+    if (iter == 1) { lambdabark = alphak; gammabark = betak1; }
+    T ck, sk, lambdak;
+    sym_givens<T>(lambdabark, betak1, &ck, &sk, &lambdak);   // Qₖ.ₖ₊₁
+
+    // wₖ, the last column of Wₖ = Vₖ(Rₖ)⁻¹, then the Lanczos step βₖ₊₂vₖ₊₂ = (A + λI)vₖ₊₁ - αₖ₊₁vₖ₊₁ - βₖ₊₁vₖ
+    T* wk = iter == 1 ? wk1 : wk2;
+    T alphak1 = 0, betak2 = 0;
+    bool scale_v = false;
+    if (fusedM) {
+      T vv = 0;
+      minares_fused_lanczos<T>(ws, *A.csr, k <= ell - 1, iter, vk, vk1, wk, wk1, epsk2, gammak1, lambdak, betak1, lambda,
+                               &alphak1, &vv);
+      if (k <= ell - 1) betak2 = std::sqrt(vv);
+    } else {
+      if (iter == 1) {
+        k_divcopy<T>(c, n, wk, vk, lambdak);
+      } else {
+        if (iter >= 3) k_scal<T>(c, n, -epsk2, wk2);
+        k_axpy<T>(c, n, -gammak1, wk1, wk);
+        k_axpy<T>(c, n, T(1), vk, wk);
+        k_scal<T>(c, n, T(1) / lambdak, wk);                  // kdiv!
+      }
+      if (k <= ell - 1) {
+        op_apply(c, A, vk1, q);                               // q ← Avₖ₊₁
+        k_axpby<T>(c, n, T(1), q, -betak1, vk);               // vₖ ← Avₖ₊₁ - βₖ₊₁vₖ
+        if (lambda != 0) k_axpy<T>(c, n, lambda, vk1, vk);
+        alphak1 = k_dot<T>(c, n, vk, vk1);
+        k_axpy<T>(c, n, -alphak1, vk1, vk);
+        betak2 = k_nrm2<T>(c, n, vk);
+      }
+    }
+    if (k <= ell - 1) {
+      if ((double)betak2 <= btol) ell = k + 1;                // early termination
+      else scale_v = true;
+      if (!fusedM && scale_v) k_scal<T>(c, n, T(1) / betak2, vk);
+    }
+
+    T epsk = 0, gammabark1 = 0, gammak = 0, lambdabark1 = 0;
+    if (k <= ell - 2) { epsk = sk * betak2; gammabark1 = -ck * betak2; }
+    if (k <= ell - 1) { gammak = ck * gammabark + sk * alphak1; lambdabark1 = sk * gammabark - ck * alphak1; }
+
+    // QR factorization of Nₖ = Q̃ₖ [Uₖ; 0]
+    T rhok2 = 0, lambdahatk = 0, phibark1 = 0, mubark = 0, phik1 = 0, gammahatk = 0, mubisk = 0, muk = 0;
+    if (iter >= 3) { rhok2 = st4 * lambdak; lambdahatk = -ct4 * lambdak; }
+    if (iter == 2) lambdahatk = lambdak;
+    if (iter >= 2) {
+      phibark1 = st3 * lambdahatk;
+      mubark = -ct3 * lambdahatk;
+      if (k <= ell - 1) { phik1 = ct2 * phibark1 + st2 * gammak; gammahatk = st2 * phibark1 - ct2 * gammak; }
+      else phik1 = phibark1;
+    }
+    if (iter == 1) { mubark = lambdak; gammahatk = gammak; }
+    if (k <= ell - 1) sym_givens<T>(mubark, gammahatk, &ct1, &st1, &mubisk);
+    else mubisk = mubark;
+    if (k <= ell - 2) sym_givens<T>(mubisk, epsk, &ct0, &st0, &muk);
+    else muk = mubisk;
+
+    // zₖ = (Q̃ₖ)ᵀ(β₁α₁e₁ + β₁β₂e₂)
+    if (iter == 1) { zetabisk = b1a1; zetabark1 = b1b2; }
+    T zetaringk, zetabisk1 = 0, zetak, zetabark2 = 0;
+    if (k <= ell - 1) { zetaringk = ct1 * zetabisk + st1 * zetabark1; zetabisk1 = st1 * zetabisk - ct1 * zetabark1; }
+    else zetaringk = zetabisk;
+    if (k <= ell - 2) { zetak = ct0 * zetaringk; zetabark2 = st0 * zetaringk; }
+    else zetak = zetaringk;
+
+    // dₖ, the last column of Dₖ = Wₖ(Uₖ)⁻¹, and x = x₋₁ + ζₖdₖ (v_k's scaling rides in the same pass when fused)
+    T* dk = iter == 1 ? dk1 : dk2;
+    if (fusedM) {
+      minares_fused_update<T>(ws, iter, vk, scale_v, betak2, dk, dk1, wk, rhok2, phik1, muk, zetak);
+    } else {
+      if (iter == 1) {
+        k_divcopy<T>(c, n, dk, wk, muk);
+      } else {
+        if (iter >= 3) k_scal<T>(c, n, -rhok2, dk2);
+        k_axpy<T>(c, n, -phik1, dk1, dk);
+        k_axpy<T>(c, n, T(1), wk, dk);
+        k_scal<T>(c, n, T(1) / muk, dk);                      // kdiv!
+      }
+      k_axpy<T>(c, n, zetak, dk, x);
+    }
+
+    if (k <= ell - 2) ArNorm = std::sqrt(zetabisk1 * zetabisk1 + zetabark2 * zetabark2);
+    if (k == ell - 1) ArNorm = std::fabs(zetabisk1);
+    if (k == ell) ArNorm = T(0);
+    if (history) stats.Aresiduals.push_back(ArNorm);
+
+    // LQ factorization Uₖ = L̂ₖP̂ₖ
+    T psibark = 0, ch3 = 0, sh3 = 0, psibisk1 = 0, thetabark1 = 0, ch4 = 0, sh4 = 0, psik2 = 0, thetak2 = 0, deltak = 0;
+    T omegak2 = 0, etak = 0;
+    if (iter == 1) {
+      psibark = muk;
+    } else if (iter == 2) {
+      sym_givens<T>(psibark1, phik1, &ch3, &sh3, &psibisk1);
+      thetabark1 = sh3 * muk;
+      psibark = -ch3 * muk;
+    } else {
+      sym_givens<T>(psibisk2, rhok2, &ch4, &sh4, &psik2);
+      thetak2 = ch4 * thetabark2 + sh4 * phik1;
+      deltak = sh4 * thetabark2 - ch4 * phik1;
+      omegak2 = sh4 * muk;
+      etak = -ch4 * muk;
+      sym_givens<T>(psibark1, deltak, &ch3, &sh3, &psibisk1);
+      thetabark1 = sh3 * etak;
+      psibark = -ch3 * etak;
+    }
+
+    // L̂ₖtₖ = zₖ
+    T xik = 0;
+    if (iter == 1) {
+      tauk = zetak / psibark;
+    } else if (iter == 2) {
+      tauk1 = tauk;
+      tauk1 = tauk1 * psibark1 / psibisk1;
+      xik = zetak;
+      tauk = (xik - thetabark1 * tauk1) / psibark;
+    } else {
+      tauk2 = tauk1;
+      tauk2 = tauk2 * psibisk2 / psik2;
+      tauk1 = (xik1 - thetak2 * tauk2) / psibisk1;
+      xik = zetak - omegak2 * tauk2;
+      tauk = (xik - thetabark1 * tauk1) / psibark;
+    }
+
+    // (Qₖ)ᵀβ₁e₁ = (χ₁, ..., χₖ, χbarₖ₊₁)
+    if (iter == 1) chibark = beta1;
+    const T chik = ck * chibark;
+    const T chibark1 = sk * chibark;
+
+    // pₖ₊₁ = [P̂ₖ 0; 0 1](Qₖ)ᵀβ₁e₁
+    if (iter == 1) {
+      pik = chik;
+    } else if (iter == 2) {
+      const T piaux1 = pik1;
+      pik1 = ch3 * piaux1 + sh3 * chik;
+      pik = sh3 * piaux1 - ch3 * chik;
+    } else {
+      const T piaux2 = pik2;
+      pik2 = ch4 * piaux2 + sh4 * chik;
+      pik = sh4 * piaux2 - ch4 * chik;
+      const T piaux1 = pik1;
+      pik1 = ch3 * piaux1 + sh3 * pik;
+      pik = sh3 * piaux1 - ch3 * pik;
+    }
+    const T pik_1 = chibark1;                                 // πₖ₊₁
+
+    if (iter == 1) rNorm = std::sqrt((pik - tauk) * (pik - tauk) + pik_1 * pik_1);
+    else rNorm = std::sqrt((pik1 - tauk1) * (pik1 - tauk1) + (pik - tauk) * (pik - tauk) + pik_1 * pik_1);
+    if (history) stats.residuals.push_back(rNorm);
+
+    breakdown = (double)betak1 <= btol;
+    solved = (rNorm <= eps_tol) || (ArNorm <= kappa);
+    tired = iter >= itmax;
+    run.poll(iter, user_exit, overtimed);
+
+    std::swap(vk, vk1);
+    if (iter >= 2) {
+      std::swap(wk2, wk1);
+      std::swap(dk2, dk1);
+      epsk2 = epsk1;
+      ct4 = ct2; st4 = st2;
+      xik1 = xik;
+      psibisk2 = psibisk1;
+      thetabark2 = thetabark1;
+      pik2 = pik1;
+    }
+    ct3 = ct1; st3 = st1;
+    ct2 = ct0; st2 = st0;
+    betak = betak1;
+    chibark = chibark1;
+    psibark1 = psibark;
+    pik1 = pik;
+    if (k <= ell - 1) {
+      alphak = alphak1;
+      betak1 = betak2;
+      gammak1 = gammak;
+      lambdabark = lambdabark1;
+      zetabisk = zetabisk1;
+    }
+    if (k <= ell - 2) {
+      epsk1 = epsk;
+      gammabark = gammabark1;
+      zetabark1 = zetabark2;
+    }
+    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %7.1e  %7.1e  %8.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm, (double)betak, (double)zetak, run.elapsed());
+  }
+  if (o.verbose > 0) printf("\n");
+  std::string status = "unknown";                             // a breakdown alone leaves it so
+  if (solved) status = "solution good enough given atol, rtol and Artol";
+  if (tired) status = "maximum number of iterations exceeded";
+  if (user_exit) status = "user-requested exit";
+  if (overtimed) status = "time limit exceeded";
+  run.finish(iter, solved, false, status);
+}
+
 #define INST(T)                                                                                                          \
+  template void car_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);             \
+  template void minares_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);         \
   template void cgs_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
   template void cg_lanczos_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&);        \
   template void dqgmres_solve<T>(Workspace<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \

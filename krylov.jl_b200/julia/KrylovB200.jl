@@ -196,7 +196,7 @@ end
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
                        :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25, :bilq => 12, :qmr => 13,
-                       :cg_lanczos => 100)
+                       :car => 32, :minares => 33, :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -284,15 +284,16 @@ function fill_stats!(ws, h::Handle, ::Type{T}) where T
   st
 end
 
-# kwargs: the union of cg.jl:100-111, minres.jl:138-151, gmres.jl:96-108, bicgstab.jl:105-116 (a solver ignores the
-# ones it does not have, exactly like the C layer's option families, interfaces/src/c_stores.jl:287-398)
+# kwargs: the union of cg.jl:100-111, minres.jl:138-151, gmres.jl:96-108, bicgstab.jl:105-116, car.jl:90-99 and
+# minares.jl:93-104 (a solver ignores the ones it does not have, exactly like the C layer's option families,
+# interfaces/src/c_stores.jl:287-398); MINARES's Artol travels in the axtol field of the extended options
 function fused_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; c::Union{Nothing,B200Vector{T}} = nothing,
                       M = I, N = I, ldiv::Bool = false, atol::T = √eps(T), rtol::T = √eps(T), etol::T = √eps(T),
                       conlim::T = 1 / √eps(T), itmax::Int = 0, timemax::Float64 = Inf, verbose::Int = 0,
                       history::Bool = false, callback = workspace -> false, iostream::IO = stdout,
                       radius::T = zero(T), linesearch::Bool = false, λ::T = zero(T), γ::T = √eps(T),
                       check_curvature::Bool = false, restart::Bool = false, reorthogonalization::Bool = false,
-                      memory::Int = 0, window::Int = 0) where T
+                      memory::Int = 0, window::Int = 0, Artol::T = √eps(T)) where T
   A.m == A.n || error("System must be square")
   length(b) == A.m || error("Inconsistent problem size")
   h = handle_for(method, ws, A, memory, window)
@@ -300,7 +301,7 @@ function fused_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; c::Un
   set_precond!(h, 1, N)
   user = Ref{Any}((callback, ws))
   cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
-  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, NaN, NaN, 0.0, NaN, 0, 1))
+  ext = Ref(CExt(history, ldiv, etol, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, γ, Artol, NaN, 0.0, NaN, 0, 1))
   o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, radius, restart, reorthogonalization, linesearch))
   GC.@preserve user ext o begin
     check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
@@ -332,7 +333,9 @@ for (fn, WS, sym, memexpr) in ((:cg!, :CgWorkspace, :cg, :(0)),
                                (:cr!, :CrWorkspace, :cr, :(0)), (:cgs!, :CgsWorkspace, :cgs, :(0)),
                                (:cg_lanczos!, :CgLanczosWorkspace, :cg_lanczos, :(0)), (:fom!, :FomWorkspace, :fom, :(length(ws.l))),
                                (:fgmres!, :FgmresWorkspace, :fgmres, :(length(ws.c))), (:dqgmres!, :DqgmresWorkspace, :dqgmres, :(length(ws.V))),
-                               (:diom!, :DiomWorkspace, :diom, :(length(ws.V))))
+                               (:diom!, :DiomWorkspace, :diom, :(length(ws.V))),
+                               # car! (M only) and minares! (λ, Artol; no preconditioner): fused passes on a B200CSR
+                               (:car!, :CarWorkspace, :car, :(0)), (:minares!, :MinaresWorkspace, :minares, :(0)))
   @eval begin
     Krylov.$fn(ws::Krylov.$WS{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
       fused_solve!($(QuoteNode(sym)), ws, A, b; memory = $memexpr, kw...)

@@ -39,7 +39,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "diom_", "dqgmres", "dqgmres_", "BlockGmresWorkspace", "block_gmres", "block_gmres_", "CsrOperator",
            "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_",
            "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_",
-           "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_"]
+           "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_",
+           "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_"]
 
 
 class B200Error(RuntimeError):
@@ -352,7 +353,7 @@ class KrylovWorkspace:
     def solve(self, A, b, *, c=None, M=None, N=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
               history=False, callback=None, radius=0.0, linesearch=False, lambda_=0.0, etol=None, conlim=None,
               restart=False, reorthogonalization=False, ldiv=False, fused=True, batch=0, time_kernels=False,
-              check_curvature=False, gamma=None):
+              check_curvature=False, gamma=None, artol=None):
         """solver!(ws, A, b; kwargs...)  -- kwargs as in cg.jl:100-111, gmres.jl:96-108,
         bicgstab.jl:105-116, minres.jl:138-151.  M / N: None (identity), a 1-D array
         (Diagonal preconditioner) or a host callable."""
@@ -375,6 +376,8 @@ class KrylovWorkspace:
             e.etol = float(etol)
         if conlim is not None:
             e.conlim = float(conlim)
+        if artol is not None:
+            e.axtol = float(artol)   # MINARES's Artol travels in the axtol field
         keep = []
         if callback is not None:
             wsref = self
@@ -547,6 +550,32 @@ class DiomWorkspace(KrylovWorkspace):
 
 class DqgmresWorkspace(KrylovWorkspace):
     solver = "dqgmres"
+
+
+class CarWorkspace(KrylovWorkspace):
+    solver = "car"
+
+    def solve(self, A, b, *, M=None, ldiv=False, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
+              history=False, callback=None, fused=True, **unknown):
+        """car!(ws, A, b; kwargs...)  -- kwargs as in car.jl:90-99: atol and rtol default to sqrt(eps), itmax = 0
+        means 2n.  M: None, the diagonal of a Diagonal preconditioner, or a host callable."""
+        if unknown:
+            raise B200Error(f"car!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        return super().solve(A, b, M=M, ldiv=ldiv, atol=atol, rtol=rtol, itmax=itmax, timemax=timemax, verbose=verbose,
+                             history=history, callback=callback, fused=fused)
+
+
+class MinaresWorkspace(KrylovWorkspace):
+    solver = "minares"
+
+    def solve(self, A, b, *, M=None, ldiv=False, lambda_=0.0, atol=None, rtol=None, artol=None, itmax=0,
+              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
+        """minares!(ws, A, b; kwargs...)  -- kwargs as in minares.jl:93-104 (λ is lambda_, Artol is artol; atol, rtol
+        and artol default to sqrt(eps)).  M must be None: the reference does not support preconditioners yet."""
+        if unknown:
+            raise B200Error(f"minares!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        return super().solve(A, b, M=M, ldiv=ldiv, lambda_=lambda_, atol=atol, rtol=rtol, artol=artol, itmax=itmax,
+                             timemax=timemax, verbose=verbose, history=history, callback=callback, fused=fused)
 
 
 class BlockGmresWorkspace(KrylovWorkspace):
@@ -964,7 +993,8 @@ _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "b
        "fom": FomWorkspace, "fgmres": FgmresWorkspace, "cgs": CgsWorkspace, "cg_lanczos": CgLanczosWorkspace,
        "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
        "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
-       "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace}
+       "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace, "car": CarWorkspace,
+       "minares": MinaresWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -1020,12 +1050,14 @@ cgls_, crls_, lslq_ = (_make_inplace(s) for s in ("cgls", "crls", "lslq"))
 cgls, crls, lslq = (_make_least_squares(s) for s in ("cgls", "crls", "lslq"))
 bilq_, qmr_ = (_make_inplace(s) for s in ("bilq", "qmr"))
 bilq, qmr = (_make_outofplace(s) for s in ("bilq", "qmr"))
+car_, minares_ = (_make_inplace(s) for s in ("car", "minares"))
+car, minares = (_make_outofplace(s) for s in ("car", "minares"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):
     return {"cg": cg, "gmres": gmres, "bicgstab": bicgstab, "minres": minres, "fom": fom, "fgmres": fgmres, "cgs": cgs,
             "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres, "bilq": bilq,
-            "qmr": qmr}[method](A, b, x0, **kw)
+            "qmr": qmr, "car": car, "minares": minares}[method](A, b, x0, **kw)
 
 
 # workspace_accessors.jl:140-152

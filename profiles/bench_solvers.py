@@ -1,7 +1,9 @@
 """Throughput of the other three solvers on the BASELINE configs 3 and 4 (+ MINRES on the Poisson matrix), fused
 phases vs the primitive path, with the algorithmic-byte roofline of SURVEY.md section 8(d).  One JSON line each.
 
-    python profiles/bench_solvers.py [gmres] [bicgstab] [minres] [--small]
+    python profiles/bench_solvers.py [gmres] [bicgstab] [minres] [car_minares] [--small]
+
+car_minares runs only when named.
 """
 import json
 import os
@@ -119,3 +121,19 @@ if "siblings" in which:   # SURVEY.md 8f-3: the sibling solvers on the same two 
                               iterations_per_s=round(niter / sec, 1), us_per_iteration=round(1e6 * sec / niter, 1),
                               launches_per_iteration=round(launches / niter, 2))), flush=True)
         ws.free()
+
+if "car_minares" in which:  # CAR and MINARES on the config-2 matrix (DESIGN.md §3a byte models)
+    N = 64 if small else 215
+    rp, ci, va = P.div_grad_csr(N, xp=torch, device=dev)
+    n, nnz = N ** 3, int(va.numel())
+    b = torch.ones(n, dtype=torch.float64, device=dev)
+    for name, vecs, kw in (("car", 20, dict(atol=0.0, rtol=0.0, itmax=100)),
+                           ("minares", 17, dict(atol=0.0, rtol=0.0, artol=0.0, itmax=100))):
+        res = {}
+        for fused in (1, 0):
+            ws = kb.krylov_workspace(name, n, n, np.float64, device="cuda")
+            ws.set_operator((rp, ci, va))
+            res[fused] = timed(ws, b, 2, fused=bool(fused), **kw)
+            ws.free()
+        B = nnz * 12 + (n + 1) * 4 + vecs * n * 8                  # nnz (v + i) + (n + 1) i + vecs n v, v = 8, i = 4
+        report(name, f"get_div_grad({N}) f64, 100 iterations/solve", B, res)
