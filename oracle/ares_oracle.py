@@ -1,8 +1,7 @@
 """ctypes front-end of the CPU restatement of car! / minares! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_ares.h, built with the BLAS-1 wrappers of krylov_oracle_impl.h into libkrylov_oracle_ares.so by ares.mk.
-The symmetric problem generators of test/test_utils.jl that test/test_car.jl and test/test_minares.jl use are
+krylov_oracle_ares.h, built into the oracle library that oracle.py builds and loads.  The symmetric problem generators of test/test_utils.jl that test/test_car.jl and test/test_minares.jl use are
 re-exported from oracle.py; symmetric_inconsistent (test/test_utils.jl:128-132) is restated here.  Parity pinning:
 tests/test_oracle_car_minares.py and tests/golden/oracle_car_minares.json (frozen histories).
 """
@@ -10,49 +9,14 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle.oracle import (Stats, _csr, _opts, _p, _result, _suf, _vec, almost_singular, cartesian_poisson,  # noqa: F401
-                           get_div_grad, sparse_laplacian, singular_consistent, square_inconsistent,
-                           square_preconditioned, symmetric_definite, symmetric_indefinite, zero_rhs)
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_ITER_CB = C.CFUNCTYPE(C.c_int, C.c_int, C.c_void_p)
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_ares.so with the committed ares.mk (when missing or older than its sources)."""
-    so = os.path.join(_HERE, "libkrylov_oracle_ares.so")
-    srcs = [os.path.join(_HERE, f) for f in ("krylov_oracle_ares.c", "krylov_oracle_ares.h", "krylov_oracle_impl.h", "ares.mk")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "ares.mk", "-s"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-    return _LIB
-
-
-class dot_mode:
-    """with dot_mode(1): ...  -- this library's dot products accumulate in double and round once (test knob,
-    krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision."""
-
-    def __init__(self, mode):
-        self.mode = int(mode)
-
-    def __enter__(self):
-        lib().oracle_set_dot_mode(self.mode)
-
-    def __exit__(self, *a):
-        lib().oracle_set_dot_mode(0)
+from oracle.oracle import (_ITER_CB, Stats, _csr, _opts, _p, _result, _suf, _vec, almost_singular,  # noqa: F401
+                           cartesian_poisson, dot_mode, get_div_grad, lib, sparse_laplacian, singular_consistent,
+                           square_inconsistent, square_preconditioned, symmetric_definite, symmetric_indefinite,
+                           zero_rhs)
 
 
 def symmetric_inconsistent():

@@ -1,8 +1,7 @@
 """ctypes front-end of the CPU restatement of bilq! / qmr! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_biorth.h, built with the BLAS-1 wrappers of krylov_oracle_impl.h into libkrylov_oracle_biorth.so by
-biorth.mk.  The square problem generators of test/test_utils.jl that test/test_bilq.jl and test/test_qmr.jl use are
+krylov_oracle_biorth.h, built into the oracle library that oracle.py builds and loads.  The square problem generators of test/test_utils.jl that test/test_bilq.jl and test/test_qmr.jl use are
 re-exported from oracle.py; unsymmetric_breakdown (test/test_utils.jl:196-201) is restated here.  Parity pinning:
 tests/test_oracle_bilq_qmr.py and tests/golden/oracle_bilq_qmr.json (frozen histories).
 """
@@ -10,50 +9,14 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle.oracle import (Stats, _csr, _opts, _p, _result, _suf, _vec, bc_breakdown, kron_unsymmetric,  # noqa: F401
-                           nonsymmetric_definite, nonsymmetric_indefinite, polar_poisson, sparse_laplacian,
-                           square_preconditioned, symmetric_definite, symmetric_indefinite, two_preconditioners,
-                           zero_rhs)
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_ITER_CB = C.CFUNCTYPE(C.c_int, C.c_int, C.c_void_p)
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_biorth.so with the committed biorth.mk (when missing or older than its sources)."""
-    so = os.path.join(_HERE, "libkrylov_oracle_biorth.so")
-    srcs = [os.path.join(_HERE, f) for f in ("krylov_oracle_biorth.c", "krylov_oracle_biorth.h", "krylov_oracle_impl.h", "biorth.mk")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "biorth.mk", "-s"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-    return _LIB
-
-
-class dot_mode:
-    """with dot_mode(1): ...  -- this library's dot products accumulate in double and round once (test knob,
-    krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision."""
-
-    def __init__(self, mode):
-        self.mode = int(mode)
-
-    def __enter__(self):
-        lib().oracle_set_dot_mode(self.mode)
-
-    def __exit__(self, *a):
-        lib().oracle_set_dot_mode(0)
+from oracle.oracle import (_ITER_CB, Stats, _csr, _opts, _p, _result, _suf, _vec, bc_breakdown, dot_mode,  # noqa: F401
+                           kron_unsymmetric, lib, nonsymmetric_definite, nonsymmetric_indefinite, polar_poisson,
+                           sparse_laplacian, square_preconditioned, symmetric_definite, symmetric_indefinite,
+                           two_preconditioners, zero_rhs)
 
 
 def unsymmetric_breakdown():

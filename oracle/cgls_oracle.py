@@ -1,43 +1,21 @@
 """ctypes front-end of the CPU restatement of cgls! / crls! / lslq! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_cgls.h and krylov_oracle_lslq.h, built with the BLAS-1 wrappers of krylov_oracle_impl.h and the rectangular products of
-krylov_oracle_lsq.h into libkrylov_oracle_cgls.so by cgls.mk.  The least-squares problem generators are re-exported
-from lsq_oracle.py.  Parity pinning: tests/test_oracle_cgls.py (the reference's assertions of test/test_cgls.jl and
+krylov_oracle_cgls.h and krylov_oracle_lslq.h, on the rectangular products of krylov_oracle_lsq.h, built into the
+oracle library that oracle.py builds and loads.  The least-squares problem generators are re-exported from
+lsq_oracle.py.  Parity pinning: tests/test_oracle_cgls.py (the reference's assertions of test/test_cgls.jl and
 test/test_crls.jl) and tests/golden/oracle_cgls.json (frozen histories).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
 from oracle.lsq_oracle import lsq_test, lstp, regularization, saddle_point, sqd  # noqa: F401
-from oracle.oracle import Stats, _p, _result, _suf, _vec, zero_rhs  # noqa: F401
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_cgls.so with the committed cgls.mk (when missing or older than its sources)."""
-    so = os.path.join(_HERE, "libkrylov_oracle_cgls.so")
-    srcs = [os.path.join(_HERE, f) for f in ("krylov_oracle_cgls.c", "krylov_oracle_cgls.h", "krylov_oracle_lslq.h", "krylov_oracle_lsq.h",
-                                             "krylov_oracle_impl.h", "cgls.mk")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "cgls.mk", "-s"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-    return _LIB
+from oracle.oracle import Stats, _p, _result, _suf, _vec, lib, zero_rhs  # noqa: F401
 
 
 class CglsOpts(C.Structure):

@@ -1,14 +1,16 @@
 /*
  * krylov_oracle.c -- TEST INFRASTRUCTURE ONLY.  CPU restatement of the
- * Krylov.jl hot path (see krylov_oracle_impl.h for the per-function
- * reference citations and the parity-pinning status).  Built by
- * oracle/Makefile into oracle/libkrylov_oracle.so; loaded by oracle/oracle.py.
+ * Krylov.jl solvers (see krylov_oracle_impl.h for the per-function
+ * reference citations and the parity-pinning status): every solver family's
+ * header, instantiated in Float64 and Float32.  Built by oracle/Makefile into
+ * oracle/libkrylov_oracle.so; loaded by oracle/oracle.py.
  * The product library (krylov.jl_b200/) never links, loads or calls this.
  */
 #include <math.h>
 #include <float.h>
 #include <stdlib.h>
 #include <string.h>
+#include <time.h>
 
 int oracle_dot_mode = 0;
 void oracle_set_dot_mode(int m) { oracle_dot_mode = m; }
@@ -23,9 +25,15 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #define COPYSIGN copysign
 #define POW pow
 #define EPS DBL_EPSILON
+#define FLTMAX_OF DBL_MAX
 #include "krylov_oracle_impl.h"
 #include "krylov_oracle_siblings.h"
 #include "krylov_oracle_block.h"
+#include "krylov_oracle_lsq.h"
+#include "krylov_oracle_cgls.h"
+#include "krylov_oracle_lslq.h"
+#include "krylov_oracle_biorth.h"
+#include "krylov_oracle_ares.h"
 #undef REAL
 #undef SUF
 #undef SQRT
@@ -33,6 +41,7 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #undef COPYSIGN
 #undef POW
 #undef EPS
+#undef FLTMAX_OF
 
 /* ---- Float32 instantiation ---- */
 #define REAL float
@@ -42,9 +51,15 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #define COPYSIGN copysignf
 #define POW powf
 #define EPS FLT_EPSILON
+#define FLTMAX_OF FLT_MAX
 #include "krylov_oracle_impl.h"
 #include "krylov_oracle_siblings.h"
 #include "krylov_oracle_block.h"
+#include "krylov_oracle_lsq.h"
+#include "krylov_oracle_cgls.h"
+#include "krylov_oracle_lslq.h"
+#include "krylov_oracle_biorth.h"
+#include "krylov_oracle_ares.h"
 
 
 /* ---------------------------------------------------------------------------

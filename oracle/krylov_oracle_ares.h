@@ -1,19 +1,13 @@
 /*
  * krylov_oracle_ares.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included
  * first).  Literal restatement of car! (src/car.jl:108-256) and minares! (src/minares.jl:113-595) for real element
- * types, built with the BLAS-1 wrappers of krylov_oracle_impl.h into libkrylov_oracle_ares.so by ares.mk and loaded by
+ * types on the BLAS-1 wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle.c and loaded by
  * oracle/ares_oracle.py.  Parity pinning: tests/test_oracle_car_minares.py (the reference's assertions of
  * test/test_car.jl and test/test_minares.jl) and tests/golden/oracle_car_minares.json (frozen histories).
  * Both solvers minimize ||A r_k|| over the same Krylov space: CAR through CG-like short recurrences, MINARES through
  * the symmetric Lanczos process.  The callback (NULL: none) returns nonzero to stop; timemax < 0 means no limit.
  */
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
-#ifndef ORACLE_ARES_DEFINED
-#define ORACLE_ARES_DEFINED
-#include <time.h>
-typedef int (*oracle_iter_cb)(int iter, void *user);
-static double oracle_now(void) { struct timespec ts; timespec_get(&ts, TIME_UTC); return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec; }
-#endif
 
 /* ============ car!  (src/car.jl:108-256) ============
  * Mdiag: NULL => M === I (then Mu aliases u), else M = Diagonal(Mdiag) applied with mul! or ldiv!. */

@@ -1,7 +1,7 @@
 /*
  * krylov_oracle_biorth.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included
- * first).  Literal restatement of bilq! (src/bilq.jl:118-407) and qmr! (src/qmr.jl:124-405), built with the BLAS-1
- * wrappers of krylov_oracle_impl.h into libkrylov_oracle_biorth.so by biorth.mk and loaded by oracle/biorth_oracle.py.
+ * first).  Literal restatement of bilq! (src/bilq.jl:118-407) and qmr! (src/qmr.jl:124-405) on the BLAS-1 wrappers of
+ * krylov_oracle_impl.h, instantiated by krylov_oracle.c and loaded by oracle/biorth_oracle.py.
  * Parity pinning: tests/test_oracle_bilq_qmr.py (the reference's assertions of test/test_bilq.jl and test/test_qmr.jl)
  * and tests/golden/oracle_bilq_qmr.json (frozen histories).
  */
@@ -13,12 +13,6 @@
  * as its own CSR (rows ascending in each column of A: the order of the reference's adjoint product).  The callback
  * (NULL: none) returns nonzero to stop; timemax < 0 means no limit.  Unlike the reference, v / u / w are copied and
  * swapped exactly as written (kcopy!, @kswap!). */
-#ifndef ORACLE_BIORTH_DEFINED
-#define ORACLE_BIORTH_DEFINED
-#include <time.h>
-typedef int (*oracle_iter_cb)(int iter, void *user);
-static double oracle_now(void) { struct timespec ts; timespec_get(&ts, TIME_UTC); return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec; }
-#endif
 int SUF(oracle_biorth)(int qmr, int n, const int *rowptr, const int *colind, const REAL *val,
                        const int *trowptr, const int *tcolind, const REAL *tval,
                        const REAL *b, const REAL *c_in, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,

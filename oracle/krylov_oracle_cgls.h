@@ -1,6 +1,6 @@
 /*
  * krylov_oracle_cgls.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h; include it and
- * krylov_oracle_lsq.h first, instantiated by krylov_oracle_cgls.c).  Literal restatements of the least-squares solvers
+ * krylov_oracle_lsq.h first, instantiated by krylov_oracle.c).  Literal restatements of the least-squares solvers
  * on the normal equations, on an m x n CSR matrix:
  *   cgls!  src/cgls.jl:129-243
  *   crls!  src/crls.jl:120-268

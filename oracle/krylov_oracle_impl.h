@@ -244,6 +244,11 @@ static void set_status(oracle_stats *st, const char *s) {
   strncpy(st->status, s, sizeof(st->status) - 1);
   st->status[sizeof(st->status) - 1] = 0;
 }
+
+/* Per-iteration callback of the solvers that take one (NULL: none): returns nonzero to stop. */
+typedef int (*oracle_iter_cb)(int iter, void *user);
+/* Wall clock in seconds, for timemax. */
+static double oracle_now(void) { struct timespec ts; timespec_get(&ts, TIME_UTC); return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec; }
 #endif
 
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)

@@ -1,6 +1,6 @@
 /*
  * krylov_oracle_lslq.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h; include it and
- * krylov_oracle_lsq.h first, instantiated by krylov_oracle_cgls.c).  Literal restatement of lslq! (src/lslq.jl:201-520)
+ * krylov_oracle_lsq.h first, instantiated by krylov_oracle.c).  Literal restatement of lslq! (src/lslq.jl:201-520)
  * on an m x n CSR matrix, with the products of krylov_oracle_lsq.h (A^T u in ascending row order of A).  M (m entries)
  * and N (n entries) are diagonals or NULL.
  * Parity pinning: the reference's own assertions of test/test_lslq.jl (tests/test_oracle_cgls.py).

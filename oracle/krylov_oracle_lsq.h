@@ -1,6 +1,6 @@
 /*
  * krylov_oracle_lsq.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included
- * first; instantiated by krylov_oracle_lsq.c).  Literal restatements of the least-squares solvers on an m x n CSR matrix:
+ * first; instantiated by krylov_oracle.c).  Literal restatements of the least-squares solvers on an m x n CSR matrix:
  *   lsqr!  src/lsqr.jl:174-440
  *   lsmr!  src/lsmr.jl:178-455
  * A v sums each row in ascending column order; A^T u sums each column in ascending row order of A (what a

@@ -1,8 +1,7 @@
 """ctypes front-end of the CPU restatement of lsqr! / lsmr! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_lsq.h, built with the BLAS-1 wrappers of krylov_oracle_impl.h into libkrylov_oracle_lsq.so by lsq.mk.
-The problem generators restate test/gen_lsq.jl and the least-squares helpers of test/test_utils.jl; the square
+krylov_oracle_lsq.h, built into the oracle library that oracle.py builds and loads.  The problem generators restate test/gen_lsq.jl and the least-squares helpers of test/test_utils.jl; the square
 generators the reference's LSQR / LSMR tests also use (zero_rhs, two_preconditioners, ddx) are re-exported from
 oracle.py.  Parity pinning: tests/test_oracle_lsq.py (the reference's assertions of test/test_lsqr.jl and
 test/test_lsmr.jl) and tests/golden/oracle_lsq.json (frozen histories).
@@ -11,32 +10,11 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle.oracle import Stats, _p, _result, _suf, _vec, ddx, two_preconditioners, zero_rhs  # noqa: F401
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_lsq.so with the committed lsq.mk (when missing or older than its sources)."""
-    so = os.path.join(_HERE, "libkrylov_oracle_lsq.so")
-    srcs = [os.path.join(_HERE, f) for f in ("krylov_oracle_lsq.c", "krylov_oracle_lsq.h", "krylov_oracle_impl.h", "lsq.mk")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "lsq.mk", "-s"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-    return _LIB
+from oracle.oracle import Stats, _p, _result, _suf, _vec, ddx, lib, two_preconditioners, zero_rhs  # noqa: F401
 
 
 class LsqOpts(C.Structure):

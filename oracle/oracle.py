@@ -22,6 +22,10 @@ import scipy.sparse as sp
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
+_SOURCES = ("krylov_oracle.c", "krylov_oracle_impl.h", "krylov_oracle_siblings.h", "krylov_oracle_block.h",
+            "krylov_oracle_lsq.h", "krylov_oracle_cgls.h", "krylov_oracle_lslq.h", "krylov_oracle_biorth.h",
+            "krylov_oracle_ares.h", "Makefile")
+_ITER_CB = C.CFUNCTYPE(C.c_int, C.c_int, C.c_void_p)    # oracle_iter_cb: nonzero stops the solve
 
 
 class Stats(C.Structure):
@@ -39,9 +43,10 @@ class Opts(C.Structure):
 
 
 def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle.so with the committed Makefile."""
+    """Compile oracle/libkrylov_oracle.so, every solver family's oracle, with the committed Makefile (when missing or
+    older than its sources)."""
     so = os.path.join(_HERE, "libkrylov_oracle.so")
-    srcs = [os.path.join(_HERE, f) for f in ("krylov_oracle.c", "krylov_oracle_impl.h", "krylov_oracle_siblings.h", "krylov_oracle_block.h", "Makefile")]
+    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
     if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["make", "-C", _HERE, "-s"])
     return so
@@ -113,8 +118,8 @@ def _result(st, x, res, extra=None):
 
 
 class dot_mode:
-    """with dot_mode(1): ...  -- the oracle's dot products accumulate in double and round once (test knob,
-    krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision."""
+    """with dot_mode(1): ...  -- the oracle's dot products, in every solver family, accumulate in double and round once
+    (test knob, krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision."""
 
     def __init__(self, mode):
         self.mode = int(mode)

@@ -59,6 +59,45 @@ def test_staged_spmv_family_register_budget():
                 assert regs <= 72, (name, regs)                        # the single-GPU variants keep 3 CTAs per SM
 
 
+# The fused passes of each solver family (fused_phases.cu): family -> [(filter on the demangled kernel name,
+# {kernel template: instantiations it matches, Float32 and Float64 together})].
+PHASE_KERNELS = {
+    "lsq": [(r"kb::(LsqP|LsqrP3|LsmrP3)", {"spmv_epi_tma": 6,        # P1, P2 (LSQR), P2 (LSMR) x Float32 / Float64
+                                           "stream_epi": 4})],       # the LSQR and LSMR P3 passes x 2
+    "cgls": [(r"kb::(Cgls|Crls)", {"spmv_epi_tma": 8,                # CGLS K1, K3 and CRLS L2, L4 x Float32 / Float64
+                                   "spmv_epi_rows": 8,
+                                   "stream_epi": 8}),                # CGLS K2, K4 and CRLS L1, L3 x 2
+             (r"kb::LslqUpdateBody", {"stream_epi": 2})],            # LSLQ's update pass (P1 / P2 are LSQR's)
+    "biorth": [(r"kb::Biorth", {"spmv_epi_tma": 4,                   # B1, B2 x Float32 / Float64
+                                "spmv_epi_rows": 4,
+                                "stream_epi": 6})],                  # QMR (first / later iterations), BiLQ x 2
+    "car_minares": [(r"kb::Car", {"spmv_epi_tma": 4,                 # C2 on a plain or gathered x, x Float32 / Float64
+                                  "stream_epi": 4}),                 # C1, C3 x 2
+                    (r"kb::Minares", {"spmv_epi_tma": 4,             # M1 on a plain or gathered x, x Float32 / Float64
+                                      "stream_epi": 6})],            # M2, M3 and the w-only pass x 2
+}
+
+
+@pytest.mark.parametrize("family", sorted(PHASE_KERNELS))
+def test_phase_kernels_fit_three_ctas_per_sm(family):
+    """The fused passes keep the 3-CTA/SM budget of the staged SpMV family: every spmv_epi_tma instantiation uses at
+    most 72 registers (288 threads x 72 x 3 CTAs fill the 64K register file), and no kernel of the family spills."""
+    ents = _entries("fused_phases")
+    if not shutil.which("c++filt"):
+        pytest.skip("c++filt not available")
+    dm = _demangle([e[0] for e in ents])
+    for pat, counts in PHASE_KERNELS[family]:
+        hit = [(dm[n], r, s) for n, r, s in ents if re.search(pat, dm[n])]
+        for tmpl, count in counts.items():
+            assert len([e for e in hit if e[0].startswith(f"void kb::{tmpl}<")]) == count, (pat, tmpl, hit)
+        f32 = sorted(e[0].replace("float", "double") for e in hit if "<float" in e[0])
+        assert f32 == sorted(e[0] for e in hit if "<double" in e[0]), (pat, hit)     # both precisions, in pairs
+        for name, regs, spill in hit:
+            assert spill == 0, (name, regs, spill)
+            if "spmv_epi_tma<" in name:
+                assert regs <= 72, (name, regs)
+
+
 def test_block_fast_kernels_do_not_spill():
     ents = _entries("block")
     dm = _demangle([e[0] for e in ents])

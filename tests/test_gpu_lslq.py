@@ -2,6 +2,7 @@
 of tests/test_gpu_cgls.py: same iteration count, status and `inconsistent`; residual, Aᴴ-residual and error-bound
 histories within 1e-6 relative (or 10x the oracle's own sensitivity to a few-ulp change of b); x within 1e-6."""
 import ctypes as C
+import functools
 import importlib.util
 import os
 
@@ -9,23 +10,16 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+import parity
 from krylov_b200 import _lib
 from krylov_b200 import problems as P
+from parity import TOL
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
-TOL = 1e-6
-
-
-def _load(name, path):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-H = _load("gpu_cgls_helpers", os.path.join(HERE, "test_gpu_cgls.py"))        # _compare, _shapes, _xsens
-G = _load("gen_golden_lslq", os.path.join(HERE, "golden", "gen_golden_lslq.py"))
+_spec = importlib.util.spec_from_file_location("gen_golden_lslq", os.path.join(HERE, "golden", "gen_golden_lslq.py"))
+G = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(G)
 BOUNDS = ("err_lbnds", "err_ubnds_lq", "err_ubnds_cg")
 
 
@@ -36,40 +30,18 @@ def CO():
     return cgls_oracle
 
 
-def _bsens(CO, A, b, kw):
-    """Running max of the oracle's relative change of each error-bound history under the perturbations of b that
-    test_gpu_cgls._sens uses (the bounds are built from the LQ iterates ζ, far more sensitive than the residuals)."""
-    _, s0 = CO.lslq(A, b, **kw)
-    out = {k: np.zeros(len(s0[k])) for k in BOUNDS}
-    for seed in range(3):
-        for ulps in (1, 8):
-            sign = np.random.default_rng(seed).choice([-1.0, 1.0], size=len(b))
-            _, s1 = CO.lslq(A, b * (1 + ulps * 2.2e-16 * sign), **kw)
-            for k in BOUNDS:
-                r0, r1 = np.asarray(s0[k]), np.asarray(s1[k])
-                n = min(len(r0), len(r1))
-                s = np.full(len(r0), np.inf)
-                s[:n] = np.abs(r0[:n] - r1[:n]) / np.maximum(np.abs(r0[:n]), 1e-300)
-                if len(s):
-                    out[k] = np.maximum(out[k], np.maximum.accumulate(s))
-    return out
-
-
 def _compare(CO, kb, A, b, **kw):
-    x, st, so = H._compare(CO, kb, "lslq", A, b, **kw)
+    """The bar of tests/test_gpu_cgls.py, and the error-bound histories against the oracle's with the same perturbations
+    of b (the bounds are built from the LQ iterates ζ, far more sensitive than the residuals)."""
+    x, st, so = parity.compare(CO.lslq, functools.partial(kb.lslq, n=A.shape[1]), A, b,
+                               keys=("residuals", "Aresiduals"), flags=("inconsistent",), floor=1e-9, **kw)
     assert st.error_with_bnd == so["error_with_bnd"]
     okw = {k: v for k, v in kw.items() if k not in ("fused", "gpu_A", "xtol")}
-    sens = None
+    runs = functools.cache(lambda: parity.perturbed_runs(CO.lslq, A, b, **okw))
     for key in BOUNDS:
         r, ro = np.asarray(getattr(st, key)), np.asarray(so[key])
         assert len(r) == len(ro), key
-        tol = np.full(len(ro), TOL)
-        ok = np.abs(r - ro) <= tol * np.abs(ro) + 1e-300
-        if not ok.all():
-            sens = sens or _bsens(CO, A, b, okw)
-            tol = np.maximum(TOL, 10 * sens[key][:len(ro)])
-            ok = np.abs(r - ro) <= tol * np.abs(ro) + 1e-300
-        assert ok.all(), f"{key}: max rel deviation {np.max(np.abs(r - ro) / np.maximum(np.abs(ro), 1e-300)):.3e}"
+        parity.assert_history(key, r, ro, lambda: parity.sens(ro, runs(), key), 1e-300)
     return x, st, so
 
 
@@ -80,14 +52,10 @@ def _compare_early(CO, kb, A, b, fused, **kw):
     k + 1 iterations), x against 10x the oracle's own change under the same perturbations; the full solve must stop
     within two iterations of the range of the perturbed runs."""
     _, so = CO.lslq(A, b, **kw)
-    stops = [so["niter"]]
-    for seed in range(3):
-        for ulps in (1, 8):
-            sign = np.random.default_rng(seed).choice([-1.0, 1.0], size=len(b))
-            stops.append(CO.lslq(A, b * (1 + ulps * 2.2e-16 * sign), **kw)[1]["niter"])
+    stops = [so["niter"]] + [s["niter"] for _, s in parity.perturbed_runs(CO.lslq, A, b, **kw)]
     if min(stops) > 3:
         kk = dict(kw, itmax=min(stops) - 3)
-        _compare(CO, kb, A, b, fused=fused, xtol=max(TOL, 10 * H._xsens(CO, "lslq", A, b, kk)), **kk)
+        _compare(CO, kb, A, b, fused=fused, xtol=None, **kk)
     else:
         _compare(CO, kb, A, b, fused=fused, **kw)
     _, st = kb.lslq(A, b, fused=fused, **kw)
@@ -97,13 +65,13 @@ def _compare_early(CO, kb, A, b, fused, **kw):
 @pytest.mark.parametrize("shape", ["square", "tall_lstp", "wide_lstp", "ddx", "grad7", "tall_gaps", "wide_gaps"])
 @pytest.mark.parametrize("fused", [True, False])
 def test_shapes_match_oracle(kb, CO, shape, fused):
-    A, b = H._shapes(CO)[shape]
+    A, b = parity.shapes()[shape]
     _compare_early(CO, kb, A, b, fused, itmax=200)
 
 
 @pytest.mark.parametrize("fused", [True, False])
 def test_options_match_oracle(kb, CO, fused):
-    A, b = H._shapes(CO)["tall_gaps"]
+    A, b = parity.shapes()["tall_gaps"]
     m, n = A.shape
     dm, dn = np.linspace(0.5, 2.0, m), np.linspace(1.0, 3.0, n)
     _compare_early(CO, kb, A, b, fused, lambda_=1e-2, itmax=300)                  # λ > 0 stays fused
@@ -139,7 +107,7 @@ def test_error_bounds_of_the_reference(kb, CO):
 def test_host_callbacks_and_device_b(kb, CO):
     import torch
     from scipy.sparse.linalg import aslinearoperator
-    A, b = H._shapes(CO)["grad7"]
+    A, b = parity.shapes()["grad7"]
     _compare(CO, kb, A, b, gpu_A=aslinearoperator(A), itmax=100)
     _compare(CO, kb, A, b, gpu_A=(lambda x: A @ x, lambda y: A.T @ y), itmax=100, sigma=1e-2)
     xo, so = CO.lslq(A, b, itmax=100)
@@ -161,7 +129,7 @@ def test_zero_rhs_and_zero_adjoint_residual(kb, CO, fused):
 
 
 def test_callback_unsupported_kwargs_and_abi(kb, CO):
-    A, b = H._shapes(CO)["grad7"]
+    A, b = parity.shapes()["grad7"]
     seen = []
 
     def cb(ws):
@@ -224,7 +192,7 @@ def test_bench_size_parity(kb, CO):
 
 
 def test_float32(kb, CO):
-    A, _ = H._shapes(CO)["square"]
+    A, _ = parity.shapes()["square"]
     b = A @ np.ones(A.shape[1])
     A32, b32 = A.astype(np.float32), b.astype(np.float32)
     _, so = CO.lslq(A32, b32, dtype=np.float32)

@@ -2,6 +2,7 @@
 same iteration count, status and `inconsistent`; residual and Aᴴ-residual histories within 1e-6 relative at every
 iteration (or 10x the oracle's own sensitivity to a few-ulp change of b, where that is larger); x within 1e-6."""
 import ctypes as C
+import functools
 import os
 import subprocess
 
@@ -9,12 +10,13 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+import parity
 from krylov_b200 import _lib
 from krylov_b200 import problems as P
+from parity import TOL
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TOL = 1e-6
 
 
 @pytest.fixture(scope="module")
@@ -25,80 +27,17 @@ def LO():
     return lsq_oracle
 
 
-def _sens(LO, solver, A, b, kw):
-    """Running max of the oracle's relative history change under small relative perturbations of b (three random sign
-    patterns of 1 and 8 ulps: the device's tree-ordered dot products differ from the oracle's sequential sums by a few
-    roundings, not one)."""
-    _, s0 = getattr(LO, solver)(A, b, **kw)
-    out = [np.zeros(len(s0["residuals"])), np.zeros(len(s0["Aresiduals"]))]
-    for seed in range(3):
-        for ulps in (1, 8):
-            sign = np.random.default_rng(seed).choice([-1.0, 1.0], size=len(b))
-            _, s1 = getattr(LO, solver)(A, b * (1 + ulps * 2.2e-16 * sign), **kw)
-            for i, key in enumerate(("residuals", "Aresiduals")):
-                r0, r1 = np.asarray(s0[key]), np.asarray(s1[key])
-                k = min(len(r0), len(r1))
-                s = np.full(len(r0), np.inf)
-                s[:k] = np.abs(r0[:k] - r1[:k]) / np.maximum(np.abs(r0[:k]), 1e-300)
-                out[i] = np.maximum(out[i], np.maximum.accumulate(s))
-    return out
-
-
-def _compare(LO, kb, solver, A, b, gpu_A=None, xtol=TOL, **kw):
+def _compare(LO, kb, solver, A, b, **kw):
     """Solve on the GPU (operator gpu_A, default A) and with the oracle; assert the parity bar."""
-    okw = {k: v for k, v in kw.items() if k not in ("fused",)}
-    xo, so = getattr(LO, solver)(A, b, **okw)
-    x, st = getattr(kb, solver)(A if gpu_A is None else gpu_A, b, history=True, n=A.shape[1], **kw)
-    x = x.cpu().numpy() if hasattr(x, "cpu") else x
-    assert (st.niter, st.status, st.inconsistent) == (so["niter"], so["status"], so["inconsistent"]), \
-        ((st.niter, st.status, st.inconsistent), (so["niter"], so["status"], so["inconsistent"]))
-    sens = None
-    for i, key in enumerate(("residuals", "Aresiduals")):
-        r, ro = np.asarray(getattr(st, key)), np.asarray(so[key])
-        assert len(r) == len(ro), key
-        tol = np.full(len(ro), TOL)
-        ok = np.abs(r - ro) <= tol * np.abs(ro) + 1e-9 * abs(ro[0])
-        if not ok.all():
-            sens = sens or _sens(LO, solver, A, b, okw)
-            tol = np.maximum(TOL, 10 * sens[i][:len(ro)])
-            ok = np.abs(r - ro) <= tol * np.abs(ro) + 1e-9 * abs(ro[0])
-        assert ok.all(), f"{key}: max rel deviation {np.max(np.abs(r - ro) / np.maximum(np.abs(ro), 1e-300)):.3e}"
-    assert np.linalg.norm(x - xo) <= xtol * max(np.linalg.norm(xo), 1e-300), np.linalg.norm(x - xo) / np.linalg.norm(xo)
-    return x, st, so
-
-
-def _rect_with_gaps(m, n, seed, density=0.08):
-    """Random m x n matrix with empty rows and empty columns."""
-    A = sp.random(m, n, density=density, random_state=seed, format="lil")
-    A[3, :] = 0
-    A[m - 1, :] = 0
-    A[:, 1] = 0
-    A[:, n - 2] = 0
-    A = sp.csr_matrix(A)
-    A.eliminate_zeros()
-    return A
-
-
-def _shapes(LO):
-    rng = np.random.default_rng(5)
-    b40, A40, *_ = LO.lsq_test(40, 40, 4, 2, 0)
-    b60, A60, *_ = LO.lsq_test(60, 30, 3, 3, 0)
-    Aw = sp.csr_matrix(A60.T)                                   # 30 x 60: m < n
-    D = sp.csr_matrix(LO.ddx(50))                                # 50 x 51
-    rp, ci, va = P.grad_csr(7)
-    G = sp.csr_matrix((va, ci, rp), shape=(len(rp) - 1, 7 ** 3))
-    R1, R2 = _rect_with_gaps(300, 120, 1), _rect_with_gaps(90, 200, 2)
-    Sq = sp.csr_matrix(sp.random(200, 200, density=0.05, random_state=3) + 4 * sp.identity(200))
-    return {"square": (Sq, rng.standard_normal(200)), "tall_lstp": (A60, b60), "wide_lstp": (Aw, rng.standard_normal(30)),
-            "ddx": (D, rng.standard_normal(50)), "grad7": (G, rng.standard_normal(G.shape[0])),
-            "tall_gaps": (R1, rng.standard_normal(300)), "wide_gaps": (R2, rng.standard_normal(90))}
+    return parity.compare(getattr(LO, solver), functools.partial(getattr(kb, solver), n=A.shape[1]), A, b,
+                          keys=("residuals", "Aresiduals"), flags=("inconsistent",), floor=1e-9, **kw)
 
 
 @pytest.mark.parametrize("solver", ["lsqr", "lsmr"])
 @pytest.mark.parametrize("shape", ["square", "tall_lstp", "wide_lstp", "ddx", "grad7", "tall_gaps", "wide_gaps"])
 @pytest.mark.parametrize("fused", [True, False])
 def test_shapes_match_oracle(kb, LO, solver, shape, fused):
-    A, b = _shapes(LO)[shape]
+    A, b = parity.shapes()[shape]
     _compare(LO, kb, solver, A, b, fused=fused, itmax=200)
 
 
@@ -113,7 +52,7 @@ def test_square_lstp_before_exhaustion(kb, LO, solver):
 
 @pytest.mark.parametrize("solver", ["lsqr", "lsmr"])
 def test_options_match_oracle(kb, LO, solver):
-    A, b = _shapes(LO)["tall_gaps"]
+    A, b = parity.shapes()["tall_gaps"]
     m, n = A.shape
     dm = np.linspace(0.5, 2.0, m)
     dn = np.linspace(1.0, 3.0, n)
@@ -133,7 +72,7 @@ def test_options_match_oracle(kb, LO, solver):
 def test_host_callbacks_and_device_b(kb, LO, solver):
     import torch
     from scipy.sparse.linalg import aslinearoperator
-    A, b = _shapes(LO)["grad7"]
+    A, b = parity.shapes()["grad7"]
     _compare(LO, kb, solver, A, b, gpu_A=aslinearoperator(A), itmax=100)
     _compare(LO, kb, solver, A, b, gpu_A=(lambda x: A @ x, lambda y: A.T @ y), itmax=100)
     xo, so = getattr(LO, solver)(A, b, itmax=100)
@@ -159,7 +98,7 @@ def test_exact_breakdowns(kb, LO, solver, fused):
 
 @pytest.mark.parametrize("solver", ["lsqr", "lsmr"])
 def test_callback_user_exit(kb, LO, solver):
-    A, b = _shapes(LO)["grad7"]
+    A, b = parity.shapes()["grad7"]
     seen = []
 
     def cb(ws):
@@ -210,7 +149,7 @@ def test_bench_size_parity(kb, LO, solver):
 
 @pytest.mark.parametrize("solver", ["lsqr", "lsmr"])
 def test_float32(kb, LO, solver):
-    A, _ = _shapes(LO)["square"]
+    A, _ = parity.shapes()["square"]
     b = A @ np.ones(A.shape[1])
     A32, b32 = A.astype(np.float32), b.astype(np.float32)
     xo, so = getattr(LO, solver)(A32, b32, dtype=np.float32)
@@ -242,7 +181,7 @@ def test_rectangular_spmv_and_transpose_bit_exact(shape):
     L = _lib.lib()
     m, n = shape
     rng = np.random.default_rng(4)
-    A = _rect_with_gaps(m, n, 9, density=0.01)
+    A = parity.rect_with_gaps(m, n, 9, density=0.01)
     A.data = rng.integers(-4, 5, size=A.nnz).astype(np.float64)
     A.eliminate_zeros()
     A.sort_indices()
