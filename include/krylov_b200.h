@@ -45,10 +45,11 @@ typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
 /* positional, frozen (krylov.h:48-83).  Implemented here: CG, MINRES, GMRES, BICGSTAB (the hot path), the
  * siblings CR, DIOM, DQGMRES, FOM, FGMRES, CGS that run on the same kernels, CAR and MINARES on a symmetric operator
  * (CAR takes M, MINARES the shift `lambda` and no preconditioner; neither takes N), BILQ and QMR on a square operator and
- * its adjoint (matvec_At with matvec_A, or the transpose of an attached CSR operator; `c` is accepted, default b), and
- * the least-squares solvers LSQR, LSMR, LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A
- * maps n -> m and matvec_At m -> n, or a CSR operator of m rows and n columns is attached); every other value returns
- * -2. */
+ * its adjoint (matvec_At with matvec_A, or the transpose of an attached CSR operator; `c` is accepted, default b), the
+ * adjoint pairs A x = b, A^T y = c of BILQR (square A) and TRILQR (A m x n: b and y have m entries, c and x have n),
+ * which require c, take no preconditioner and return y through krylov_get_y, and the least-squares solvers LSQR, LSMR,
+ * LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a
+ * CSR operator of m rows and n columns is attached); every other value returns -2. */
 typedef enum {
   KRYLOV_CG = 0, KRYLOV_CR = 1, KRYLOV_SYMMLQ = 2, KRYLOV_MINRES = 3, KRYLOV_MINRES_QLP = 4, KRYLOV_DIOM = 5,
   KRYLOV_DQGMRES = 6, KRYLOV_FOM = 7, KRYLOV_GMRES = 8, KRYLOV_FGMRES = 9, KRYLOV_BICGSTAB = 10, KRYLOV_CGS = 11,
@@ -99,12 +100,14 @@ void krylov_get_version(int *major, int *minor, int *patch);
 int krylov_solve(void *ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, KrylovMatvec matvec_M, KrylovMatvec matvec_N,
                  const void *b, const void *c, void *userdata, const KrylovOptions *opts);
 int krylov_get_x(void *ws, void *x, int n);
-int krylov_get_y(void *ws, void *y, int m); /* -2: single-solution solver */
+int krylov_get_y(void *ws, void *y, int m); /* BILQR, TRILQR: y (m entries); -2: single-solution solver */
 int krylov_is_solved(void *ws);             /* 1 | 0 | -1 */
 int krylov_niter(void *ws);
 double krylov_elapsed_time(void *ws);
 int krylov_warm_start(void *ws, const void *x0, int n);
-int krylov_warm_start2(void *ws, const void *x0, const void *y0, int nx, int ny); /* -2 here */
+/* BILQR, TRILQR: x0 (n entries) and y0 (m entries), -1 when the lengths differ; -2: single-solution solver.
+ * krylov_warm_start on a BILQR / TRILQR workspace returns -1. */
+int krylov_warm_start2(void *ws, const void *x0, const void *y0, int nx, int ny);
 int krylov_workspace_free(void *ws); /* 0 | 1 if the handle is unknown (double free is safe) */
 
 /* Block solvers (krylov.h:250-285): KRYLOV_BLOCK_GMRES is implemented (p <= 32, Float32 / Float64; the tall-skinny
@@ -138,7 +141,8 @@ const char *krylov_b200_last_error(void);
  * cg.jl:196, gmres.jl:257, bicgstab.jl:221,228, minres.jl:289.
  *   rowptr[n+1], colind[nnz], values[nnz] (element type = workspace dtype);
  *   least-squares workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
- *   least-squares, BiLQ and QMR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
+ *   TriLQR workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
+ *   least-squares, BiLQ, QMR, BiLQR and TriLQR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
  *   until the operator changes;
  *   index_base 0|1, index_bytes 4|8 (Julia's SparseMatrixCSC{T,Int64} passes
  *   1 and 8 -- for a symmetric matrix its CSC arrays ARE the CSR arrays);
@@ -187,7 +191,8 @@ typedef struct {
   double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0                       */
   double utol;         /* LSLQ: kwarg `utol`; NaN -> sqrt(eps)                                                       */
   int transfer_to_lsqr; /* LSLQ: 1 -> return the LSQR point (kwarg `transfer_to_lsqr`)                                */
-  int transfer_to_bicg; /* BiLQ: 1 (default) -> return the BiCG point when it converges first (kwarg `transfer_to_bicg`) */
+  int transfer_to_bicg; /* BiLQ, BiLQR: 1 (default) -> return the BiCG point when it converges first (kwarg `transfer_to_bicg`);
+                          TriLQR: its kwarg `transfer_to_usymcg` (the USYMCG point), in the same field                  */
 } KrylovB200Options;
 KrylovB200Options krylov_b200_default_options(void);
 int krylov_b200_set_options(void *ws, const KrylovB200Options *opts);
@@ -210,13 +215,18 @@ typedef struct {
   int nerr_lbnds;      /* LSLQ history lengths (krylov_b200_get_history which = 3, 4, 5)                        */
   int nerr_ubnds_lq;
   int nerr_ubnds_cg;
+  int solved_primal;   /* AdjointStats (src/krylov_stats.jl:263-280) of BiLQR / TriLQR; `solved` = solved_primal && solved_dual */
+  int solved_dual;
+  int nresiduals_dual; /* length of residuals_dual (krylov_b200_get_history which = 6); residuals_primal is which = 0 */
 } KrylovB200Stats;
 int krylov_b200_get_stats(void *ws, KrylovB200Stats *out);
-/* which: 0 residuals, 1 Aresiduals, 2 Acond; LSLQ: 3 err_lbnds, 4 err_ubnds_lq, 5 err_ubnds_cg.
+/* which: 0 residuals, 1 Aresiduals, 2 Acond; LSLQ: 3 err_lbnds, 4 err_ubnds_lq, 5 err_ubnds_cg; BiLQR / TriLQR:
+ * 0 residuals_primal, 6 residuals_dual.
  * Returns the number copied (<= cap) or -1. */
 int krylov_b200_get_history(void *ws, int which, double *out, int cap);
 /* Device pointer of a workspace vector by its reference field name
- * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"). */
+ * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"; BiLQR / TriLQR: "y", "d̅",
+ * "wₖ₋₃", "wₖ₋₂", "uₖ₋₁", "uₖ", "vₖ₋₁", "vₖ", "q", "p", "Δx", "Δy"). */
 int krylov_b200_get_vector(void *ws, const char *name, void **dev_ptr);
 /* Average durations (ms) of the fused kernels measured with CUDA events on the workspace stream during the
  * last solve run with time_kernels = 1: out[0] = K1 (SpMV + p update + <p,Ap>), out[1] = K2 (x, r update + <r,r>),

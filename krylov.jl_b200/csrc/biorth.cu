@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <utility>
 
+#include "biorth_lq.h"
 #include "solver_common.h"
 
 namespace kb {
@@ -36,40 +37,6 @@ template <class T> struct QmrQR {
     zeta = c * zetabar;
     zetabar1 = s * zetabar;
     s1 = s; c1 = c;
-  }
-};
-
-// LQ factorization of T_k and the forward substitution for z̄_k (bilq.jl:265-305)
-template <class T> struct BilqLQ {
-  T c1 = -1, c = -1, s1 = 0, s = 0;          // c_{k-1}, c_k, s_{k-1}, s_k
-  T zeta2 = 0, zeta1 = 0, zetabar = 0;       // ζ_{k-2}, ζ_{k-1}, ζ̄_k
-  T eta1 = 0, eta = 0, dbar1 = 0, dbar = 0;  // η_{k-1}, η_k, δ̄_{k-1}, δ̄_k
-  T norm_v = 0;                              // ||v_k||
-  void step(int iter, T alpha, T beta, T gamma) {
-    T delta1 = 0, lambda = 0, eps2 = 0;
-    if (iter == 1) {
-      dbar = alpha;
-    } else if (iter == 2) {
-      sym_givens<T>(dbar1, gamma, &c, &s, &delta1);
-      lambda = c * beta + s * alpha;
-      dbar = s * beta - c * alpha;
-    } else {
-      sym_givens<T>(dbar1, gamma, &c, &s, &delta1);
-      eps2 = s1 * beta;
-      lambda = -c1 * c * beta + s * alpha;
-      dbar = -c1 * s * beta - c * alpha;
-    }
-    if (iter == 1) eta = beta;
-    if (iter == 2) { zeta1 = eta1 / delta1; eta = -lambda * zeta1; }
-    if (iter >= 3) { zeta2 = zeta1; zeta1 = eta1 / delta1; eta = -eps2 * zeta2 - lambda * zeta1; }
-  }
-  // ||r_k|| of the LQ point (bilq.jl:339-346); vv1 = <v_k, v_{k+1}>
-  T residual(int iter, T bNorm, T alpha, T beta, T beta1, T vv1, T norm_v1) const {
-    if (iter == 1) return bNorm;
-    const T mu = beta * (s1 * zeta2 - c1 * c * zeta1) + alpha * s * zeta1;
-    const T om = beta1 * s * zeta1;
-    const T th = mu * om * vv1;
-    return std::sqrt((mu * mu) * (norm_v * norm_v) + (om * om) * (norm_v1 * norm_v1) + 2 * th);
   }
 };
 

@@ -42,7 +42,7 @@ struct Handle {
   int p = 0;
   void* ws = nullptr;
   std::shared_ptr<CsrAny> csr;
-  std::shared_ptr<CsrAny> csrT;        // least squares, BiLQ, QMR: A^T of the attached operator, built on first use ...
+  std::shared_ptr<CsrAny> csrT;        // least squares, BiLQ, QMR, BiLQR, TriLQR: A^T of the attached operator, built on first use ...
   const CsrAny* csrT_for = nullptr;    // ... for this operator
   void* Mdiag = nullptr;
   void* Ndiag = nullptr;
@@ -79,7 +79,8 @@ int fail(const char* where, const char* msg) {
 bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
          s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
-         s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR || s == S_CAR || s == S_MINARES;
+         s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR || s == S_CAR || s == S_MINARES ||
+         s == S_BILQR || s == S_TRILQR;
 }
 
 int pick_device() {
@@ -116,6 +117,7 @@ int m_of(Handle* h) {
 bool is_ls(const Handle* h) { return !h->block && is_ls_kind(h->solver); }
 bool is_cg_ls(int s) { return s == S_CGLS || s == S_CRLS; }     // CGLS / CRLS: M on the residual space, no N
 bool is_biorth(int s) { return s == S_BILQ || s == S_QMR; }      // BiLQ / QMR: square, apply A and its adjoint
+bool is_adjoint(const Handle* h) { return !h->block && is_adjoint_kind(h->solver); }   // BiLQR / TriLQR: x and y
 template <class T> Csr<T>& csr_of(CsrAny& a);
 template <> Csr<double>& csr_of<double>(CsrAny& a) { return a.d; }
 template <> Csr<float>& csr_of<float>(CsrAny& a) { return a.f; }
@@ -186,6 +188,7 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   s.utol = std::isnan(h->ext.utol) ? -1 : h->ext.utol;
   s.transfer_to_lsqr = h->ext.transfer_to_lsqr != 0;
   s.transfer_to_bicg = h->ext.transfer_to_bicg != 0;
+  s.transfer_to_usymcg = h->ext.transfer_to_bicg != 0;   // TriLQR's kwarg travels in the same field
   // _typed_solve_gmres! serves GMRES, FGMRES and FOM (c_stores.jl:376-398)
   if (h->solver == S_GMRES || h->solver == S_FGMRES || h->solver == S_FOM) {
     s.restart = o->restart != 0; s.reorthogonalization = o->reorthogonalization != 0;
@@ -206,11 +209,16 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   return s;
 }
 
-// A^T of a CSR operator as a new object on context c (host-side transpose, once per operator)
-std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src) {
+// A^T of a CSR operator as a new object on context c (host-side transpose, once per operator).  rows > 0: at least
+// that many rows, the ones beyond A's columns empty.
+std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src, int rows = 0) {
   HostCsr hs, ht;
   if (src.dtype == KRYLOV_FLOAT64) csr_to_host<double>(c, src.d, hs); else csr_to_host<float>(c, src.f, hs);
   transpose_csr(hs, ht);
+  if (rows > ht.n) {
+    ht.rowptr.resize((size_t)rows + 1, ht.rowptr.back());
+    ht.n = rows;
+  }
   auto a = std::make_shared<CsrAny>();
   a->dtype = src.dtype; a->owner_ctx = &c;
   if (a->dtype == KRYLOV_FLOAT64) csr_from_host<double>(c, a->d, ht); else csr_from_host<float>(c, a->f, ht);
@@ -218,10 +226,11 @@ std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src) {
 }
 
 // A^T of the handle's CSR operator, formed once per attached operator and kept on the handle until it changes
+// TriLQR's has max(m, n) rows: its fused T2 pass finishes every row of q (m entries) in the launch over A^T's rows.
 template <class T> const Csr<T>* adjoint_csr(Handle* h, Workspace<T>* ws) {
   if (!h->csrT || h->csrT_for != h->csr.get()) {
     h->csrT.reset();
-    h->csrT = transpose_any(ws->ctx, *h->csr);
+    h->csrT = transpose_any(ws->ctx, *h->csr, h->solver == S_TRILQR ? std::max(ws->m, ws->n) : 0);
     h->csrT_for = h->csr.get();
   }
   return &csr_of<T>(*h->csrT);
@@ -350,6 +359,80 @@ int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, Kryl
   return 0;
 }
 
+// bilqr! / trilqr!: x (n entries) solves A x = b and y (m entries) solves A^T y = c; b has m entries, c has n.  A maps
+// n -> m (square for BiLQR) and needs its adjoint.  Neither solver takes a preconditioner.
+template <class T>
+int do_solve_adjoint(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, const void* c,
+                     void* ud, const KrylovOptions* opts) {
+  Workspace<T>* ws = W<T>(h);
+  const char* name = h->solver == S_BILQR ? "bilqr" : "trilqr";
+  if (fM || fN || h->Mdiag || h->Ndiag || h->Pblk[0] || h->Pblk[1])
+    throw std::runtime_error(std::string(name) + " takes no preconditioner (matvec_M, matvec_N or an attached M / N)");
+  if (!b) throw std::runtime_error("b is NULL");
+  if (!c) throw std::runtime_error(std::string(name) + " solves A^T y = c as well: c must be given");
+  KB_CUDA(cudaSetDevice(ws->ctx.device));
+  SolveOpts so = map_opts(h, opts);
+  const int m = ws->m, n = ws->n;
+  LinOp<T> A, At;
+  if (fA) {
+    if (!fAt) throw std::runtime_error(std::string(name) + " applies the adjoint of A: matvec_At must be given with matvec_A");
+    A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
+    At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
+  } else if (h->csr) {
+    const Csr<T>& C = csr_of<T>(*h->csr);
+    if (C.n != m || C.max_col >= n)
+      throw std::runtime_error("CSR operator: size inconsistent with the workspace ((m, n) = (" + std::to_string(m) + ", " +
+                               std::to_string(n) + "), operator rows = " + std::to_string(C.n) + ", largest column = " +
+                               std::to_string(C.max_col) + ")");
+    A.kind = LinOp<T>::CSR; A.csr = &C; A.n = m;
+    At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = At.csr->n;
+  } else {
+    throw std::runtime_error("no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr");
+  }
+  const T* bd = stage_in<T>(h, ws, b, ws->bbuf);                 // m entries
+  const T* cd = (const T*)c;                                     // n entries
+  if (h->device_kind != KRYLOV_CUDA) {
+    if (!ws->cbuf) ws->cbuf = dev_alloc<T>((size_t)n);
+    KB_CUDA(cudaMemcpyAsync(ws->cbuf, c, sizeof(T) * (size_t)n, cudaMemcpyHostToDevice, ws->ctx.stream));
+    cd = ws->cbuf;
+  }
+  if (h->solver == S_BILQR) bilqr_solve<T>(*ws, A, At, bd, cd, so);
+  else trilqr_solve<T>(*ws, A, At, bd, cd, so);
+  return 0;
+}
+
+template <class T> int do_get_y(Handle* h, void* y, int m) {
+  Workspace<T>* ws = W<T>(h);
+  if (m > ws->m) m = ws->m;
+  KB_CUDA(cudaSetDevice(ws->ctx.device));
+  KB_CUDA(cudaMemcpyAsync(y, ws->y, sizeof(T) * (size_t)m,
+                          h->device_kind == KRYLOV_CUDA ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ws->ctx.stream));
+  ws->ctx.sync();
+  return 0;
+}
+
+// warm_start!(workspace, x0, y0): x0 has n entries, y0 m
+template <class T> int do_warm_start2(Handle* h, const void* x0, const void* y0, int nx, int ny) {
+  Workspace<T>* ws = W<T>(h);
+  if (!x0 || !y0) throw std::runtime_error("x0 and y0 must be given");
+  if (nx != ws->n || ny != ws->m)
+    throw std::runtime_error("x0 should have size " + std::to_string(ws->n) + " and y0 size " + std::to_string(ws->m));
+  KB_CUDA(cudaSetDevice(ws->ctx.device));
+  const T* xd = (const T*)x0;
+  const T* yd = (const T*)y0;
+  T* stage = nullptr;
+  if (h->device_kind != KRYLOV_CUDA) {
+    stage = dev_alloc<T>((size_t)nx + (size_t)ny);
+    KB_CUDA(cudaMemcpyAsync(stage, x0, sizeof(T) * (size_t)nx, cudaMemcpyHostToDevice, ws->ctx.stream));
+    KB_CUDA(cudaMemcpyAsync(stage + nx, y0, sizeof(T) * (size_t)ny, cudaMemcpyHostToDevice, ws->ctx.stream));
+    xd = stage; yd = stage + nx;
+  }
+  ws_warm_start2<T>(ws, xd, yd);
+  ws->ctx.sync();
+  dev_free(stage);
+  return 0;
+}
+
 template <class T> int do_get_x(Handle* h, void* x, int n) {
   Workspace<T>* ws = W<T>(h);
   if (n > ws->n) n = ws->n;
@@ -362,6 +445,9 @@ template <class T> int do_get_x(Handle* h, void* x, int n) {
 
 template <class T> int do_warm_start(Handle* h, const void* x0, int n) {
   Workspace<T>* ws = W<T>(h);
+  if (is_adjoint_kind(h->solver))
+    throw std::runtime_error(std::string(h->solver == S_BILQR ? "bilqr" : "trilqr") +
+                             " solves two systems: warm-start it with krylov_warm_start2 (x0 and y0)");
   if (is_ls_kind(h->solver))
     throw std::runtime_error(is_cg_ls(h->solver)      ? "cgls and crls do not support warm-start (they take no x0)"
                              : h->solver == S_LSLQ ? "lslq does not support warm-start (it takes no x0)"
@@ -396,7 +482,14 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
   if (!strcmp(nm, "Mr") || !strcmp(nm, "Ms")) return ws->Mr;
   if (!strcmp(nm, "Mq")) return ws->kind == S_CGLS ? ws->Mr : ws->z;   // CGLS: Mq aliases Mr (cgls.jl:156)
   if (!strcmp(nm, "w̄") || !strcmp(nm, "wbar")) return ws->kind == S_LSLQ ? ws->w : nullptr;
-  if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ ? ws->w : nullptr;
+  if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ || is_adjoint_kind(ws->kind) ? ws->w : nullptr;
+  if (is_adjoint_kind(ws->kind)) {                 // BilqrWorkspace / TrilqrWorkspace (w_{k-3} / w_{k-2} rotate by pointer)
+    if (!strcmp(nm, "y") || !strcmp(nm, "t")) return ws->y;
+    if (!strcmp(nm, "Δx")) return ws->dx;
+    if (!strcmp(nm, "Δy") || !strcmp(nm, "dy")) return ws->dy;
+    if (!strcmp(nm, "wₖ₋₃") || !strcmp(nm, "w_prev3")) return ws->w1;
+    if (!strcmp(nm, "wₖ₋₂") || !strcmp(nm, "w_prev2")) return ws->w2;
+  }
   if (!strcmp(nm, "uₖ₋₁") || !strcmp(nm, "u_prev")) return ws->u_prev;      // BiLQ / QMR (rotated by pointer)
   if (!strcmp(nm, "vₖ₋₁") || !strcmp(nm, "v_prev")) return ws->v_prev;
   if (!strcmp(nm, "uₖ")) return ws->u;
@@ -461,6 +554,9 @@ int krylov_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, Krylov
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_solve", "unknown workspace handle");
+    if (is_adjoint(h))
+      return h->dtype == KRYLOV_FLOAT64 ? do_solve_adjoint<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts)
+                                        : do_solve_adjoint<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts);
     if (is_ls(h))                    // the square solvers never apply the adjoint
       return h->dtype == KRYLOV_FLOAT64 ? do_solve_ls<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts)
                                         : do_solve_ls<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts);
@@ -478,10 +574,13 @@ int krylov_get_x(void* ws, void* x, int n) {
 }
 
 int krylov_get_y(void* ws, void* y, int m) {
-  (void)y; (void)m;
-  Handle* h = lookup(ws);
-  if (!h) return fail("krylov_get_y", "unknown workspace handle");
-  return -2;   // solution_count == 1 for the four solvers (c_stores.jl:211-216)
+  try {
+    Handle* h = lookup(ws);
+    if (!h) return fail("krylov_get_y", "unknown workspace handle");
+    if (!is_adjoint(h)) return -2;   // solution_count == 1 (c_stores.jl:211-216): only BiLQR and TriLQR have a y
+    if (!y) return fail("krylov_get_y", "y is NULL");
+    return h->dtype == KRYLOV_FLOAT64 ? do_get_y<double>(h, y, m) : do_get_y<float>(h, y, m);
+  } catch (const std::exception& e) { return fail("krylov_get_y", e); }
 }
 
 int krylov_is_solved(void* ws) { Handle* h = lookup(ws); return h ? (stats_any(h).solved ? 1 : 0) : -1; }
@@ -497,10 +596,12 @@ int krylov_warm_start(void* ws, const void* x0, int n) {
 }
 
 int krylov_warm_start2(void* ws, const void* x0, const void* y0, int nx, int ny) {
-  (void)x0; (void)y0; (void)nx; (void)ny;
-  Handle* h = lookup(ws);
-  if (!h) return fail("krylov_warm_start2", "unknown workspace handle");
-  return -2;
+  try {
+    Handle* h = lookup(ws);
+    if (!h) return fail("krylov_warm_start2", "unknown workspace handle");
+    if (!is_adjoint(h)) return -2;
+    return h->dtype == KRYLOV_FLOAT64 ? do_warm_start2<double>(h, x0, y0, nx, ny) : do_warm_start2<float>(h, x0, y0, nx, ny);
+  } catch (const std::exception& e) { return fail("krylov_warm_start2", e); }
 }
 
 // One destroy routine for both handle kinds: sets the handle's device, drops the operator and the preconditioner
@@ -692,7 +793,7 @@ int krylov_b200_set_operator_csr(void* ws, int n, long long nnz, const void* row
     KB_CUDA(cudaSetDevice(cx.device));
     // n: number of rows (m of a least-squares workspace, whose operator has the workspace's n columns)
     if (n != m_of(h)) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
-    const int ncols = is_ls(h) ? n_of(h) : -1;
+    const int ncols = is_ls(h) || (!h->block && h->solver == S_TRILQR) ? n_of(h) : -1;
     if (h->dtype == KRYLOV_FLOAT64)
       csr_upload<double>(cx, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, ncols, &a->dd);
     else
@@ -800,6 +901,8 @@ int krylov_b200_get_stats(void* ws, KrylovB200Stats* out) {
   out->error_with_bnd = s.error_with_bnd;
   out->nerr_lbnds = (int)s.err_lbnds.size(); out->nerr_ubnds_lq = (int)s.err_ubnds_lq.size();
   out->nerr_ubnds_cg = (int)s.err_ubnds_cg.size();
+  out->solved_primal = s.solved_primal; out->solved_dual = s.solved_dual;
+  out->nresiduals_dual = (int)s.residuals_dual.size();
   return 0;
 }
 
@@ -809,7 +912,8 @@ int krylov_b200_get_history(void* ws, int which, double* out, int cap) {
   if (!out || cap < 0) return fail("krylov_b200_get_history", "bad arguments (out is NULL or cap < 0)");
   const Stats& s = stats_any(h);
   const std::vector<double>& v = which == 0 ? s.residuals : which == 1 ? s.Aresiduals : which == 3 ? s.err_lbnds
-                                : which == 4 ? s.err_ubnds_lq : which == 5 ? s.err_ubnds_cg : s.Acond;
+                                : which == 4 ? s.err_ubnds_lq : which == 5 ? s.err_ubnds_cg : which == 6 ? s.residuals_dual
+                                : s.Acond;
   int k = (int)v.size() < cap ? (int)v.size() : cap;
   for (int i = 0; i < k; i++) out[i] = v[i];
   return k;
@@ -976,6 +1080,7 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
       return fail("krylov_b200_dist_init", "row-partitioned BiLQ / QMR solves are not available");
     if (h->solver == S_CAR || h->solver == S_MINARES)
       return fail("krylov_b200_dist_init", "row-partitioned CAR / MINARES solves are not available");
+    if (is_adjoint(h)) return fail("krylov_b200_dist_init", "row-partitioned BiLQR / TriLQR solves are not available");
     return h->dtype == KRYLOV_FLOAT64 ? dist_init_t<double>(h, rank, world, nhalo, halo_rank, halo_off)
                                       : dist_init_t<float>(h, rank, world, nhalo, halo_rank, halo_off);
   } catch (const std::exception& e) { return fail("krylov_b200_dist_init", e); }

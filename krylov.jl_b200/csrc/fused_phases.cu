@@ -1175,6 +1175,169 @@ void minares_fused_update(Workspace<T>& ws, int iter, T* vk, bool scale, T beta,
                       NoFin(), 5);
 }
 
+// ===========================================================================
+// BiLQR / TriLQR  (src/bilqr.jl:227-418, src/trilqr.jl:210-397; adjoint pairs A x = b, A^T y = c)
+// BiLQR runs BiLQ's B1 / B2 unchanged and one update pass U over n.  TriLQR's SSY step is T1 (SpMV on A, alpha on the
+// device) and T2 (SpMV on A^T, which also finishes q over all m rows: beta_{k+1} = ||q|| is needed before U), then one
+// update pass over max(m, n).  U carries the primal half (x, d̅), the dual half (w_{k-1}, y) and the next v, u; a half
+// that has converged gets an instantiation without its vectors.
+// ===========================================================================
+template <class T> struct AdjointState { T alpha, qq, pp; };
+
+// Dual direction and solution (bilqr.jl:363-392, trilqr.jl:339-368), iteration >= 2: w_{k-1} = src / delta at iteration
+// 2 (kdivcopy!), else (w_{k-3} + src - lam2 w_{k-2}) / delta with w_{k-3} first scaled by -eps3 from iteration 4 on, in
+// the kscal!/kaxpy!/kaxpy!/kdiv! order; y += psi w_{k-1}.  wk is the buffer of w_{k-2} at iteration 2, of w_{k-3} after.
+// w_{k-3} is still the reference's zero vector at iteration 3: it is not read then, so the fused path needs no fill.
+template <class T> struct AdjointW {
+  T* wk; const T* w2; T* y; T eps3, lam2, delta, inv_delta, psi; int iter;
+  __device__ __forceinline__ void operator()(int i, T src) const {
+    T w;
+    if (iter == 2) {
+      w = div_rn(src, delta);
+    } else {
+      w = iter >= 4 ? mul_rn(-eps3, wk[i]) : T(0);
+      w = add_rn(w, mul_rn(T(1), src));
+      w = add_rn(w, mul_rn(-lam2, w2[i]));
+      w = mul_rn(inv_delta, w);
+    }
+    wk[i] = w;
+    y[i] = add_rn(y[i], mul_rn(psi, w));
+  }
+};
+// Primal direction and solution (bilqr.jl:299-311, trilqr.jl:283-295): d̅ = a at iteration 1, else x += (zeta c) d̅,
+// x += (zeta s) a, d̅ = -c a + s d̅ (a = v_k for BiLQR, u_k for TriLQR).
+template <class T> struct AdjointD {
+  T* dbar; T* x; T czeta, szeta, c, s; int iter;
+  __device__ __forceinline__ void operator()(int i, T a) const {
+    if (iter == 1) {
+      dbar[i] = a;
+    } else {
+      const T di = dbar[i];
+      x[i] = add_rn(add_rn(x[i], mul_rn(czeta, di)), mul_rn(szeta, a));
+      dbar[i] = add_rn(mul_rn(-c, a), mul_rn(s, di));
+    }
+  }
+};
+
+// The next v and u are written into the buffers of v_{k-1} and u_{k-1}, and the dual direction reads one of those
+// same buffers (u_{k-1} in BiLQR, v_{k-1} in TriLQR).  So every element of it is read, by the thread that then
+// overwrites it, before the next vector is stored: each body below calls the dual update first.
+template <class T, bool PRIMAL, bool DUAL> struct AdjointBilqrBody {
+  AdjointD<T> dd; AdjointW<T> w; const T* v; const T* q; const T* p; const T* u; T* vnext; T* unext; T beta1, gamma1; int keep;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    if (DUAL && w.iter >= 2) w(i, unext[i]);          // u_{k-1}, read before u_{k+1} overwrites it
+    const T qi = q[i];
+    if (PRIMAL) {
+      const T vi = v[i];
+      dd(i, vi);
+      d[0] += vi * qi; d[1] += qi * qi;
+    }
+    vnext[i] = keep ? v[i] : div_rn(qi, beta1);
+    const T un = keep ? u[i] : div_rn(p[i], gamma1);
+    unext[i] = un;
+    if (DUAL) d[2] += un * un;
+  }
+};
+template <class T, bool PRIMAL, bool DUAL> struct AdjointTrilqrBody {
+  AdjointD<T> dd; AdjointW<T> w; const T* v; const T* q; const T* p; const T* u; T* vnext; T* unext; T beta1, gamma1;
+  int m, n;
+  __device__ __forceinline__ void operator()(int i, T*) const {
+    if (i < m) {
+      if (DUAL && w.iter >= 2) w(i, vnext[i]);        // v_{k-1}, read before v_{k+1} overwrites it
+      vnext[i] = beta1 != T(0) ? div_rn(q[i], beta1) : v[i];
+    }
+    if (i < n) {
+      const T ui = u[i];
+      if (PRIMAL) dd(i, ui);
+      unext[i] = gamma1 != T(0) ? div_rn(p[i], gamma1) : ui;
+    }
+  }
+};
+template <class T> struct AdjointT1Epi {   // q = A u - gamma v_{k-1} ; <v, q>           (trilqr.jl:210,214,218)
+  T* q; const T* vprev; const T* v; T gamma; int first;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T qn = first ? acc : add_rn(acc, mul_rn(-gamma, vprev[row]));
+    q[row] = qn;
+    d[0] += v[row] * qn;
+  }
+};
+template <class T> struct AdjointT1Fin {
+  AdjointState<T>* s;
+  __device__ void operator()(const T* tot) const { s->alpha = tot[0]; }
+};
+// p = A^T v - beta u_{k-1} - alpha u (rows < n) ; q -= alpha v (rows < m) ; ||q||^2, ||p||^2   (trilqr.jl:211,215,220-224)
+template <class T> struct AdjointT2Epi {
+  T* p; T* q; const T* uprev; const T* u; const T* v; const AdjointState<T>* s; T beta; int m, n, first;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T alpha = s->alpha;
+    if (row < n) {
+      T pn = first ? acc : add_rn(acc, mul_rn(-beta, uprev[row]));
+      pn = add_rn(pn, mul_rn(-alpha, u[row]));
+      p[row] = pn;
+      d[1] += pn * pn;
+    }
+    if (row < m) {
+      const T qn = add_rn(q[row], mul_rn(-alpha, v[row]));
+      q[row] = qn;
+      d[0] += qn * qn;
+    }
+  }
+};
+template <class T> struct AdjointT2Fin {
+  AdjointState<T>* s;
+  __device__ void operator()(const T* tot) const { s->qq = tot[0]; s->pp = tot[1]; }
+};
+
+template <class T>
+void bilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T czeta, T szeta, T cs, T sn, T* wk, const T* w2,
+                        T eps3, T lam2, T delta1, T psi1, T beta1, T gamma1, bool keep, T* out3) {
+  Ctx& c = ws.ctx;
+  const AdjointD<T> dd{ws.w, ws.x, czeta, szeta, cs, sn, iter};
+  const AdjointW<T> w{wk, w2, ws.y, eps3, lam2, delta1, T(1) / delta1, psi1, iter};
+  const StoreFin<T, 3> fin{sib_slots<T>(c)};
+  const int k = keep ? 1 : 0;
+  if (primal && dual)
+    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, true, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin, 5);
+  else if (primal)
+    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, true, false>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin, 5);
+  else
+    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, false, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin, 5);
+  sib_read<T, 3>(c, out3);
+}
+
+template <class T>
+void trilqr_fused_ssy(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool first, T beta, T gamma, T* alpha, T* qq, T* pp) {
+  Ctx& c = ws.ctx;
+  typedef AdjointState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  St* H = (St*)ws.fused_host;
+  const int f = first ? 1 : 0;
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.u}, AdjointT1Epi<T>{ws.q, ws.v_prev, ws.v, gamma, f}, AdjointT1Fin<T>{S}, 4);
+  launch_spmv_epi_g<T, 2>(c, At, XPlain<T>{ws.v}, AdjointT2Epi<T>{ws.p, ws.q, ws.u_prev, ws.u, ws.v, S, beta, ws.m, ws.n, f},
+                          AdjointT2Fin<T>{S}, 4);
+  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
+  c.sync();
+  *alpha = H[1].alpha; *qq = H[1].qq; *pp = H[1].pp;
+}
+
+template <class T>
+void trilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T czeta, T szeta, T cs, T sn, T* wk, const T* w2,
+                         T eps3, T lam2, T delta1, T psi1, T beta1, T gamma1) {
+  Ctx& c = ws.ctx;
+  const AdjointD<T> dd{ws.w, ws.x, czeta, szeta, cs, sn, iter};
+  const AdjointW<T> w{wk, w2, ws.y, eps3, lam2, delta1, T(1) / delta1, psi1, iter};
+  const int len = std::max(ws.m, ws.n);
+  if (primal && dual)
+    launch_stream<T, 0>(c, len, AdjointTrilqrBody<T, true, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1,
+                                                                 ws.m, ws.n}, NoFin(), 5);
+  else if (primal)
+    launch_stream<T, 0>(c, len, AdjointTrilqrBody<T, true, false>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1,
+                                                                  ws.m, ws.n}, NoFin(), 5);
+  else
+    launch_stream<T, 0>(c, len, AdjointTrilqrBody<T, false, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1,
+                                                                  ws.m, ws.n}, NoFin(), 5);
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1205,7 +1368,10 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void car_fused_directions<T>(Workspace<T>&, const Csr<T>&, T, T*, T*);                                    \
   template void minares_fused_lanczos<T>(Workspace<T>&, const Csr<T>&, bool, int, T*, const T*, T*, const T*, T, T, T, T, T, \
                                          T*, T*);                                                                    \
-  template void minares_fused_update<T>(Workspace<T>&, int, T*, bool, T, T*, const T*, const T*, T, T, T, T);
+  template void minares_fused_update<T>(Workspace<T>&, int, T*, bool, T, T*, const T*, const T*, T, T, T, T);       \
+  template void bilqr_fused_update<T>(Workspace<T>&, bool, bool, int, T, T, T, T, T*, const T*, T, T, T, T, T, T, bool, T*); \
+  template void trilqr_fused_ssy<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T*, T*, T*);             \
+  template void trilqr_fused_update<T>(Workspace<T>&, bool, bool, int, T, T, T, T, T*, const T*, T, T, T, T, T, T);
 INST(double)
 INST(float)
 #undef INST

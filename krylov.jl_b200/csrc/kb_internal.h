@@ -11,6 +11,7 @@
 //   solver_common.h  host helpers of the drivers, among them SolveRun: the callback / clock / exit protocol
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
 //   biorth.cu     host control flow of bilq!/qmr! (one Lanczos biorthogonalization driver; A and A^T)
+//   adjoint.cu    host control flow of bilqr!/trilqr! (adjoint system pairs A x = b, A^T y = c; two solutions)
 //   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! on rectangular operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
@@ -176,7 +177,8 @@ struct SolveOpts {
   double axtol = -1, btol = -1;     // LSQR, LSMR (<0 => sqrt(eps(T))); btol: LSLQ too
   double sigma = 0, utol = -1;      // LSLQ: σ (Gauss-Radau bounds when > 0), utol (<0 => sqrt(eps(T)))
   bool transfer_to_lsqr = false;    // LSLQ
-  bool transfer_to_bicg = true;     // BiLQ
+  bool transfer_to_bicg = true;     // BiLQ, BiLQR
+  bool transfer_to_usymcg = true;   // TriLQR
   bool restart = false;             // GMRES, FOM, FGMRES
   bool reorthogonalization = false; // GMRES, FOM, FGMRES
   bool check_curvature = false;     // CG-Lanczos
@@ -199,19 +201,25 @@ struct Stats {
   double Anorm = NAN;                  // LanczosStats (cg_lanczos!)
   bool error_with_bnd = false;         // LSLQStats (lslq!)
   std::vector<double> err_lbnds, err_ubnds_lq, err_ubnds_cg;
+  bool solved_primal = false, solved_dual = false;   // AdjointStats (bilqr!, trilqr!): residuals holds residuals_primal
+  std::vector<double> residuals_dual;
   std::string status = "unknown";
   void reset() {
     residuals.clear(); Aresiduals.clear(); Acond.clear(); indefinite = false; npcCount = 0;
     err_lbnds.clear(); err_ubnds_lq.clear(); err_ubnds_cg.clear(); error_with_bnd = false;
+    residuals_dual.clear(); solved_primal = false; solved_dual = false;
   }
 };
 
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
-                  S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
+                  S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_TRILQR = 18, S_BILQR = 19, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
                   S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
 // the least-squares solvers: A is m x n, b has m entries and x has n
 inline bool is_ls_kind(int k) { return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS; }
+// the adjoint-pair solvers: two solutions, x (A x = b) and y (A^T y = c).  TriLQR: A is m x n, b and y have m entries,
+// c and x have n; BiLQR: square
+inline bool is_adjoint_kind(int k) { return k == S_BILQR || k == S_TRILQR; }
 
 // One workspace per (solver, dtype): owns every device vector of the solver
 // (src/krylov_workspaces.jl; SURVEY.md appendix B for fields and aliasing).
@@ -234,6 +242,8 @@ struct Workspace {
   T *Nv = nullptr, *Mu = nullptr, *Av = nullptr, *Atu = nullptr;                     // LSQR / LSMR (+ w, u, v; Mu, Av, u: m)
   T *h = nullptr, *hbar = nullptr;                                                   // LSMR
   T *u_prev = nullptr, *v_prev = nullptr;                                             // BiLQ / QMR (+ u, v, q, p; w1, w2 / w)
+  T *dy = nullptr;                     // BiLQR / TriLQR: Δy of a warm start (+ x, y = t, u, v, u_prev, v_prev, q, p,
+                                       // w = d̅, w1 = w_{k-3}, w2 = w_{k-2}; TriLQR: v-space vectors have m entries)
   T *d1 = nullptr, *d2 = nullptr;      // MINARES: d_{k-1}, d_{k-2} (+ v = v_k, vv = v_{k+1}, w1 = w_{k-1}, w2 = w_{k-2}, q)
                                        // CAR: r, p, s, q, t, u (+ Mu, lazy)
   T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
@@ -422,6 +432,30 @@ template <class T> T qmr_fused_update(Workspace<T>& ws, T* wk, const T* w1, int 
 // returns <v, v_next> and ||v_next||^2.
 template <class T> void bilq_fused_update(Workspace<T>& ws, bool first, T czeta, T szeta, T c, T s, T beta1, T gamma1, bool keep,
                                           T* vv1, T* v1v1);
+// BiLQR (fused_phases.cu): the update pass after B1 / B2.  Primal half (primal): d̅ = v when iter == 1, else
+// x += czeta d̅ + szeta v, d̅ = -c v + s d̅, and <v, q>, ||q||^2.  Dual half (dual): w_{k-1} from u_{k-1} into wk (iter >= 2,
+// as bilqr.jl:363-381; w3 = w_{k-3}, w2 = w_{k-2}), y += psi w_{k-1}, and ||u_{k+1}||^2.  Then v_{k+1} = q / beta1 and
+// u_{k+1} = p / gamma1 into the buffers of v_{k-1}, u_{k-1} (keep: copies of v, u).  out: {<v, q>, ||q||^2, ||u_{k+1}||^2}.
+template <class T> void bilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T czeta, T szeta, T c, T s,
+                                           T* wk, const T* w2, T eps3, T lam2, T delta1, T psi1, T beta1, T gamma1, bool keep,
+                                           T* out3);
+// TriLQR (fused_phases.cu), A (m x n) and At (A^T, max(m, n) rows: rows beyond n are empty) CSR operators.  One SSY step:
+// T1 (SpMV on A gathering u: q = A u - gamma v_prev, alpha = <v, q> on the device) and T2 (SpMV on A^T gathering v:
+// p = A^T v - beta u_prev - alpha u, q -= alpha v over all m rows, ||p||^2 and ||q||^2), then one read-back of
+// {alpha, ||q||^2, ||p||^2}.  `first`: iteration 1 (no gamma / beta terms).
+template <class T> void trilqr_fused_ssy(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool first, T beta, T gamma,
+                                         T* alpha, T* qq, T* pp);
+// TriLQR's update pass over max(m, n): primal half on the n-space (d̅ = u or x += czeta d̅ + szeta u, d̅ = -c u + s d̅),
+// dual half on the m-space (w_{k-1} from v_{k-1}, y += psi w_{k-1}), then v_{k+1} = q / beta1 (beta1 != 0) and
+// u_{k+1} = p / gamma1 (gamma1 != 0) into the buffers of v_{k-1}, u_{k-1}, else copies of v, u.  No read-back.
+template <class T> void trilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T czeta, T szeta, T c, T s,
+                                            T* wk, const T* w2, T eps3, T lam2, T delta1, T psi1, T beta1, T gamma1);
+// bilqr! / trilqr! (adjoint.cu): A with its adjoint At (a CSR operator holding A^T, or a callback); b, c required.
+template <class T> void bilqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const T* c,
+                                    const SolveOpts& o);
+template <class T> void trilqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const T* c,
+                                     const SolveOpts& o);
+template <class T> void ws_warm_start2(Workspace<T>* ws, const T* x0_dev, const T* y0_dev);
 // bilq! / qmr! (biorth.cu): square A with its adjoint At (a CSR operator holding A^T, or a callback); c = nullptr: c = b.
 template <class T> void bilq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const T* c,
                                    const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);

@@ -4,6 +4,7 @@
 // strings and aliasing rules (files cited per function); every vector operation
 // is a kernel from blas1.cu / spmv.cu / fused_phases.cu, nothing is computed on
 // the host except O(1)/O(k^2) scalar work the reference also does on the host.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <limits>
@@ -18,7 +19,7 @@ namespace kb {
 // ---------------------------------------------------------------------------
 template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int memory, int window, int device) {
   const double t0 = now_seconds();
-  if (m != n && !is_ls_kind(kind)) throw std::runtime_error("System must be square");
+  if (m != n && !is_ls_kind(kind) && kind != S_TRILQR) throw std::runtime_error("System must be square");
   Workspace<T>* ws = new Workspace<T>();
   try {
     ws->kind = kind; ws->m = m; ws->n = n;
@@ -79,6 +80,14 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         ws->u_prev = A(); ws->u = A(); ws->q = A(); ws->v_prev = A(); ws->v = A(); ws->p = A();
         if (kind == S_QMR) { ws->w1 = A(); ws->w2 = A(); } else { ws->w = A(); }   // w_{k-2}, w_{k-1} / d̅
         break;
+      case S_BILQR: case S_TRILQR: {                // BilqrWorkspace / TrilqrWorkspace (Δx, Δy by warm_start2)
+        // TriLQR: x, d̅, u_{k-1}, u_k, p live in the n-space and y, v_{k-1}, v_k, q, w_{k-3}, w_{k-2} in the m-space.  p
+        // has max(m, n) entries: the cached A^T has that many rows (the fused T2 pass covers every row of q with them).
+        auto Am = [&]() { return dev_alloc<T>((size_t)m); };
+        ws->u_prev = A(); ws->u = A(); ws->w = A(); ws->p = dev_alloc<T>((size_t)std::max(m, n));
+        ws->v_prev = Am(); ws->v = Am(); ws->q = Am(); ws->y = Am(); ws->w1 = Am(); ws->w2 = Am();
+        break;
+      }
       case S_CAR:                                   // CarWorkspace (Mu is allocated by the solve)
         ws->r = A(); ws->p = A(); ws->s = A(); ws->q = A(); ws->t = A(); ws->u = A();
         break;
@@ -101,7 +110,7 @@ template <class T> void ws_destroy(Workspace<T>* ws) {
   T* vecs[] = {ws->x, ws->dx, ws->r, ws->p, ws->Ap, ws->z, ws->npc_dir, ws->p2, ws->v, ws->s, ws->qd, ws->t, ws->yz,
                ws->r1, ws->r2, ws->w1, ws->w2, ws->y, ws->vv, ws->w, ws->q, ws->pp, ws->bbuf, ws->cbuf,
                ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next, ws->Nv, ws->Mu, ws->Av, ws->Atu, ws->h, ws->hbar,
-               ws->Ar, ws->Mr, ws->u_prev, ws->v_prev, ws->d1, ws->d2};
+               ws->Ar, ws->Mr, ws->u_prev, ws->v_prev, ws->d1, ws->d2, ws->dy};
   for (T* p : vecs) dev_free(p);
   for (T* p : ws->V) dev_free(p);
   for (T* p : ws->Z) dev_free(p);

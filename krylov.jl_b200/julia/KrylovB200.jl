@@ -196,7 +196,7 @@ end
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
                        :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25, :bilq => 12, :qmr => 13,
-                       :car => 32, :minares => 33, :cg_lanczos => 100)
+                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -211,6 +211,7 @@ struct CStats  # KrylovB200Stats (include/krylov_b200.h)
   nresiduals::Cint; nAresiduals::Cint; nAcond::Cint
   allocation_timer::Cdouble; timer::Cdouble; status::NTuple{96,UInt8}; Anorm::Cdouble
   error_with_bnd::Cint; nerr_lbnds::Cint; nerr_ubnds_lq::Cint; nerr_ubnds_cg::Cint
+  solved_primal::Cint; solved_dual::Cint; nresiduals_dual::Cint
 end
 
 mutable struct Handle
@@ -481,6 +482,62 @@ Krylov.bilq!(ws::Krylov.BilqWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200
   biorth_solve!(:bilq, ws, A, b; kw...)
 Krylov.qmr!(ws::Krylov.QmrWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
   biorth_solve!(:qmr, ws, A, b; kw...)
+
+# ---- bilqr! / trilqr! (src/bilqr.jl:99-113, src/trilqr.jl:98-112) on a B200CSR: one krylov_solve per solve ----------
+# A x = b and Aᵀ y = c together; the library forms Aᵀ once per operator and runs the fused passes.  TriLQR's
+# transfer_to_usymcg travels in the transfer_to_bicg field of the extended options.  The workspace's y receives y, its
+# stats (AdjointStats, src/krylov_stats.jl:263-280) both flags and both histories.
+function adjoint_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}, c::B200Vector{T};
+                        transfer_to_bicg::Bool = true, transfer_to_usymcg::Bool = true, atol::T = √eps(T),
+                        rtol::T = √eps(T), itmax::Int = 0, timemax::Float64 = Inf, verbose::Int = 0, history::Bool = false,
+                        callback = workspace -> false, iostream::IO = stdout) where T
+  method === :bilqr && A.m != A.n && error("Systems must be square")
+  length(b) == A.m || error("Inconsistent problem size")
+  length(c) == A.n || error("Inconsistent problem size")
+  h = handle_for(method, ws, A, 0, 0)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  transfer = method === :bilqr ? transfer_to_bicg : transfer_to_usymcg
+  ext = Ref(CExt(history, false, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0,
+                 transfer))
+  o = Ref(COpts(atol, rtol, itmax, verbose, 0.0, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    if ws.warm_start                      # warm_start!(ws, x0, y0) stored them in ws.Δx and ws.Δy
+      check(ccall((:krylov_warm_start2, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint), h.ptr, ws.Δx.ptr,
+                  ws.Δy.ptr, A.n, A.m))
+      ws.warm_start = false
+    end
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, c.ptr, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+    check(ccall((:krylov_get_y, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.y.ptr, A.m))
+  end
+  fill_adjoint_stats!(ws, h, T)
+  ws
+end
+function fill_adjoint_stats!(ws, h::Handle, ::Type{T}) where T
+  cs = Ref{CStats}()
+  check(ccall((:krylov_b200_get_stats, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, cs))
+  s = cs[]
+  st = ws.stats
+  st.niter = s.niter; st.solved_primal = s.solved_primal != 0; st.solved_dual = s.solved_dual != 0; st.timer = s.timer
+  bytes = collect(s.status); z = findfirst(==(0x00), bytes)
+  st.status = String(bytes[1:(z === nothing ? length(bytes) : z - 1)])
+  for (which, field, cnt) in ((0, :residuals_primal, s.nresiduals), (6, :residuals_dual, s.nresiduals_dual))
+    buf = Vector{Cdouble}(undef, cnt)
+    got = cnt == 0 ? 0 : ccall((:krylov_b200_get_history, lib), Cint, (Ptr{Cvoid}, Cint, Ptr{Cdouble}, Cint), h.ptr, which, buf, cnt)
+    v = getproperty(st, field); empty!(v); append!(v, T.(buf[1:got]))
+  end
+  st
+end
+Krylov.bilqr!(ws::Krylov.BilqrWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}, c::B200Vector{T}; kw...) where T =
+  adjoint_solve!(:bilqr, ws, A, b, c; kw...)
+Krylov.trilqr!(ws::Krylov.TrilqrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}, c::B200Vector{T};
+               kw...) where T =
+  adjoint_solve!(:trilqr, ws, A, b, c; kw...)
 
 # ---- block_gmres! (src/block_gmres.jl:78-110; C ABI krylov.h:250-285): one krylov_block_solve per solve ------------------
 # B, X, X0 are column-major n x p device matrices; the library keeps row-major panels internally and runs the

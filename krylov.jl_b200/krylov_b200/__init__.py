@@ -40,7 +40,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_",
            "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_",
            "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_",
-           "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_"]
+           "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_",
+           "AdjointStats", "BilqrWorkspace", "TrilqrWorkspace", "bilqr", "bilqr_", "trilqr", "trilqr_"]
 
 
 class B200Error(RuntimeError):
@@ -62,6 +63,22 @@ class SimpleStats:
     timer: float = 0.0
     status: str = "unknown"
     Anorm: float = math.nan          # LanczosStats (src/krylov_stats.jl), cg_lanczos! only
+
+
+@dataclass
+class AdjointStats:
+    """src/krylov_stats.jl:263-280: the statistics of bilqr! / trilqr!; `solved` is solved_primal and solved_dual."""
+    niter: int = 0
+    solved_primal: bool = False
+    solved_dual: bool = False
+    residuals_primal: list = field(default_factory=list)
+    residuals_dual: list = field(default_factory=list)
+    timer: float = 0.0
+    status: str = "unknown"
+
+    @property
+    def solved(self) -> bool:
+        return self.solved_primal and self.solved_dual
 
 
 def device_count() -> int:
@@ -786,8 +803,9 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
                 setattr(e, name, float(val))
         return self._run(A, b, M, N, o, e, callback)
 
-    def _run(self, A, b, M, N, o, e, callback, c=None):
-        """Set the options, the operator pair and the preconditioners, stage b (and c) and call krylov_solve."""
+    def _run(self, A, b, M, N, o, e, callback, c=None, c_len=None):
+        """Set the options, the operator pair and the preconditioners, stage b (and c, of c_len entries, default m) and
+        call krylov_solve."""
         m, n = self.m, self.n
         keep = []
         if callback is not None:
@@ -835,7 +853,7 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
         if c is not None:
             if not _is_torch(c):
                 c = np.ascontiguousarray(c, dtype=self.dtype)
-            if c.shape[0] != m:
+            if c.shape[0] != (m if c_len is None else c_len):
                 raise B200Error("Inconsistent problem size")
         pc, kc = _ptr(c)
         self._order_after(kb_, kc)
@@ -968,6 +986,135 @@ class QmrWorkspace(_BiorthWorkspace):
         return self._solve(A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown)
 
 
+class _AdjointWorkspace(_LeastSquaresWorkspace):
+    """Workspace of bilqr! / trilqr! (src/krylov_workspaces.jl BilqrWorkspace / TrilqrWorkspace): the primal system
+    A x = b and the adjoint system A^T y = c, solved together.  A is m x n (square for BiLQR): b and y have m entries,
+    c and x have n.  Both apply A and its adjoint: a CSR operator (its transpose is formed once and cached), or a
+    scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables.  Neither takes a preconditioner."""
+    nA = 2
+
+    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
+        super().__init__(m_or_A, n_or_b, dtype, device=device)
+
+    def _solve(self, A, b, c, transfer, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown):
+        if unknown:
+            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        if c is None:
+            raise B200Error(f"{self.solver}! solves A^T y = c as well: c must be given")
+        o = lib().krylov_default_options()
+        if atol is not None:
+            o.atol = float(atol)
+        if rtol is not None:
+            o.rtol = float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        e = lib().krylov_b200_default_options()
+        e.history, e.fused = int(history), int(fused)
+        e.transfer_to_bicg = int(transfer)           # TriLQR's transfer_to_usymcg travels in the same field
+        return self._run(A, b, None, None, o, e, callback, c, c_len=self.n)
+
+    def warm_start(self, x0, y0):
+        """warm_start!(workspace, x0, y0): x0 has n entries, y0 m."""
+        if not _is_torch(x0):
+            x0 = np.ascontiguousarray(x0, dtype=self.dtype)
+        if not _is_torch(y0):
+            y0 = np.ascontiguousarray(y0, dtype=self.dtype)
+        px, kx = _ptr(x0)
+        py, ky = _ptr(y0)
+        self._order_after(kx, ky)
+        if lib().krylov_warm_start2(self._h, px, py, int(x0.shape[0]), int(y0.shape[0])) != 0:
+            raise B200Error(_lib.last_error())
+        return self
+
+    @property
+    def y(self):
+        """The solution of A^T y = c: a host copy (or a torch CUDA tensor for device workspaces)."""
+        if self.device == "cuda":
+            import torch
+            out = torch.empty(self.m, dtype=torch.float64 if self.dtype == np.float64 else torch.float32, device="cuda")
+            if lib().krylov_get_y(self._h, C.c_void_p(out.data_ptr()), self.m) != 0:
+                raise B200Error(_lib.last_error())
+            return out
+        out = np.empty(self.m, dtype=self.dtype)
+        if lib().krylov_get_y(self._h, out.ctypes.data_as(C.c_void_p), self.m) != 0:
+            raise B200Error(_lib.last_error())
+        return out
+
+    @property
+    def stats(self) -> AdjointStats:
+        s = KrylovB200Stats()
+        if lib().krylov_b200_get_stats(self._h, C.byref(s)) != 0:
+            raise B200Error(_lib.last_error())
+
+        def hist(which, cnt):
+            buf = (C.c_double * max(cnt, 1))()
+            k = lib().krylov_b200_get_history(self._h, which, buf, cnt)
+            return list(buf[:max(k, 0)])
+        return AdjointStats(s.niter, bool(s.solved_primal), bool(s.solved_dual), hist(0, s.nresiduals),
+                            hist(6, s.nresiduals_dual), s.timer, s.status.decode("utf-8"))
+
+
+class BilqrWorkspace(_AdjointWorkspace):
+    solver = "bilqr"
+
+    def solve(self, A, b, c, *, transfer_to_bicg=True, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
+              history=False, callback=None, fused=True, **unknown):
+        """bilqr!(ws, A, b, c; kwargs...)  -- kwargs as in bilqr.jl:99-107: atol and rtol default to sqrt(eps),
+        itmax = 0 means 2n."""
+        return self._solve(A, b, c, transfer_to_bicg, atol, rtol, itmax, timemax, verbose, history, callback, fused,
+                           unknown)
+
+
+class TrilqrWorkspace(_AdjointWorkspace):
+    solver = "trilqr"
+
+    def solve(self, A, b, c, *, transfer_to_usymcg=True, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
+              history=False, callback=None, fused=True, **unknown):
+        """trilqr!(ws, A, b, c; kwargs...)  -- kwargs as in trilqr.jl: atol and rtol default to sqrt(eps), itmax = 0
+        means m + n.  A is m x n, b has m entries and c n."""
+        return self._solve(A, b, c, transfer_to_usymcg, atol, rtol, itmax, timemax, verbose, history, callback, fused,
+                           unknown)
+
+
+def _make_adjoint(name):
+    def f(A, b, c, x0=None, y0=None, **kw):
+        m, n = b.shape[0], c.shape[0]
+        if _is_torch(b):                      # the element type, without copying a device b to the host
+            import torch
+            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
+        else:
+            dt = np.asarray(b).dtype
+        if dt not in (np.float32, np.float64):
+            dt = np.float64
+        ws = _WS[name](m, n, dt, device="cuda" if _is_torch(b) else "host")
+        try:
+            if (x0 is None) != (y0 is None):
+                raise B200Error(f"{name}: pass both x0 and y0, or neither")
+            if x0 is not None:
+                ws.warm_start(x0, y0)
+            ws.solve(A, b, c, **kw)
+            return ws.x, ws.y, ws.stats
+        finally:
+            ws.free()
+    f.__name__ = name
+    f.__doc__ = f"(x, y, stats) = {name}(A, b, c[, x0, y0]; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, c n"
+    return f
+
+
+def _make_adjoint_inplace(name):
+    def f(ws, A, b, c, x0=None, y0=None, **kw):
+        if ws.solver != name:
+            raise B200Error(f"{name}! needs a {_WS[name].__name__}")
+        if (x0 is None) != (y0 is None):
+            raise B200Error(f"{name}!: pass both x0 and y0, or neither")
+        if x0 is not None:
+            ws.warm_start(x0, y0)
+        return ws.solve(A, b, c, **kw)
+    f.__name__ = name + "_"
+    f.__doc__ = f"{name}!(workspace, A, b, c[, x0, y0]; kwargs...)"
+    return f
+
+
 def _make_least_squares(name):
     def f(A, b, *, n=None, window=0, **kw):
         m = b.shape[0]
@@ -994,7 +1141,7 @@ _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "b
        "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
        "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
        "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace, "car": CarWorkspace,
-       "minares": MinaresWorkspace}
+       "minares": MinaresWorkspace, "bilqr": BilqrWorkspace, "trilqr": TrilqrWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -1052,6 +1199,8 @@ bilq_, qmr_ = (_make_inplace(s) for s in ("bilq", "qmr"))
 bilq, qmr = (_make_outofplace(s) for s in ("bilq", "qmr"))
 car_, minares_ = (_make_inplace(s) for s in ("car", "minares"))
 car, minares = (_make_outofplace(s) for s in ("car", "minares"))
+bilqr_, trilqr_ = (_make_adjoint_inplace(s) for s in ("bilqr", "trilqr"))
+bilqr, trilqr = (_make_adjoint(s) for s in ("bilqr", "trilqr"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):

@@ -23,7 +23,7 @@ KRYLOV_LSLQ, KRYLOV_LSQR, KRYLOV_LSMR, KRYLOV_CGLS, KRYLOV_CRLS = 20, 21, 22, 24
 SOLVER_IDS = {"lslq": KRYLOV_LSLQ, "lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cgls": KRYLOV_CGLS, "crls": KRYLOV_CRLS, "cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
               "fom": KRYLOV_FOM, "fgmres": KRYLOV_FGMRES, "cgs": KRYLOV_CGS, "cg_lanczos": KRYLOV_B200_CG_LANCZOS,
               "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES, "bilq": 12, "qmr": 13,
-              "car": 32, "minares": 33}
+              "car": 32, "minares": 33, "trilqr": 18, "bilqr": 19}
 
 MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p)
 BLOCK_MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p)
@@ -54,7 +54,8 @@ class KrylovB200Stats(C.Structure):
                 ("npcCount", C.c_int), ("nresiduals", C.c_int), ("nAresiduals", C.c_int), ("nAcond", C.c_int),
                 ("allocation_timer", C.c_double), ("timer", C.c_double), ("status", C.c_char * 96),
                 ("Anorm", C.c_double), ("error_with_bnd", C.c_int), ("nerr_lbnds", C.c_int), ("nerr_ubnds_lq", C.c_int),
-                ("nerr_ubnds_cg", C.c_int)]
+                ("nerr_ubnds_cg", C.c_int), ("solved_primal", C.c_int), ("solved_dual", C.c_int),
+                ("nresiduals_dual", C.c_int)]
 
 
 # every symbol include/krylov_b200.h declares: name -> (restype, argtypes)
