@@ -263,12 +263,17 @@ template <class T> void csr_plan(Ctx& c, Csr<T>& A, CsrDict<T>* dict) {
   const size_t two_cta = 110 * 1024, one_cta = 220 * 1024;
   A.tma_ok = false;
   int per_sm = 2;
-  // tuning overrides (profiles/sweep_k1.py): KB200_STAGES, KB200_CTAS_PER_SM
+  // tuning overrides (profiles/sweep_k1.py): KB200_STAGES, KB200_CTAS_PER_SM.  A forced ring gets the per-CTA ceiling
+  // of the default rule for the same CTAs per SM (and never more than the 220 KB every staged launcher opts in to);
+  // one that does not fit falls through to the default choice.
   const char* es = getenv("KB200_STAGES");
   const char* ec = getenv("KB200_CTAS_PER_SM");
   if (es && ec) {
     const int s = atoi(es), cps = atoi(ec);
-    if (s >= 1 && s <= 8 && cps >= 1 && cps <= 8 && L.total_bytes(s) * cps <= 226 * 1024) { A.tma_ok = true; A.stages = s; per_sm = cps; }
+    if (s >= 1 && s <= 8 && cps >= 1 && cps <= 8) {
+      const size_t per_cta = cps == 1 ? one_cta : cps == 2 ? two_cta : 226 * 1024 / cps;
+      if (L.total_bytes(s) <= per_cta) { A.tma_ok = true; A.stages = s; per_sm = cps; }
+    }
   }
   // default: 3 CTAs/SM x 2 stages when it fits (profiles/sweep_k1.py sweeps the alternatives): the gather latency
   // wants 27 warps/SM, and a shallower ring leaves more of the SM's 228 KB to L1 for the gathered vectors.

@@ -77,15 +77,32 @@ def test_fused_cg_with_jacobi_preconditioner(kb, O):
     assert out[True][2] < out[False][2]
 
 
+def _arrow_csr(N, dt):
+    """div_grad(N) with a dense first row and column of small entries (corner raised above the row's sum): its first
+    tile does not fit the shared-memory ring in either type, so CG runs cg_k1_rows."""
+    import scipy.sparse as sp
+    from krylov_b200 import problems as P
+    rp, ci, va = P.div_grad_csr(N)
+    n = N ** 3
+    w = 1e-4 * (1.0 + np.arange(n) % 5)
+    w[0] = w[1:].sum() + 1.0
+    R = sp.csr_matrix((w, (np.zeros(n, np.int64), np.arange(n))), shape=(n, n))
+    A = sp.csr_matrix(sp.csr_matrix((va, ci, rp), shape=(n, n)) + R + R.T - sp.csr_matrix(([w[0]], ([0], [0])), shape=(n, n)))
+    A.sort_indices()
+    return A.indptr.astype(np.int32), A.indices.astype(np.int32), A.data.astype(dt)
+
+
 def test_cg_x_update_in_k1_is_bit_identical(kb):
     """Moving x += alpha p from K2 into the next K1 (XUP) changes no arithmetic: x, r and the residual history are
-    bit-identical to the K2 placement, for convergence exits, itmax exits and Float32."""
+    bit-identical to the K2 placement, for convergence exits, itmax exits and Float32, on a staged operator
+    (cg_k1_tma) and on an untiled one (cg_k1_rows)."""
     import os
     from krylov_b200 import problems as P
-    for dt, kw in ((np.float64, dict(atol=0.0, rtol=1e-8)), (np.float64, dict(atol=0.0, rtol=0.0, itmax=7)),
-                   (np.float64, dict(atol=0.0, rtol=0.0, itmax=8)), (np.float32, dict())):
-        rp, ci, va = P.div_grad_csr(20, dtype=dt)
-        n = 20 ** 3
+    for op, dt, kw in ((op, dt, kw) for op in ("stencil", "arrow") for dt, kw in (
+            (np.float64, dict(atol=0.0, rtol=1e-8)), (np.float64, dict(atol=0.0, rtol=0.0, itmax=7)),
+            (np.float64, dict(atol=0.0, rtol=0.0, itmax=8)), (np.float32, dict()))):
+        rp, ci, va = P.div_grad_csr(20, dtype=dt) if op == "stencil" else _arrow_csr(31, dt)
+        n = len(rp) - 1
         b = (np.arange(n) % 7 + 1).astype(dt)
         outs = []
         for flag in ("1", "0"):
