@@ -49,7 +49,9 @@ typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
  * adjoint pairs A x = b, A^T y = c of BILQR (square A) and TRILQR (A m x n: b and y have m entries, c and x have n),
  * which require c, take no preconditioner and return y through krylov_get_y, and the least-squares solvers LSQR, LSMR,
  * LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a
- * CSR operator of m rows and n columns is attached); every other value returns -2. */
+ * CSR operator of m rows and n columns is attached), and the least-norm solvers CRAIG and CRAIGMR on the same m x n
+ * operators (min ||x|| subject to A x = b; x = A^T y, and y, m entries, is returned through krylov_get_y; `c` is
+ * ignored); every other value returns -2. */
 typedef enum {
   KRYLOV_CG = 0, KRYLOV_CR = 1, KRYLOV_SYMMLQ = 2, KRYLOV_MINRES = 3, KRYLOV_MINRES_QLP = 4, KRYLOV_DIOM = 5,
   KRYLOV_DQGMRES = 6, KRYLOV_FOM = 7, KRYLOV_GMRES = 8, KRYLOV_FGMRES = 9, KRYLOV_BICGSTAB = 10, KRYLOV_CGS = 11,
@@ -100,7 +102,7 @@ void krylov_get_version(int *major, int *minor, int *patch);
 int krylov_solve(void *ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, KrylovMatvec matvec_M, KrylovMatvec matvec_N,
                  const void *b, const void *c, void *userdata, const KrylovOptions *opts);
 int krylov_get_x(void *ws, void *x, int n);
-int krylov_get_y(void *ws, void *y, int m); /* BILQR, TRILQR: y (m entries); -2: single-solution solver */
+int krylov_get_y(void *ws, void *y, int m); /* BILQR, TRILQR, CRAIG, CRAIGMR: y (m entries); -2: single-solution solver */
 int krylov_is_solved(void *ws);             /* 1 | 0 | -1 */
 int krylov_niter(void *ws);
 double krylov_elapsed_time(void *ws);
@@ -140,9 +142,10 @@ const char *krylov_b200_last_error(void);
 /* Attach a CSR matrix as the operator A of `ws`: replaces mul!(y, A, x) at
  * cg.jl:196, gmres.jl:257, bicgstab.jl:221,228, minres.jl:289.
  *   rowptr[n+1], colind[nnz], values[nnz] (element type = workspace dtype);
- *   least-squares workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
+ *   least-squares and least-norm (CRAIG, CRAIGMR) workspaces: n is the number of rows (the workspace's m) and the
+ *   columns are the workspace's n;
  *   TriLQR workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
- *   least-squares, BiLQ, QMR, BiLQR and TriLQR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
+ *   least-squares, least-norm, BiLQ, QMR, BiLQR and TriLQR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
  *   until the operator changes;
  *   index_base 0|1, index_bytes 4|8 (Julia's SparseMatrixCSC{T,Int64} passes
  *   1 and 8 -- for a symmetric matrix its CSC arrays ARE the CSR arrays);
@@ -156,7 +159,7 @@ int krylov_b200_share_operator(void *ws, void *src);
 int krylov_b200_attach_csr(void *ws, void *csr);
 /* Diagonal preconditioner: which = 0 -> M, 1 -> N; d[n] holds the diagonal of
  * the operator the solver applies (P^-1 with the default ldiv=false). NULL detaches.
- * LSQR / LSMR / LSLQ: M acts on the data space (d[m]), N on the solution space (d[n]).  CGLS / CRLS: M acts on the
+ * LSQR / LSMR / LSLQ / CRAIG / CRAIGMR: M acts on the data space (d[m]), N on the solution space (d[n]).  CGLS / CRLS: M acts on the
  * residual space (d[m]); they take no N (a solve with N attached or matvec_N given is refused). */
 int krylov_b200_set_preconditioner_diag(void *ws, int which, const void *d, int location);
 /* Block-Jacobi preconditioner (docs/src/preconditioners.md:33,159): which = 0 -> M, 1 -> N; blocks[ceil(n/bs)][bs][bs]
@@ -187,10 +190,10 @@ typedef struct {
   double cr_gamma;     /* CR: kwarg `γ` (src/cr.jl:112); NaN -> sqrt(eps)                                        */
   double axtol;        /* LSQR, LSMR: kwarg `axtol` (src/lsqr.jl:152); MINARES: kwarg `Artol`, the relative
                           tolerance on ||A r|| (src/minares.jl:99); NaN -> sqrt(eps)                                  */
-  double btol;         /* LSQR, LSMR, LSLQ: kwarg `btol`; NaN -> sqrt(eps)                                        */
+  double btol;         /* LSQR, LSMR, LSLQ, CRAIG: kwarg `btol`; NaN -> sqrt(eps)                                 */
   double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0                       */
   double utol;         /* LSLQ: kwarg `utol`; NaN -> sqrt(eps)                                                       */
-  int transfer_to_lsqr; /* LSLQ: 1 -> return the LSQR point (kwarg `transfer_to_lsqr`)                                */
+  int transfer_to_lsqr; /* LSLQ, CRAIG (acts when lambda > 0): 1 -> return the LSQR point (kwarg `transfer_to_lsqr`)  */
   int transfer_to_bicg; /* BiLQ, BiLQR: 1 (default) -> return the BiCG point when it converges first (kwarg `transfer_to_bicg`);
                           TriLQR: its kwarg `transfer_to_usymcg` (the USYMCG point), in the same field                  */
 } KrylovB200Options;
@@ -225,7 +228,8 @@ int krylov_b200_get_stats(void *ws, KrylovB200Stats *out);
  * Returns the number copied (<= cap) or -1. */
 int krylov_b200_get_history(void *ws, int which, double *out, int cap);
 /* Device pointer of a workspace vector by its reference field name
- * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"; BiLQR / TriLQR: "y", "d̅",
+ * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"; CRAIG / CRAIGMR: "y", "Nv",
+ * "Mu", "Av", "Aᴴu", "u", "v", "w", CRAIG "w2", CRAIGMR "d", "w̄" and "q"; BiLQR / TriLQR: "y", "d̅",
  * "wₖ₋₃", "wₖ₋₂", "uₖ₋₁", "uₖ", "vₖ₋₁", "vₖ", "q", "p", "Δx", "Δy"). */
 int krylov_b200_get_vector(void *ws, const char *name, void **dev_ptr);
 /* Average durations (ms) of the fused kernels measured with CUDA events on the workspace stream during the

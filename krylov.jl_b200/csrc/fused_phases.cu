@@ -1338,6 +1338,152 @@ void trilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T c
                                                                   ws.m, ws.n}, NoFin(), 5);
 }
 
+// ===========================================================================
+// CRAIG / CRAIGMR  (src/craig.jl:276-379, src/craigmr.jl:280-379; lambda = 0, M = N = I)
+// As for LSQR, kdiv!(u, beta) and kdiv!(v, alpha) are left pending: Mu and Nv stay unscaled in memory and every reader
+// applies s_u = 1/beta or s_v = 1/alpha (1 when the reference skips the division), which is the rounding kdiv! does.
+// The SpMV gathers take the factor from the device block (written by the Fin of the pass that produced the norm); the
+// epilogues take it by value from the host, which computed the same quotient from the same read-back.
+// ===========================================================================
+template <class T> struct CraigState { T s_u, s_v, alpha, beta, ww, ia, mba; };
+
+template <class T> struct CraigNormFin {     // tot[0] = ||z||^2 -> s = ||z|| ; inverse = 1/s (1 when s = 0)
+  T* out; T* inv;
+  __device__ void operator()(const T* tot) const {
+    const T s = sqrt_rn(tot[0]);
+    *out = s;
+    *inv = s == T(0) ? T(1) : div_rn(T(1), s);
+  }
+};
+// CRAIG C1 on A^T, gathering u: x += xi v (the previous iteration's, pending) ; Nv = A^T u - beta v ; ||Nv||^2
+template <class T> struct CraigP1Epi {
+  T* nv; T* x; T beta, s_v, xi; int xup;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T v = mul_rn(nv[row], s_v);
+    if (xup) x[row] = add_rn(x[row], mul_rn(xi, v));
+    const T nn = add_rn(mul_rn(T(1), acc), mul_rn(-beta, v));
+    nv[row] = nn;
+    d[0] += nn * nn;
+  }
+};
+// CRAIG C2 on A, gathering v: w = u + tw w ; y += ty w ; ||w||^2 ; Mu = A v - alpha u ; ||Mu||^2
+template <class T> struct CraigP2Epi {
+  T* mu; T* w; T* y; T s_u, alpha, tw, ty;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T u = mul_rn(mu[row], s_u);
+    const T wn = add_rn(mul_rn(T(1), u), mul_rn(tw, w[row]));
+    w[row] = wn;
+    y[row] = add_rn(y[row], mul_rn(ty, wn));
+    d[1] += wn * wn;
+    const T nm = add_rn(mul_rn(T(1), acc), mul_rn(-alpha, u));
+    mu[row] = nm;
+    d[0] += nm * nm;
+  }
+};
+template <class T> struct CraigP2Fin {
+  CraigState<T>* s;
+  __device__ void operator()(const T* tot) const {
+    CraigNormFin<T>{&s->beta, &s->s_u}(tot);
+    s->ww = tot[1];
+  }
+};
+template <class T> struct CraigFlushBody {   // x += xi v, v = Nv s_v
+  T* x; const T* nv; T xi, s_v;
+  __device__ __forceinline__ void operator()(int i, T*) const { x[i] = add_rn(x[i], mul_rn(xi, mul_rn(nv[i], s_v))); }
+};
+
+template <class T> static CraigState<T>* craig_state(Workspace<T>& ws, bool init) {
+  typedef CraigState<T> St;
+  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
+  if (init) {                     // u_1 and v_0 = 0 are stored scaled: both factors start at 1
+    St* H = (St*)ws.fused_host;
+    memset(H, 0, sizeof(St));
+    H->s_u = T(1); H->s_v = T(1);
+    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, ws.ctx.stream));
+  }
+  return S;
+}
+template <class T> static CraigState<T> craig_read(Workspace<T>& ws) {
+  typedef CraigState<T> St;
+  St* H = (St*)ws.fused_host;
+  KB_CUDA(cudaMemcpyAsync(H + 1, ws.fused_state, sizeof(St), cudaMemcpyDeviceToHost, ws.ctx.stream));
+  ws.ctx.sync();
+  return H[1];
+}
+
+template <class T> T craig_fused_p1(Workspace<T>& ws, const Csr<T>& At, bool init, T beta, T s_v, bool xup, T xi) {
+  CraigState<T>* S = craig_state<T>(ws, init);
+  launch_spmv_epi_g<T, 1>(ws.ctx, At, XScaled<T>{ws.Mu, &S->s_u, T(1)}, CraigP1Epi<T>{ws.Nv, ws.x, beta, s_v, xi, xup ? 1 : 0},
+                          CraigNormFin<T>{&S->alpha, &S->s_v}, 4);
+  return craig_read<T>(ws).alpha;
+}
+template <class T> void craig_fused_p2(Workspace<T>& ws, const Csr<T>& A, T s_u, T alpha, T tw, T ty, T* beta, T* ww) {
+  CraigState<T>* S = (CraigState<T>*)ws.fused_state;
+  launch_spmv_epi_g<T, 2>(ws.ctx, A, XScaled<T>{ws.Nv, &S->s_v, T(1)}, CraigP2Epi<T>{ws.Mu, ws.w, ws.y, s_u, alpha, tw, ty},
+                          CraigP2Fin<T>{S}, 4);
+  const CraigState<T> H = craig_read<T>(ws);
+  *beta = H.beta; *ww = H.ww;
+}
+template <class T> void craig_fused_flush(Workspace<T>& ws, T xi, T s_v) {
+  launch_stream<T, 0>(ws.ctx, ws.n, CraigFlushBody<T>{ws.x, ws.Nv, xi, s_v}, NoFin(), 5);
+}
+
+// CRAIGMR R1 on A, gathering v: Mu = A v - alpha u ; ||Mu||^2
+template <class T> struct CraigmrP1Epi {
+  T* mu; T s_u, alpha;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T nm = add_rn(mul_rn(T(1), acc), mul_rn(-alpha, mul_rn(mu[row], s_u)));
+    mu[row] = nm;
+    d[0] += nm * nm;
+  }
+};
+// CRAIGMR R2 on A^T, gathering u: d = v / rho (first) or d = (1/rho) v + tr d ; x += zeta d ; Nv = A^T u - beta v ; ||Nv||^2
+template <class T> struct CraigmrP2Epi {
+  T* nv; T* dd; T* x; T s_v, rho, inv_rho, tr, zeta, beta; int first;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T v = mul_rn(nv[row], s_v);
+    const T dn = first ? div_rn(v, rho) : add_rn(mul_rn(inv_rho, v), mul_rn(tr, dd[row]));
+    dd[row] = dn;
+    x[row] = add_rn(x[row], mul_rn(zeta, dn));
+    const T nn = add_rn(mul_rn(T(1), acc), mul_rn(-beta, v));
+    nv[row] = nn;
+    d[0] += nn * nn;
+  }
+};
+template <class T> struct CraigmrP2Fin {     // alpha, s_v and the coefficients of the w̄ update: 1/alpha, -beta/alpha
+  CraigState<T>* s;
+  __device__ void operator()(const T* tot) const {
+    CraigNormFin<T>{&s->alpha, &s->s_v}(tot);
+    if (s->alpha != T(0)) { s->ia = div_rn(T(1), s->alpha); s->mba = div_rn(-s->beta, s->alpha); }
+  }
+};
+// CRAIGMR R3 over m: w = (1/rho) w̄ + tr w ; y += zeta w ; alpha != 0: w̄ = (1/alpha) u - (beta/alpha) w̄
+template <class T> struct CraigmrP3Body {
+  T* w; T* y; T* wbar; const T* mu; const CraigState<T>* s; T s_u, inv_rho, tr, zeta;
+  __device__ __forceinline__ void operator()(int i, T*) const {
+    const T wb = wbar[i];
+    const T wn = add_rn(mul_rn(inv_rho, wb), mul_rn(tr, w[i]));
+    w[i] = wn;
+    y[i] = add_rn(y[i], mul_rn(zeta, wn));
+    if (s->alpha != T(0)) wbar[i] = add_rn(mul_rn(s->ia, mul_rn(mu[i], s_u)), mul_rn(s->mba, wb));
+  }
+};
+
+template <class T> T craigmr_fused_p1(Workspace<T>& ws, const Csr<T>& A, bool init, T s_u, T alpha) {
+  CraigState<T>* S = craig_state<T>(ws, init);
+  launch_spmv_epi_g<T, 1>(ws.ctx, A, XScaled<T>{ws.Nv, &S->s_v, T(1)}, CraigmrP1Epi<T>{ws.Mu, s_u, alpha},
+                          CraigNormFin<T>{&S->beta, &S->s_u}, 4);
+  return craig_read<T>(ws).beta;
+}
+template <class T>
+T craigmr_fused_p23(Workspace<T>& ws, const Csr<T>& At, bool first, T s_u, T s_v, T beta, T rho, T inv_rho, T tr, T zeta) {
+  CraigState<T>* S = (CraigState<T>*)ws.fused_state;
+  launch_spmv_epi_g<T, 1>(ws.ctx, At, XScaled<T>{ws.Mu, &S->s_u, T(1)},
+                          CraigmrP2Epi<T>{ws.Nv, ws.d1, ws.x, s_v, rho, inv_rho, tr, zeta, beta, first ? 1 : 0}, CraigmrP2Fin<T>{S}, 4);
+  launch_stream<T, 0>(ws.ctx, ws.m, CraigmrP3Body<T>{ws.w, ws.y, ws.w1, ws.Mu, S, s_u, inv_rho, tr, zeta}, NoFin(), 5);
+  return craig_read<T>(ws).alpha;
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1371,7 +1517,12 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void minares_fused_update<T>(Workspace<T>&, int, T*, bool, T, T*, const T*, const T*, T, T, T, T);       \
   template void bilqr_fused_update<T>(Workspace<T>&, bool, bool, int, T, T, T, T, T*, const T*, T, T, T, T, T, T, bool, T*); \
   template void trilqr_fused_ssy<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T*, T*, T*);             \
-  template void trilqr_fused_update<T>(Workspace<T>&, bool, bool, int, T, T, T, T, T*, const T*, T, T, T, T, T, T);
+  template void trilqr_fused_update<T>(Workspace<T>&, bool, bool, int, T, T, T, T, T*, const T*, T, T, T, T, T, T); \
+  template T craig_fused_p1<T>(Workspace<T>&, const Csr<T>&, bool, T, T, bool, T);                                 \
+  template void craig_fused_p2<T>(Workspace<T>&, const Csr<T>&, T, T, T, T, T*, T*);                              \
+  template void craig_fused_flush<T>(Workspace<T>&, T, T);                                                         \
+  template T craigmr_fused_p1<T>(Workspace<T>&, const Csr<T>&, bool, T, T);                                         \
+  template T craigmr_fused_p23<T>(Workspace<T>&, const Csr<T>&, bool, T, T, T, T, T, T, T);
 INST(double)
 INST(float)
 #undef INST

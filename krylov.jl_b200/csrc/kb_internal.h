@@ -12,7 +12,8 @@
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
 //   biorth.cu     host control flow of bilq!/qmr! (one Lanczos biorthogonalization driver; A and A^T)
 //   adjoint.cu    host control flow of bilqr!/trilqr! (adjoint system pairs A x = b, A^T y = c; two solutions)
-//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! on rectangular operators (primitive and fused paths)
+//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! and of the least-norm craig!/craigmr! on rectangular
+//                 operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
 #pragma once
@@ -214,9 +215,13 @@ struct Stats {
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
                   S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_TRILQR = 18, S_BILQR = 19, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
-                  S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
-// the least-squares solvers: A is m x n, b has m entries and x has n
-inline bool is_ls_kind(int k) { return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS; }
+                  S_CRAIG = 28, S_CRAIGMR = 29, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
+// the least-squares and least-norm solvers: A is m x n, b has m entries and x has n
+inline bool is_ls_kind(int k) {
+  return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS || k == S_CRAIG || k == S_CRAIGMR;
+}
+// the least-norm solvers: min ||x|| subject to A x = b, with x = A^T y; they return the multipliers y (m entries) too
+inline bool is_leastnorm_kind(int k) { return k == S_CRAIG || k == S_CRAIGMR; }
 // the adjoint-pair solvers: two solutions, x (A x = b) and y (A^T y = c).  TriLQR: A is m x n, b and y have m entries,
 // c and x have n; BiLQR: square
 inline bool is_adjoint_kind(int k) { return k == S_BILQR || k == S_TRILQR; }
@@ -246,6 +251,8 @@ struct Workspace {
                                        // w = d̅, w1 = w_{k-3}, w2 = w_{k-2}; TriLQR: v-space vectors have m entries)
   T *d1 = nullptr, *d2 = nullptr;      // MINARES: d_{k-1}, d_{k-2} (+ v = v_k, vv = v_{k+1}, w1 = w_{k-1}, w2 = w_{k-2}, q)
                                        // CAR: r, p, s, q, t, u (+ Mu, lazy)
+                                       // CRAIG: x, Nv, Atu (n), y, w, Mu, Av (m) (+ u, v, w2: lazy)
+                                       // CRAIGMR: d in d1, w̄ in w1 (+ x, Nv, Atu, y, w, Mu, Av; u, v, q: lazy)
   T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
                                        // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
   std::vector<T*> V;
@@ -320,6 +327,11 @@ template <class T> void lsmr_solve(Workspace<T>& ws, const LinOp<T>& A, const Li
                                    const LinOp<T>& N, const SolveOpts& o);
 template <class T> void lslq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const LinOp<T>& N, const SolveOpts& o);
+// Least norm (lsq.cu): min ||x|| subject to A x = b, x = A^T y; M acts on the m-space, N on the n-space.
+template <class T> void craig_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                    const LinOp<T>& N, const SolveOpts& o);
+template <class T> void craigmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                      const LinOp<T>& N, const SolveOpts& o);
 // CGLS / CRLS: M (m x m) acts on the residual space; they take no N.
 template <class T> void cgls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const SolveOpts& o);
@@ -410,6 +422,20 @@ template <class T> void lsq_fused_bidiag(Workspace<T>& ws, const Csr<T>& A, cons
 template <class T> T lsq_fused_update(Workspace<T>& ws, bool lsmr, bool scale_v, T inv_alpha, T sigma, T tau, T delta);
 // LSLQ's update after P1 / P2 (w = w̄): v = Nv / alpha (scale_v), x += (c zeta) w̄, x += (s zeta) v, w̄ = -c v + s w̄.
 template <class T> void lslq_fused_update(Workspace<T>& ws, bool scale_v, T inv_alpha, T czeta, T szeta, T c, T s);
+// CRAIG (fused_phases.cu), lambda = 0, M = N = I, A and A^T CSR operators; Mu and Nv stay unscaled (s_u = 1/beta and
+// s_v = 1/alpha are applied by their readers).  C1: SpMV on A^T gathering u with x += xi v (the previous iteration's
+// update, pending when xup), Nv = A^T u - beta v; returns alpha (one read-back).  `init`: first iteration.
+template <class T> T craig_fused_p1(Workspace<T>& ws, const Csr<T>& At, bool init, T beta, T s_v, bool xup, T xi);
+// C2: SpMV on A gathering v with w = u + tw w, y += ty w, Mu = A v - alpha u; one read-back of beta and <w, w>.
+template <class T> void craig_fused_p2(Workspace<T>& ws, const Csr<T>& A, T s_u, T alpha, T tw, T ty, T* beta, T* ww);
+// the pending x += xi v (before a callback and after the last iteration)
+template <class T> void craig_fused_flush(Workspace<T>& ws, T xi, T s_v);
+// CRAIGMR (fused_phases.cu), same conditions.  R1: SpMV on A gathering v, Mu = A v - alpha u; returns beta.
+template <class T> T craigmr_fused_p1(Workspace<T>& ws, const Csr<T>& A, bool init, T s_u, T alpha);
+// R2: SpMV on A^T gathering u, d = v / rho (first) or (1/rho) v + tr d, x += zeta d, Nv = A^T u - beta v; R3 over m:
+// w = (1/rho) w̄ + tr w, y += zeta w and, when alpha != 0, w̄ = (1/alpha) u - (beta/alpha) w̄.  Returns alpha.
+template <class T> T craigmr_fused_p23(Workspace<T>& ws, const Csr<T>& At, bool first, T s_u, T s_v, T beta, T rho, T inv_rho,
+                                       T tr, T zeta);
 // One CGLS iteration, M = I, no trust region, 4 launches: K1 q = A p (alpha on the device), K2 r -= alpha q, K3 s = A^T r
 // with x += alpha p and s -= lambda x, K4 p = s + beta p.  One read-back: <r, r> and gamma = <s, s>.
 // `init`: first iteration, sets gamma (and <p, p> = gamma) on the device from the host.

@@ -906,7 +906,369 @@ void crls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   run.finish(iter, solved, false, st);
 }
 
+// ===========================================================================
+// craig!  (src/craig.jl:174-405): CG on A Aᴴ y = b, x = Aᴴ y.  The Golub-Kahan products run in the opposite order from
+// LSQR's: Aᴴu first, then A v.  Fused (λ = 0, M = N = I, CSR A and Aᴴ): C1 on Aᴴ, then C2 on A, one read-back each;
+// x += ξ v rides in the next C1 and is flushed before a callback and after the last iteration.
+// ===========================================================================
+template <class T>
+void craig_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                 const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CRAIG: system of %d equations in %d variables\n", m, n);
+  const T lambda = (T)o.lambda;
+  const T conlim = o.conlim < 0 ? T(1) / std::sqrt(eps_of<T>()) : (T)o.conlim;
+  const T btol = tol_of<T>(o.btol), atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  Stats& stats = ws.stats;
+
+  T beta1;
+  Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta1);
+  s.fused = s.fused && lambda == 0;                             // the fused passes carry no regularization
+  allocate_if(!s.fused, ws, ws.Av, m);
+  allocate_if(!s.fused, ws, ws.Atu);
+  allocate_if(lambda > 0, ws, ws.w2);
+  T* u = s.MisI ? ws.Mu : ws.u;
+  T* v = s.NisI ? ws.Nv : ws.v;
+  k_fill<T>(c, m, ws.y, T(0));
+  T rNorm = beta1;
+  if (history) stats.residuals.push_back(rNorm);
+  if (beta1 == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    return;
+  }
+  const T beta1_2 = beta1 * beta1;
+  T beta = beta1, theta = beta1, xi = T(-1), delta = lambda, rho_prev = T(1);
+
+  k_scal<T>(c, m, T(1) / beta1, u);                            // β₁Mu₁ = b
+  if (!s.MisI) k_scal<T>(c, m, T(1) / beta1, ws.Mu);
+  k_fill<T>(c, n, ws.Nv, T(0));
+  k_fill<T>(c, m, ws.w, T(0));
+  if (lambda > 0) k_fill<T>(c, n, ws.w2, T(0));
+
+  T Anorm2 = 0, Anorm = 0, Dnorm2 = 0, Acond = 0, xNorm2 = 0, xNorm = 0;
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+  const T eps_c = atol + rtol * rNorm;
+  const T ctol = conlim > 0 ? T(1) / conlim : T(0);
+  if (o.verbose > 0) printf("%5s  %8s  %8s  %8s  %8s  %8s  %7s  %5s\n", "k", "‖r‖", "‖x‖", "‖A‖", "κ(A)", "α", "β", "timer");
+  if (kdisplay(iter, o.verbose))
+    printf("%5d  %8.2e  %8.2e  %8.2e  %8.2e  %8s  %7s  %.2fs\n", iter, (double)rNorm, (double)xNorm, (double)Anorm, (double)Acond,
+           " ✗ ✗ ✗ ✗", "✗ ✗ ✗ ✗", run.elapsed());
+
+  T bkwerr = 1;
+  bool solved_lim = bkwerr <= btol, solved_mach = T(1) + bkwerr <= T(1), solved_resid_tol = rNorm <= eps_c;
+  bool solved_resid_lim = rNorm <= btol + atol * Anorm * xNorm / beta1;
+  bool solved = solved_mach || solved_lim || solved_resid_tol || solved_resid_lim;
+  bool ill_cond = false, ill_cond_mach = false, ill_cond_lim = false, inconsistent = false;
+  bool tired = iter >= itmax, user_exit = false, overtimed = false;
+  // fused: the x update of the last completed iteration waits for the next C1 (factor s_v = 1/α of that iteration)
+  // fused: s_u = 1/β and s_v = 1/α of the stored Mu and Nv (1 while they hold u₁ and v₀ = 0)
+  bool xpend = false;
+  T xi_pend = 0, s_u = 1, s_v = 1;
+
+  while (!(solved || inconsistent || ill_cond || tired || user_exit || overtimed)) {
+    // 1. αₖ₊₁Nvₖ₊₁ = Aᴴuₖ₊₁ - βₖ₊₁Nvₖ
+    T alpha;
+    if (s.fused) {
+      alpha = craig_fused_p1<T>(ws, *At.csr, iter == 0 && !xpend, beta, s_v, xpend, xi_pend);
+      xpend = false;
+    } else {
+      op_apply(c, At, u, ws.Atu);
+      k_axpby<T>(c, n, T(1), ws.Atu, -beta, ws.Nv);
+      if (!s.NisI) op_apply(c, N, ws.Nv, v, ldiv);
+      alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+    }
+    if (alpha == 0) {
+      inconsistent = true;
+      continue;
+    }
+    if (s.fused) {
+      s_v = T(1) / alpha;                                       // kdiv!(n, v, α), applied by v's readers
+    } else {
+      k_scal<T>(c, n, T(1) / alpha, v);
+      if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+    }
+
+    Anorm2 += alpha * alpha + lambda * lambda;
+    T c1 = 1, s1 = 0, rho;
+    if (lambda > 0) sym_givens<T>(alpha, delta, &c1, &s1, &rho);
+    else rho = alpha;
+    xi = -theta / rho * xi;
+
+    if (lambda > 0) {
+      // w1 = c₁ v + s₁ w2 ; w2 = s₁ v - c₁ w2 ; x = x + ξ w1
+      k_axpy<T>(c, n, xi * c1, v, ws.x);
+      k_axpy<T>(c, n, xi * s1, ws.w2, ws.x);
+      k_axpby<T>(c, n, s1, v, -c1, ws.w2);
+    } else if (s.fused) {
+      xpend = true; xi_pend = xi;
+    } else {
+      k_axpy<T>(c, n, xi, v, ws.x);
+    }
+
+    // Recur y, then 2. βₖ₊₁Muₖ₊₁ = Avₖ - αₖMuₖ
+    if (s.fused) {
+      T ww;
+      craig_fused_p2<T>(ws, *A.csr, s_u, alpha, -theta / rho_prev, xi / rho, &beta, &ww);
+      s_u = beta == 0 ? T(1) : T(1) / beta;                     // kdiv!(m, u, β), applied by u's readers
+      Dnorm2 += std::sqrt(ww);
+    } else {
+      k_axpby<T>(c, m, T(1), u, -theta / rho_prev, ws.w);      // w = u - θ/ρ_prev * w
+      k_axpy<T>(c, m, xi / rho, ws.w, ws.y);                    // y = y + ξ/ρ * w
+      Dnorm2 += k_nrm2<T>(c, m, ws.w);                          // knorm(m, w): a norm, as the reference has it
+      op_apply(c, A, v, ws.Av);
+      k_axpby<T>(c, m, T(1), ws.Av, -alpha, ws.Mu);
+      if (!s.MisI) op_apply(c, M, ws.Mu, u, ldiv);
+      beta = knorm_elliptic<T>(c, m, u, ws.Mu);
+      if (beta != 0) {
+        k_scal<T>(c, m, T(1) / beta, u);
+        if (!s.MisI) k_scal<T>(c, m, T(1) / beta, ws.Mu);
+      }
+    }
+
+    // Finish the updates from the first Givens rotation.
+    T gamma = 0;
+    if (lambda > 0) {
+      theta = beta * c1;
+      gamma = beta * s1;
+      T c2, s2;
+      sym_givens<T>(lambda, gamma, &c2, &s2, &delta);
+      k_scal<T>(c, n, s2, ws.w2);
+    } else {
+      theta = beta;
+    }
+
+    Anorm2 += beta * beta;
+    Anorm = std::sqrt(Anorm2);
+    Acond = Anorm * std::sqrt(Dnorm2);
+    xNorm2 += xi * xi;
+    xNorm = std::sqrt(xNorm2);
+    rNorm = beta * std::fabs(xi);                               // r = - β ξ u
+    if (lambda > 0) rNorm *= std::fabs(c1);                     // r = - c₁ β ξ u when λ > 0
+    if (history) stats.residuals.push_back(rNorm);
+    iter = iter + 1;
+    bkwerr = rNorm / std::sqrt(beta1_2 + Anorm2 * xNorm2);
+    rho_prev = rho;
+    if (kdisplay(iter, o.verbose))
+      printf("%5d  %8.2e  %8.2e  %8.2e  %8.2e  %8.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)xNorm, (double)Anorm,
+             (double)Acond, (double)alpha, (double)beta, run.elapsed());
+
+    solved_lim = bkwerr <= btol;
+    solved_mach = T(1) + bkwerr <= T(1);
+    solved_resid_tol = rNorm <= eps_c;
+    solved_resid_lim = rNorm <= btol + atol * Anorm * xNorm / beta1;
+    solved = solved_mach || solved_lim || solved_resid_tol || solved_resid_lim;
+    ill_cond_mach = T(1) + T(1) / Acond <= T(1);
+    ill_cond_lim = T(1) / Acond <= ctol;
+    ill_cond = ill_cond_mach || ill_cond_lim;
+    if (xpend && o.callback) {                                  // the callback reads x
+      craig_fused_flush<T>(ws, xi_pend, s_v);
+      xpend = false;
+    }
+    run.poll(iter, user_exit, overtimed);
+    inconsistent = false;
+    tired = iter >= itmax;
+  }
+  if (xpend) craig_fused_flush<T>(ws, xi_pend, s_v);
+  if (o.verbose > 0) printf("\n");
+
+  if (lambda > 0 && o.transfer_to_lsqr) {                       // the LSQR point
+    xi *= -theta / delta;
+    k_axpy<T>(c, n, xi, ws.w2, ws.x);
+  }
+
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (solved) st = "solution good enough for the tolerances given";
+  if (ill_cond_mach) st = "condition number seems too large for this machine";
+  if (ill_cond_lim) st = "condition number exceeds tolerance";
+  if (inconsistent) st = "system may be inconsistent";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  run.finish(iter, solved, inconsistent, st);
+}
+
+// ===========================================================================
+// craigmr!  (src/craigmr.jl:161-396): MINRES on A Aᴴ y = b, x = Aᴴ y.  Fused (λ = 0, M = N = I, CSR A and Aᴴ): R1 on A,
+// read β, the Givens step on the host, then R2 on Aᴴ and R3 over m, read α: 3 launches and 2 read-backs.
+// ===========================================================================
+template <class T>
+void craigmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                   const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CRAIGMR: system of %d equations in %d variables\n", m, n);
+  const T lambda = (T)o.lambda;
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  Stats& stats = ws.stats;
+
+  T beta;
+  Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta);
+  s.fused = s.fused && lambda == 0;                             // the fused passes carry no regularization
+  allocate_if(!s.fused, ws, ws.Av, m);
+  allocate_if(!s.fused, ws, ws.Atu);
+  allocate_if(lambda > 0, ws, ws.q);
+  T* u = s.MisI ? ws.Mu : ws.u;
+  T* v = s.NisI ? ws.Nv : ws.v;
+  k_fill<T>(c, m, ws.y, T(0));
+  if (beta == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    if (history) { stats.residuals.push_back(beta); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  lsq_start<T>(ws, s, At, N, ldiv, beta);                       // u /= β₁, Nv = Aᴴu, v = N Nv
+  T alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+  T Anorm2 = alpha * alpha;
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+  if (o.verbose > 0) printf("%5s  %7s  %7s  %7s  %7s  %8s  %8s  %7s  %5s\n", "k", "‖r‖", "‖Aᴴr‖", "β", "α", "cos", "sin", "‖A‖²", "timer");
+  if (kdisplay(iter, o.verbose))
+    printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %.2fs\n", iter, (double)beta, (double)alpha, (double)beta,
+           (double)alpha, 0.0, 1.0, (double)Anorm2, run.elapsed());
+  if (alpha == 0) {                                             // Aᴴb = 0: x = 0 is a minimum least-squares solution
+    run.finish(0, true, false, "x is a minimum least-squares solution");
+    if (history) { stats.residuals.push_back(beta); stats.Aresiduals.push_back(0); }
+    return;
+  }
+  k_scal<T>(c, n, T(1) / alpha, v);
+  if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+
+  // Regularization
+  const T lambdak = lambda;                                     // λ₁ = λ
+  T cpk = 1, spk = 1, cdk = 1, sdk = 1, alphahat;
+  if (lambda > 0) k_copy<T>(c, n, ws.q, v);                     // q₀ = 0 by definition
+  if (lambda > 0) {
+    sym_givens<T>(alpha, lambdak, &cpk, &spk, &alphahat);
+    k_scal<T>(c, n, spk, ws.q);                                 // q̄₁ = sp₁ v₁
+  } else {
+    alphahat = alpha;
+  }
+  (void)cdk;
+
+  T zetabar = beta, rhobar = alphahat, theta = 0;
+  T rNorm = zetabar;
+  if (history) stats.residuals.push_back(rNorm);
+  T ArNorm = alpha;
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  const T eps_c = atol + rtol * rNorm;
+  const T eps_i = atol + rtol * ArNorm;
+  k_divcopy<T>(c, m, ws.w1, u, alphahat);                       // w̄ = u / α̂
+  k_fill<T>(c, m, ws.w, T(0));
+  k_fill<T>(c, n, ws.d1, T(0));
+
+  bool solved = rNorm <= eps_c;
+  bool inconsistent = (rNorm > 100 * eps_c) && (ArNorm <= eps_i);
+  bool tired = iter >= itmax, user_exit = false, overtimed = false;
+  T s_u = 1, s_v = 1;                                           // fused: 1/β and 1/α of the stored Mu and Nv (u₁, v₁ are scaled)
+
+  while (!(solved || inconsistent || tired || user_exit || overtimed)) {
+    iter = iter + 1;
+    // 1. βₖ₊₁Muₖ₊₁ = Avₖ - αₖMuₖ
+    if (s.fused) {
+      beta = craigmr_fused_p1<T>(ws, *A.csr, iter == 1, s_u, alpha);
+    } else {
+      op_apply(c, A, v, ws.Av);
+      k_axpby<T>(c, m, T(1), ws.Av, -alpha, ws.Mu);
+      if (!s.MisI) op_apply(c, M, ws.Mu, u, ldiv);
+      beta = knorm_elliptic<T>(c, m, u, ws.Mu);
+      if (beta != 0) {
+        k_scal<T>(c, m, T(1) / beta, u);
+        if (!s.MisI) k_scal<T>(c, m, T(1) / beta, ws.Mu);
+      }
+    }
+    Anorm2 = Anorm2 + beta * beta;                              // = ‖B_{k-1}‖²
+
+    T betahat, lambda_aux = 0;
+    if (lambda > 0) {
+      betahat = cpk * beta;
+      lambda_aux = spk * beta;
+    } else {
+      betahat = beta;
+    }
+
+    // Continue QR factorization
+    T cs, sn, rho;
+    sym_givens<T>(rhobar, betahat, &cs, &sn, &rho);
+    const T zeta = cs * zetabar;
+    zetabar = sn * zetabar;
+    rNorm = std::fabs(zetabar);
+    if (history) stats.residuals.push_back(rNorm);
+
+    if (s.fused) {
+      s_u = beta == 0 ? T(1) : T(1) / beta;
+      alpha = craigmr_fused_p23<T>(ws, *At.csr, iter == 1, s_u, s_v, beta, rho, T(1) / rho, -theta / rho, zeta);
+      s_v = alpha == 0 ? T(1) : T(1) / alpha;
+    } else {
+      k_axpby<T>(c, m, T(1) / rho, ws.w1, -theta / rho, ws.w); // w = (w̄ - θ w) / ρ
+      k_axpy<T>(c, m, zeta, ws.w, ws.y);                        // y = y + ζ w
+      if (lambda > 0) {                                         // DₖRₖ = V̅ₖ with v̅ₖ = cpₖvₖ + spₖqₖ₋₁
+        if (iter == 1) {
+          k_axpy<T>(c, n, cpk / rho, v, ws.d1);
+        } else {
+          k_axpby<T>(c, n, cpk / rho, v, -theta / rho, ws.d1);
+          k_axpy<T>(c, n, spk / rho, ws.q, ws.d1);
+          k_axpby<T>(c, n, spk, v, -cpk, ws.q);                 // q̄ₖ ← spₖ vₖ - cpₖ qₖ₋₁
+        }
+      } else {                                                  // DₖRₖ = Vₖ
+        if (iter == 1) k_divcopy<T>(c, n, ws.d1, v, rho);
+        else k_axpby<T>(c, n, T(1) / rho, v, -theta / rho, ws.d1);
+      }
+      k_axpy<T>(c, n, zeta, ws.d1, ws.x);                       // xₖ = Dₖzₖ
+      // 2. αₖ₊₁Nvₖ₊₁ = Aᴴuₖ₊₁ - βₖ₊₁Nvₖ
+      op_apply(c, At, u, ws.Atu);
+      k_axpby<T>(c, n, T(1), ws.Atu, -beta, ws.Nv);
+      if (!s.NisI) op_apply(c, N, ws.Nv, v, ldiv);
+      alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+    }
+    Anorm2 = Anorm2 + alpha * alpha;                            // = ‖Lₖ‖
+    ArNorm = alpha * beta * std::fabs(zeta / rho);
+    if (history) stats.Aresiduals.push_back(ArNorm);
+    if (kdisplay(iter, o.verbose))
+      printf("%5d  %7.1e  %7.1e  %7.1e  %7.1e  %8.1e  %8.1e  %7.1e  %.2fs\n", iter, (double)rNorm, (double)ArNorm, (double)beta,
+             (double)alpha, (double)cs, (double)sn, (double)Anorm2, run.elapsed());
+
+    if (lambda > 0) {
+      T lambdak1;
+      sym_givens<T>(lambda, lambda_aux, &cdk, &sdk, &lambdak1);
+      k_scal<T>(c, n, sdk, ws.q);                               // qₖ ← sdₖ q̄ₖ
+      sym_givens<T>(alpha, lambdak1, &cpk, &spk, &alphahat);
+    } else {
+      alphahat = alpha;
+    }
+    if (alpha != 0 && !s.fused) {                               // fused: R3 updated w̄ and v's readers apply 1/α
+      k_scal<T>(c, n, T(1) / alpha, v);
+      if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+      k_axpby<T>(c, m, T(1) / alphahat, u, -betahat / alphahat, ws.w1);   // w̄ = (u - β̂ w̄) / α̂
+    }
+    theta = sn * alphahat;
+    rhobar = -cs * alphahat;
+
+    run.poll(iter, user_exit, overtimed);
+    solved = rNorm <= eps_c;
+    inconsistent = (rNorm > 100 * eps_c) && (ArNorm <= eps_i);
+    tired = iter >= itmax;
+  }
+  if (o.verbose > 0) printf("\n");
+
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (solved) st = "found approximate minimum-norm solution";
+  if (!tired && !solved) st = "found approximate minimum least-squares solution";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  run.finish(iter, solved, inconsistent, st);
+}
+
 #define INST(T)                                                                                                         \
+  template void craig_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
+                               const SolveOpts&);                                                                       \
+  template void craigmr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
+                                 const SolveOpts&);                                                                     \
   template void lslq_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
                               const SolveOpts&);                                                                        \
   template void cgls_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&); \

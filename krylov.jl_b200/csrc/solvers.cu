@@ -88,6 +88,12 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         ws->v_prev = Am(); ws->v = Am(); ws->q = Am(); ws->y = Am(); ws->w1 = Am(); ws->w2 = Am();
         break;
       }
+      case S_CRAIG: case S_CRAIGMR: {               // CraigWorkspace / CraigmrWorkspace (Av, Aᴴu, u, v, w2 / q: by the solve)
+        auto Am = [&]() { return dev_alloc<T>((size_t)m); };
+        ws->Nv = A(); ws->Mu = Am(); ws->y = Am(); ws->w = Am();
+        if (kind == S_CRAIGMR) { ws->d1 = A(); ws->w1 = Am(); }   // d, w̄
+        break;
+      }
       case S_CAR:                                   // CarWorkspace (Mu is allocated by the solve)
         ws->r = A(); ws->p = A(); ws->s = A(); ws->q = A(); ws->t = A(); ws->u = A();
         break;

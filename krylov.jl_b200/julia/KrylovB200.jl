@@ -196,7 +196,7 @@ end
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
                        :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25, :bilq => 12, :qmr => 13,
-                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :cg_lanczos => 100)
+                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :craig => 28, :craigmr => 29, :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -446,6 +446,43 @@ Krylov.cgls!(ws::Krylov.CglsWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200C
   normal_ls_solve!(:cgls, ws, A, b; kw...)
 Krylov.crls!(ws::Krylov.CrlsWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
   normal_ls_solve!(:crls, ws, A, b; kw...)
+
+# ---- craig! / craigmr! (src/craig.jl:151-166, src/craigmr.jl:141-153) on a rectangular B200CSR: one krylov_solve ----
+# The least-norm solution of A x = b with x = Aᵀ y: the workspace's x receives x and its y the multipliers y.  The
+# library forms Aᵀ once per operator; the fused Golub-Kahan passes run when M = N = I and λ = 0, B200Diagonal M
+# (m entries) / N (n entries) and λ > 0 run its primitive path.  btol, conlim and transfer_to_lsqr are CRAIG's only.
+function leastnorm_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N = I, ldiv::Bool = false,
+                          transfer_to_lsqr::Bool = false, sqd::Bool = false, λ::T = zero(T), btol::T = √eps(T),
+                          conlim::T = 1/√eps(T), atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0,
+                          timemax::Float64 = Inf, verbose::Int = 0, history::Bool = false, callback = workspace -> false,
+                          iostream::IO = stdout) where T
+  length(b) == A.m || error("Inconsistent problem size")
+  sqd && (λ ≠ 0) && error("sqd cannot be set to true if λ ≠ 0 !")
+  sqd && (λ = one(T))
+  h = handle_for(method, ws, A, 0, 0)
+  set_precond!(h, 0, M)
+  set_precond!(h, 1, N)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, NaN, conlim, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, btol, 0.0, NaN,
+                 transfer_to_lsqr, 1))
+  o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, C_NULL, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+    check(ccall((:krylov_get_y, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.y.ptr, A.m))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.craig!(ws::Krylov.CraigWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  leastnorm_solve!(:craig, ws, A, b; kw...)
+Krylov.craigmr!(ws::Krylov.CraigmrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  leastnorm_solve!(:craigmr, ws, A, b; kw...)
 
 # ---- bilq! / qmr! (src/bilq.jl:97-115, src/qmr.jl:104-114) on a square B200CSR: one krylov_solve per solve ------------
 # The library forms Aᵀ once per operator and runs the fused Lanczos biorthogonalization when M = N = I; `c` defaults to b.

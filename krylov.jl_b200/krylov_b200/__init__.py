@@ -41,7 +41,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_",
            "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_",
            "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_",
-           "AdjointStats", "BilqrWorkspace", "TrilqrWorkspace", "bilqr", "bilqr_", "trilqr", "trilqr_"]
+           "AdjointStats", "BilqrWorkspace", "TrilqrWorkspace", "bilqr", "bilqr_", "trilqr", "trilqr_",
+           "CraigWorkspace", "CraigmrWorkspace", "craig", "craig_", "craigmr", "craigmr_"]
 
 
 class B200Error(RuntimeError):
@@ -1076,6 +1077,93 @@ class TrilqrWorkspace(_AdjointWorkspace):
                            unknown)
 
 
+class _LeastNormWorkspace(_LeastSquaresWorkspace):
+    """Workspace of craig! / craigmr! on an m x n operator (src/krylov_workspaces.jl CraigWorkspace / CraigmrWorkspace):
+    the least-norm solution of A x = b, x = A^T y.  b and y have m entries, x has n.  A and its adjoint: a CSR operator
+    (its transpose is formed once and cached), or a scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host
+    callables.  M (m entries) and N (n entries): None, the diagonal of a Diagonal preconditioner, or a host callable."""
+    nA = 2
+
+    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
+        super().__init__(m_or_A, n_or_b, dtype, device=device)
+
+    def _solve(self, A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
+               unknown, transfer_to_lsqr=False, btol=None, conlim=None):
+        if unknown:
+            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        if sqd and lambda_ != 0:
+            raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
+        if sqd:
+            lambda_ = 1.0
+        o = lib().krylov_default_options()
+        if atol is not None:
+            o.atol = float(atol)
+        if rtol is not None:
+            o.rtol = float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        o.lambda_ = float(lambda_)
+        e = lib().krylov_b200_default_options()
+        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        e.transfer_to_lsqr = int(transfer_to_lsqr)
+        for name, val in (("btol", btol), ("conlim", conlim)):
+            if val is not None:
+                setattr(e, name, float(val))
+        return self._run(A, b, M, N, o, e, callback)
+
+    y = _AdjointWorkspace.y
+
+
+class CraigWorkspace(_LeastNormWorkspace):
+    solver = "craig"
+
+    def solve(self, A, b, *, M=None, N=None, ldiv=False, transfer_to_lsqr=False, sqd=False, lambda_=0.0, btol=None,
+              conlim=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False, callback=None,
+              fused=True, **unknown):
+        """craig!(ws, A, b; kwargs...)  -- kwargs as in craig.jl:151-166: btol, atol and rtol default to sqrt(eps),
+        conlim to 1/sqrt(eps), itmax = 0 means m + n; transfer_to_lsqr acts when λ > 0."""
+        return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
+                           unknown, transfer_to_lsqr, btol, conlim)
+
+
+class CraigmrWorkspace(_LeastNormWorkspace):
+    solver = "craigmr"
+
+    def solve(self, A, b, *, M=None, N=None, ldiv=False, sqd=False, lambda_=0.0, atol=None, rtol=None, itmax=0,
+              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
+        """craigmr!(ws, A, b; kwargs...)  -- kwargs as in craigmr.jl:141-153: atol and rtol default to sqrt(eps),
+        itmax = 0 means m + n."""
+        return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
+                           unknown)
+
+
+def _make_least_norm(name):
+    def f(A, b, x0=None, *, n=None, **kw):
+        if x0 is not None:
+            raise B200Error(f"{name} does not support warm-start (it takes no x0)")
+        m = b.shape[0]
+        if n is None:
+            if not hasattr(A, "shape"):
+                raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
+            n = A.shape[1]
+        if _is_torch(b):                      # the element type, without copying a device b to the host
+            import torch
+            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
+        else:
+            dt = np.asarray(b).dtype
+        if dt not in (np.float32, np.float64):
+            dt = np.float64
+        ws = _WS[name](m, int(n), dt, device="cuda" if _is_torch(b) else "host")
+        try:
+            ws.solve(A, b, **kw)
+            return ws.x, ws.y, ws.stats
+        finally:
+            ws.free()
+    f.__name__ = name
+    f.__doc__ = f"(x, y, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
+    return f
+
+
 def _make_adjoint(name):
     def f(A, b, c, x0=None, y0=None, **kw):
         m, n = b.shape[0], c.shape[0]
@@ -1141,7 +1229,8 @@ _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "b
        "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
        "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
        "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace, "car": CarWorkspace,
-       "minares": MinaresWorkspace, "bilqr": BilqrWorkspace, "trilqr": TrilqrWorkspace}
+       "minares": MinaresWorkspace, "bilqr": BilqrWorkspace, "trilqr": TrilqrWorkspace, "craig": CraigWorkspace,
+       "craigmr": CraigmrWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -1201,12 +1290,14 @@ car_, minares_ = (_make_inplace(s) for s in ("car", "minares"))
 car, minares = (_make_outofplace(s) for s in ("car", "minares"))
 bilqr_, trilqr_ = (_make_adjoint_inplace(s) for s in ("bilqr", "trilqr"))
 bilqr, trilqr = (_make_adjoint(s) for s in ("bilqr", "trilqr"))
+craig_, craigmr_ = (_make_inplace(s) for s in ("craig", "craigmr"))
+craig, craigmr = (_make_least_norm(s) for s in ("craig", "craigmr"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):
     return {"cg": cg, "gmres": gmres, "bicgstab": bicgstab, "minres": minres, "fom": fom, "fgmres": fgmres, "cgs": cgs,
             "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres, "bilq": bilq,
-            "qmr": qmr, "car": car, "minares": minares}[method](A, b, x0, **kw)
+            "qmr": qmr, "car": car, "minares": minares, "craig": craig, "craigmr": craigmr}[method](A, b, x0, **kw)
 
 
 # workspace_accessors.jl:140-152

@@ -96,6 +96,44 @@ def csr_matvec_ones(rowptr, colind, values):
     return out
 
 
+def div_csr(N, dtype=np.float64, xp=np, device=None):
+    """Divergence D = G^T of the N x N x N grid, assembled in closed form (xp=torch with device="cuda": on the GPU):
+    m = N^3 rows (the points), n = 3 N^2 (N-1) columns (the rows of grad_csr(N)), at most six nonzeros per row.  Row p
+    holds, in ascending column order, +1 where p is the neighbour and -1 where p is the base point of a difference
+    along x, then y, then z.  Equal to grad_csr(N).T entry by entry.  Returns (rowptr, colind, values) as int32 CSR."""
+    is_t = xp is not np
+    kw = dict(device=device) if is_t else {}
+    i64 = xp.int64
+    p = xp.arange(N ** 3, dtype=i64, **kw)
+    i, j, k = p % N, (p // N) % N, p // (N * N)
+    mx = N * N * (N - 1)                                # rows of Dx (= of Dy, of Dz)
+
+    def rx(q):
+        return (q // N) * (N - 1) + q % N
+
+    def ry(q):
+        return mx + (q // (N * N)) * (N * (N - 1)) + q % (N * N)
+
+    def rz(q):
+        return 2 * mx + q
+    cols = [rx(p - 1), rx(p), ry(p - N), ry(p), rz(p - N * N), rz(p)]
+    keep = [i > 0, i < N - 1, j > 0, j < N - 1, k > 0, k < N - 1]
+    cols, keep = xp.stack(cols, 1), xp.stack(keep, 1)
+    sign = xp.tile(xp.asarray([1.0, -1.0], dtype=xp.float64, **kw), (3,)) if not is_t else \
+        xp.tensor([1.0, -1.0] * 3, dtype=xp.float64, **kw)
+    vals = (sign.reshape(1, 6) + xp.zeros((N ** 3, 6), dtype=xp.float64, **kw))[keep]
+    colind = cols[keep]
+    counts = keep.sum(1)
+    if is_t:
+        import torch
+        rowptr = torch.zeros(N ** 3 + 1, dtype=torch.int64, **kw)
+        rowptr[1:] = torch.cumsum(counts, 0)
+        tdt = torch.float64 if np.dtype(dtype) == np.float64 else torch.float32
+        return rowptr.to(torch.int32), colind.to(torch.int32), vals.to(tdt)
+    rowptr = np.concatenate([[0], np.cumsum(counts)])
+    return rowptr.astype(np.int32), colind.astype(np.int32), vals.astype(dtype)
+
+
 def grad_csr(N, dtype=np.float64, xp=np, device=None):
     """Forward-difference gradient G = [Dx; Dy; Dz] of an N x N x N grid (unknown (i,j,k) -> i + N*(j + N*k)), the
     rectangular operator of the least-squares benchmark: m = 3 N^2 (N-1) rows, n = N^3 columns, two nonzeros per row
