@@ -703,16 +703,17 @@ template <class T> void cg_dist_push_r(Workspace<T>& ws) {
 // ---------------------------------------------------------------------------
 // Everything the fused loops need besides the solver's vectors is allocated when the workspace is created
 // (ws_create) -- the in-place call allocates nothing (test/test_allocations.jl:54-57).
-constexpr size_t kOffGridBar = 1024, kOffPeerTab = 2048, kOffHostSeq = 3072;     // layout of the 4 KB device / pinned blocks
+constexpr size_t kOffGridBar = 1024, kOffPeerTab = 2048, kOffHostSeq = 3072;     // CG's layout of the 4 KB blocks
+
+template <class T> void fused_block_alloc(Workspace<T>& ws) {
+  KB_CUDA(cudaMalloc(&ws.fused_state, kFusedBlockBytes));
+  KB_CUDA(cudaMemset(ws.fused_state, 0, kFusedBlockBytes));
+  KB_CUDA(cudaHostAlloc(&ws.fused_host, kFusedBlockBytes, cudaHostAllocPortable | cudaHostAllocMapped));
+  memset(ws.fused_host, 0, kFusedBlockBytes);
+}
 
 template <class T> void cg_fused_prepare(Workspace<T>& ws) {
   static_assert(sizeof(CgState<T>) <= kOffGridBar && sizeof(CgPeerTab<T>) <= kFusedBlockBytes - kOffPeerTab, "block layout");
-  if (!ws.fused_state) {
-    KB_CUDA(cudaMalloc(&ws.fused_state, kFusedBlockBytes));
-    KB_CUDA(cudaMemset(ws.fused_state, 0, kFusedBlockBytes));
-    KB_CUDA(cudaHostAlloc(&ws.fused_host, kFusedBlockBytes, cudaHostAllocPortable | cudaHostAllocMapped));
-    memset(ws.fused_host, 0, kFusedBlockBytes);
-  }
   if (!ws.p2) ws.p2 = dev_alloc<T>((size_t)ws.n);
   for (int i = 0; i < 2; i++)
     if (!ws.fused_ev[i]) KB_CUDA(cudaEventCreateWithFlags(&ws.fused_ev[i], cudaEventDisableTiming));
@@ -1075,6 +1076,7 @@ CgFusedExit cg_fused_loop(Workspace<T>& ws, const CgFusedPlan<T>& pl, const Solv
 
 #define INST(T)                                                                                              \
   template CgFusedPlan<T> cg_fused_plan<T>(const Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const SolveOpts&); \
+  template void fused_block_alloc<T>(Workspace<T>&);                                                         \
   template void cg_fused_prepare<T>(Workspace<T>&);                                                          \
   template void cg_dist_push_r<T>(Workspace<T>&);                                                            \
   template CgFusedExit cg_fused_loop<T>(Workspace<T>&, const CgFusedPlan<T>&, const SolveOpts&, T, T, int, double);

@@ -1,16 +1,13 @@
-// fused_phases.cu -- fused iteration phases of bicgstab!, minres!, gmres!, the siblings and the least-squares solvers
-// (SURVEY.md section 8a phase structures).  Each phase is ONE launch: an SpMV
-// or a streaming pass whose epilogue applies the adjacent axpy/axpby/scal
-// updates and accumulates the dot products the next scalar needs; the CTA that
-// finishes the grid reduction derives that scalar on the device, so the phases
-// of one iteration chain through device memory and the host reads the scalar
-// block back once (BiCGSTAB, GMRES) or twice (MINRES) per iteration to run the
-// reference's stopping logic unchanged.
+// fused_phases.cu -- fused iteration phases of every solver family with a fused path except CG (cg_fused.cu)
+// (SURVEY.md section 8a phase structures).  Each phase is ONE launch: an SpMV or a streaming pass whose epilogue applies
+// the adjacent axpy/axpby/scal updates and accumulates the dot products the next scalar needs; the CTA that finishes
+// the grid reduction stores them, or the scalar derived from them, in the family's state struct on the device.  The
+// phases of one iteration chain through that struct, and the host reads it back (StateBlock) to run the reference's
+// stopping logic unchanged.
 //
-// Arithmetic is the reference's, operation by operation (non-contracted
-// mul/add in the same order as the kaxpy!/kaxpby!/kscal! sequence it replaces),
-// so these paths produce the same vectors as the primitive path given the same
-// scalars; tests assert that equality.
+// Arithmetic is the reference's, operation by operation (non-contracted mul/add in the same order as the
+// kaxpy!/kaxpby!/kscal! sequence it replaces), so these paths produce the same vectors as the primitive path given the
+// same scalars; tests assert that equality.
 #include "kb_internal.h"
 #include "spmv_tiles.cuh"
 
@@ -94,49 +91,70 @@ struct NoFin {
 };
 
 template <class T, int K, class Epi, class Fin, class G>
-static void launch_spmv_epi_g(Ctx& c, const Csr<T>& A, G xg, Epi epi, Fin fin, int ticket) {
+static void launch_spmv_epi_g(Ctx& c, const Csr<T>& A, G xg, Epi epi, Fin fin) {
+  unsigned* ticket = c.tickets + 4;       // the SpMV passes' grid reduction ticket (the streaming passes take 5)
   if (A.tma_ok) {
     ensure_dyn_smem((const void*)spmv_epi_tma<T, K, Epi, Fin, G>, 220 * 1024);
     int occ = 0;          // persistent grid = what is really co-resident (never more than one wave)
     KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, spmv_epi_tma<T, K, Epi, Fin, G>, kTileThreads, A.smem_bytes));
     if (occ < 1) throw std::runtime_error("spmv_epi_tma does not fit on an SM with the planned shared-memory ring");
     const int grid = std::min(std::min(occ, A.ctas_per_sm) * sm_count(), std::max(1, A.ntiles));
-    spmv_epi_tma<T, K, Epi, Fin, G><<<grid, kTileThreads, A.smem_bytes, c.stream>>>(A, xg, epi, fin, (T*)c.partials, c.tickets + ticket, c.dcomm);
+    spmv_epi_tma<T, K, Epi, Fin, G><<<grid, kTileThreads, A.smem_bytes, c.stream>>>(A, xg, epi, fin, (T*)c.partials, ticket, c.dcomm);
   } else {
-    spmv_epi_rows<T, K, Epi, Fin, G><<<stream_grid(A.n, 1, 8), kBlock, 0, c.stream>>>(A, xg, epi, fin, (T*)c.partials, c.tickets + ticket, c.dcomm);
+    spmv_epi_rows<T, K, Epi, Fin, G><<<stream_grid(A.n, 1, 8), kBlock, 0, c.stream>>>(A, xg, epi, fin, (T*)c.partials, ticket, c.dcomm);
   }
   KB_CUDA(cudaGetLastError());
   c.launches++;
 }
 
 template <class T, int K, class Epi, class Fin>
-static void launch_spmv_epi(Ctx& c, const Csr<T>& A, const T* x, Epi epi, Fin fin, int ticket) {
+static void launch_spmv_epi(Ctx& c, const Csr<T>& A, const T* x, Epi epi, Fin fin) {
   if (A.n <= 0) return;
   if (c.dex) {                               // row-partitioned operator: exchange the halo of x, gather [local | halo]
     k_halo_exchange<T>(c, x);
-    launch_spmv_epi_g<T, K, Epi, Fin, XGather<T>>(c, A, xgather_of<T>(c, x), epi, fin, ticket);
+    launch_spmv_epi_g<T, K, Epi, Fin, XGather<T>>(c, A, xgather_of<T>(c, x), epi, fin);
   } else {
-    launch_spmv_epi_g<T, K, Epi, Fin, XPlain<T>>(c, A, XPlain<T>{x}, epi, fin, ticket);
+    launch_spmv_epi_g<T, K, Epi, Fin, XPlain<T>>(c, A, XPlain<T>{x}, epi, fin);
   }
 }
 
 template <class T, int K, class Body, class Fin>
-static void launch_stream(Ctx& c, int n, Body body, Fin fin, int ticket) {
+static void launch_stream(Ctx& c, int n, Body body, Fin fin) {
   if (n <= 0) return;
-  stream_epi<T, K, Body, Fin><<<stream_grid(n, 2, 8), kBlock, 0, c.stream>>>(n, body, fin, (T*)c.partials, c.tickets + ticket, c.dcomm);
+  stream_epi<T, K, Body, Fin><<<stream_grid(n, 2, 8), kBlock, 0, c.stream>>>(n, body, fin, (T*)c.partials, c.tickets + 5, c.dcomm);
   KB_CUDA(cudaGetLastError());
   c.launches++;
 }
 
-template <class S> static S* state_buf(void*& dev, void*& host) {
-  if (!dev) {
-    KB_CUDA(cudaMalloc(&dev, kFusedBlockBytes));
-    KB_CUDA(cudaMemset(dev, 0, kFusedBlockBytes));
-    KB_CUDA(cudaHostAlloc(&host, kFusedBlockBytes, cudaHostAllocPortable | cudaHostAllocMapped));
+// Every scalar the host needs from a family's passes is written by their Fin into the family's state struct S<T>,
+// which sits at the start of the workspace's device block (ws.fused_state), next to the values the passes carry from
+// one launch to the next.  The pinned mirror (ws.fused_host) holds two copies of S<T>: slot 0 stages a seed, slot 1
+// receives the read-back.  post() and wait() are apart because some passes are queued behind the copy and must stay
+// queued before the host blocks.
+template <template <class> class S, class T> struct StateBlock {
+  typedef S<T> St;
+  static_assert(2 * sizeof(St) <= kFusedBlockBytes, "the state struct and its two host slots must fit the block");
+  Ctx& c;
+  St* dev;
+  St* host;
+  size_t posted = 0;
+  explicit StateBlock(Workspace<T>& ws) : c(ws.ctx), dev((St*)ws.fused_state), host((St*)ws.fused_host) {}
+  void seed(const St& s) {                  // host slot 0 -> device
+    host[0] = s;
+    KB_CUDA(cudaMemcpyAsync(dev, host, sizeof(St), cudaMemcpyHostToDevice, c.stream));
   }
-  static_assert(sizeof(S) <= 1024, "state block too large");
-  return (S*)dev;
-}
+  void post(size_t bytes = sizeof(St)) {    // device -> host slot 1, queued on the stream
+    KB_CUDA(cudaMemcpyAsync(host + 1, dev, bytes, cudaMemcpyDeviceToHost, c.stream));
+    posted = bytes;
+  }
+  const St& wait() {                        // slot 1 once the stream has drained; every posted word passes the guard
+    c.sync();
+    const T* w = reinterpret_cast<const T*>(host + 1);
+    for (size_t i = 0; i < posted / sizeof(T); i++) dist_nan_guard(c, (double)w[i]);
+    return host[1];
+  }
+  const St& read() { post(); return wait(); }
+};
 
 // ===========================================================================
 // BiCGSTAB  (src/bicgstab.jl:215-256, N = I, M = I or a diagonal applied by multiplication)
@@ -204,25 +222,23 @@ void bicgstab_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const T* cvec, 
                               T* next_rho, T* rNorm) {
   Ctx& c = ws.ctx;
   const int n = ws.n;
-  typedef BicgState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<BicgState, T> sb(ws);
+  BicgState<T>* S = sb.dev;
   if (first) {
-    memset(H, 0, sizeof(St));
-    H->rho = rho_in;
-    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+    BicgState<T> s{};
+    s.rho = rho_in;
+    sb.seed(s);
   }
   const T* m = ws.mdiag_fused;          // left diagonal preconditioner fused into the two SpMV epilogues
   T* t = m ? ws.t : ws.qd;              // t == d == qd when M = I  (bicgstab.jl:153-154)
-  launch_spmv_epi<T, 1>(c, A, ws.p, BicgK1Epi<T>{ws.v, cvec, m}, BicgK1Fin<T>{S}, 4);
-  launch_stream<T, 0>(c, n, BicgK2Body<T>{ws.r, ws.v, ws.s, S}, NoFin(), 5);
-  launch_spmv_epi<T, 2>(c, A, ws.s, BicgK3Epi<T>{t, ws.s, m}, BicgK3Fin<T>{S}, 4);
-  launch_stream<T, 2>(c, n, BicgK4Body<T>{ws.x, ws.p, ws.s, t, cvec, ws.r, S}, BicgK4Fin<T>{S}, 5);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));   // scalars of this iteration
-  launch_stream<T, 0>(c, n, BicgK5Body<T>{ws.p, ws.r, ws.v, S}, NoFin(), 5);
-  c.sync();
-  *alpha = H[1].alpha; *omega = H[1].omega; *next_rho = H[1].next_rho; *rNorm = H[1].rNorm;
-  dist_nan_guard(c, (double)*rNorm);
+  launch_spmv_epi<T, 1>(c, A, ws.p, BicgK1Epi<T>{ws.v, cvec, m}, BicgK1Fin<T>{S});
+  launch_stream<T, 0>(c, n, BicgK2Body<T>{ws.r, ws.v, ws.s, S}, NoFin());
+  launch_spmv_epi<T, 2>(c, A, ws.s, BicgK3Epi<T>{t, ws.s, m}, BicgK3Fin<T>{S});
+  launch_stream<T, 2>(c, n, BicgK4Body<T>{ws.x, ws.p, ws.s, t, cvec, ws.r, S}, BicgK4Fin<T>{S});
+  sb.post();                            // scalars of this iteration
+  launch_stream<T, 0>(c, n, BicgK5Body<T>{ws.p, ws.r, ws.v, S}, NoFin());
+  const BicgState<T>& h = sb.wait();
+  *alpha = h.alpha; *omega = h.omega; *next_rho = h.next_rho; *rNorm = h.rNorm;
 }
 
 // ===========================================================================
@@ -301,21 +317,18 @@ void minres_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, int iter, T lambda,
                           T eps_rot, T* w, T* alpha, T* beta2) {
   Ctx& c = ws.ctx;
   const int n = ws.n;
-  typedef MinresState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<MinresState, T> sb(ws);
+  MinresState<T>* S = sb.dev;
   const T inv_beta = T(1) / beta;
   const T c1 = iter >= 2 ? -beta / oldbeta : T(0);
   const T* m = ws.mdiag_fused;
   T* v = m ? ws.vv : ws.r2;                                 // minres.jl:193
-  launch_spmv_epi<T, 1>(c, A, v, MinresK1Epi<T>{ws.y, v, ws.r1, lambda, inv_beta, c1, iter}, MinresK1Fin<T>{S, beta}, 4);
+  launch_spmv_epi<T, 1>(c, A, v, MinresK1Epi<T>{ws.y, v, ws.r1, lambda, inv_beta, c1, iter}, MinresK1Fin<T>{S, beta});
   launch_stream<T, 1>(c, n, MinresK2Body<T>{ws.y, ws.r2, w, ws.w2, S, beta, inv_beta, cs, sn, deltabar, eps_rot, iter,
                                             m ? ws.vv : nullptr, m},
-                      MinresK2Fin<T>{S}, 5);
-  KB_CUDA(cudaMemcpyAsync(H, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  *alpha = H->alpha; *beta2 = H->beta2;
-  dist_nan_guard(c, (double)*alpha + (double)*beta2);
+                      MinresK2Fin<T>{S});
+  const MinresState<T>& h = sb.read();
+  *alpha = h.alpha; *beta2 = h.beta2;
   T* old_r1 = ws.r1;          // r1 <- r2 ; r2 <- y   (minres.jl:309-310) by rotating the bindings
   ws.r1 = ws.r2; ws.r2 = ws.y; ws.y = old_r1;
 }
@@ -323,15 +336,9 @@ void minres_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, int iter, T lambda,
 // Phase B: w /= gamma ; x += phi w ; returns ||x||.
 template <class T>
 T minres_fused_update(Workspace<T>& ws, T* w, T gamma, T phi) {
-  Ctx& c = ws.ctx;
-  typedef MinresState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
-  launch_stream<T, 1>(c, ws.n, MinresK3Body<T>{w, ws.x, T(1) / gamma, phi}, MinresK3Fin<T>{S}, 5);
-  KB_CUDA(cudaMemcpyAsync(H, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  dist_nan_guard(c, (double)H->xx);
-  return std::sqrt(H->xx);
+  StateBlock<MinresState, T> sb(ws);
+  launch_stream<T, 1>(ws.ctx, ws.n, MinresK3Body<T>{w, ws.x, T(1) / gamma, phi}, MinresK3Fin<T>{sb.dev});
+  return std::sqrt(sb.read().xx);
 }
 
 // ===========================================================================
@@ -367,20 +374,18 @@ template <class T>
 void fused_orth_chain(Workspace<T>& ws, const Csr<T>& A, const T* xin, T* q, const T* const* vecs, int cnt, T* h_out, T* Hbis) {
   Ctx& c = ws.ctx;
   const int n = ws.n;
-  typedef GmresState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<GmresState, T> sb(ws);
+  GmresState<T>* S = sb.dev;
   const T* m = ws.mdiag_fused;
-  launch_spmv_epi<T, 1>(c, A, xin, GmresSpmvEpi<T>{q, vecs[0], m}, GmresHFin<T>{S, 0}, 4);
+  launch_spmv_epi<T, 1>(c, A, xin, GmresSpmvEpi<T>{q, vecs[0], m}, GmresHFin<T>{S, 0});
   for (int i = 0; i < cnt; i++) {
     const T* vnext = (i + 1 < cnt) ? vecs[i + 1] : nullptr;
-    launch_stream<T, 1>(c, n, GmresMgsBody<T>{q, vecs[i], vnext, S, i}, GmresHFin<T>{S, (i + 1 < cnt) ? i + 1 : -1}, 5);
+    launch_stream<T, 1>(c, n, GmresMgsBody<T>{q, vecs[i], vnext, S, i}, GmresHFin<T>{S, (i + 1 < cnt) ? i + 1 : -1});
   }
-  KB_CUDA(cudaMemcpyAsync(H, S, sizeof(T) * (size_t)(cnt + 1), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  for (int i = 0; i < cnt; i++) h_out[i] = H->h[i];
-  *Hbis = std::sqrt(H->hbis2);
-  dist_nan_guard(c, (double)H->hbis2);
+  sb.post(sizeof(T) * (size_t)(cnt + 1));                   // hbis2 and h[0..cnt-1]
+  const GmresState<T>& h = sb.wait();
+  for (int i = 0; i < cnt; i++) h_out[i] = h.h[i];
+  *Hbis = std::sqrt(h.hbis2);
 }
 
 // Arnoldi step k (1-based inner_iter): w = A V[k]; MGS against V[1..k]; returns h[0..k-1] and Hbis.
@@ -407,7 +412,7 @@ void fused_multi_axpy(Workspace<T>& ws, T* xr, int k, const T* y, T* const* vecs
     MultiAxpyBody<T, NV> body;
     body.xr = xr; body.cnt = std::min(NV, k - base);
     for (int i = 0; i < NV; i++) { body.v[i] = vecs[std::min(base + i, k - 1)]; body.y[i] = (base + i < k) ? y[base + i] : T(0); }
-    launch_stream<T, 0>(ws.ctx, ws.n, body, NoFin(), 5);
+    launch_stream<T, 0>(ws.ctx, ws.n, body, NoFin());
   }
 }
 
@@ -423,22 +428,6 @@ void fused_multi_axpy(Workspace<T>& ws, T* xr, int k, const T* y, T* const* vecs
 // Every element update repeats the k* sequence it replaces operation by operation (non-contracted), so vectors are
 // bit-identical to the primitive path given the same scalars.
 // ===========================================================================
-template <class T, int K> struct StoreFin {          // K grid totals -> K consecutive device scalars
-  T* out;
-  __device__ void operator()(const T* tot) const {
-#pragma unroll
-    for (int k = 0; k < K; k++) out[k] = tot[k];
-  }
-};
-template <class T> static T* sib_slots(Ctx& c) { return reinterpret_cast<T*>(reinterpret_cast<double*>(c.dscal) + 8); }
-template <class T, int K> static void sib_read(Ctx& c, T* out) {
-  T* h = reinterpret_cast<T*>(reinterpret_cast<double*>(c.hscal) + 8);
-  KB_CUDA(cudaMemcpyAsync(h, sib_slots<T>(c), sizeof(T) * K, cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  for (int k = 0; k < K; k++) out[k] = h[k];
-  dist_nan_guard(c, (double)out[0]);
-}
-
 // ---- dqgmres! / diom!: direction update (dqgmres.jl:279-289, diom.jl:279-289) in one pass per 8 stack vectors ----
 //   for every live i: P[ppos] = -H_i P[ppos] (same slot) or P[ppos] -= H_i P[ipos];  then P[ppos] += z; P[ppos] /= H_1;
 //   x += step P[ppos]
@@ -470,12 +459,14 @@ void trunc_fused_direction(Workspace<T>& ws, T* pp, int cnt, T* const* pvecs, co
       body.pv[i] = cnt > 0 ? pvecs[k] : pp; body.coef[i] = (cnt > 0 && base + i < cnt) ? coefs[base + i] : T(0);
       body.same[i] = (cnt > 0 && pvecs[k] == pp) ? 1 : 0;
     }
-    launch_stream<T, 0>(ws.ctx, ws.n, body, NoFin(), 5);
+    launch_stream<T, 0>(ws.ctx, ws.n, body, NoFin());
     base += NV;
   } while (base < cnt);
 }
 
 // ---- cgs! (src/cgs.jl:196-239) ----
+template <class T> struct CgsState { T sigma, rho_next, rr; };
+
 template <class T> struct CgsK1Epi {               // t = A p ; sigma = <c, t>
   T* t; const T* cv;
   __device__ __forceinline__ void operator()(int row, T acc, T* d) const { t[row] = acc; d[0] += __ldg(&cv[row]) * acc; }
@@ -499,6 +490,8 @@ template <class T> struct CgsK3Epi {               // s = A u ; r -= alpha s ; <
     d[0] += __ldg(&cv[row]) * rn; d[1] += rn * rn;
   }
 };
+template <class T> struct CgsK1Fin { CgsState<T>* s; __device__ void operator()(const T* tot) const { s->sigma = tot[0]; } };
+template <class T> struct CgsK3Fin { CgsState<T>* s; __device__ void operator()(const T* tot) const { s->rho_next = tot[0]; s->rr = tot[1]; } };
 template <class T> struct CgsK4Body {              // u = r + beta q ; p = u + beta (q + beta p)
   T* u; T* p; const T* r; const T* q; T beta;
   __device__ __forceinline__ void operator()(int j, T*) const {
@@ -509,23 +502,25 @@ template <class T> struct CgsK4Body {              // u = r + beta q ; p = u + b
   }
 };
 template <class T> T cgs_fused_sigma(Workspace<T>& ws, const Csr<T>& A, const T* cvec) {
-  Ctx& c = ws.ctx;
-  launch_spmv_epi<T, 1>(c, A, ws.p, CgsK1Epi<T>{ws.ts, cvec}, StoreFin<T, 1>{sib_slots<T>(c)}, 4);
-  T out[1]; sib_read<T, 1>(c, out);
-  return out[0];
+  StateBlock<CgsState, T> sb(ws);
+  launch_spmv_epi<T, 1>(ws.ctx, A, ws.p, CgsK1Epi<T>{ws.ts, cvec}, CgsK1Fin<T>{sb.dev});
+  return sb.read().sigma;
 }
 template <class T> void cgs_fused_update(Workspace<T>& ws, const Csr<T>& A, const T* cvec, T alpha, T* rho_next, T* rr) {
   Ctx& c = ws.ctx;
-  launch_stream<T, 0>(c, ws.n, CgsK2Body<T>{ws.q, ws.u, ws.ts, ws.x, alpha}, NoFin(), 5);
-  launch_spmv_epi<T, 2>(c, A, ws.u, CgsK3Epi<T>{ws.ts, ws.r, cvec, alpha}, StoreFin<T, 2>{sib_slots<T>(c)}, 4);
-  T out[2]; sib_read<T, 2>(c, out);
-  *rho_next = out[0]; *rr = out[1];
+  StateBlock<CgsState, T> sb(ws);
+  launch_stream<T, 0>(c, ws.n, CgsK2Body<T>{ws.q, ws.u, ws.ts, ws.x, alpha}, NoFin());
+  launch_spmv_epi<T, 2>(c, A, ws.u, CgsK3Epi<T>{ws.ts, ws.r, cvec, alpha}, CgsK3Fin<T>{sb.dev});
+  const CgsState<T>& h = sb.read();
+  *rho_next = h.rho_next; *rr = h.rr;
 }
 template <class T> void cgs_fused_directions(Workspace<T>& ws, T beta) {
-  launch_stream<T, 0>(ws.ctx, ws.n, CgsK4Body<T>{ws.u, ws.p, ws.r, ws.q, beta}, NoFin(), 5);
+  launch_stream<T, 0>(ws.ctx, ws.n, CgsK4Body<T>{ws.u, ws.p, ws.r, ws.q, beta}, NoFin());
 }
 
 // ---- cg_lanczos! (src/cg_lanczos.jl:186-216), M = I so v === Mv ----
+template <class T> struct LanState { T delta, mm; };
+
 template <class T> struct LanK1Epi {               // Mv_next = A v ; delta = <v, Mv_next>
   T* mvn; const T* v;
   __device__ __forceinline__ void operator()(int row, T acc, T* d) const { mvn[row] = acc; d[0] += __ldg(&v[row]) * acc; }
@@ -539,6 +534,8 @@ template <class T> struct LanK2Body {              // Mv_next -= delta Mv (- bet
     d[0] += m * m;
   }
 };
+template <class T> struct LanK1Fin { LanState<T>* s; __device__ void operator()(const T* tot) const { s->delta = tot[0]; } };
+template <class T> struct LanK2Fin { LanState<T>* s; __device__ void operator()(const T* tot) const { s->mm = tot[0]; } };
 template <class T> struct LanK3Body {              // v /= beta ; x += gamma p ; p = sigma v + omega p
   T* v; T* x; T* p; T inv_beta; T gamma; T sigma; T omega;
   __device__ __forceinline__ void operator()(int j, T*) const {
@@ -549,22 +546,22 @@ template <class T> struct LanK3Body {              // v /= beta ; x += gamma p ;
   }
 };
 template <class T> T lanczos_fused_delta(Workspace<T>& ws, const Csr<T>& A) {
-  Ctx& c = ws.ctx;
-  launch_spmv_epi<T, 1>(c, A, ws.Mv, LanK1Epi<T>{ws.Mv_next, ws.Mv}, StoreFin<T, 1>{sib_slots<T>(c)}, 4);
-  T out[1]; sib_read<T, 1>(c, out);
-  return out[0];
+  StateBlock<LanState, T> sb(ws);
+  launch_spmv_epi<T, 1>(ws.ctx, A, ws.Mv, LanK1Epi<T>{ws.Mv_next, ws.Mv}, LanK1Fin<T>{sb.dev});
+  return sb.read().delta;
 }
 template <class T> T lanczos_fused_recur(Workspace<T>& ws, T delta, T beta, bool later) {
-  Ctx& c = ws.ctx;
-  launch_stream<T, 1>(c, ws.n, LanK2Body<T>{ws.Mv_next, ws.Mv, ws.Mv_prev, delta, beta, later ? 1 : 0}, StoreFin<T, 1>{sib_slots<T>(c)}, 5);
-  T out[1]; sib_read<T, 1>(c, out);
-  return std::sqrt(out[0]);
+  StateBlock<LanState, T> sb(ws);
+  launch_stream<T, 1>(ws.ctx, ws.n, LanK2Body<T>{ws.Mv_next, ws.Mv, ws.Mv_prev, delta, beta, later ? 1 : 0}, LanK2Fin<T>{sb.dev});
+  return std::sqrt(sb.read().mm);
 }
 template <class T> void lanczos_fused_update(Workspace<T>& ws, T beta, T gamma, T sigma, T omega) {
-  launch_stream<T, 0>(ws.ctx, ws.n, LanK3Body<T>{ws.Mv, ws.x, ws.p, T(1) / beta, gamma, sigma, omega}, NoFin(), 5);
+  launch_stream<T, 0>(ws.ctx, ws.n, LanK3Body<T>{ws.Mv, ws.x, ws.p, T(1) / beta, gamma, sigma, omega}, NoFin());
 }
 
 // ---- cr! (src/cr.jl:375-445), M = I, no trust region, no linesearch ----
+template <class T> struct CrState { T xx, rr, ArAr, rAr, qq; };
+
 template <class T> struct CrK1Body {               // x += alpha p ; r -= alpha q ; ||x||^2, ||r||^2
   T* x; T* r; const T* p; const T* q; T alpha;
   __device__ __forceinline__ void operator()(int j, T* d) const {
@@ -588,18 +585,21 @@ template <class T> struct CrK3Body {               // p = r + beta p ; q = Ar + 
     d[0] += qn * qn;
   }
 };
+template <class T> struct CrK1Fin { CrState<T>* s; __device__ void operator()(const T* tot) const { s->xx = tot[0]; s->rr = tot[1]; } };
+template <class T> struct CrK2Fin { CrState<T>* s; __device__ void operator()(const T* tot) const { s->ArAr = tot[0]; s->rAr = tot[1]; } };
+template <class T> struct CrK3Fin { CrState<T>* s; __device__ void operator()(const T* tot) const { s->qq = tot[0]; } };
 template <class T> void cr_fused_step(Workspace<T>& ws, const Csr<T>& A, T alpha, T* xx, T* rr, T* ArAr, T* rAr) {
   Ctx& c = ws.ctx;
-  launch_stream<T, 2>(c, ws.n, CrK1Body<T>{ws.x, ws.r, ws.p, ws.q, alpha}, StoreFin<T, 2>{sib_slots<T>(c)}, 5);
-  launch_spmv_epi<T, 2>(c, A, ws.r, CrK2Epi<T>{ws.Ap, ws.r}, StoreFin<T, 2>{sib_slots<T>(c) + 2}, 4);
-  T out[4]; sib_read<T, 4>(c, out);
-  *xx = out[0]; *rr = out[1]; *ArAr = out[2]; *rAr = out[3];
+  StateBlock<CrState, T> sb(ws);
+  launch_stream<T, 2>(c, ws.n, CrK1Body<T>{ws.x, ws.r, ws.p, ws.q, alpha}, CrK1Fin<T>{sb.dev});
+  launch_spmv_epi<T, 2>(c, A, ws.r, CrK2Epi<T>{ws.Ap, ws.r}, CrK2Fin<T>{sb.dev});
+  const CrState<T>& h = sb.read();
+  *xx = h.xx; *rr = h.rr; *ArAr = h.ArAr; *rAr = h.rAr;
 }
 template <class T> T cr_fused_directions(Workspace<T>& ws, T beta) {
-  Ctx& c = ws.ctx;
-  launch_stream<T, 1>(c, ws.n, CrK3Body<T>{ws.p, ws.q, ws.r, ws.Ap, beta}, StoreFin<T, 1>{sib_slots<T>(c)}, 5);
-  T out[1]; sib_read<T, 1>(c, out);
-  return out[0];
+  StateBlock<CrState, T> sb(ws);
+  launch_stream<T, 1>(ws.ctx, ws.n, CrK3Body<T>{ws.p, ws.q, ws.r, ws.Ap, beta}, CrK3Fin<T>{sb.dev});
+  return sb.read().qq;
 }
 
 // ===========================================================================
@@ -608,7 +608,7 @@ template <class T> T cr_fused_directions(Workspace<T>& ws, T beta) {
 // s_u = 1/beta (the scaled gather of P2 and the Mu read of the next P1), which are the two roundings the reference
 // performs.  v === Nv is scaled in place by P3, as kdiv!(v, alpha) does.
 // ===========================================================================
-template <class T> struct LsqState { T alpha, beta, s_u, ww; int beta_zero; };
+template <class T> struct LsqState { T alpha, beta, s_u, ww, xx; };   // alpha, s_u: carried from one pass to the next
 
 template <class T> struct LsqP1Epi {      // Mu = A v - alpha (Mu s_u) ; ||Mu||^2   (kaxpby!(m, one, Av, -alpha, Mu))
   T* mu; const LsqState<T>* s;
@@ -624,7 +624,6 @@ template <class T> struct LsqP1Fin {      // beta = ||Mu|| ; s_u = 1/beta (1 whe
   __device__ void operator()(const T* tot) const {
     const T beta = sqrt_rn(tot[0]);
     s->beta = beta;
-    s->beta_zero = beta == T(0);
     s->s_u = beta == T(0) ? T(1) : div_rn(T(1), beta);
   }
 };
@@ -632,7 +631,7 @@ template <class T, bool WW> struct LsqP2Epi {   // Nv = A^T u - beta Nv ; ||Nv||
   T* nv; const T* w; const LsqState<T>* s;
   __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
     if (WW) { const T wr = w[row]; d[1] += wr * wr; }
-    if (s->beta_zero) return;                     // beta = 0: the reference skips this product (lsqr.jl:303)
+    if (s->beta == T(0)) return;                  // beta = 0: the reference skips this product (lsqr.jl:303)
     const T nn = add_rn(mul_rn(T(1), acc), mul_rn(-s->beta, nv[row]));
     nv[row] = nn;
     d[0] += nn * nn;
@@ -642,7 +641,7 @@ template <class T, int K> struct LsqP2Fin {
   LsqState<T>* s;
   __device__ void operator()(const T* tot) const {
     if (K > 1) s->ww = tot[K - 1];
-    if (!s->beta_zero) s->alpha = sqrt_rn(tot[0]);
+    if (s->beta != T(0)) s->alpha = sqrt_rn(tot[0]);
   }
 };
 template <class T> struct LsqrP3Body {    // v = Nv / alpha ; x += sigma w ; w = v - tau w   (lsqr.jl:315,361-362)
@@ -669,39 +668,37 @@ template <class T> struct LsmrP3Body {    // v = Nv / alpha ; hbar = h - delta h
     d[0] += xn * xn;
   }
 };
+template <class T> struct LsmrP3Fin { LsqState<T>* s; __device__ void operator()(const T* tot) const { s->xx = tot[0]; } };
 
 template <class T>
 void lsq_fused_bidiag(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, bool want_ww, T* beta, T* alpha_out,
                       T* ww) {
   Ctx& c = ws.ctx;
-  typedef LsqState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<LsqState, T> sb(ws);
+  LsqState<T>* S = sb.dev;
   if (init) {                     // Mu holds u_1 already scaled (the initialisation runs on the primitives)
-    memset(H, 0, sizeof(St));
-    H->alpha = alpha; H->s_u = T(1);
-    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+    LsqState<T> s{};
+    s.alpha = alpha; s.s_u = T(1);
+    sb.seed(s);
   }
-  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.Nv}, LsqP1Epi<T>{ws.Mu, S}, LsqP1Fin<T>{S}, 4);
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.Nv}, LsqP1Epi<T>{ws.Mu, S}, LsqP1Fin<T>{S});
   const XScaled<T> ug{ws.Mu, &S->s_u, T(1)};
-  if (want_ww) launch_spmv_epi_g<T, 2>(c, At, ug, LsqP2Epi<T, true>{ws.Nv, ws.w, S}, LsqP2Fin<T, 2>{S}, 4);
-  else launch_spmv_epi_g<T, 1>(c, At, ug, LsqP2Epi<T, false>{ws.Nv, ws.w, S}, LsqP2Fin<T, 1>{S}, 4);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  *beta = H[1].beta; *alpha_out = H[1].alpha; *ww = H[1].ww;
+  if (want_ww) launch_spmv_epi_g<T, 2>(c, At, ug, LsqP2Epi<T, true>{ws.Nv, ws.w, S}, LsqP2Fin<T, 2>{S});
+  else launch_spmv_epi_g<T, 1>(c, At, ug, LsqP2Epi<T, false>{ws.Nv, ws.w, S}, LsqP2Fin<T, 1>{S});
+  const LsqState<T>& h = sb.read();
+  *beta = h.beta; *alpha_out = h.alpha; *ww = h.ww;
 }
 
 template <class T> T lsq_fused_update(Workspace<T>& ws, bool lsmr, bool scale_v, T inv_alpha, T sigma, T tau, T delta) {
   Ctx& c = ws.ctx;
   if (!lsmr) {
-    launch_stream<T, 0>(c, ws.n, LsqrP3Body<T>{ws.Nv, ws.x, ws.w, inv_alpha, sigma, tau, scale_v ? 1 : 0}, NoFin(), 5);
+    launch_stream<T, 0>(c, ws.n, LsqrP3Body<T>{ws.Nv, ws.x, ws.w, inv_alpha, sigma, tau, scale_v ? 1 : 0}, NoFin());
     return T(0);
   }
-  T* out = sib_slots<T>(c);
+  StateBlock<LsqState, T> sb(ws);
   launch_stream<T, 1>(c, ws.n, LsmrP3Body<T>{ws.Nv, ws.x, ws.h, ws.hbar, inv_alpha, sigma, tau, delta, scale_v ? 1 : 0},
-                      StoreFin<T, 1>{out}, 5);
-  T xx[1]; sib_read<T, 1>(c, xx);
-  return std::sqrt(xx[0]);
+                      LsmrP3Fin<T>{sb.dev});
+  return std::sqrt(sb.read().xx);
 }
 
 // LSLQ (src/lslq.jl:302-320,411-416): after LSQR's P1 / P2 (want_ww = false), one pass over n:
@@ -718,7 +715,7 @@ template <class T> struct LslqUpdateBody {
 };
 template <class T> void lslq_fused_update(Workspace<T>& ws, bool scale_v, T inv_alpha, T czeta, T szeta, T c, T s) {
   launch_stream<T, 0>(ws.ctx, ws.n, LslqUpdateBody<T>{ws.Nv, ws.x, ws.w, inv_alpha, czeta, szeta, c, s, scale_v ? 1 : 0},
-                      NoFin(), 5);
+                      NoFin());
 }
 
 // ===========================================================================
@@ -783,21 +780,20 @@ template <class T> struct CglsK4Fin {
 template <class T>
 void cgls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T lambda, T* rr, T* gamma_out) {
   Ctx& c = ws.ctx;
-  typedef CglsState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<CglsState, T> sb(ws);
+  CglsState<T>* S = sb.dev;
   if (init) {                     // p = s, so <p, p> is the gamma the host computed
-    memset(H, 0, sizeof(St));
-    H->gamma = gamma; H->pp = gamma;
-    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+    CglsState<T> s{};
+    s.gamma = gamma; s.pp = gamma;
+    sb.seed(s);
   }
-  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.p}, CglsK1Epi<T>{ws.q}, CglsK1Fin<T>{S, lambda}, 4);
-  launch_stream<T, 1>(c, ws.m, CglsK2Body<T>{ws.r, ws.q, S}, CglsK2Fin<T>{S}, 5);
-  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.r}, CglsK3Epi<T>{ws.x, ws.p, ws.s, S, lambda}, CglsK3Fin<T>{S}, 4);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  launch_stream<T, 1>(c, ws.n, CglsK4Body<T>{ws.p, ws.s, S}, CglsK4Fin<T>{S}, 5);
-  c.sync();
-  *rr = H[1].rr; *gamma_out = H[1].gamma;
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.p}, CglsK1Epi<T>{ws.q}, CglsK1Fin<T>{S, lambda});
+  launch_stream<T, 1>(c, ws.m, CglsK2Body<T>{ws.r, ws.q, S}, CglsK2Fin<T>{S});
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.r}, CglsK3Epi<T>{ws.x, ws.p, ws.s, S, lambda}, CglsK3Fin<T>{S});
+  sb.post();
+  launch_stream<T, 1>(c, ws.n, CglsK4Body<T>{ws.p, ws.s, S}, CglsK4Fin<T>{S});
+  const CglsState<T>& h = sb.wait();
+  *rr = h.rr; *gamma_out = h.gamma;
 }
 
 // ===========================================================================
@@ -865,21 +861,20 @@ template <class T>
 void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, T gamma, T lambda, T* ArAr,
                           T* xx, T* rr, T* gamma_out) {
   Ctx& c = ws.ctx;
-  typedef CrlsState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<CrlsState, T> sb(ws);
+  CrlsState<T>* S = sb.dev;
   if (init) {
-    memset(H, 0, sizeof(St));
-    H->alpha = alpha; H->gamma = gamma;
-    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, c.stream));
+    CrlsState<T> s{};
+    s.alpha = alpha; s.gamma = gamma;
+    sb.seed(s);
   }
-  launch_stream<T, 2>(c, ws.n, CrlsL1Body<T>{ws.x, ws.Ar, ws.p, ws.q, S}, CrlsL1Fin<T>{S}, 5);
-  launch_spmv_epi_g<T, 2>(c, A, XPlain<T>{ws.Ar}, CrlsL2Epi<T>{ws.r, ws.Ap, ws.s, S}, CrlsL2Fin<T>{S, lambda}, 4);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  launch_stream<T, 0>(c, ws.m, CrlsL3Body<T>{ws.Ap, ws.s, S}, NoFin(), 5);
-  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.Ap}, CrlsL4Epi<T>{ws.p, ws.Ar, ws.q, S, lambda}, CrlsL4Fin<T>{S}, 4);
-  c.sync();
-  *ArAr = H[1].ArAr; *xx = H[1].xx; *rr = H[1].rr; *gamma_out = H[1].gamma;
+  launch_stream<T, 2>(c, ws.n, CrlsL1Body<T>{ws.x, ws.Ar, ws.p, ws.q, S}, CrlsL1Fin<T>{S});
+  launch_spmv_epi_g<T, 2>(c, A, XPlain<T>{ws.Ar}, CrlsL2Epi<T>{ws.r, ws.Ap, ws.s, S}, CrlsL2Fin<T>{S, lambda});
+  sb.post();
+  launch_stream<T, 0>(c, ws.m, CrlsL3Body<T>{ws.Ap, ws.s, S}, NoFin());
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.Ap}, CrlsL4Epi<T>{ws.p, ws.Ar, ws.q, S, lambda}, CrlsL4Fin<T>{S});
+  const CrlsState<T>& h = sb.wait();
+  *ArAr = h.ArAr; *xx = h.xx; *rr = h.rr; *gamma_out = h.gamma;
 }
 
 // ===========================================================================
@@ -889,7 +884,7 @@ void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, b
 // the direction / solution update and forms v_{k+1}, u_{k+1} in the buffers of v_{k-1}, u_{k-1} (the caller rotates
 // the pointers).  When <p, q> = 0 the reference keeps v_k and u_k: U then copies them instead of dividing.
 // ===========================================================================
-template <class T> struct BiorthState { T alpha, pq; };
+template <class T> struct BiorthState { T alpha, pq, vv1, v1v1; };   // alpha: B1 -> B2; vv1, v1v1: the update pass
 
 template <class T> struct BiorthB1Epi {   // q = A v - gamma v_{k-1} ; <u, q>          (bilq.jl:236,244,247)
   T* q; const T* vprev; const T* u; T gamma;
@@ -967,44 +962,48 @@ template <class T> struct BiorthBilqBody {
   }
 };
 
+template <class T> struct BiorthQmrFin { BiorthState<T>* s; __device__ void operator()(const T* tot) const { s->v1v1 = tot[0]; } };
+template <class T> struct BiorthBilqFin {
+  BiorthState<T>* s;
+  __device__ void operator()(const T* tot) const { s->vv1 = tot[0]; s->v1v1 = tot[1]; }
+};
+
 template <class T>
 void biorth_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, T beta, T gamma, T* alpha, T* pq) {
   Ctx& c = ws.ctx;
-  typedef BiorthState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
-  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.v}, BiorthB1Epi<T>{ws.q, ws.v_prev, ws.u, gamma}, BiorthB1Fin<T>{S}, 4);
+  StateBlock<BiorthState, T> sb(ws);
+  BiorthState<T>* S = sb.dev;
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.v}, BiorthB1Epi<T>{ws.q, ws.v_prev, ws.u, gamma}, BiorthB1Fin<T>{S});
   launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.u}, BiorthB2Epi<T>{ws.p, ws.q, ws.u_prev, ws.u, ws.v, S, beta},
-                          BiorthB2Fin<T>{S}, 4);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  *alpha = H[1].alpha; *pq = H[1].pq;
+                          BiorthB2Fin<T>{S});
+  const BiorthState<T>& h = sb.read();
+  *alpha = h.alpha; *pq = h.pq;
 }
 
 template <class T>
 T qmr_fused_update(Workspace<T>& ws, T* wk, const T* w1, int iter, T eps2, T lambda, T delta, T zeta, T beta1, T gamma1,
                    bool keep) {
   Ctx& c = ws.ctx;
+  StateBlock<BiorthState, T> sb(ws);
   const BiorthNext<T> nx{ws.v_prev, ws.u_prev, ws.q, ws.p, ws.v, ws.u, beta1, gamma1, keep ? 1 : 0};
   if (iter == 1)
     launch_stream<T, 1>(c, ws.n, BiorthQmrBody<T, true>{wk, w1, ws.x, ws.v, nx, eps2, lambda, T(1) / delta, delta, zeta, iter},
-                        StoreFin<T, 1>{sib_slots<T>(c)}, 5);
+                        BiorthQmrFin<T>{sb.dev});
   else
     launch_stream<T, 1>(c, ws.n, BiorthQmrBody<T, false>{wk, w1, ws.x, ws.v, nx, eps2, lambda, T(1) / delta, delta, zeta, iter},
-                        StoreFin<T, 1>{sib_slots<T>(c)}, 5);
-  T out[1]; sib_read<T, 1>(c, out);
-  return out[0];
+                        BiorthQmrFin<T>{sb.dev});
+  return sb.read().v1v1;
 }
 
 template <class T>
 void bilq_fused_update(Workspace<T>& ws, bool first, T czeta, T szeta, T cs, T sn, T beta1, T gamma1, bool keep, T* vv1,
                        T* v1v1) {
-  Ctx& c = ws.ctx;
+  StateBlock<BiorthState, T> sb(ws);
   const BiorthNext<T> nx{ws.v_prev, ws.u_prev, ws.q, ws.p, ws.v, ws.u, beta1, gamma1, keep ? 1 : 0};
-  launch_stream<T, 2>(c, ws.n, BiorthBilqBody<T>{ws.w, ws.x, ws.v, nx, czeta, szeta, cs, sn, first ? 1 : 0},
-                      StoreFin<T, 2>{sib_slots<T>(c)}, 5);
-  T out[2]; sib_read<T, 2>(c, out);
-  *vv1 = out[0]; *v1v1 = out[1];
+  launch_stream<T, 2>(ws.ctx, ws.n, BiorthBilqBody<T>{ws.w, ws.x, ws.v, nx, czeta, szeta, cs, sn, first ? 1 : 0},
+                      BiorthBilqFin<T>{sb.dev});
+  const BiorthState<T>& h = sb.read();
+  *vv1 = h.vv1; *v1v1 = h.v1v1;
 }
 
 // ===========================================================================
@@ -1013,7 +1012,7 @@ void bilq_fused_update(Workspace<T>& ws, bool first, T czeta, T szeta, T cs, T s
 // leaves rho_next = <t, s> and beta = rho_next / rho in the device block, C3 reads beta and updates the directions,
 // and the host reads {rho_next, <u, u>} once and re-derives beta with the same division.
 // ===========================================================================
-template <class T> struct CarState { T rho_next, beta, uu; };
+template <class T> struct CarState { T rho_next, beta, uu, rr, ss; };   // beta: C2 -> C3
 
 template <class T> struct CarC1Body {     // x += alpha p ; r -= alpha q ; s -= alpha u ; ||r||^2, ||s||^2   (car.jl:189-191)
   T* x; T* r; T* s; const T* p; const T* q; const T* u; T alpha;
@@ -1026,6 +1025,7 @@ template <class T> struct CarC1Body {     // x += alpha p ; r -= alpha q ; s -= 
     d[0] += rn * rn; d[1] += sn * sn;
   }
 };
+template <class T> struct CarC1Fin { CarState<T>* st; __device__ void operator()(const T* tot) const { st->rr = tot[0]; st->ss = tot[1]; } };
 template <class T> struct CarC2Epi {      // t = A s ; <t, s>                       (car.jl:203-204)
   T* t; const T* s;
   __device__ __forceinline__ void operator()(int row, T acc, T* d) const { t[row] = acc; d[0] += acc * __ldg(&s[row]); }
@@ -1051,21 +1051,19 @@ template <class T> struct CarC3Fin {
 };
 
 template <class T> void car_fused_step(Workspace<T>& ws, T alpha, T* rr, T* ss) {
-  Ctx& c = ws.ctx;
-  launch_stream<T, 2>(c, ws.n, CarC1Body<T>{ws.x, ws.r, ws.s, ws.p, ws.q, ws.u, alpha}, StoreFin<T, 2>{sib_slots<T>(c)}, 5);
-  T out[2]; sib_read<T, 2>(c, out);
-  *rr = out[0]; *ss = out[1];
+  StateBlock<CarState, T> sb(ws);
+  launch_stream<T, 2>(ws.ctx, ws.n, CarC1Body<T>{ws.x, ws.r, ws.s, ws.p, ws.q, ws.u, alpha}, CarC1Fin<T>{sb.dev});
+  const CarState<T>& h = sb.read();
+  *rr = h.rr; *ss = h.ss;
 }
 template <class T> void car_fused_directions(Workspace<T>& ws, const Csr<T>& A, T rho, T* rho_next, T* uu) {
   Ctx& c = ws.ctx;
-  typedef CarState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
-  launch_spmv_epi<T, 1>(c, A, ws.s, CarC2Epi<T>{ws.t, ws.s}, CarC2Fin<T>{S, rho}, 4);
-  launch_stream<T, 1>(c, ws.n, CarC3Body<T>{ws.p, ws.q, ws.u, ws.r, ws.s, ws.t, S}, CarC3Fin<T>{S}, 5);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  *rho_next = H[1].rho_next; *uu = H[1].uu;
+  StateBlock<CarState, T> sb(ws);
+  CarState<T>* S = sb.dev;
+  launch_spmv_epi<T, 1>(c, A, ws.s, CarC2Epi<T>{ws.t, ws.s}, CarC2Fin<T>{S, rho});
+  launch_stream<T, 1>(c, ws.n, CarC3Body<T>{ws.p, ws.q, ws.u, ws.r, ws.s, ws.t, S}, CarC3Fin<T>{S});
+  const CarState<T>& h = sb.read();
+  *rho_next = h.rho_next; *uu = h.uu;
 }
 
 // ===========================================================================
@@ -1153,17 +1151,15 @@ void minares_fused_lanczos(Workspace<T>& ws, const Csr<T>& A, bool lanczos, int 
   Ctx& c = ws.ctx;
   const MinaresW<T> w{wk, w1, eps2, gamma1, lam, T(1) / lam, iter};
   if (!lanczos) {
-    launch_stream<T, 0>(c, ws.n, MinaresWBody<T>{w, vk}, NoFin(), 5);
+    launch_stream<T, 0>(c, ws.n, MinaresWBody<T>{w, vk}, NoFin());
     return;
   }
-  typedef MinaresState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
-  launch_spmv_epi<T, 1>(c, A, vk1, MinaresM1Epi<T>{w, vk, vk1, beta1, shift, shift != T(0) ? 1 : 0}, MinaresM1Fin<T>{S}, 4);
-  launch_stream<T, 1>(c, ws.n, MinaresM2Body<T>{vk, vk1, S}, MinaresM2Fin<T>{S}, 5);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  *alpha = H[1].alpha; *vv = H[1].vv;
+  StateBlock<MinaresState, T> sb(ws);
+  MinaresState<T>* S = sb.dev;
+  launch_spmv_epi<T, 1>(c, A, vk1, MinaresM1Epi<T>{w, vk, vk1, beta1, shift, shift != T(0) ? 1 : 0}, MinaresM1Fin<T>{S});
+  launch_stream<T, 1>(c, ws.n, MinaresM2Body<T>{vk, vk1, S}, MinaresM2Fin<T>{S});
+  const MinaresState<T>& h = sb.read();
+  *alpha = h.alpha; *vv = h.vv;
 }
 
 template <class T>
@@ -1172,7 +1168,7 @@ void minares_fused_update(Workspace<T>& ws, int iter, T* vk, bool scale, T beta,
   launch_stream<T, 0>(ws.ctx, ws.n,
                       MinaresM3Body<T>{vk, dk, d1, wk, ws.x, scale ? T(1) / beta : T(1), rho2, phi1, mu, T(1) / mu, zeta,
                                        scale ? 1 : 0, iter},
-                      NoFin(), 5);
+                      NoFin());
 }
 
 // ===========================================================================
@@ -1182,7 +1178,7 @@ void minares_fused_update(Workspace<T>& ws, int iter, T* vk, bool scale, T beta,
 // update pass over max(m, n).  U carries the primal half (x, d̅), the dual half (w_{k-1}, y) and the next v, u; a half
 // that has converged gets an instantiation without its vectors.
 // ===========================================================================
-template <class T> struct AdjointState { T alpha, qq, pp; };
+template <class T> struct AdjointState { T alpha, qq, pp, vq, uu; };   // alpha: T1 -> T2; qq: ||q||^2 of T2 or of U
 
 // Dual direction and solution (bilqr.jl:363-392, trilqr.jl:339-368), iteration >= 2: w_{k-1} = src / delta at iteration
 // 2 (kdivcopy!), else (w_{k-3} + src - lam2 w_{k-2}) / delta with w_{k-3} first scaled by -eps3 from iteration 4 on, in
@@ -1237,6 +1233,10 @@ template <class T, bool PRIMAL, bool DUAL> struct AdjointBilqrBody {
     unext[i] = un;
     if (DUAL) d[2] += un * un;
   }
+};
+template <class T> struct AdjointBilqrFin {
+  AdjointState<T>* s;
+  __device__ void operator()(const T* tot) const { s->vq = tot[0]; s->qq = tot[1]; s->uu = tot[2]; }
 };
 template <class T, bool PRIMAL, bool DUAL> struct AdjointTrilqrBody {
   AdjointD<T> dd; AdjointW<T> w; const T* v; const T* q; const T* p; const T* u; T* vnext; T* unext; T beta1, gamma1;
@@ -1294,30 +1294,30 @@ void bilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T cz
   Ctx& c = ws.ctx;
   const AdjointD<T> dd{ws.w, ws.x, czeta, szeta, cs, sn, iter};
   const AdjointW<T> w{wk, w2, ws.y, eps3, lam2, delta1, T(1) / delta1, psi1, iter};
-  const StoreFin<T, 3> fin{sib_slots<T>(c)};
+  StateBlock<AdjointState, T> sb(ws);
+  const AdjointBilqrFin<T> fin{sb.dev};
   const int k = keep ? 1 : 0;
   if (primal && dual)
-    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, true, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin, 5);
+    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, true, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin);
   else if (primal)
-    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, true, false>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin, 5);
+    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, true, false>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin);
   else
-    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, false, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin, 5);
-  sib_read<T, 3>(c, out3);
+    launch_stream<T, 3>(c, ws.n, AdjointBilqrBody<T, false, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1, k}, fin);
+  const AdjointState<T>& h = sb.read();
+  out3[0] = h.vq; out3[1] = h.qq; out3[2] = h.uu;
 }
 
 template <class T>
 void trilqr_fused_ssy(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool first, T beta, T gamma, T* alpha, T* qq, T* pp) {
   Ctx& c = ws.ctx;
-  typedef AdjointState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  St* H = (St*)ws.fused_host;
+  StateBlock<AdjointState, T> sb(ws);
+  AdjointState<T>* S = sb.dev;
   const int f = first ? 1 : 0;
-  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.u}, AdjointT1Epi<T>{ws.q, ws.v_prev, ws.v, gamma, f}, AdjointT1Fin<T>{S}, 4);
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.u}, AdjointT1Epi<T>{ws.q, ws.v_prev, ws.v, gamma, f}, AdjointT1Fin<T>{S});
   launch_spmv_epi_g<T, 2>(c, At, XPlain<T>{ws.v}, AdjointT2Epi<T>{ws.p, ws.q, ws.u_prev, ws.u, ws.v, S, beta, ws.m, ws.n, f},
-                          AdjointT2Fin<T>{S}, 4);
-  KB_CUDA(cudaMemcpyAsync(H + 1, S, sizeof(St), cudaMemcpyDeviceToHost, c.stream));
-  c.sync();
-  *alpha = H[1].alpha; *qq = H[1].qq; *pp = H[1].pp;
+                          AdjointT2Fin<T>{S});
+  const AdjointState<T>& h = sb.read();
+  *alpha = h.alpha; *qq = h.qq; *pp = h.pp;
 }
 
 template <class T>
@@ -1329,13 +1329,13 @@ void trilqr_fused_update(Workspace<T>& ws, bool primal, bool dual, int iter, T c
   const int len = std::max(ws.m, ws.n);
   if (primal && dual)
     launch_stream<T, 0>(c, len, AdjointTrilqrBody<T, true, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1,
-                                                                 ws.m, ws.n}, NoFin(), 5);
+                                                                 ws.m, ws.n}, NoFin());
   else if (primal)
     launch_stream<T, 0>(c, len, AdjointTrilqrBody<T, true, false>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1,
-                                                                  ws.m, ws.n}, NoFin(), 5);
+                                                                  ws.m, ws.n}, NoFin());
   else
     launch_stream<T, 0>(c, len, AdjointTrilqrBody<T, false, true>{dd, w, ws.v, ws.q, ws.p, ws.u, ws.v_prev, ws.u_prev, beta1, gamma1,
-                                                                  ws.m, ws.n}, NoFin(), 5);
+                                                                  ws.m, ws.n}, NoFin());
 }
 
 // ===========================================================================
@@ -1392,40 +1392,28 @@ template <class T> struct CraigFlushBody {   // x += xi v, v = Nv s_v
   __device__ __forceinline__ void operator()(int i, T*) const { x[i] = add_rn(x[i], mul_rn(xi, mul_rn(nv[i], s_v))); }
 };
 
-template <class T> static CraigState<T>* craig_state(Workspace<T>& ws, bool init) {
-  typedef CraigState<T> St;
-  St* S = state_buf<St>(ws.fused_state, ws.fused_host);
-  if (init) {                     // u_1 and v_0 = 0 are stored scaled: both factors start at 1
-    St* H = (St*)ws.fused_host;
-    memset(H, 0, sizeof(St));
-    H->s_u = T(1); H->s_v = T(1);
-    KB_CUDA(cudaMemcpyAsync(S, H, sizeof(St), cudaMemcpyHostToDevice, ws.ctx.stream));
-  }
-  return S;
-}
-template <class T> static CraigState<T> craig_read(Workspace<T>& ws) {
-  typedef CraigState<T> St;
-  St* H = (St*)ws.fused_host;
-  KB_CUDA(cudaMemcpyAsync(H + 1, ws.fused_state, sizeof(St), cudaMemcpyDeviceToHost, ws.ctx.stream));
-  ws.ctx.sync();
-  return H[1];
-}
-
 template <class T> T craig_fused_p1(Workspace<T>& ws, const Csr<T>& At, bool init, T beta, T s_v, bool xup, T xi) {
-  CraigState<T>* S = craig_state<T>(ws, init);
+  StateBlock<CraigState, T> sb(ws);
+  CraigState<T>* S = sb.dev;
+  if (init) {                     // u_1 and v_0 = 0 are stored scaled: both factors start at 1
+    CraigState<T> s{};
+    s.s_u = T(1); s.s_v = T(1);
+    sb.seed(s);
+  }
   launch_spmv_epi_g<T, 1>(ws.ctx, At, XScaled<T>{ws.Mu, &S->s_u, T(1)}, CraigP1Epi<T>{ws.Nv, ws.x, beta, s_v, xi, xup ? 1 : 0},
-                          CraigNormFin<T>{&S->alpha, &S->s_v}, 4);
-  return craig_read<T>(ws).alpha;
+                          CraigNormFin<T>{&S->alpha, &S->s_v});
+  return sb.read().alpha;
 }
 template <class T> void craig_fused_p2(Workspace<T>& ws, const Csr<T>& A, T s_u, T alpha, T tw, T ty, T* beta, T* ww) {
-  CraigState<T>* S = (CraigState<T>*)ws.fused_state;
+  StateBlock<CraigState, T> sb(ws);
+  CraigState<T>* S = sb.dev;
   launch_spmv_epi_g<T, 2>(ws.ctx, A, XScaled<T>{ws.Nv, &S->s_v, T(1)}, CraigP2Epi<T>{ws.Mu, ws.w, ws.y, s_u, alpha, tw, ty},
-                          CraigP2Fin<T>{S}, 4);
-  const CraigState<T> H = craig_read<T>(ws);
-  *beta = H.beta; *ww = H.ww;
+                          CraigP2Fin<T>{S});
+  const CraigState<T>& h = sb.read();
+  *beta = h.beta; *ww = h.ww;
 }
 template <class T> void craig_fused_flush(Workspace<T>& ws, T xi, T s_v) {
-  launch_stream<T, 0>(ws.ctx, ws.n, CraigFlushBody<T>{ws.x, ws.Nv, xi, s_v}, NoFin(), 5);
+  launch_stream<T, 0>(ws.ctx, ws.n, CraigFlushBody<T>{ws.x, ws.Nv, xi, s_v}, NoFin());
 }
 
 // CRAIGMR R1 on A, gathering v: Mu = A v - alpha u ; ||Mu||^2
@@ -1470,18 +1458,25 @@ template <class T> struct CraigmrP3Body {
 };
 
 template <class T> T craigmr_fused_p1(Workspace<T>& ws, const Csr<T>& A, bool init, T s_u, T alpha) {
-  CraigState<T>* S = craig_state<T>(ws, init);
+  StateBlock<CraigState, T> sb(ws);
+  CraigState<T>* S = sb.dev;
+  if (init) {
+    CraigState<T> s{};
+    s.s_u = T(1); s.s_v = T(1);
+    sb.seed(s);
+  }
   launch_spmv_epi_g<T, 1>(ws.ctx, A, XScaled<T>{ws.Nv, &S->s_v, T(1)}, CraigmrP1Epi<T>{ws.Mu, s_u, alpha},
-                          CraigNormFin<T>{&S->beta, &S->s_u}, 4);
-  return craig_read<T>(ws).beta;
+                          CraigNormFin<T>{&S->beta, &S->s_u});
+  return sb.read().beta;
 }
 template <class T>
 T craigmr_fused_p23(Workspace<T>& ws, const Csr<T>& At, bool first, T s_u, T s_v, T beta, T rho, T inv_rho, T tr, T zeta) {
-  CraigState<T>* S = (CraigState<T>*)ws.fused_state;
+  StateBlock<CraigState, T> sb(ws);
+  CraigState<T>* S = sb.dev;
   launch_spmv_epi_g<T, 1>(ws.ctx, At, XScaled<T>{ws.Mu, &S->s_u, T(1)},
-                          CraigmrP2Epi<T>{ws.Nv, ws.d1, ws.x, s_v, rho, inv_rho, tr, zeta, beta, first ? 1 : 0}, CraigmrP2Fin<T>{S}, 4);
-  launch_stream<T, 0>(ws.ctx, ws.m, CraigmrP3Body<T>{ws.w, ws.y, ws.w1, ws.Mu, S, s_u, inv_rho, tr, zeta}, NoFin(), 5);
-  return craig_read<T>(ws).alpha;
+                          CraigmrP2Epi<T>{ws.Nv, ws.d1, ws.x, s_v, rho, inv_rho, tr, zeta, beta, first ? 1 : 0}, CraigmrP2Fin<T>{S});
+  launch_stream<T, 0>(ws.ctx, ws.m, CraigmrP3Body<T>{ws.w, ws.y, ws.w1, ws.Mu, S, s_u, inv_rho, tr, zeta}, NoFin());
+  return sb.read().alpha;
 }
 
 int gmres_fused_max() { return kGmresMaxFused; }

@@ -5,7 +5,8 @@
 //   blas1.cu      k* primitives on device vectors   (src/krylov_utils.jl:309-349)
 //   spmv.cu       CSR operator: plain and TMA-staged SpMV (kmul!, krylov_utils.jl:305)
 //   cg_fused.cu   two-launch CG iteration               (src/cg.jl:195-268)
-//   fused_phases.cu  fused iteration phases of bicgstab!/minres! and the Arnoldi step of gmres!/fom!/fgmres!
+//   fused_phases.cu  fused iteration phases of every solver family with a fused path except cg!, and their scalar
+//                 read-back (one state struct per family in the workspace's device block)
 //   solvers.cu    host control flow of cg!/bicgstab!/minres! and the one Arnoldi driver of gmres!/fom!/fgmres!
 //   siblings.cu   cgs!, cg_lanczos!, dqgmres!, diom!, cr!, car!, minares! on the same kernels (SURVEY.md 8f-3)
 //   solver_common.h  host helpers of the drivers, among them SolveRun: the callback / clock / exit protocol
@@ -37,7 +38,8 @@ struct Ctx {
   bool own_stream = false;
   void* partials = nullptr;      // kMaxPartials * 4 doubles of reduction scratch
   unsigned* tickets = nullptr;   // 8 tickets (zero-initialised, self re-arming)
-  void* dscal = nullptr;         // 16 device scalars (doubles) written by reductions
+  void* dscal = nullptr;         // 16 device scalars (doubles) written by reductions: slot 0 the dots of blas1.cu,
+                                 // slot 1 the SpMV's, slot 15 k_dist_sum (the fused passes use ws.fused_state)
   void* hscal = nullptr;         // pinned mirror of dscal
   long long launches = 0;        // kernels launched through this context (bench: gpu_launches)
   DistComm* dcomm = nullptr;     // device-resident communicator of a row-partitioned solve (nullptr: single GPU)
@@ -264,8 +266,9 @@ struct Workspace {
   const T* mdiag_fused = nullptr;      // diagonal of M for the fused phases (set per solve; nullptr: M = I)
   double k1_ms = 0, k2_ms = 0;         // average event-timed duration of the fused kernels (time_kernels)
   int timed_pairs = 0;
-  void* fused_state = nullptr;         // device scalar block of the fused paths
-  void* fused_host = nullptr;          // pinned mirror (2 slots)
+  void* fused_state = nullptr;         // device scalar block of the fused paths (4 KB; CG: cg_fused.cu's layout, else
+                                       // one state struct per family at its start, fused_phases.cu)
+  void* fused_host = nullptr;          // pinned mirror: CG's layout, else two copies of the state struct (seed, read-back)
   cudaEvent_t fused_ev[2] = {nullptr, nullptr};   // fused CG: one event per read-back slot
   unsigned long long fused_seq = 0;               // persistent CG: sequence number of the last launch (host-polled report)
   T* bbuf = nullptr;                   // device copies of host b / c for the C ABI
@@ -373,7 +376,9 @@ template <class T> CgFusedPlan<T> cg_fused_plan(const Workspace<T>& ws, const Li
 template <class T> CgFusedExit cg_fused_loop(Workspace<T>& ws, const CgFusedPlan<T>& plan, const SolveOpts& o, T gamma0, T eps_tol,
                                              int itmax, double start_time);
 template <class T> void cg_dist_push_r(Workspace<T>& ws);
-template <class T> void cg_fused_prepare(Workspace<T>& ws);   // device/pinned scalar blocks, p2, events (ws_create)
+template <class T> void cg_fused_prepare(Workspace<T>& ws);   // p2 and the read-back events (ws_create)
+// the 4 KB device block ws.fused_state and its pinned mirror ws.fused_host, zeroed (ws_create, every kind)
+template <class T> void fused_block_alloc(Workspace<T>& ws);
 constexpr size_t kFusedBlockBytes = 4096;
 
 // Fused iteration phases of BiCGSTAB / MINRES / GMRES (fused_phases.cu); eligible when A is a CSR operator,

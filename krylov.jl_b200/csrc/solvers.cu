@@ -24,6 +24,7 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
   try {
     ws->kind = kind; ws->m = m; ws->n = n;
     ws->ctx.init(device);
+    fused_block_alloc<T>(*ws);
     auto A = [&]() { return dev_alloc<T>((size_t)n); };
     ws->x = A();
     switch (kind) {

@@ -10,7 +10,10 @@ Prints the differences and exits 1 when any configuration differs.  The configur
 right-hand-side solvers with the fused paths on and off: diagonal M and N, ldiv, warm starts, restart and growth past
 `memory`, reorthogonalization, b = 0, itmax = 3, a callback exit, timemax = 0, the solver-specific exits and Float32,
 and CG on a constant-coefficient operator (the path of the CsrDict encoding, M = I and a diagonal M, both types), CG's
-two-launch kernels (fused = 2), a block-Jacobi M and the in-kernel phase timing (time_kernels).
+two-launch kernels (fused = 2), a block-Jacobi M and the in-kernel phase timing (time_kernels).  LSQR and LSMR get the
+same treatment; LSLQ, CGLS, CRLS, CRAIG, CRAIGMR, BiLQ, QMR, BiLQR, TriLQR, CAR and MINARES run compactly (defaults,
+Float32, itmax = 3 and a callback exit, fused and not).  For the two-solution solvers y and the dual history are
+compared too.
 """
 import json
 import os
@@ -26,6 +29,9 @@ SQUARE = {"cg": "lap", "cr": "lap", "minres": "lap", "cg_lanczos": "lap", "bicgs
           "gmres": "kron", "fom": "kron", "fgmres": "kron", "dqgmres": "kron", "diom": "kron"}
 TAKES_N = {"bicgstab", "cgs", "gmres", "fom", "fgmres", "dqgmres", "diom"}
 ARNOLDI = {"gmres", "fom", "fgmres"}
+COMPACT = {"lslq": "grad", "cgls": "grad", "crls": "grad", "craig": "div", "craigmr": "div", "bilq": "kron",
+           "qmr": "kron", "bilqr": "kron", "trilqr": "grad", "car": "lap", "minares": "lap"}
+ADJOINT = {"bilqr", "trilqr"}
 CHUNK = 12
 
 
@@ -53,6 +59,7 @@ def problems():
         "dg": (dg, rng.standard_normal(6000)),
         "kron": (kron, kron @ np.ones(216)),
         "grad": (grad, rng.standard_normal(grad.shape[0])),
+        "div": (grad.T, rng.standard_normal(grad.shape[1])),              # underdetermined: the least-norm solvers
         "indef": (indef, indef @ np.arange(1.0, 11.0)),
         "indef12": (indef12, indef12 @ np.arange(1.0, 13.0)),
         "negcurv": (negcurv, negcurv @ np.arange(1.0, 11.0)),
@@ -138,6 +145,12 @@ def configs():
         add(s, p, lambda_=0.1)
         add(s, p, radius=0.5)
         add(s, p, dtype="float32")
+    for s, p in COMPACT.items():
+        c = {"c": "ramp"} if s in ADJOINT else {}
+        add(s, p, **c)
+        add(s, p, dtype="float32", **c)
+        add(s, p, itmax=3, **c)
+        add(s, p, callback=3, **c)
     return out
 
 
@@ -165,8 +178,11 @@ def run_chunk(lo, hi, path):
         for which, ln in (("M", m), ("N", n)):
             if which in kw:
                 kw[which] = vec["pos"](ln) if kw[which] == "pos" else vec[kw[which]]()
-        if kw.pop("c", None):
+        c = kw.pop("c", None)
+        if c == "e1":
             kw["c"] = np.eye(n)[0]
+        elif c == "ramp":                           # the adjoint system's right-hand side: n entries
+            kw["c"] = np.linspace(-1.0, 2.0, n)
         x0 = 0.5 * np.ones(n) if kw.pop("x0", False) else None
         memory = kw.pop("memory", 0)
         stop_at = kw.pop("callback", None)
@@ -184,9 +200,17 @@ def run_chunk(lo, hi, path):
             ws.solve(A, b.astype(dtype), **kw)
             st = ws.stats
             res = dict(x=np.ascontiguousarray(ws.x).tobytes().hex(), niter=st.niter, status=st.status, solved=st.solved,
-                       inconsistent=st.inconsistent, indefinite=st.indefinite, npcCount=st.npcCount, Anorm=hexf(st.Anorm),
-                       residuals=[hexf(v) for v in st.residuals], Aresiduals=[hexf(v) for v in st.Aresiduals],
-                       Acond=[hexf(v) for v in st.Acond], launches=ws.launches)
+                       launches=ws.launches)
+            if cfg["solver"] in ADJOINT:             # AdjointStats
+                res.update(solved_primal=st.solved_primal, solved_dual=st.solved_dual,
+                           residuals=[hexf(v) for v in st.residuals_primal],
+                           residuals_dual=[hexf(v) for v in st.residuals_dual])
+            else:
+                res.update(inconsistent=st.inconsistent, indefinite=st.indefinite, npcCount=st.npcCount,
+                           Anorm=hexf(st.Anorm), residuals=[hexf(v) for v in st.residuals],
+                           Aresiduals=[hexf(v) for v in st.Aresiduals], Acond=[hexf(v) for v in st.Acond])
+            if hasattr(ws, "y"):                     # the two-solution workspaces
+                res["y"] = np.ascontiguousarray(ws.y).tobytes().hex()
         except kb.B200Error as e:
             res = dict(error=str(e))
         finally:

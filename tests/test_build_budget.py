@@ -75,6 +75,14 @@ PHASE_KERNELS = {
                                   "stream_epi": 4}),                 # C1, C3 x 2
                     (r"kb::Minares", {"spmv_epi_tma": 4,             # M1 on a plain or gathered x, x Float32 / Float64
                                       "stream_epi": 6})],            # M2, M3 and the w-only pass x 2
+    # the BiLQR and TriLQR update passes: both halves, primal only, dual only, x Float32 / Float64
+    "adjoint_update": [(r"kb::AdjointBilqrBody", {"stream_epi": 6}),
+                       (r"kb::AdjointTrilqrBody", {"stream_epi": 6})],
+    "adjoint_ssy": [(r"kb::AdjointT[12]", {"spmv_epi_tma": 4,        # TriLQR's T1, T2 x Float32 / Float64
+                                           "spmv_epi_rows": 4})],
+    "leastnorm": [(r"kb::Craig", {"spmv_epi_tma": 8,                 # CRAIG C1, C2 and CRAIGMR R1, R2 x 2
+                                  "spmv_epi_rows": 8,
+                                  "stream_epi": 4})],                # CRAIG's x flush and CRAIGMR's R3 x 2
 }
 
 
