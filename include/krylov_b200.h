@@ -49,7 +49,7 @@ typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
  * adjoint pairs A x = b, A^T y = c of BILQR (square A) and TRILQR (A m x n: b and y have m entries, c and x have n),
  * which require c, take no preconditioner and return y through krylov_get_y, and the least-squares solvers LSQR, LSMR,
  * LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a
- * CSR operator of m rows and n columns is attached), and the least-norm solvers CRAIG and CRAIGMR on the same m x n
+ * CSR operator of m rows and n columns is attached), and the least-norm solvers CRAIG, CRAIGMR and LNLQ on the same m x n
  * operators (min ||x|| subject to A x = b; x = A^T y, and y, m entries, is returned through krylov_get_y; `c` is
  * ignored); every other value returns -2. */
 typedef enum {
@@ -102,7 +102,7 @@ void krylov_get_version(int *major, int *minor, int *patch);
 int krylov_solve(void *ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, KrylovMatvec matvec_M, KrylovMatvec matvec_N,
                  const void *b, const void *c, void *userdata, const KrylovOptions *opts);
 int krylov_get_x(void *ws, void *x, int n);
-int krylov_get_y(void *ws, void *y, int m); /* BILQR, TRILQR, CRAIG, CRAIGMR: y (m entries); -2: single-solution solver */
+int krylov_get_y(void *ws, void *y, int m); /* BILQR, TRILQR, CRAIG, CRAIGMR, LNLQ: y (m entries); -2: single-solution solver */
 int krylov_is_solved(void *ws);             /* 1 | 0 | -1 */
 int krylov_niter(void *ws);
 double krylov_elapsed_time(void *ws);
@@ -142,7 +142,7 @@ const char *krylov_b200_last_error(void);
 /* Attach a CSR matrix as the operator A of `ws`: replaces mul!(y, A, x) at
  * cg.jl:196, gmres.jl:257, bicgstab.jl:221,228, minres.jl:289.
  *   rowptr[n+1], colind[nnz], values[nnz] (element type = workspace dtype);
- *   least-squares and least-norm (CRAIG, CRAIGMR) workspaces: n is the number of rows (the workspace's m) and the
+ *   least-squares and least-norm (CRAIG, CRAIGMR, LNLQ) workspaces: n is the number of rows (the workspace's m) and the
  *   columns are the workspace's n;
  *   TriLQR workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
  *   least-squares, least-norm, BiLQ, QMR, BiLQR and TriLQR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
@@ -159,7 +159,7 @@ int krylov_b200_share_operator(void *ws, void *src);
 int krylov_b200_attach_csr(void *ws, void *csr);
 /* Diagonal preconditioner: which = 0 -> M, 1 -> N; d[n] holds the diagonal of
  * the operator the solver applies (P^-1 with the default ldiv=false). NULL detaches.
- * LSQR / LSMR / LSLQ / CRAIG / CRAIGMR: M acts on the data space (d[m]), N on the solution space (d[n]).  CGLS / CRLS: M acts on the
+ * LSQR / LSMR / LSLQ / CRAIG / CRAIGMR / LNLQ: M acts on the data space (d[m]), N on the solution space (d[n]).  CGLS / CRLS: M acts on the
  * residual space (d[m]); they take no N (a solve with N attached or matvec_N given is refused). */
 int krylov_b200_set_preconditioner_diag(void *ws, int which, const void *d, int location);
 /* Block-Jacobi preconditioner (docs/src/preconditioners.md:33,159): which = 0 -> M, 1 -> N; blocks[ceil(n/bs)][bs][bs]
@@ -178,7 +178,7 @@ int krylov_b200_set_preconditioner_blockdiag(void *ws, int which, int bs, const 
 typedef struct {
   int history;        /* 1: record residual history (kwarg `history`)              */
   int ldiv;           /* 1: preconditioners are applied with ldiv! (kwarg `ldiv`)   */
-  double etol;        /* MINRES; NaN -> sqrt(eps)                                   */
+  double etol;        /* MINRES; LNLQ: kwarg `utoly`; NaN -> sqrt(eps)                 */
   double conlim;      /* MINRES; NaN -> 1/sqrt(eps)                                 */
   int fused;          /* 1 (default): fused kernels when eligible (CG: one persistent cooperative launch per
                        * batch of iterations); 2: fused CG as two launches per iteration; 0: primitives */
@@ -191,11 +191,12 @@ typedef struct {
   double axtol;        /* LSQR, LSMR: kwarg `axtol` (src/lsqr.jl:152); MINARES: kwarg `Artol`, the relative
                           tolerance on ||A r|| (src/minares.jl:99); NaN -> sqrt(eps)                                  */
   double btol;         /* LSQR, LSMR, LSLQ, CRAIG: kwarg `btol`; NaN -> sqrt(eps)                                 */
-  double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0                       */
-  double utol;         /* LSLQ: kwarg `utol`; NaN -> sqrt(eps)                                                       */
+  double sigma;        /* LSLQ: kwarg `σ` (src/lslq.jl:178), Gauss-Radau error bounds when > 0; LNLQ: kwarg `σ`      */
+  double utol;         /* LSLQ: kwarg `utol`; LNLQ: kwarg `utolx`; NaN -> sqrt(eps)                                  */
   int transfer_to_lsqr; /* LSLQ, CRAIG (acts when lambda > 0): 1 -> return the LSQR point (kwarg `transfer_to_lsqr`)  */
   int transfer_to_bicg; /* BiLQ, BiLQR: 1 (default) -> return the BiCG point when it converges first (kwarg `transfer_to_bicg`);
-                          TriLQR: its kwarg `transfer_to_usymcg` (the USYMCG point), in the same field                  */
+                          TriLQR: its kwarg `transfer_to_usymcg` (the USYMCG point), in the same field.
+                          LNLQ: its kwarg `transfer_to_craig` (the CRAIG point), default 1 as the reference's `true`   */
 } KrylovB200Options;
 KrylovB200Options krylov_b200_default_options(void);
 int krylov_b200_set_options(void *ws, const KrylovB200Options *opts);
@@ -214,8 +215,9 @@ typedef struct {
   double timer;
   char status[96];
   double Anorm;       /* LanczosStats.Anorm (cg_lanczos!); NaN for the other solvers */
-  int error_with_bnd;  /* LSLQStats (src/krylov_stats.jl:352-365): the error bounds became complex              */
-  int nerr_lbnds;      /* LSLQ history lengths (krylov_b200_get_history which = 3, 4, 5)                        */
+  int error_with_bnd;  /* LSLQStats (src/krylov_stats.jl:352-365), LNLQStats: the error bounds became complex */
+  int nerr_lbnds;      /* LSLQ history lengths (krylov_b200_get_history which = 3, 4, 5); LNLQ: error_bnd_x and
+                          error_bnd_y in nerr_lbnds / nerr_ubnds_lq (which = 3, 4)                              */
   int nerr_ubnds_lq;
   int nerr_ubnds_cg;
   int solved_primal;   /* AdjointStats (src/krylov_stats.jl:263-280) of BiLQR / TriLQR; `solved` = solved_primal && solved_dual */
@@ -223,12 +225,13 @@ typedef struct {
   int nresiduals_dual; /* length of residuals_dual (krylov_b200_get_history which = 6); residuals_primal is which = 0 */
 } KrylovB200Stats;
 int krylov_b200_get_stats(void *ws, KrylovB200Stats *out);
-/* which: 0 residuals, 1 Aresiduals, 2 Acond; LSLQ: 3 err_lbnds, 4 err_ubnds_lq, 5 err_ubnds_cg; BiLQR / TriLQR:
+/* which: 0 residuals, 1 Aresiduals, 2 Acond; LSLQ: 3 err_lbnds, 4 err_ubnds_lq, 5 err_ubnds_cg; LNLQ: 3 error_bnd_x,
+ * 4 error_bnd_y; BiLQR / TriLQR:
  * 0 residuals_primal, 6 residuals_dual.
  * Returns the number copied (<= cap) or -1. */
 int krylov_b200_get_history(void *ws, int which, double *out, int cap);
 /* Device pointer of a workspace vector by its reference field name
- * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"; CRAIG / CRAIGMR: "y", "Nv",
+ * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"; LNLQ: "x", "Nv", "Aᴴu", "y", "w̄", "Mu", "Av", "u", "v", "q"; CRAIG / CRAIGMR: "y", "Nv",
  * "Mu", "Av", "Aᴴu", "u", "v", "w", CRAIG "w2", CRAIGMR "d", "w̄" and "q"; BiLQR / TriLQR: "y", "d̅",
  * "wₖ₋₃", "wₖ₋₂", "uₖ₋₁", "uₖ", "vₖ₋₁", "vₖ", "q", "p", "Δx", "Δy"). */
 int krylov_b200_get_vector(void *ws, const char *name, void **dev_ptr);

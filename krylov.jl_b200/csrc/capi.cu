@@ -80,7 +80,7 @@ bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
          s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
          s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR || s == S_CAR || s == S_MINARES ||
-         s == S_BILQR || s == S_TRILQR || s == S_CRAIG || s == S_CRAIGMR;
+         s == S_BILQR || s == S_TRILQR || s == S_CRAIG || s == S_CRAIGMR || s == S_LNLQ;
 }
 
 int pick_device() {
@@ -252,6 +252,7 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
                              : h->solver == S_LSLQ ? "lslq applies the adjoint of A: matvec_At must be given with matvec_A"
                              : h->solver == S_CRAIG ? "craig applies the adjoint of A: matvec_At must be given with matvec_A"
                              : h->solver == S_CRAIGMR ? "craigmr applies the adjoint of A: matvec_At must be given with matvec_A"
+                             : h->solver == S_LNLQ ? "lnlq applies the adjoint of A: matvec_At must be given with matvec_A"
                                                    : "lsqr and lsmr apply the adjoint of A: matvec_At must be given with matvec_A");
     A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
     At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
@@ -283,6 +284,7 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
     case S_CRLS: crls_solve<T>(*ws, A, At, bd, M, so); break;
     case S_CRAIG: craig_solve<T>(*ws, A, At, bd, M, N, so); break;
     case S_CRAIGMR: craigmr_solve<T>(*ws, A, At, bd, M, N, so); break;
+    case S_LNLQ: lnlq_solve<T>(*ws, A, At, bd, M, N, so); break;
   }
   return 0;
 }
@@ -457,6 +459,7 @@ template <class T> int do_warm_start(Handle* h, const void* x0, int n) {
                              : h->solver == S_LSLQ ? "lslq does not support warm-start (it takes no x0)"
                              : h->solver == S_CRAIG ? "craig does not support warm-start (it takes no x0)"
                              : h->solver == S_CRAIGMR ? "craigmr does not support warm-start (it takes no x0)"
+                             : h->solver == S_LNLQ ? "lnlq does not support warm-start (it takes no x0)"
                                                  : "lsqr and lsmr do not support warm-start (they take no x0)");
   if (n != ws->n) throw std::runtime_error("x0 should have size n");
   KB_CUDA(cudaSetDevice(ws->ctx.device));
@@ -487,7 +490,7 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
   if (!strcmp(nm, "Ar")) return ws->Ar ? ws->Ar : ws->Ap;   // CRLS has its own Ar; CR's Ar is Ap
   if (!strcmp(nm, "Mr") || !strcmp(nm, "Ms")) return ws->Mr;
   if (!strcmp(nm, "Mq")) return ws->kind == S_CGLS ? ws->Mr : ws->z;   // CGLS: Mq aliases Mr (cgls.jl:156)
-  if (!strcmp(nm, "w̄") || !strcmp(nm, "wbar")) return ws->kind == S_LSLQ ? ws->w : ws->kind == S_CRAIGMR ? ws->w1 : nullptr;
+  if (!strcmp(nm, "w̄") || !strcmp(nm, "wbar")) return ws->kind == S_LSLQ || ws->kind == S_LNLQ ? ws->w : ws->kind == S_CRAIGMR ? ws->w1 : nullptr;
   if (ws->kind == S_CRAIGMR && !strcmp(nm, "d")) return ws->d1;   // CraigmrWorkspace
   if (!strcmp(nm, "Aᴴu")) return ws->Atu;
   if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ || is_adjoint_kind(ws->kind) ? ws->w : nullptr;
@@ -585,7 +588,7 @@ int krylov_get_y(void* ws, void* y, int m) {
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_get_y", "unknown workspace handle");
-    // solution_count (c_stores.jl:211-216) is 2 for BiLQR, TriLQR, CRAIG and CRAIGMR only
+    // solution_count (c_stores.jl:211-216) is 2 for BiLQR, TriLQR, CRAIG, CRAIGMR and LNLQ only
     if (!is_adjoint(h) && !is_leastnorm_kind(h->solver)) return -2;
     if (!y) return fail("krylov_get_y", "y is NULL");
     return h->dtype == KRYLOV_FLOAT64 ? do_get_y<double>(h, y, m) : do_get_y<float>(h, y, m);
@@ -857,7 +860,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
     h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0;
     if (!blocks) return 0;
-    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on least-squares (LSQR, LSMR, CGLS, CRLS) or least-norm (CRAIG, CRAIGMR) workspaces");
+    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on least-squares (LSQR, LSMR, CGLS, CRLS) or least-norm (CRAIG, CRAIGMR, LNLQ) workspaces");
     if (bs < 2 || bs > 8) return fail("krylov_b200_set_preconditioner_blockdiag", "block size must be in 2..8");
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
     const int n = n_of(h);
@@ -1084,7 +1087,7 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_b200_dist_init", "unknown workspace handle");
-    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) and least-norm (CRAIG, CRAIGMR) solves are not available");
+    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) and least-norm (CRAIG, CRAIGMR, LNLQ) solves are not available");
     if (is_biorth(h->solver))        // A^T of a row block needs the column halo of A, not its row halo
       return fail("krylov_b200_dist_init", "row-partitioned BiLQ / QMR solves are not available");
     if (h->solver == S_CAR || h->solver == S_MINARES)

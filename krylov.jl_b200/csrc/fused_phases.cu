@@ -1479,6 +1479,86 @@ T craigmr_fused_p23(Workspace<T>& ws, const Csr<T>& At, bool first, T s_u, T s_v
   return sb.read().alpha;
 }
 
+// ===========================================================================
+// LNLQ  (src/lnlq.jl:326-552; lambda = 0, M = N = I)
+// The products run in LSQR's order, A v then A^T u, with kdiv!(u, beta) and kdiv!(v, alpha) pending as in CRAIG.  The
+// y / w̄ update of a pass needs u_{k+1}, so it rides in the next L1, which reads u before overwriting Mu.
+// ===========================================================================
+template <class T> struct LnlqState { T s_u, s_v, alpha, beta; };
+
+template <class T> struct LnlqNormFin {      // tot[0] = ||z||^2 -> s = ||z|| ; inverse = 1/s (1 when s = 0)
+  T* out; T* inv;
+  __device__ void operator()(const T* tot) const {
+    const T s = sqrt_rn(tot[0]);
+    *out = s;
+    *inv = s == T(0) ? T(1) : div_rn(T(1), s);
+  }
+};
+// y += yc w̄ ; y += ys u ; w̄ = wc u + ws w̄   (kaxpy!, kaxpy!, kaxpby!: lnlq.jl:449-453)
+template <class T> __device__ __forceinline__ void lnlq_y_update(T* y, T* wbar, int i, T u, T yc, T ys, T wc, T ws) {
+  const T wb = wbar[i];
+  y[i] = add_rn(add_rn(y[i], mul_rn(yc, wb)), mul_rn(ys, u));
+  wbar[i] = add_rn(mul_rn(wc, u), mul_rn(ws, wb));
+}
+// L1 on A, gathering v: the previous pass's y / w̄ update (pending when yup), then Mu = A v - alpha u ; ||Mu||^2
+template <class T> struct LnlqL1Epi {
+  T* mu; T* y; T* wbar; T s_u, alpha, yc, ys, wc, ws; int yup;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T u = mul_rn(mu[row], s_u);
+    if (yup) lnlq_y_update(y, wbar, row, u, yc, ys, wc, ws);
+    const T nm = add_rn(mul_rn(T(1), acc), mul_rn(-alpha, u));
+    mu[row] = nm;
+    d[0] += nm * nm;
+  }
+};
+// L2 on A^T, gathering u: x += tau v ; Nv = A^T u - beta v ; ||Nv||^2
+template <class T> struct LnlqL2Epi {
+  T* nv; T* x; T s_v, beta, tau;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T v = mul_rn(nv[row], s_v);
+    x[row] = add_rn(x[row], mul_rn(tau, v));
+    const T nn = add_rn(mul_rn(T(1), acc), mul_rn(-beta, v));
+    nv[row] = nn;
+    d[0] += nn * nn;
+  }
+};
+template <class T> struct LnlqFlushBody {    // the pending y / w̄ update over m, u = Mu s_u
+  T* y; T* wbar; const T* mu; T s_u, yc, ys, wc, ws;
+  __device__ __forceinline__ void operator()(int i, T*) const { lnlq_y_update(y, wbar, i, mul_rn(mu[i], s_u), yc, ys, wc, ws); }
+};
+template <class T> struct LnlqXBody {        // x += a v, v = Nv s_v
+  T* x; const T* nv; T a, s_v;
+  __device__ __forceinline__ void operator()(int i, T*) const { x[i] = add_rn(x[i], mul_rn(a, mul_rn(nv[i], s_v))); }
+};
+
+template <class T>
+T lnlq_fused_l1(Workspace<T>& ws, const Csr<T>& A, bool init, T s_u, T alpha, bool yup, T yc, T ys, T wc, T wsn) {
+  StateBlock<LnlqState, T> sb(ws);
+  LnlqState<T>* S = sb.dev;
+  if (init) {                     // u_1 and v_1 are stored scaled: both factors start at 1
+    LnlqState<T> s{};
+    s.s_u = T(1); s.s_v = T(1);
+    sb.seed(s);
+  }
+  launch_spmv_epi_g<T, 1>(ws.ctx, A, XScaled<T>{ws.Nv, &S->s_v, T(1)},
+                          LnlqL1Epi<T>{ws.Mu, ws.y, ws.w, s_u, alpha, yc, ys, wc, wsn, yup ? 1 : 0},
+                          LnlqNormFin<T>{&S->beta, &S->s_u});
+  return sb.read().beta;
+}
+template <class T> T lnlq_fused_l2(Workspace<T>& ws, const Csr<T>& At, T s_v, T beta, T tau) {
+  StateBlock<LnlqState, T> sb(ws);
+  LnlqState<T>* S = sb.dev;
+  launch_spmv_epi_g<T, 1>(ws.ctx, At, XScaled<T>{ws.Mu, &S->s_u, T(1)}, LnlqL2Epi<T>{ws.Nv, ws.x, s_v, beta, tau},
+                          LnlqNormFin<T>{&S->alpha, &S->s_v});
+  return sb.read().alpha;
+}
+template <class T> void lnlq_fused_flush(Workspace<T>& ws, T s_u, T yc, T ys, T wc, T wsn) {
+  launch_stream<T, 0>(ws.ctx, ws.m, LnlqFlushBody<T>{ws.y, ws.w, ws.Mu, s_u, yc, ys, wc, wsn}, NoFin());
+}
+template <class T> void lnlq_fused_xup(Workspace<T>& ws, T a, T s_v) {
+  launch_stream<T, 0>(ws.ctx, ws.n, LnlqXBody<T>{ws.x, ws.Nv, a, s_v}, NoFin());
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1517,7 +1597,11 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void craig_fused_p2<T>(Workspace<T>&, const Csr<T>&, T, T, T, T, T*, T*);                              \
   template void craig_fused_flush<T>(Workspace<T>&, T, T);                                                         \
   template T craigmr_fused_p1<T>(Workspace<T>&, const Csr<T>&, bool, T, T);                                         \
-  template T craigmr_fused_p23<T>(Workspace<T>&, const Csr<T>&, bool, T, T, T, T, T, T, T);
+  template T craigmr_fused_p23<T>(Workspace<T>&, const Csr<T>&, bool, T, T, T, T, T, T, T);                        \
+  template T lnlq_fused_l1<T>(Workspace<T>&, const Csr<T>&, bool, T, T, bool, T, T, T, T);                          \
+  template T lnlq_fused_l2<T>(Workspace<T>&, const Csr<T>&, T, T, T);                                               \
+  template void lnlq_fused_flush<T>(Workspace<T>&, T, T, T, T, T);                                                  \
+  template void lnlq_fused_xup<T>(Workspace<T>&, T, T);
 INST(double)
 INST(float)
 #undef INST

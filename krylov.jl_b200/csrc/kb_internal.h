@@ -13,7 +13,7 @@
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
 //   biorth.cu     host control flow of bilq!/qmr! (one Lanczos biorthogonalization driver; A and A^T)
 //   adjoint.cu    host control flow of bilqr!/trilqr! (adjoint system pairs A x = b, A^T y = c; two solutions)
-//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! and of the least-norm craig!/craigmr! on rectangular
+//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! and of the least-norm craig!/craigmr!/lnlq! on rectangular
 //                 operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
@@ -217,13 +217,14 @@ struct Stats {
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
                   S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_TRILQR = 18, S_BILQR = 19, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
-                  S_CRAIG = 28, S_CRAIGMR = 29, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
+                  S_CRAIG = 28, S_CRAIGMR = 29, S_LNLQ = 30, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
 // the least-squares and least-norm solvers: A is m x n, b has m entries and x has n
 inline bool is_ls_kind(int k) {
-  return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS || k == S_CRAIG || k == S_CRAIGMR;
+  return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS || k == S_CRAIG || k == S_CRAIGMR ||
+         k == S_LNLQ;
 }
 // the least-norm solvers: min ||x|| subject to A x = b, with x = A^T y; they return the multipliers y (m entries) too
-inline bool is_leastnorm_kind(int k) { return k == S_CRAIG || k == S_CRAIGMR; }
+inline bool is_leastnorm_kind(int k) { return k == S_CRAIG || k == S_CRAIGMR || k == S_LNLQ; }
 // the adjoint-pair solvers: two solutions, x (A x = b) and y (A^T y = c).  TriLQR: A is m x n, b and y have m entries,
 // c and x have n; BiLQR: square
 inline bool is_adjoint_kind(int k) { return k == S_BILQR || k == S_TRILQR; }
@@ -255,6 +256,7 @@ struct Workspace {
                                        // CAR: r, p, s, q, t, u (+ Mu, lazy)
                                        // CRAIG: x, Nv, Atu (n), y, w, Mu, Av (m) (+ u, v, w2: lazy)
                                        // CRAIGMR: d in d1, w̄ in w1 (+ x, Nv, Atu, y, w, Mu, Av; u, v, q: lazy)
+                                       // LNLQ: w̄ in w (+ x, Nv, y, Mu; Atu, Av, u, v, q: lazy)
   T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
                                        // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
   std::vector<T*> V;
@@ -335,6 +337,8 @@ template <class T> void craig_solve(Workspace<T>& ws, const LinOp<T>& A, const L
                                     const LinOp<T>& N, const SolveOpts& o);
 template <class T> void craigmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                       const LinOp<T>& N, const SolveOpts& o);
+template <class T> void lnlq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
+                                   const LinOp<T>& N, const SolveOpts& o);
 // CGLS / CRLS: M (m x m) acts on the residual space; they take no N.
 template <class T> void cgls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const SolveOpts& o);
@@ -441,6 +445,16 @@ template <class T> T craigmr_fused_p1(Workspace<T>& ws, const Csr<T>& A, bool in
 // w = (1/rho) w̄ + tr w, y += zeta w and, when alpha != 0, w̄ = (1/alpha) u - (beta/alpha) w̄.  Returns alpha.
 template <class T> T craigmr_fused_p23(Workspace<T>& ws, const Csr<T>& At, bool first, T s_u, T s_v, T beta, T rho, T inv_rho,
                                        T tr, T zeta);
+// LNLQ (fused_phases.cu), same conditions and the same pending factors.  L1: SpMV on A gathering v; first the previous
+// pass's update (when yup: y += yc w̄, y += ys u, w̄ = wc u + ws w̄ with u = Mu s_u), then Mu = A v - alpha u; returns
+// beta.  `init`: first pass (u_1 and v_1 stored scaled).
+template <class T>
+T lnlq_fused_l1(Workspace<T>& ws, const Csr<T>& A, bool init, T s_u, T alpha, bool yup, T yc, T ys, T wc, T wsn);
+// L2: SpMV on A^T gathering u, x += tau v (v = Nv s_v), Nv = A^T u - beta v; returns alpha.
+template <class T> T lnlq_fused_l2(Workspace<T>& ws, const Csr<T>& At, T s_v, T beta, T tau);
+// the pending y / w̄ update over m (before a callback and after the last pass), and the terminal x += a v
+template <class T> void lnlq_fused_flush(Workspace<T>& ws, T s_u, T yc, T ys, T wc, T wsn);
+template <class T> void lnlq_fused_xup(Workspace<T>& ws, T a, T s_v);
 // One CGLS iteration, M = I, no trust region, 4 launches: K1 q = A p (alpha on the device), K2 r -= alpha q, K3 s = A^T r
 // with x += alpha p and s -= lambda x, K4 p = s + beta p.  One read-back: <r, r> and gamma = <s, s>.
 // `init`: first iteration, sets gamma (and <p, p> = gamma) on the device from the host.

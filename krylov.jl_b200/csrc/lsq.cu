@@ -1264,7 +1264,290 @@ void craigmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, cons
   run.finish(iter, solved, inconsistent, st);
 }
 
+// ===========================================================================
+// lnlq!  (src/lnlq.jl:168-568): SYMMLQ on A Aᴴ y = b, x = Aᴴ y.  `iter` is incremented once before the loop and once
+// at the end of each pass, so niter = passes + 1.  σ-based upper bounds on ‖x - x*‖ (stats.err_lbnds) and ‖y - y*‖
+// (stats.err_ubnds_lq) when √(σ² + λ²) > 0.  Fused (λ = 0, M = N = I, CSR A and Aᴴ): L1 on A, read β, then L2 on Aᴴ,
+// read α; the y / w̄ update of a pass rides in the next L1 and is flushed before a callback and after the last pass.
+// ===========================================================================
+template <class T>
+void lnlq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M, const LinOp<T>& N,
+                const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv, transfer_to_craig = o.transfer_to_bicg;
+  if (o.verbose > 0) printf("LNLQ: system of %d equations in %d variables\n", m, n);
+  const T lambda = (T)o.lambda, sigma = (T)o.sigma;
+  const T utolx = tol_of<T>(o.utol), utoly = tol_of<T>(o.etol), atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  const T eps = eps_of<T>();
+  Stats& stats = ws.stats;
+  std::vector<double>& xNorms = stats.err_lbnds;                // error_bnd_x
+  std::vector<double>& yNorms = stats.err_ubnds_lq;             // error_bnd_y
+
+  T beta;
+  Setup s = lsq_prologue<T>(ws, A, At, b, M, N, o, &beta);      // x = 0, Mu = b, u = M⁻¹Mu, β₁ = ‖u‖_M
+  s.fused = s.fused && lambda == 0;                             // the fused passes carry no regularization
+  allocate_if(!s.fused, ws, ws.Av, m);
+  allocate_if(!s.fused, ws, ws.Atu);
+  allocate_if(lambda > 0, ws, ws.q);
+  T* u = s.MisI ? ws.Mu : ws.u;
+  T* v = s.NisI ? ws.Nv : ws.v;
+  T* wbar = ws.w;
+  const T sigma_est = std::sqrt(sigma * sigma + lambda * lambda);
+  bool complex_error_bnd = false;
+  k_fill<T>(c, m, ws.y, T(0));
+
+  const T bNorm = s.MisI ? beta : (m > 0 ? k_nrm2<T>(c, m, b) : T(0));   // M = I: β₁ is knorm(m, b)
+  if (bNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    stats.error_with_bnd = false;
+    if (history) stats.residuals.push_back(bNorm);
+    return;
+  }
+  if (history) stats.residuals.push_back(bNorm);
+  const T eps_c = atol + rtol * bNorm;
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+  if (o.verbose > 0) printf("%5s  %7s  %5s\n", "k", "‖rₖ‖", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)bNorm, run.elapsed());
+  iter = iter + 1;
+
+  // β₁Mu₁ = b ; α₁Nv₁ = Aᴴu₁
+  if (beta != 0) {
+    k_scal<T>(c, m, T(1) / beta, u);
+    if (!s.MisI) k_scal<T>(c, m, T(1) / beta, ws.Mu);
+  }
+  if (s.fused) {
+    op_apply(c, At, u, ws.Nv);                                  // kmul!(Aᴴu, Aᴴ, u) ; kcopy!(n, Nv, Aᴴu) without the copy
+  } else {
+    op_apply(c, At, u, ws.Atu);
+    k_copy<T>(c, n, ws.Nv, ws.Atu);
+  }
+  if (!s.NisI) op_apply(c, N, ws.Nv, v, ldiv);
+  T alpha = knorm_elliptic<T>(c, n, v, ws.Nv);
+  if (alpha != 0) {
+    k_scal<T>(c, n, T(1) / alpha, v);
+    if (!s.NisI) k_scal<T>(c, n, T(1) / alpha, ws.Nv);
+  }
+  k_copy<T>(c, m, wbar, u);                                     // w̄₁ = u₁
+
+  T sk = 0, zeta_km1 = 0, etak = 0;
+  T cpk = 1, spk = 1;                                           // Givens rotation that zeroes out λₖ
+  if (lambda > 0) k_copy<T>(c, n, ws.q, v);                     // q₀ = 0 by definition
+  T alphahat;
+  if (lambda > 0) {
+    sym_givens<T>(alpha, lambda, &cpk, &spk, &alphahat);
+    k_scal<T>(c, n, spk, ws.q);                                 // q̄₁ = sp₁ v₁
+  } else {
+    alphahat = alpha;
+  }
+  T epsbar = alphahat;
+  T tau = beta / alphahat;                                      // τ₁ = β₁ / α̂₁
+  T zetabar = tau / epsbar;
+  T thetak = tau;
+
+  bool solved_lq = false, solved_cg = false, tired = false, user_exit = false, overtimed = false;
+  T err_x = 0, err_y = 0, tautilde = 0, rhobar = 0, csig = 0;
+  if (sigma_est > 0) {
+    tautilde = beta / sigma_est;
+    const T zetatilde = tautilde / sigma_est;
+    err_x = tautilde;
+    err_y = zetatilde;
+    solved_lq = err_x <= utolx || err_y <= utoly;
+    if (history) { xNorms.push_back(err_x); yNorms.push_back(err_y); }
+    rhobar = -sigma_est;
+    csig = -1;
+  }
+  // fused: s_u = 1/β and s_v = 1/α of the stored Mu and Nv (1 while they hold u₁ and v₁, scaled above); the y / w̄
+  // update of the last pass waits for the next L1 with its coefficients ζc, ζs, -c, s
+  T s_u = 1, s_v = 1;
+  bool ypend = false;
+  T yc = 0, ys = 0, wc = 0, wsn = 0;
+
+  while (!(solved_lq || solved_cg || tired || user_exit || overtimed)) {
+    // (xᵃᵘˣ)ₖ ← (xᵃᵘˣ)ₖ₋₁ + τₖ v̄ₖ  (fused: in L2, before Nv is overwritten)
+    if (lambda > 0) {
+      k_axpy<T>(c, n, tau * cpk, v, ws.x);
+      if (iter >= 2) {
+        k_axpy<T>(c, n, tau * spk, ws.q, ws.x);
+        k_axpby<T>(c, n, spk, v, -cpk, ws.q);                   // q̄ₖ ← spₖ vₖ - cpₖ qₖ₋₁
+      }
+    } else if (!s.fused) {
+      k_axpy<T>(c, n, tau, v, ws.x);
+    }
+
+    // βₖ₊₁Muₖ₊₁ = Avₖ - αₖMuₖ ; αₖ₊₁Nvₖ₊₁ = Aᴴuₖ₊₁ - βₖ₊₁Nvₖ
+    T beta_next, alpha_next;
+    if (s.fused) {
+      beta_next = lnlq_fused_l1<T>(ws, *A.csr, iter == 1, s_u, alpha, ypend, yc, ys, wc, wsn);
+      ypend = false;
+      const T s_v_old = s_v;
+      s_u = beta_next == 0 ? T(1) : T(1) / beta_next;           // kdiv!(m, u, β), applied by u's readers
+      alpha_next = lnlq_fused_l2<T>(ws, *At.csr, s_v_old, beta_next, tau);
+      s_v = alpha_next == 0 ? T(1) : T(1) / alpha_next;         // kdiv!(n, v, α), applied by v's readers
+    } else {
+      op_apply(c, A, v, ws.Av);
+      k_axpby<T>(c, m, T(1), ws.Av, -alpha, ws.Mu);
+      if (!s.MisI) op_apply(c, M, ws.Mu, u, ldiv);
+      beta_next = knorm_elliptic<T>(c, m, u, ws.Mu);
+      if (beta_next != 0) {
+        k_scal<T>(c, m, T(1) / beta_next, u);
+        if (!s.MisI) k_scal<T>(c, m, T(1) / beta_next, ws.Mu);
+      }
+      op_apply(c, At, u, ws.Atu);
+      k_axpby<T>(c, n, T(1), ws.Atu, -beta_next, ws.Nv);
+      if (!s.NisI) op_apply(c, N, ws.Nv, v, ldiv);
+      alpha_next = knorm_elliptic<T>(c, n, v, ws.Nv);
+      if (alpha_next != 0) {
+        k_scal<T>(c, n, T(1) / alpha_next, v);
+        if (!s.NisI) k_scal<T>(c, n, T(1) / alpha_next, ws.Nv);
+      }
+    }
+
+    // Continue the regularization.
+    T betahat, alphahat_next, cp_next = cpk, sp_next = spk;
+    if (lambda > 0) {
+      betahat = cpk * beta_next;
+      const T theta_reg = spk * beta_next;
+      T cdk, sdk, lambda_next;
+      sym_givens<T>(lambda, theta_reg, &cdk, &sdk, &lambda_next);
+      k_scal<T>(c, n, sdk, ws.q);                               // qₖ ← sdₖ q̄ₖ
+      sym_givens<T>(alpha_next, lambda_next, &cp_next, &sp_next, &alphahat_next);
+    } else {
+      betahat = beta_next;
+      alphahat_next = alpha_next;
+    }
+
+    T omega = 0;
+    if (sigma_est > 0 && !complex_error_bnd) {                  // QR factorization for the Gauss-Radau estimate
+      T mubar = -csig * alphahat;
+      T rho = std::sqrt(rhobar * rhobar + alphahat * alphahat);
+      csig = rhobar / rho;
+      T ssig = alphahat / rho;
+      rhobar = ssig * mubar + csig * sigma_est;
+      mubar = -csig * betahat;
+      const T theta = betahat * csig / rhobar;
+      const T omega_disc = sigma_est * sigma_est - sigma_est * betahat * theta;
+      if (omega_disc < 0) {
+        complex_error_bnd = true;
+      } else {
+        omega = std::sqrt(omega_disc);
+        tautilde = -tau * betahat / omega;
+      }
+      rho = std::sqrt(rhobar * rhobar + betahat * betahat);
+      csig = rhobar / rho;
+      ssig = betahat / rho;
+      rhobar = ssig * mubar + csig * sigma_est;
+    }
+
+    // Lₖ₊₁tₖ₊₁ = β₁e₁, the LQ factorization of (Lₖ₊₁)ᴴ and M̅ₖ₊₁z̅ₖ₊₁ = tₖ₊₁
+    const T tau_next = -betahat * tau / alphahat_next;
+    T c_next, s_next, epsk;
+    sym_givens<T>(epsbar, betahat, &c_next, &s_next, &epsk);
+    const T eta_next = alphahat_next * s_next;
+    const T epsbar_next = -alphahat_next * c_next;
+    const T zetak = thetak / epsk;
+    const T theta_next = tau_next - eta_next * zetak;
+    const T zetabar_next = theta_next / epsbar_next;
+
+    // (yᴸ)ₖ₊₁ ← (yᴸ)ₖ + ζₖ wₖ with wₖ = cₖ₊₁ w̄ₖ + sₖ₊₁ uₖ₊₁ ; w̄ₖ₊₁ = sₖ₊₁ w̄ₖ - cₖ₊₁ uₖ₊₁
+    if (s.fused) {
+      ypend = true;
+      yc = zetak * c_next; ys = zetak * s_next; wc = -c_next; wsn = s_next;
+    } else {
+      k_axpy<T>(c, m, zetak * c_next, wbar, ws.y);
+      k_axpy<T>(c, m, zetak * s_next, u, ws.y);
+      k_axpby<T>(c, m, -c_next, u, s_next, wbar);
+    }
+
+    if (sigma_est > 0 && !complex_error_bnd) {
+      if (transfer_to_craig) {
+        const T disc_x = tautilde * tautilde - tau_next * tau_next;
+        if (disc_x < 0) complex_error_bnd = true; else err_x = std::sqrt(disc_x);
+      } else {
+        const T d = tau_next - eta_next * zetak;
+        const T disc_xL = tautilde * tautilde - tau_next * tau_next + d * d;
+        if (disc_xL < 0) complex_error_bnd = true; else err_x = std::sqrt(disc_xL);
+      }
+      const T etatilde = omega * s_next;
+      const T epstilde = -omega * c_next;
+      const T zetatilde = (tautilde - etatilde * zetak) / epstilde;
+      if (transfer_to_craig) {
+        const T disc_y = zetatilde * zetatilde - zetabar_next * zetabar_next;
+        if (disc_y < 0) complex_error_bnd = true; else err_y = std::sqrt(disc_y);
+      } else {
+        err_y = std::fabs(zetatilde);
+      }
+      if (history) { xNorms.push_back(err_x); yNorms.push_back(err_y); }
+    }
+
+    // ‖(rᴸ)ₖ‖ = |α̂ₖ| √(|ϵ̄ₖζ̄ₖ|² + |β̂ₖ₊₁sₖζₖ₋₁|²) ; the first pass reports ‖b‖ again
+    T rNorm_lq;
+    if (iter == 1) {
+      rNorm_lq = bNorm;
+    } else {
+      const T ra = epsbar * zetabar, rb = betahat * sk * zeta_km1;
+      rNorm_lq = std::fabs(alphahat) * std::sqrt(ra * ra + rb * rb);
+    }
+    if (history) stats.residuals.push_back(rNorm_lq);
+    const T rNorm_cg = transfer_to_craig ? std::fabs(betahat * tau) : T(0);   // ‖(rᶜ)ₖ‖ = |β̂ₖ₊₁τₖ|
+
+    if (ypend && o.callback) {                                  // the callback reads y
+      lnlq_fused_flush<T>(ws, s_u, yc, ys, wc, wsn);
+      ypend = false;
+    }
+    run.poll(iter, user_exit, overtimed);
+    tired = iter >= itmax;
+    solved_lq = rNorm_lq <= eps_c;
+    solved_cg = transfer_to_craig && (std::fabs(zetabar) > eps) && (rNorm_cg <= eps_c);
+    if (sigma_est > 0) {
+      solved_lq = solved_lq || err_x <= utolx || err_y <= utoly;
+      solved_cg = transfer_to_craig && (solved_cg || err_x <= utolx || err_y <= utoly);
+    }
+    if (kdisplay(iter, o.verbose)) printf("%5d  %7.1e  %.2fs\n", iter, (double)rNorm_lq, run.elapsed());
+
+    sk = s_next;
+    alpha = alpha_next;
+    alphahat = alphahat_next;
+    etak = eta_next;
+    thetak = theta_next;
+    epsbar = epsbar_next;
+    tau = tau_next;
+    zeta_km1 = zetak;
+    zetabar = zetabar_next;
+    if (lambda > 0) { cpk = cp_next; spk = sp_next; }
+    iter = iter + 1;
+  }
+  if (o.verbose > 0) printf("\n");
+  if (ypend) lnlq_fused_flush<T>(ws, s_u, yc, ys, wc, wsn);
+
+  // The CRAIG point (signed test on ζ̄, unlike the loop's) or the LNLQ point
+  const bool craig_point = solved_cg && (zetabar > eps);
+  const T xcoef = craig_point ? tau : etak * zeta_km1;
+  if (lambda > 0) {
+    k_axpy<T>(c, n, xcoef * cpk, v, ws.x);
+    if (iter >= 2) k_axpy<T>(c, n, xcoef * spk, ws.q, ws.x);
+  } else if (s.fused) {
+    lnlq_fused_xup<T>(ws, xcoef, s_v);
+  } else {
+    k_axpy<T>(c, n, xcoef, v, ws.x);
+  }
+  if (craig_point) k_axpy<T>(c, m, zetabar, wbar, ws.y);        // (yᶜ)ₖ ← (yᴸ)ₖ₋₁ + ζ̄ₖ w̄ₖ
+
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (solved_lq) st = "solutions (xᴸ, yᴸ) good enough for the tolerances given";
+  if (solved_cg) st = "solutions (xᶜ, yᶜ) good enough for the tolerances given";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  stats.error_with_bnd = complex_error_bnd;
+  run.finish(iter, solved_lq || solved_cg, false, st);
+}
+
 #define INST(T)                                                                                                         \
+  template void lnlq_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
+                              const SolveOpts&);                                                                        \
   template void craig_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
                                const SolveOpts&);                                                                       \
   template void craigmr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \

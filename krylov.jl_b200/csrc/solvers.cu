@@ -95,6 +95,11 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         if (kind == S_CRAIGMR) { ws->d1 = A(); ws->w1 = Am(); }   // d, w̄
         break;
       }
+      case S_LNLQ: {                                // LnlqWorkspace: w̄ in w (Av, Aᴴu, u, v, q: by the solve)
+        auto Am = [&]() { return dev_alloc<T>((size_t)m); };
+        ws->Nv = A(); ws->Mu = Am(); ws->y = Am(); ws->w = Am();
+        break;
+      }
       case S_CAR:                                   // CarWorkspace (Mu is allocated by the solve)
         ws->r = A(); ws->p = A(); ws->s = A(); ws->q = A(); ws->t = A(); ws->u = A();
         break;

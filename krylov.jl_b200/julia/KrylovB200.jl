@@ -196,7 +196,7 @@ end
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
                        :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25, :bilq => 12, :qmr => 13,
-                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :craig => 28, :craigmr => 29, :cg_lanczos => 100)
+                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :craig => 28, :craigmr => 29, :lnlq => 30, :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -272,11 +272,12 @@ function fill_stats!(ws, h::Handle, ::Type{T}) where T
   hasproperty(st, :indefinite) && (st.indefinite = s.indefinite != 0)
   hasproperty(st, :npcCount) && (st.npcCount = s.npcCount)
   hasproperty(st, :Anorm) && (st.Anorm = T(s.Anorm))            # LanczosStats (cg_lanczos!)
-  hasproperty(st, :error_with_bnd) && (st.error_with_bnd = s.error_with_bnd != 0)   # LSLQStats (lslq!)
+  hasproperty(st, :error_with_bnd) && (st.error_with_bnd = s.error_with_bnd != 0)   # LSLQStats, LNLQStats
   bytes = collect(s.status); z = findfirst(==(0x00), bytes)
   st.status = String(bytes[1:(z === nothing ? length(bytes) : z - 1)])
   for (which, field, cnt) in ((0, :residuals, s.nresiduals), (1, :Aresiduals, s.nAresiduals), (2, :Acond, s.nAcond),
-                              (3, :err_lbnds, s.nerr_lbnds), (4, :err_ubnds_lq, s.nerr_ubnds_lq), (5, :err_ubnds_cg, s.nerr_ubnds_cg))
+                              (3, :err_lbnds, s.nerr_lbnds), (4, :err_ubnds_lq, s.nerr_ubnds_lq), (5, :err_ubnds_cg, s.nerr_ubnds_cg),
+                              (3, :error_bnd_x, s.nerr_lbnds), (4, :error_bnd_y, s.nerr_ubnds_lq))   # LNLQStats
     hasproperty(st, field) || continue
     buf = Vector{Cdouble}(undef, cnt)
     got = cnt == 0 ? 0 : ccall((:krylov_b200_get_history, lib), Cint, (Ptr{Cvoid}, Cint, Ptr{Cdouble}, Cint), h.ptr, which, buf, cnt)
@@ -483,6 +484,40 @@ Krylov.craig!(ws::Krylov.CraigWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B20
   leastnorm_solve!(:craig, ws, A, b; kw...)
 Krylov.craigmr!(ws::Krylov.CraigmrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
   leastnorm_solve!(:craigmr, ws, A, b; kw...)
+
+# ---- lnlq! (src/lnlq.jl:144-160) on a rectangular B200CSR: one krylov_solve ----
+# A sibling of leastnorm_solve!, whose kwargs are CRAIG's and CRAIGMR's.  The fused Golub-Kahan passes run when
+# M = N = I and λ = 0.  The extended options carry σ in `sigma`, utolx in `utol`, utoly in `etol` and transfer_to_craig
+# in `transfer_to_bicg`; the bounds come back in stats.error_bnd_x / error_bnd_y (history slots 3 and 4).
+function lnlq_solve!(ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N = I, ldiv::Bool = false, transfer_to_craig::Bool = true,
+                     sqd::Bool = false, λ::T = zero(T), σ::T = zero(T), utolx::T = √eps(T), utoly::T = √eps(T),
+                     atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0, timemax::Float64 = Inf, verbose::Int = 0,
+                     history::Bool = false, callback = workspace -> false, iostream::IO = stdout) where T
+  length(b) == A.m || error("Inconsistent problem size")
+  sqd && (λ ≠ 0) && error("sqd cannot be set to true if λ ≠ 0 !")
+  sqd && (λ = one(T))
+  h = handle_for(:lnlq, ws, A, 0, 0)
+  set_precond!(h, 0, M)
+  set_precond!(h, 1, N)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, utoly, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, σ, utolx,
+                 0, transfer_to_craig))
+  o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, C_NULL, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+    check(ccall((:krylov_get_y, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.y.ptr, A.m))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.lnlq!(ws::Krylov.LnlqWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  lnlq_solve!(ws, A, b; kw...)
 
 # ---- bilq! / qmr! (src/bilq.jl:97-115, src/qmr.jl:104-114) on a square B200CSR: one krylov_solve per solve ------------
 # The library forms Aᵀ once per operator and runs the fused Lanczos biorthogonalization when M = N = I; `c` defaults to b.

@@ -42,7 +42,7 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_",
            "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_",
            "AdjointStats", "BilqrWorkspace", "TrilqrWorkspace", "bilqr", "bilqr_", "trilqr", "trilqr_",
-           "CraigWorkspace", "CraigmrWorkspace", "craig", "craig_", "craigmr", "craigmr_"]
+           "CraigWorkspace", "CraigmrWorkspace", "craig", "craig_", "craigmr", "craigmr_", "LnlqWorkspace", "lnlq", "lnlq_"]
 
 
 class B200Error(RuntimeError):
@@ -505,6 +505,9 @@ class KrylovWorkspace:
         if self.solver == "lslq":    # LSLQStats (src/krylov_stats.jl:352-365)
             out.err_lbnds, out.err_ubnds_lq = hist(3, s.nerr_lbnds), hist(4, s.nerr_ubnds_lq)
             out.err_ubnds_cg, out.error_with_bnd = hist(5, s.nerr_ubnds_cg), bool(s.error_with_bnd)
+        elif self.solver == "lnlq":  # LNLQStats (src/krylov_stats.jl): the bounds travel in LSLQ's history slots 3 and 4
+            out.error_bnd_x, out.error_bnd_y = hist(3, s.nerr_lbnds), hist(4, s.nerr_ubnds_lq)
+            out.error_with_bnd = bool(s.error_with_bnd)
         return out
 
     @property
@@ -1088,7 +1091,7 @@ class _LeastNormWorkspace(_LeastSquaresWorkspace):
         super().__init__(m_or_A, n_or_b, dtype, device=device)
 
     def _solve(self, A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-               unknown, transfer_to_lsqr=False, btol=None, conlim=None):
+               unknown, transfer_to_lsqr=False, btol=None, conlim=None, ext=None):
         if unknown:
             raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
         if sqd and lambda_ != 0:
@@ -1109,6 +1112,8 @@ class _LeastNormWorkspace(_LeastSquaresWorkspace):
         for name, val in (("btol", btol), ("conlim", conlim)):
             if val is not None:
                 setattr(e, name, float(val))
+        for name, val in (ext or {}).items():
+            setattr(e, name, val)
         return self._run(A, b, M, N, o, e, callback)
 
     y = _AdjointWorkspace.y
@@ -1135,6 +1140,23 @@ class CraigmrWorkspace(_LeastNormWorkspace):
         itmax = 0 means m + n."""
         return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
                            unknown)
+
+
+class LnlqWorkspace(_LeastNormWorkspace):
+    solver = "lnlq"
+
+    def solve(self, A, b, *, M=None, N=None, ldiv=False, transfer_to_craig=True, sqd=False, lambda_=0.0, sigma=0.0,
+              utolx=None, utoly=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False,
+              callback=None, fused=True, **unknown):
+        """lnlq!(ws, A, b; kwargs...)  -- kwargs as in lnlq.jl:144-160: utolx, utoly, atol and rtol default to sqrt(eps),
+        itmax = 0 means m + n; σ (`sigma`) > 0, or λ > 0, turns on the upper bounds on ‖x - x*‖ and ‖y - y*‖
+        (stats.error_bnd_x / error_bnd_y)."""
+        ext = {"sigma": float(sigma), "transfer_to_bicg": int(transfer_to_craig)}
+        for name, val in (("utol", utolx), ("etol", utoly)):          # the C ABI carries utolx in utol, utoly in etol
+            if val is not None:
+                ext[name] = float(val)
+        return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
+                           unknown, ext=ext)
 
 
 def _make_least_norm(name):
@@ -1230,7 +1252,7 @@ _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "b
        "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
        "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace, "car": CarWorkspace,
        "minares": MinaresWorkspace, "bilqr": BilqrWorkspace, "trilqr": TrilqrWorkspace, "craig": CraigWorkspace,
-       "craigmr": CraigmrWorkspace}
+       "craigmr": CraigmrWorkspace, "lnlq": LnlqWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -1292,12 +1314,14 @@ bilqr_, trilqr_ = (_make_adjoint_inplace(s) for s in ("bilqr", "trilqr"))
 bilqr, trilqr = (_make_adjoint(s) for s in ("bilqr", "trilqr"))
 craig_, craigmr_ = (_make_inplace(s) for s in ("craig", "craigmr"))
 craig, craigmr = (_make_least_norm(s) for s in ("craig", "craigmr"))
+lnlq_, lnlq = _make_inplace("lnlq"), _make_least_norm("lnlq")
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):
     return {"cg": cg, "gmres": gmres, "bicgstab": bicgstab, "minres": minres, "fom": fom, "fgmres": fgmres, "cgs": cgs,
             "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres, "bilq": bilq,
-            "qmr": qmr, "car": car, "minares": minares, "craig": craig, "craigmr": craigmr}[method](A, b, x0, **kw)
+            "qmr": qmr, "car": car, "minares": minares, "craig": craig, "craigmr": craigmr,
+            "lnlq": lnlq}[method](A, b, x0, **kw)
 
 
 # workspace_accessors.jl:140-152

@@ -1,5 +1,5 @@
-"""Throughput of craig! and craigmr! (Float64), the fused passes against the primitive path (fused = 0), alternated in
-the same run, with the algorithmic-byte model of DESIGN.md section 3f.  One JSON line per (solver, path), then one line
+"""Throughput of craig!, craigmr! and lnlq! (Float64), the fused passes against the primitive path (fused = 0), alternated
+in the same run, with the algorithmic-byte models of DESIGN.md sections 3f and 3g.  One JSON line per (solver, path), then one line
 with the card it ran on.
 
     python profiles/bench_leastnorm.py [--N 215] [--itmax 100] [--reps 3] [--out FILE]
@@ -7,8 +7,9 @@ with the card it ran on.
 Workload, assembled on the GPU (A^T is formed once by the library, outside the timed solves): the divergence D = G^T of
 the N^3 grid (problems.div_csr; N = 215: m = 9 938 375 rows, n = 29 676 450 columns, 59 352 900 nonzeros) and
 b = D cos(0, 1, ..., n - 1), a consistent system whose least-norm solution is the Helmholtz projection of the cosine
-field.  All tolerances are 0 (CRAIG: btol = 0 and conlim = 0, so ctol = 0) so that every solve runs itmax iterations;
-a warm-up solve with history checks that it does.
+field.  All tolerances are 0 (CRAIG: btol = 0 and conlim = 0, so ctol = 0; LNLQ: σ = 0 and utolx = utoly = 0) so that
+every solve runs itmax iterations; a warm-up solve with history checks that it does.  An LNLQ iteration is one pass of
+its loop (lnlq! reports niter = passes + 1).
 """
 import argparse
 import json
@@ -34,9 +35,10 @@ def matrix_bytes(rows, nnz, v=8, i=4):
 def bytes_per_iteration(solver, m, n, nnz, v=8):
     """Algorithmic bytes of one fused iteration (DESIGN.md section 3f, SURVEY 8d counting): each product streams its
     matrix and row pointers once; every vector is counted once per read and once per write.
-    CRAIG: C1 on A^T (m + 4n)v, C2 on A (n + 6m)v.  CRAIGMR: R1 on A (n + 2m)v, R2 on A^T (m + 6n)v, R3 7m v."""
+    CRAIG: C1 on A^T (m + 4n)v, C2 on A (n + 6m)v.  CRAIGMR: R1 on A (n + 2m)v, R2 on A^T (m + 6n)v, R3 7m v.
+    LNLQ: L1 on A (n + 6m)v, L2 on A^T (m + 4n)v: the same total as CRAIG."""
     mats = matrix_bytes(m, nnz) + matrix_bytes(n, nnz)
-    if solver == "craig":
+    if solver in ("craig", "lnlq"):
         return mats + (5 * n + 7 * m) * v
     return mats + (7 * n + 10 * m) * v
 
@@ -65,8 +67,10 @@ def main():
     del z, rows
     work = f"div({a.N}) = grad({a.N})^T f64, m={m} n={n} nnz={nnz}, b = D cos(0:n-1), {a.itmax} iterations/solve"
     lines = []
-    for solver in ("craig", "craigmr"):
-        kw = dict(atol=0.0, rtol=0.0, itmax=a.itmax, **({"btol": 0.0, "conlim": 0.0} if solver == "craig" else {}))
+    for solver in ("craig", "craigmr", "lnlq"):
+        extra = {"craig": {"btol": 0.0, "conlim": 0.0}, "craigmr": {}, "lnlq": {"utolx": 0.0, "utoly": 0.0}}[solver]
+        kw = dict(atol=0.0, rtol=0.0, itmax=a.itmax, **extra)
+        niter = a.itmax + (solver == "lnlq")     # lnlq! counts one more than its passes
         ws = kb.krylov_workspace(solver, m, n, np.float64, device="cuda")
         ws.set_operator((rp, ci, va))
         st = torch.cuda.ExternalStream(kb.lib().krylov_b200_stream(ws._h), device=dev)
@@ -74,7 +78,7 @@ def main():
         launches = {}
         for fused in (1, 0):                     # warm-up: forms A^T, loads the modules
             ws.solve(None, b, fused=bool(fused), history=True, **kw)
-            assert ws.stats.niter == a.itmax and len(ws.stats.residuals) == a.itmax + 1, (solver, fused, ws.stats.status)
+            assert ws.stats.niter == niter and len(ws.stats.residuals) == a.itmax + 1, (solver, fused, ws.stats.status)
         for _ in range(a.reps):
             for fused in (1, 0):                 # alternated, so both paths see the same machine state
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -86,7 +90,7 @@ def main():
                 torch.cuda.synchronize()
                 times[fused].append(e0.elapsed_time(e1) * 1e-3)
                 launches[fused] = ws.launches - l0
-                assert ws.stats.niter == a.itmax, ws.stats
+                assert ws.stats.niter == niter, ws.stats
         ws.free()
         torch.cuda.empty_cache()
         B = bytes_per_iteration(solver, m, n, nnz)
