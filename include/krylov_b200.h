@@ -51,7 +51,9 @@ typedef enum { KRYLOV_CPU = 0, KRYLOV_CUDA = 1 } KrylovDeviceType;
  * LSLQ, CGLS and CRLS on an m x n operator (b has m entries, x has n; matvec_A maps n -> m and matvec_At m -> n, or a
  * CSR operator of m rows and n columns is attached), and the least-norm solvers CRAIG, CRAIGMR and LNLQ on the same m x n
  * operators (min ||x|| subject to A x = b; x = A^T y, and y, m entries, is returned through krylov_get_y; `c` is
- * ignored); every other value returns -2. */
+ * ignored), and the least-norm solvers CGNE and CRMR on the same operators, which return x only (krylov_get_y returns
+ * -2), take `lambda` and one preconditioner, N, on the m-dimensional residual space (a solve given matvec_M or an M
+ * diagonal is refused); every other value returns -2. */
 typedef enum {
   KRYLOV_CG = 0, KRYLOV_CR = 1, KRYLOV_SYMMLQ = 2, KRYLOV_MINRES = 3, KRYLOV_MINRES_QLP = 4, KRYLOV_DIOM = 5,
   KRYLOV_DQGMRES = 6, KRYLOV_FOM = 7, KRYLOV_GMRES = 8, KRYLOV_FGMRES = 9, KRYLOV_BICGSTAB = 10, KRYLOV_CGS = 11,
@@ -142,7 +144,7 @@ const char *krylov_b200_last_error(void);
 /* Attach a CSR matrix as the operator A of `ws`: replaces mul!(y, A, x) at
  * cg.jl:196, gmres.jl:257, bicgstab.jl:221,228, minres.jl:289.
  *   rowptr[n+1], colind[nnz], values[nnz] (element type = workspace dtype);
- *   least-squares and least-norm (CRAIG, CRAIGMR, LNLQ) workspaces: n is the number of rows (the workspace's m) and the
+ *   least-squares and least-norm (CRAIG, CRAIGMR, LNLQ, CGNE, CRMR) workspaces: n is the number of rows (the workspace's m) and the
  *   columns are the workspace's n;
  *   TriLQR workspaces: n is the number of rows (the workspace's m) and the columns are the workspace's n;
  *   least-squares, least-norm, BiLQ, QMR, BiLQR and TriLQR workspaces: the library forms A^T once (host-side) on the first solve and keeps it
@@ -160,7 +162,8 @@ int krylov_b200_attach_csr(void *ws, void *csr);
 /* Diagonal preconditioner: which = 0 -> M, 1 -> N; d[n] holds the diagonal of
  * the operator the solver applies (P^-1 with the default ldiv=false). NULL detaches.
  * LSQR / LSMR / LSLQ / CRAIG / CRAIGMR / LNLQ: M acts on the data space (d[m]), N on the solution space (d[n]).  CGLS / CRLS: M acts on the
- * residual space (d[m]); they take no N (a solve with N attached or matvec_N given is refused). */
+ * residual space (d[m]); they take no N (a solve with N attached or matvec_N given is refused).  CGNE / CRMR: N acts on
+ * the residual space (d[m]); they take no M (a solve with M attached or matvec_M given is refused). */
 int krylov_b200_set_preconditioner_diag(void *ws, int which, const void *d, int location);
 /* Block-Jacobi preconditioner (docs/src/preconditioners.md:33,159): which = 0 -> M, 1 -> N; blocks[ceil(n/bs)][bs][bs]
  * (row-major dense diagonal blocks, 2 <= bs <= 8, element type = workspace dtype; a last block of n % bs rows uses
@@ -233,7 +236,9 @@ int krylov_b200_get_history(void *ws, int which, double *out, int cap);
 /* Device pointer of a workspace vector by its reference field name
  * ("x","r","p","Ap","z","npc_dir","v","s","qd","r1","r2","w1","w2","y","w","dx","V1".."Vk"; LNLQ: "x", "Nv", "Aᴴu", "y", "w̄", "Mu", "Av", "u", "v", "q"; CRAIG / CRAIGMR: "y", "Nv",
  * "Mu", "Av", "Aᴴu", "u", "v", "w", CRAIG "w2", CRAIGMR "d", "w̄" and "q"; BiLQR / TriLQR: "y", "d̅",
- * "wₖ₋₃", "wₖ₋₂", "uₖ₋₁", "uₖ", "vₖ₋₁", "vₖ", "q", "p", "Δx", "Δy"). */
+ * "wₖ₋₃", "wₖ₋₂", "uₖ₋₁", "uₖ", "vₖ₋₁", "vₖ", "q", "p", "Δx", "Δy"; CGNE: "x", "p", "Aᴴz", "r", "q", "s", "z";
+ * CRMR: "x", "p", "Aᴴr", "r", "q", "s", "Nq".  The fused CGNE path does not write "q" or "Aᴴz": they hold what the
+ * last primitive-path solve left). */
 int krylov_b200_get_vector(void *ws, const char *name, void **dev_ptr);
 /* Average durations (ms) of the fused kernels measured with CUDA events on the workspace stream during the
  * last solve run with time_kernels = 1: out[0] = K1 (SpMV + p update + <p,Ap>), out[1] = K2 (x, r update + <r,r>),

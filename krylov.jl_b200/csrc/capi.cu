@@ -80,7 +80,7 @@ bool supported_solver(int s) {
   return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
          s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
          s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR || s == S_CAR || s == S_MINARES ||
-         s == S_BILQR || s == S_TRILQR || s == S_CRAIG || s == S_CRAIGMR || s == S_LNLQ;
+         s == S_BILQR || s == S_TRILQR || s == S_CRAIG || s == S_CRAIGMR || s == S_LNLQ || s == S_CGNE || s == S_CRMR;
 }
 
 int pick_device() {
@@ -184,6 +184,7 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   if (h->solver == S_MINARES) s.lambda = o->lambda;   // _typed_solve_sym_lambda! (CAR: _typed_solve!, M only)
   if (is_ls_kind(h->solver)) { s.lambda = o->lambda; s.radius = o->radius; }   // _typed_solve_ls_mn_radius! (c_stores.jl:403-423)
   if (h->solver == S_LSLQ || is_leastnorm_kind(h->solver)) s.radius = 0;   // _typed_solve_ls_mn!: λ and no trust region
+  if (is_normal_ln_kind(h->solver)) s.radius = 0;                          // CGNE / CRMR: λ and N (c_stores.jl:460)
   s.sigma = std::isnan(h->ext.sigma) ? 0 : h->ext.sigma;
   s.utol = std::isnan(h->ext.utol) ? -1 : h->ext.utol;
   s.transfer_to_lsqr = h->ext.transfer_to_lsqr != 0;
@@ -253,6 +254,8 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
                              : h->solver == S_CRAIG ? "craig applies the adjoint of A: matvec_At must be given with matvec_A"
                              : h->solver == S_CRAIGMR ? "craigmr applies the adjoint of A: matvec_At must be given with matvec_A"
                              : h->solver == S_LNLQ ? "lnlq applies the adjoint of A: matvec_At must be given with matvec_A"
+                             : h->solver == S_CGNE ? "cgne applies the adjoint of A: matvec_At must be given with matvec_A"
+                             : h->solver == S_CRMR ? "crmr applies the adjoint of A: matvec_At must be given with matvec_A"
                                                    : "lsqr and lsmr apply the adjoint of A: matvec_At must be given with matvec_A");
     A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
     At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
@@ -269,11 +272,16 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
   }
   LinOp<T> M = make_cb_op<T>(h, ws, fM, ud), N = make_cb_op<T>(h, ws, fN, ud);
   M.n = m; N.n = n;                      // M acts on the m-dimensional data space, N on the n-dimensional solution space
+  if (is_normal_ln_kind(h->solver)) N.n = m;   // CGNE / CRMR: N acts on the m-dimensional residual space
   if (!fM && h->Mdiag) { M.kind = LinOp<T>::DIAG; M.diag = (const T*)h->Mdiag; }
   if (!fN && h->Ndiag) { N.kind = LinOp<T>::DIAG; N.diag = (const T*)h->Ndiag; }
   // The reference's C layer drops N for CGLS / CRLS; a caller passing one expects it to act, so it is refused.
   if (is_cg_ls(h->solver) && !N.is_identity())
     throw std::runtime_error("cgls and crls take no right preconditioner N (M acts on the m-dimensional residual space)");
+  // The reference's C layer drops M for CGNE / CRMR in the same way; N is their only preconditioner.
+  if (is_normal_ln_kind(h->solver) && !M.is_identity())
+    throw std::runtime_error(std::string(h->solver == S_CGNE ? "cgne" : "crmr") +
+                             " takes no preconditioner M: N (on the m-dimensional residual space) is its only preconditioner");
   if (!b) throw std::runtime_error("b is NULL");
   const T* bd = stage_in<T>(h, ws, b, ws->bbuf);
   switch (h->solver) {
@@ -285,6 +293,8 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
     case S_CRAIG: craig_solve<T>(*ws, A, At, bd, M, N, so); break;
     case S_CRAIGMR: craigmr_solve<T>(*ws, A, At, bd, M, N, so); break;
     case S_LNLQ: lnlq_solve<T>(*ws, A, At, bd, M, N, so); break;
+    case S_CGNE: cgne_solve<T>(*ws, A, At, bd, N, so); break;
+    case S_CRMR: crmr_solve<T>(*ws, A, At, bd, N, so); break;
   }
   return 0;
 }
@@ -460,6 +470,8 @@ template <class T> int do_warm_start(Handle* h, const void* x0, int n) {
                              : h->solver == S_CRAIG ? "craig does not support warm-start (it takes no x0)"
                              : h->solver == S_CRAIGMR ? "craigmr does not support warm-start (it takes no x0)"
                              : h->solver == S_LNLQ ? "lnlq does not support warm-start (it takes no x0)"
+                             : h->solver == S_CGNE ? "cgne does not support warm-start (it takes no x0)"
+                             : h->solver == S_CRMR ? "crmr does not support warm-start (it takes no x0)"
                                                  : "lsqr and lsmr do not support warm-start (they take no x0)");
   if (n != ws->n) throw std::runtime_error("x0 should have size n");
   KB_CUDA(cudaSetDevice(ws->ctx.device));
@@ -493,6 +505,9 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
   if (!strcmp(nm, "w̄") || !strcmp(nm, "wbar")) return ws->kind == S_LSLQ || ws->kind == S_LNLQ ? ws->w : ws->kind == S_CRAIGMR ? ws->w1 : nullptr;
   if (ws->kind == S_CRAIGMR && !strcmp(nm, "d")) return ws->d1;   // CraigmrWorkspace
   if (!strcmp(nm, "Aᴴu")) return ws->Atu;
+  if (ws->kind == S_CGNE && !strcmp(nm, "Aᴴz")) return ws->Ar;   // CgneWorkspace (the fused path leaves Aᴴz and q unwritten)
+  if (ws->kind == S_CRMR && !strcmp(nm, "Aᴴr")) return ws->Ar;   // CrmrWorkspace
+  if (ws->kind == S_CRMR && !strcmp(nm, "Nq")) return ws->z;
   if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ || is_adjoint_kind(ws->kind) ? ws->w : nullptr;
   if (is_adjoint_kind(ws->kind)) {                 // BilqrWorkspace / TrilqrWorkspace (w_{k-3} / w_{k-2} rotate by pointer)
     if (!strcmp(nm, "y") || !strcmp(nm, "t")) return ws->y;
@@ -842,7 +857,8 @@ int krylov_b200_set_preconditioner_diag(void* ws, int which, const void* d, int 
     void*& slot = which == 0 ? h->Mdiag : h->Ndiag;
     if (!d) { dev_free(slot); slot = nullptr; return 0; }
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
-    const int n = which == 0 ? m_of(h) : n_of(h);     // least squares: M has m entries, N has n
+    // least squares: M has m entries, N has n; CGNE / CRMR: N acts on the residual space and has m entries
+    const int n = which == 0 || (!h->block && is_normal_ln_kind(h->solver)) ? m_of(h) : n_of(h);
     KB_CUDA(cudaSetDevice(ctx_of(h).device));
     if (!slot) slot = dev_alloc<char>(esz * (size_t)n);
     KB_CUDA(cudaMemcpy(slot, d, esz * (size_t)n, location ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
@@ -860,7 +876,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
     h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0;
     if (!blocks) return 0;
-    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on least-squares (LSQR, LSMR, CGLS, CRLS) or least-norm (CRAIG, CRAIGMR, LNLQ) workspaces");
+    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on least-squares (LSQR, LSMR, CGLS, CRLS) or least-norm (CRAIG, CRAIGMR, LNLQ, CGNE, CRMR) workspaces");
     if (bs < 2 || bs > 8) return fail("krylov_b200_set_preconditioner_blockdiag", "block size must be in 2..8");
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
     const int n = n_of(h);
@@ -1087,7 +1103,7 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_b200_dist_init", "unknown workspace handle");
-    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) and least-norm (CRAIG, CRAIGMR, LNLQ) solves are not available");
+    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) and least-norm (CRAIG, CRAIGMR, LNLQ, CGNE, CRMR) solves are not available");
     if (is_biorth(h->solver))        // A^T of a row block needs the column halo of A, not its row halo
       return fail("krylov_b200_dist_init", "row-partitioned BiLQ / QMR solves are not available");
     if (h->solver == S_CAR || h->solver == S_MINARES)

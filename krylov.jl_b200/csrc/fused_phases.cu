@@ -1559,6 +1559,126 @@ template <class T> void lnlq_fused_xup(Workspace<T>& ws, T a, T s_v) {
   launch_stream<T, 0>(ws.ctx, ws.n, LnlqXBody<T>{ws.x, ws.Nv, a, s_v}, NoFin());
 }
 
+// ===========================================================================
+// CGNE  (src/cgne.jl:201-235; N = I, lambda = 0)
+// CG on A A^T y = b with x = A^T y.  E1's Fin derives gamma_next and beta, E2's Fin delta = <p, p> and the next alpha
+// (cgne.jl:204-206 at the start of the next iteration).  q = A p and Aᴴz = A^T r are consumed in the epilogues and not
+// stored.  The host reads {gamma, delta} once, after E2.  No Fin writes a field its own pass's epilogue reads: E1 hands
+// alpha to E2 in `ax`.
+// ===========================================================================
+template <class T> struct CgneState { T gamma, delta, alpha, ax, beta; };
+
+template <class T> struct CgneE1Epi {     // q = A p ; r -= alpha q ; <r, r>            (cgne.jl:202,208,210)
+  T* r; const CgneState<T>* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T rn = add_rn(r[row], mul_rn(-s->alpha, acc));
+    r[row] = rn;
+    d[0] += rn * rn;
+  }
+};
+template <class T> struct CgneE1Fin {     // beta = gamma_next / gamma ; gamma = gamma_next   (cgne.jl:211,218)
+  CgneState<T>* s;
+  __device__ void operator()(const T* tot) const {
+    s->ax = s->alpha;
+    s->beta = div_rn(tot[0], s->gamma);
+    s->gamma = tot[0];
+  }
+};
+template <class T> struct CgneE2Epi {     // x += alpha p ; p = A^T r + beta p ; <p, p>   (cgne.jl:207,212-214)
+  T* x; T* p; const CgneState<T>* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T pv = p[row];
+    x[row] = add_rn(x[row], mul_rn(s->ax, pv));
+    const T pn = add_rn(mul_rn(T(1), acc), mul_rn(s->beta, pv));
+    p[row] = pn;
+    d[0] += pn * pn;
+  }
+};
+template <class T> struct CgneE2Fin {     // delta = <p, p> ; alpha = gamma / delta          (cgne.jl:204,206)
+  CgneState<T>* s;
+  __device__ void operator()(const T* tot) const { s->delta = tot[0]; s->alpha = div_rn(s->gamma, tot[0]); }
+};
+
+template <class T>
+void cgne_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T delta, T* gamma_out,
+                          T* delta_out) {
+  Ctx& c = ws.ctx;
+  StateBlock<CgneState, T> sb(ws);
+  CgneState<T>* S = sb.dev;
+  if (init) {
+    CgneState<T> s{};
+    s.gamma = gamma; s.delta = delta; s.alpha = gamma / delta;
+    sb.seed(s);
+  }
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.p}, CgneE1Epi<T>{ws.r, S}, CgneE1Fin<T>{S});
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.r}, CgneE2Epi<T>{ws.x, ws.p, S}, CgneE2Fin<T>{S});
+  const CgneState<T>& h = sb.read();
+  *gamma_out = h.gamma; *delta_out = h.delta;
+}
+
+// ===========================================================================
+// CRMR  (src/crmr.jl:197-227; N = I, lambda = 0)
+// CR on A A^T y = b with x = A^T y, CGLS's pass structure with the roles of the spaces swapped: R1's Fin derives alpha,
+// R3's Fin gamma and beta.  The host reads {<r, r>, gamma} once, after R3; R4 is already queued behind the copy.
+// ===========================================================================
+template <class T> struct CrmrState { T gamma, alpha, beta, rr; };
+
+template <class T> struct CrmrR1Epi {     // q = A p ; <q, q>                          (crmr.jl:198,201)
+  T* q;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const { q[row] = acc; d[0] += acc * acc; }
+};
+template <class T> struct CrmrR1Fin {     // alpha = gamma / <q, q>                    (crmr.jl:201)
+  CrmrState<T>* s;
+  __device__ void operator()(const T* tot) const { s->alpha = div_rn(s->gamma, tot[0]); }
+};
+template <class T> struct CrmrR2Body {    // r -= alpha q ; <r, r>                     (crmr.jl:203-204)
+  T* r; const T* q; const CrmrState<T>* s;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    const T rn = add_rn(r[i], mul_rn(-s->alpha, q[i]));
+    r[i] = rn;
+    d[0] += rn * rn;
+  }
+};
+template <class T> struct CrmrR2Fin {
+  CrmrState<T>* s;
+  __device__ void operator()(const T* tot) const { s->rr = tot[0]; }
+};
+template <class T> struct CrmrR3Epi {     // x += alpha p ; Aᴴr = A^T r ; <Aᴴr, Aᴴr>   (crmr.jl:202,205-206)
+  T* x; const T* p; T* ar; const CrmrState<T>* s;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    x[row] = add_rn(x[row], mul_rn(s->alpha, p[row]));
+    ar[row] = acc;
+    d[0] += acc * acc;
+  }
+};
+template <class T> struct CrmrR3Fin {     // beta = gamma_next / gamma ; gamma = gamma_next   (crmr.jl:208,215)
+  CrmrState<T>* s;
+  __device__ void operator()(const T* tot) const { s->beta = div_rn(tot[0], s->gamma); s->gamma = tot[0]; }
+};
+template <class T> struct CrmrR4Body {    // p = Aᴴr + beta p                          (crmr.jl:210)
+  T* p; const T* ar; const CrmrState<T>* s;
+  __device__ __forceinline__ void operator()(int i, T*) const { p[i] = add_rn(mul_rn(T(1), ar[i]), mul_rn(s->beta, p[i])); }
+};
+
+template <class T>
+void crmr_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T* rr, T* gamma_out) {
+  Ctx& c = ws.ctx;
+  StateBlock<CrmrState, T> sb(ws);
+  CrmrState<T>* S = sb.dev;
+  if (init) {
+    CrmrState<T> s{};
+    s.gamma = gamma;
+    sb.seed(s);
+  }
+  launch_spmv_epi_g<T, 1>(c, A, XPlain<T>{ws.p}, CrmrR1Epi<T>{ws.q}, CrmrR1Fin<T>{S});
+  launch_stream<T, 1>(c, ws.m, CrmrR2Body<T>{ws.r, ws.q, S}, CrmrR2Fin<T>{S});
+  launch_spmv_epi_g<T, 1>(c, At, XPlain<T>{ws.r}, CrmrR3Epi<T>{ws.x, ws.p, ws.Ar, S}, CrmrR3Fin<T>{S});
+  sb.post();
+  launch_stream<T, 0>(c, ws.n, CrmrR4Body<T>{ws.p, ws.Ar, S}, NoFin());
+  const CrmrState<T>& h = sb.wait();
+  *rr = h.rr; *gamma_out = h.gamma;
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1601,7 +1721,9 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template T lnlq_fused_l1<T>(Workspace<T>&, const Csr<T>&, bool, T, T, bool, T, T, T, T);                          \
   template T lnlq_fused_l2<T>(Workspace<T>&, const Csr<T>&, T, T, T);                                               \
   template void lnlq_fused_flush<T>(Workspace<T>&, T, T, T, T, T);                                                  \
-  template void lnlq_fused_xup<T>(Workspace<T>&, T, T);
+  template void lnlq_fused_xup<T>(Workspace<T>&, T, T);                                                           \
+  template void cgne_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T*, T*);          \
+  template void crmr_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T*, T*);
 INST(double)
 INST(float)
 #undef INST

@@ -13,7 +13,7 @@
 //   block.cu      block_gmres! on row-major device panels (8f-2; block.h)
 //   biorth.cu     host control flow of bilq!/qmr! (one Lanczos biorthogonalization driver; A and A^T)
 //   adjoint.cu    host control flow of bilqr!/trilqr! (adjoint system pairs A x = b, A^T y = c; two solutions)
-//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! and of the least-norm craig!/craigmr!/lnlq! on rectangular
+//   lsq.cu        host control flow of lsqr!/lsmr!/lslq!/cgls!/crls! and of the least-norm craig!/craigmr!/lnlq!/cgne!/crmr! on rectangular
 //                 operators (primitive and fused paths)
 //   mtx.cu        Matrix Market ingestion, transposed operator (8f-4; mtx.h)
 //   capi.cu       the C ABI (include/krylov_b200.h)
@@ -217,12 +217,15 @@ struct Stats {
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
                   S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_TRILQR = 18, S_BILQR = 19, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
-                  S_CRAIG = 28, S_CRAIGMR = 29, S_LNLQ = 30, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
+                  S_CGNE = 26, S_CRMR = 27, S_CRAIG = 28, S_CRAIGMR = 29, S_LNLQ = 30, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
 // the least-squares and least-norm solvers: A is m x n, b has m entries and x has n
 inline bool is_ls_kind(int k) {
   return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS || k == S_CRAIG || k == S_CRAIGMR ||
-         k == S_LNLQ;
+         k == S_LNLQ || k == S_CGNE || k == S_CRMR;
 }
+// CGNE / CRMR: CG and CR on A A^T y = b with x = A^T y; they return x only and take one preconditioner, N, on the
+// m-dimensional residual space
+inline bool is_normal_ln_kind(int k) { return k == S_CGNE || k == S_CRMR; }
 // the least-norm solvers: min ||x|| subject to A x = b, with x = A^T y; they return the multipliers y (m entries) too
 inline bool is_leastnorm_kind(int k) { return k == S_CRAIG || k == S_CRAIGMR || k == S_LNLQ; }
 // the adjoint-pair solvers: two solutions, x (A x = b) and y (A^T y = c).  TriLQR: A is m x n, b and y have m entries,
@@ -259,6 +262,8 @@ struct Workspace {
                                        // LNLQ: w̄ in w (+ x, Nv, y, Mu; Atu, Av, u, v, q: lazy)
   T *Ar = nullptr, *Mr = nullptr;      // CGLS: Mr (m, lazy; Mq aliases it) (+ x, p, s: n; r, q: m)
                                        // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
+                                       // CGNE: Aᴴz in Ar (+ x, p: n; r, q: m; s, z: m, lazy)
+                                       // CRMR: Aᴴr in Ar, Nq in z (m, lazy) (+ x, p: n; r, q: m; s: m, lazy)
   std::vector<T*> V;
   std::vector<T*> Z;                   // FGMRES: Z[k] = N_k V[k];  DQGMRES / DIOM: the direction stack P
   std::vector<T> c, sgiv, zg, R;       // GMRES host-side Givens data
@@ -339,6 +344,11 @@ template <class T> void craigmr_solve(Workspace<T>& ws, const LinOp<T>& A, const
                                       const LinOp<T>& N, const SolveOpts& o);
 template <class T> void lnlq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const LinOp<T>& N, const SolveOpts& o);
+// CGNE / CRMR: N (m x m) acts on the residual space; they take no M.
+template <class T> void cgne_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& N,
+                                   const SolveOpts& o);
+template <class T> void crmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& N,
+                                   const SolveOpts& o);
 // CGLS / CRLS: M (m x m) acts on the residual space; they take no N.
 template <class T> void cgls_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const SolveOpts& o);
@@ -465,6 +475,16 @@ template <class T> void cgls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, 
 // One read-back: <Ar, Ar>, <x, x>, <r, r> and gamma.  `init`: first iteration, sets alpha and gamma from the host.
 template <class T> void crls_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T alpha, T gamma,
                                              T lambda, T* ArAr, T* xx, T* rr, T* gamma_out);
+// One CGNE iteration, N = I, lambda = 0, 2 launches: E1 (SpMV on A gathering p) r -= alpha (A p), with gamma and beta on
+// the device; E2 (SpMV on A^T gathering r) x += alpha p, p = A^T r + beta p, delta = <p, p> and the next alpha on the
+// device.  One read-back: gamma and delta.  `init`: first iteration, sets gamma and alpha = gamma / delta from the host.
+template <class T> void cgne_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T delta,
+                                             T* gamma_out, T* delta_out);
+// One CRMR iteration, N = I, lambda = 0, 4 launches: R1 q = A p (alpha on the device), R2 r -= alpha q, R3 Aᴴr = A^T r
+// with x += alpha p (gamma, beta on the device), R4 p = Aᴴr + beta p.  One read-back: <r, r> and gamma.
+// `init`: first iteration, sets gamma on the device from the host.
+template <class T> void crmr_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, bool init, T gamma, T* rr,
+                                             T* gamma_out);
 // BiLQ / QMR (fused_phases.cu), M = N = I, A and A^T CSR operators.  One Lanczos biorthogonalization step: B1 (SpMV on A
 // gathering v: q = A v - gamma v_prev, alpha = <u, q> on the device) and B2 (SpMV on A^T gathering u: p = A^T u -
 // beta u_prev - alpha u, q -= alpha v, <p, q>), then one read-back of {alpha, <p, q>}.

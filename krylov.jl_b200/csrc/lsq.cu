@@ -7,7 +7,8 @@
 // lslq! (src/lslq.jl:201-520) runs the same Golub-Kahan step (fused: LSQR's P1 / P2 and its own update pass).
 // cgls! (src/cgls.jl:129-243) and crls! (src/crls.jl:120-268) run the normal-equations recurrences on the same operator
 // pair: 8 / 11 launches per iteration on the primitives, 4 fused ones (fused_phases.cu) and one read-back when A is a
-// CSR operator, M = I and there is no trust region.
+// CSR operator, M = I and there is no trust region.  cgne! and crmr! run them on A Aᴴ y = b, x = Aᴴ y: 2 and 4 fused
+// launches per iteration and one read-back when A is a CSR operator, N = I and λ = 0.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -1545,7 +1546,189 @@ void lnlq_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T
   run.finish(iter, solved_lq || solved_cg, false, st);
 }
 
+// ===========================================================================
+// cgne!  (src/cgne.jl:134-252): CG on A Aᴴ y = b, x = Aᴴ y (Craig's method).  N acts on the m-dimensional residual
+// space: z = N r.  The first history entry is ‖b‖, every later one √⟨r, z⟩.  Fused (N = I, λ = 0, CSR A and Aᴴ): E1 on
+// A, E2 on Aᴴ, one read-back of {γ, δ}; q and Aᴴz are not stored, x is current after every iteration.
+// ===========================================================================
+template <class T>
+void cgne_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& N, const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CGNE: system of %d equations in %d variables\n", m, n);
+  const bool NisI = N.is_identity();
+  const T lambda = (T)o.lambda;
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  const bool fused = o.fused && A.kind == LinOp<T>::CSR && At.kind == LinOp<T>::CSR && NisI && lambda == 0;
+  Stats& stats = ws.stats;
+  allocate_if(!NisI, ws, ws.z, m);
+  allocate_if(lambda > 0, ws, ws.s, m);
+  stats.reset();
+  T* z = NisI ? ws.r : ws.z;
+
+  k_fill<T>(c, n, ws.x, T(0));
+  k_copy<T>(c, m, ws.r, b);                                     // r ← b
+  if (!NisI) op_apply(c, N, ws.r, z, ldiv);
+  T rNorm = k_nrm2<T>(c, m, ws.r);
+  if (history) stats.residuals.push_back(rNorm);
+  if (rNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    return;
+  }
+  if (lambda > 0) k_copy<T>(c, m, ws.s, ws.r);                  // s ← r
+  op_apply(c, At, z, ws.p);
+  T pNorm = k_nrm2<T>(c, n, ws.p);                              // ‖p‖ detects an inconsistent system
+  T gamma = k_dot<T>(c, m, ws.r, z);
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+
+  const T eps_c = atol + rtol * rNorm;                          // consistent systems
+  const T eps_i = atol + rtol * pNorm;                          // inconsistent systems
+  if (o.verbose > 0) printf("%5s  %8s  %5s\n", "k", "‖r‖", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %.2fs\n", iter, (double)rNorm, run.elapsed());
+
+  bool solved = rNorm <= eps_c, inconsistent = (rNorm > 100 * eps_c) && (pNorm <= eps_i), tired = iter >= itmax;
+  bool user_exit = false, overtimed = false;
+  const T delta0 = fused && !(solved || inconsistent || tired) ? k_dot<T>(c, n, ws.p, ws.p) : T(0);
+  while (!(solved || inconsistent || tired || user_exit || overtimed)) {
+    if (fused) {
+      T pp;
+      cgne_fused_iteration<T>(ws, *A.csr, *At.csr, iter == 0, gamma, delta0, &gamma, &pp);
+      pNorm = std::sqrt(pp);
+      rNorm = std::sqrt(gamma);
+    } else {
+      op_apply(c, A, ws.p, ws.q);
+      if (lambda > 0) k_axpy<T>(c, m, lambda, ws.s, ws.q);
+      T delta = k_dot<T>(c, n, ws.p, ws.p);
+      if (lambda > 0) delta += lambda * k_dot<T>(c, m, ws.s, ws.s);
+      const T alpha = gamma / delta;
+      k_axpy<T>(c, n, alpha, ws.p, ws.x);
+      k_axpy<T>(c, m, -alpha, ws.q, ws.r);
+      if (!NisI) op_apply(c, N, ws.r, z, ldiv);
+      const T gamma_next = k_dot<T>(c, m, ws.r, z);
+      const T beta = gamma_next / gamma;
+      op_apply(c, At, z, ws.Ar);                                // Aᴴz
+      k_axpby<T>(c, n, T(1), ws.Ar, beta, ws.p);                // p = Aᴴz + β p
+      pNorm = k_nrm2<T>(c, n, ws.p);
+      if (lambda > 0) k_axpby<T>(c, m, T(1), ws.r, beta, ws.s); // s = r + β s
+      gamma = gamma_next;
+      rNorm = std::sqrt(gamma_next);
+    }
+    if (history) stats.residuals.push_back(rNorm);
+    iter = iter + 1;
+    if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %.2fs\n", iter, (double)rNorm, run.elapsed());
+    const bool resid_decrease_mach = rNorm + T(1) <= T(1);
+    run.poll(iter, user_exit, overtimed);
+    const bool resid_decrease_lim = rNorm <= eps_c;
+    solved = resid_decrease_lim || resid_decrease_mach;
+    inconsistent = (rNorm > 100 * eps_c) && (pNorm <= eps_i);
+    tired = iter >= itmax;
+  }
+  if (o.verbose > 0) printf("\n");
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (inconsistent) st = "system probably inconsistent";
+  if (solved) st = "solution good enough given atol and rtol";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  run.finish(iter, solved, inconsistent, st);
+}
+
+// ===========================================================================
+// crmr!  (src/crmr.jl:132-244): CR on A Aᴴ y = b, x = Aᴴ y.  N acts on the m-dimensional residual space: r = N b and
+// Nq = N q.  Fused (N = I, λ = 0, CSR A and Aᴴ): R1 on A, R2 over m, R3 on Aᴴ, R4 over n, one read-back of
+// {‖r‖², γ}; x is current after every iteration.
+// ===========================================================================
+template <class T>
+void crmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& N, const SolveOpts& o) {
+  SolveRun<T> run(ws, o);
+  Ctx& c = ws.ctx;
+  const int m = ws.m, n = ws.n;
+  const bool history = o.history, ldiv = o.ldiv;
+  if (o.verbose > 0) printf("CRMR: system of %d equations in %d variables\n", m, n);
+  const bool NisI = N.is_identity();
+  const T lambda = (T)o.lambda;
+  const T atol = tol_of<T>(o.atol), rtol = tol_of<T>(o.rtol);
+  const bool fused = o.fused && A.kind == LinOp<T>::CSR && At.kind == LinOp<T>::CSR && NisI && lambda == 0;
+  Stats& stats = ws.stats;
+  allocate_if(!NisI, ws, ws.z, m);
+  allocate_if(lambda > 0, ws, ws.s, m);
+  stats.reset();
+  T* Nq = NisI ? ws.q : ws.z;
+
+  k_fill<T>(c, n, ws.x, T(0));
+  if (NisI) k_copy<T>(c, m, ws.r, b);                           // r = N b
+  else op_apply(c, N, b, ws.r, ldiv);
+  const T bNorm = k_nrm2<T>(c, m, ws.r);
+  T rNorm = bNorm;
+  if (history) stats.residuals.push_back(rNorm);
+  if (bNorm == 0) {
+    run.finish(0, true, false, "x is a zero-residual solution");
+    if (history) stats.Aresiduals.push_back(0);
+    return;
+  }
+  if (lambda > 0) k_copy<T>(c, m, ws.s, ws.r);                  // s ← r
+  op_apply(c, At, ws.r, ws.Ar);
+  k_copy<T>(c, n, ws.p, ws.Ar);                                 // p ← Aᴴr
+  T gamma = k_dot<T>(c, n, ws.Ar, ws.Ar);
+  if (lambda > 0) gamma += lambda * rNorm * rNorm;
+  int iter = 0;
+  const int itmax = ls_itmax(ws, o.itmax);
+
+  T ArNorm = std::sqrt(gamma);
+  if (history) stats.Aresiduals.push_back(ArNorm);
+  const T eps_c = atol + rtol * rNorm;                          // consistent systems
+  const T eps_i = atol + rtol * ArNorm;                         // inconsistent systems
+  if (o.verbose > 0) printf("%5s  %8s  %8s  %5s\n", "k", "‖Aᴴr‖", "‖r‖", "timer");
+  if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %8.2e  %.2fs\n", iter, (double)ArNorm, (double)rNorm, run.elapsed());
+
+  bool solved = rNorm <= eps_c, inconsistent = (rNorm > 100 * eps_c) && (ArNorm <= eps_i), tired = iter >= itmax;
+  bool user_exit = false, overtimed = false;
+  while (!(solved || inconsistent || tired || user_exit || overtimed)) {
+    if (fused) {
+      T rr;
+      crmr_fused_iteration<T>(ws, *A.csr, *At.csr, iter == 0, gamma, &rr, &gamma);
+      rNorm = std::sqrt(rr);
+    } else {
+      op_apply(c, A, ws.p, ws.q);
+      if (lambda > 0) k_axpy<T>(c, m, lambda, ws.s, ws.q);     // q = q + λ s
+      if (!NisI) op_apply(c, N, ws.q, Nq, ldiv);
+      const T alpha = gamma / k_dot<T>(c, m, ws.q, Nq);        // qᴴ N q
+      k_axpy<T>(c, n, alpha, ws.p, ws.x);
+      k_axpy<T>(c, m, -alpha, Nq, ws.r);
+      rNorm = k_nrm2<T>(c, m, ws.r);
+      op_apply(c, At, ws.r, ws.Ar);
+      T gamma_next = k_dot<T>(c, n, ws.Ar, ws.Ar);
+      if (lambda > 0) gamma_next += lambda * rNorm * rNorm;
+      const T beta = gamma_next / gamma;
+      k_axpby<T>(c, n, T(1), ws.Ar, beta, ws.p);                // p = Aᴴr + β p
+      if (lambda > 0) k_axpby<T>(c, m, T(1), ws.r, beta, ws.s); // s = r + β s
+      gamma = gamma_next;
+    }
+    ArNorm = std::sqrt(gamma);
+    if (history) { stats.residuals.push_back(rNorm); stats.Aresiduals.push_back(ArNorm); }
+    iter = iter + 1;
+    if (kdisplay(iter, o.verbose)) printf("%5d  %8.2e  %8.2e  %.2fs\n", iter, (double)ArNorm, (double)rNorm, run.elapsed());
+    run.poll(iter, user_exit, overtimed);
+    solved = rNorm <= eps_c;
+    inconsistent = (rNorm > 100 * eps_c) && (ArNorm <= eps_i);
+    tired = iter >= itmax;
+  }
+  if (o.verbose > 0) printf("\n");
+  const char* st = "unknown";
+  if (tired) st = "maximum number of iterations exceeded";
+  if (solved) st = "solution good enough given atol and rtol";
+  if (inconsistent) st = "system probably inconsistent but least squares/norm solution found";
+  if (user_exit) st = "user-requested exit";
+  if (overtimed) st = "time limit exceeded";
+  run.finish(iter, solved, inconsistent, st);
+}
+
 #define INST(T)                                                                                                         \
+  template void cgne_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&); \
+  template void crmr_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const SolveOpts&); \
   template void lnlq_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \
                               const SolveOpts&);                                                                        \
   template void craig_solve<T>(Workspace<T>&, const LinOp<T>&, const LinOp<T>&, const T*, const LinOp<T>&, const LinOp<T>&, \

@@ -89,6 +89,9 @@ template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int me
         ws->v_prev = Am(); ws->v = Am(); ws->q = Am(); ws->y = Am(); ws->w1 = Am(); ws->w2 = Am();
         break;
       }
+      case S_CGNE: case S_CRMR:                     // CgneWorkspace / CrmrWorkspace: Aᴴz / Aᴴr in Ar (s, z / Nq: by the solve)
+        ws->p = A(); ws->Ar = A(); ws->r = dev_alloc<T>((size_t)m); ws->q = dev_alloc<T>((size_t)m);
+        break;
       case S_CRAIG: case S_CRAIGMR: {               // CraigWorkspace / CraigmrWorkspace (Av, Aᴴu, u, v, w2 / q: by the solve)
         auto Am = [&]() { return dev_alloc<T>((size_t)m); };
         ws->Nv = A(); ws->Mu = Am(); ws->y = Am(); ws->w = Am();

@@ -196,7 +196,8 @@ end
 # (test/test_allocations.jl:54-57).
 const SOLVER_ID = Dict(:cg => 0, :cr => 1, :minres => 3, :diom => 5, :dqgmres => 6, :fom => 7, :gmres => 8, :fgmres => 9,
                        :bicgstab => 10, :cgs => 11, :lslq => 20, :lsqr => 21, :lsmr => 22, :cgls => 24, :crls => 25, :bilq => 12, :qmr => 13,
-                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :craig => 28, :craigmr => 29, :lnlq => 30, :cg_lanczos => 100)
+                       :car => 32, :minares => 33, :trilqr => 18, :bilqr => 19, :craig => 28, :craigmr => 29, :lnlq => 30,
+                       :cgne => 26, :crmr => 27, :cg_lanczos => 100)
 struct COpts   # KrylovOptions, interfaces/src/c_enums.jl:40-62
   atol::Cdouble; rtol::Cdouble; itmax::Cint; verbose::Cint; lambda::Cdouble; tau::Cdouble; nu::Cdouble
   timemax::Cdouble; radius::Cdouble; restart::Cint; reorthogonalization::Cint; linesearch::Cint
@@ -518,6 +519,37 @@ function lnlq_solve!(ws, A::B200CSR{T}, b::B200Vector{T}; M = I, N = I, ldiv::Bo
 end
 Krylov.lnlq!(ws::Krylov.LnlqWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
   lnlq_solve!(ws, A, b; kw...)
+
+# ---- cgne! / crmr! (src/cgne.jl:113-131, src/crmr.jl:111-129) on a rectangular B200CSR: one krylov_solve ----------
+# A sibling of normal_ls_solve! and leastnorm_solve!, whose kwargs are CGLS's / CRLS's and CRAIG's / CRAIGMR's.  CG and
+# CR on A Aᵀ y = b with x = Aᵀ y; only x comes back.  N acts on the m-dimensional residual space (a B200Diagonal of m
+# entries) and there is no M.  The fused passes run when N = I and λ = 0.
+function normal_ln_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}; N = I, ldiv::Bool = false, λ::T = zero(T),
+                          atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0, timemax::Float64 = Inf, verbose::Int = 0,
+                          history::Bool = false, callback = workspace -> false, iostream::IO = stdout) where T
+  length(b) == A.m || error("Inconsistent problem size")
+  h = handle_for(method, ws, A, 0, 0)
+  set_precond!(h, 0, I)
+  set_precond!(h, 1, N)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, 0, NaN, NaN, NaN, 0.0, NaN, 0, 1))
+  o = Ref(COpts(atol, rtol, itmax, verbose, λ, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, 0, 0, 0))
+  GC.@preserve user ext o begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, C_NULL, b.ptr, C_NULL, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    check(ccall((:krylov_get_x, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Cint), h.ptr, ws.x.ptr, A.n))
+  end
+  fill_stats!(ws, h, T)
+  ws
+end
+Krylov.cgne!(ws::Krylov.CgneWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  normal_ln_solve!(:cgne, ws, A, b; kw...)
+Krylov.crmr!(ws::Krylov.CrmrWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T}; kw...) where T =
+  normal_ln_solve!(:crmr, ws, A, b; kw...)
 
 # ---- bilq! / qmr! (src/bilq.jl:97-115, src/qmr.jl:104-114) on a square B200CSR: one krylov_solve per solve ------------
 # The library forms Aᵀ once per operator and runs the fused Lanczos biorthogonalization when M = N = I; `c` defaults to b.

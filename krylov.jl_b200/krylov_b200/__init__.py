@@ -42,7 +42,8 @@ __all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspac
            "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_",
            "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_",
            "AdjointStats", "BilqrWorkspace", "TrilqrWorkspace", "bilqr", "bilqr_", "trilqr", "trilqr_",
-           "CraigWorkspace", "CraigmrWorkspace", "craig", "craig_", "craigmr", "craigmr_", "LnlqWorkspace", "lnlq", "lnlq_"]
+           "CraigWorkspace", "CraigmrWorkspace", "craig", "craig_", "craigmr", "craigmr_", "LnlqWorkspace", "lnlq", "lnlq_",
+           "CgneWorkspace", "CrmrWorkspace", "cgne", "cgne_", "crmr", "crmr_"]
 
 
 class B200Error(RuntimeError):
@@ -766,6 +767,7 @@ def block_gmres_(ws: BlockGmresWorkspace, A, B, X0=None, **kw):
 class _LeastSquaresWorkspace(KrylovWorkspace):
     """Workspace of lsqr! / lsmr! on an m x n operator (src/krylov_workspaces.jl LsqrWorkspace / LsmrWorkspace):
     b has m entries, x has n.  `window` (default 5) sizes the forward-error window."""
+    _N_on_residual_space = False    # CGNE / CRMR: N acts on the m-dimensional residual space
 
     def __init__(self, m_or_A, n_or_b=None, dtype=None, *, window: int = 0, device: str = "host", memory: int = 0):
         super().__init__(m_or_A, n_or_b, dtype, memory=memory, window=window, device=device)
@@ -836,7 +838,7 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
             self.set_operator(A)
         keep += [fA, fAt]
         fP = [null, null]
-        for which, (P, ln) in enumerate(((M, m), (N, n))):
+        for which, (P, ln) in enumerate(((M, m), (N, m if self._N_on_residual_space else n))):
             if P is not None and callable(P) and not hasattr(P, "shape"):
                 fP[which] = self._wrap_rect(P, ln, ln)
                 keep.append(fP[which])
@@ -1159,6 +1161,45 @@ class LnlqWorkspace(_LeastNormWorkspace):
                            unknown, ext=ext)
 
 
+class _NormalLeastNormWorkspace(_LeastSquaresWorkspace):
+    """Workspace of cgne! / crmr! on an m x n operator (src/krylov_workspaces.jl CgneWorkspace / CrmrWorkspace): the
+    least-norm solution of A x = b by CG / CR on A A^T y = b, x = A^T y.  b has m entries, x has n; only x is returned.
+    A and its adjoint: a CSR operator (its transpose is formed once and cached), or a scipy.sparse.linalg.LinearOperator
+    / (matvec, rmatvec) pair of host callables.  N (m entries) acts on the residual space: None, the diagonal of a
+    Diagonal preconditioner, or a host callable.  There is no M."""
+    nA = 2
+    _N_on_residual_space = True
+
+    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
+        super().__init__(m_or_A, n_or_b, dtype, device=device)
+
+    def solve(self, A, b, *, N=None, ldiv=False, lambda_=0.0, atol=None, rtol=None, itmax=0, timemax=math.inf,
+              verbose=0, history=False, callback=None, fused=True, **unknown):
+        """cgne!(ws, A, b; kwargs...) / crmr!(ws, A, b; kwargs...)  -- kwargs as in cgne.jl:116-126 and
+        crmr.jl:114-124: atol and rtol default to sqrt(eps), itmax = 0 means m + n, λ (`lambda_`) >= 0."""
+        if unknown:
+            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
+        o = lib().krylov_default_options()
+        if atol is not None:
+            o.atol = float(atol)
+        if rtol is not None:
+            o.rtol = float(rtol)
+        o.itmax, o.verbose = int(itmax), int(verbose)
+        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+        o.lambda_ = float(lambda_)
+        e = lib().krylov_b200_default_options()
+        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        return self._run(A, b, None, N, o, e, callback)
+
+
+class CgneWorkspace(_NormalLeastNormWorkspace):
+    solver = "cgne"
+
+
+class CrmrWorkspace(_NormalLeastNormWorkspace):
+    solver = "crmr"
+
+
 def _make_least_norm(name):
     def f(A, b, x0=None, *, n=None, **kw):
         if x0 is not None:
@@ -1183,6 +1224,33 @@ def _make_least_norm(name):
             ws.free()
     f.__name__ = name
     f.__doc__ = f"(x, y, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
+    return f
+
+
+def _make_normal_least_norm(name):
+    def f(A, b, x0=None, *, n=None, **kw):
+        if x0 is not None:
+            raise B200Error(f"{name} does not support warm-start (it takes no x0)")
+        m = b.shape[0]
+        if n is None:
+            if not hasattr(A, "shape"):
+                raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
+            n = A.shape[1]
+        if _is_torch(b):                      # the element type, without copying a device b to the host
+            import torch
+            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
+        else:
+            dt = np.asarray(b).dtype
+        if dt not in (np.float32, np.float64):
+            dt = np.float64
+        ws = _WS[name](m, int(n), dt, device="cuda" if _is_torch(b) else "host")
+        try:
+            ws.solve(A, b, **kw)
+            return ws.x, ws.stats
+        finally:
+            ws.free()
+    f.__name__ = name
+    f.__doc__ = f"(x, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
     return f
 
 
@@ -1252,7 +1320,7 @@ _WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "b
        "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
        "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace, "car": CarWorkspace,
        "minares": MinaresWorkspace, "bilqr": BilqrWorkspace, "trilqr": TrilqrWorkspace, "craig": CraigWorkspace,
-       "craigmr": CraigmrWorkspace, "lnlq": LnlqWorkspace}
+       "craigmr": CraigmrWorkspace, "lnlq": LnlqWorkspace, "cgne": CgneWorkspace, "crmr": CrmrWorkspace}
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
@@ -1315,13 +1383,15 @@ bilqr, trilqr = (_make_adjoint(s) for s in ("bilqr", "trilqr"))
 craig_, craigmr_ = (_make_inplace(s) for s in ("craig", "craigmr"))
 craig, craigmr = (_make_least_norm(s) for s in ("craig", "craigmr"))
 lnlq_, lnlq = _make_inplace("lnlq"), _make_least_norm("lnlq")
+cgne_, crmr_ = (_make_inplace(s) for s in ("cgne", "crmr"))
+cgne, crmr = (_make_normal_least_norm(s) for s in ("cgne", "crmr"))
 
 
 def krylov_solve(method: str, A, b, x0=None, **kw):
     return {"cg": cg, "gmres": gmres, "bicgstab": bicgstab, "minres": minres, "fom": fom, "fgmres": fgmres, "cgs": cgs,
             "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres, "bilq": bilq,
             "qmr": qmr, "car": car, "minares": minares, "craig": craig, "craigmr": craigmr,
-            "lnlq": lnlq}[method](A, b, x0, **kw)
+            "lnlq": lnlq, "cgne": cgne, "crmr": crmr}[method](A, b, x0, **kw)
 
 
 # workspace_accessors.jl:140-152

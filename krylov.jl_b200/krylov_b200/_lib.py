@@ -23,7 +23,8 @@ KRYLOV_LSLQ, KRYLOV_LSQR, KRYLOV_LSMR, KRYLOV_CGLS, KRYLOV_CRLS = 20, 21, 22, 24
 SOLVER_IDS = {"lslq": KRYLOV_LSLQ, "lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cgls": KRYLOV_CGLS, "crls": KRYLOV_CRLS, "cg": KRYLOV_CG, "minres": KRYLOV_MINRES, "gmres": KRYLOV_GMRES, "bicgstab": KRYLOV_BICGSTAB,
               "fom": KRYLOV_FOM, "fgmres": KRYLOV_FGMRES, "cgs": KRYLOV_CGS, "cg_lanczos": KRYLOV_B200_CG_LANCZOS,
               "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES, "bilq": 12, "qmr": 13,
-              "car": 32, "minares": 33, "trilqr": 18, "bilqr": 19, "craig": 28, "craigmr": 29, "lnlq": 30}
+              "car": 32, "minares": 33, "trilqr": 18, "bilqr": 19, "craig": 28, "craigmr": 29, "lnlq": 30,
+              "cgne": 26, "crmr": 27}
 
 MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p)
 BLOCK_MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p)

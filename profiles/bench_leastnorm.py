@@ -1,15 +1,16 @@
-"""Throughput of craig!, craigmr! and lnlq! (Float64), the fused passes against the primitive path (fused = 0), alternated
-in the same run, with the algorithmic-byte models of DESIGN.md sections 3f and 3g.  One JSON line per (solver, path), then one line
-with the card it ran on.
+"""Throughput of craig!, craigmr!, lnlq!, cgne! and crmr! (Float64), the fused passes against the primitive path
+(fused = 0), alternated in the same run, with the algorithmic-byte models of DESIGN.md sections 3f, 3g and 3h.  One JSON
+line per (solver, path), then one line with the card it ran on.
 
-    python profiles/bench_leastnorm.py [--N 215] [--itmax 100] [--reps 3] [--out FILE]
+    python profiles/bench_leastnorm.py [--N 215] [--itmax 100] [--reps 3] [--solvers craig,craigmr,lnlq,cgne,crmr]
+                                       [--out FILE]
 
 Workload, assembled on the GPU (A^T is formed once by the library, outside the timed solves): the divergence D = G^T of
 the N^3 grid (problems.div_csr; N = 215: m = 9 938 375 rows, n = 29 676 450 columns, 59 352 900 nonzeros) and
 b = D cos(0, 1, ..., n - 1), a consistent system whose least-norm solution is the Helmholtz projection of the cosine
 field.  All tolerances are 0 (CRAIG: btol = 0 and conlim = 0, so ctol = 0; LNLQ: σ = 0 and utolx = utoly = 0) so that
 every solve runs itmax iterations; a warm-up solve with history checks that it does.  An LNLQ iteration is one pass of
-its loop (lnlq! reports niter = passes + 1).
+its loop (lnlq! reports niter = passes + 1).  CGNE and CRMR take no tolerance of their own.
 """
 import argparse
 import json
@@ -36,10 +37,16 @@ def bytes_per_iteration(solver, m, n, nnz, v=8):
     """Algorithmic bytes of one fused iteration (DESIGN.md section 3f, SURVEY 8d counting): each product streams its
     matrix and row pointers once; every vector is counted once per read and once per write.
     CRAIG: C1 on A^T (m + 4n)v, C2 on A (n + 6m)v.  CRAIGMR: R1 on A (n + 2m)v, R2 on A^T (m + 6n)v, R3 7m v.
-    LNLQ: L1 on A (n + 6m)v, L2 on A^T (m + 4n)v: the same total as CRAIG."""
+    LNLQ: L1 on A (n + 6m)v, L2 on A^T (m + 4n)v: the same total as CRAIG.
+    CGNE (section 3h): E1 on A (n + 2m)v, E2 on A^T (m + 4n)v.  CRMR: R1 on A (n + m)v, R2 3m v, R3 on A^T (m + 4n)v,
+    R4 3n v: CGLS's model."""
     mats = matrix_bytes(m, nnz) + matrix_bytes(n, nnz)
     if solver in ("craig", "lnlq"):
         return mats + (5 * n + 7 * m) * v
+    if solver == "cgne":
+        return mats + (5 * n + 3 * m) * v
+    if solver == "crmr":
+        return mats + (8 * n + 5 * m) * v
     return mats + (7 * n + 10 * m) * v
 
 
@@ -54,6 +61,7 @@ def main():
     ap.add_argument("--N", type=int, default=215)
     ap.add_argument("--itmax", type=int, default=100)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--solvers", default="craig,craigmr,lnlq,cgne,crmr")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -67,8 +75,8 @@ def main():
     del z, rows
     work = f"div({a.N}) = grad({a.N})^T f64, m={m} n={n} nnz={nnz}, b = D cos(0:n-1), {a.itmax} iterations/solve"
     lines = []
-    for solver in ("craig", "craigmr", "lnlq"):
-        extra = {"craig": {"btol": 0.0, "conlim": 0.0}, "craigmr": {}, "lnlq": {"utolx": 0.0, "utoly": 0.0}}[solver]
+    for solver in a.solvers.split(","):
+        extra = {"craig": {"btol": 0.0, "conlim": 0.0}, "lnlq": {"utolx": 0.0, "utoly": 0.0}}.get(solver, {})
         kw = dict(atol=0.0, rtol=0.0, itmax=a.itmax, **extra)
         niter = a.itmax + (solver == "lnlq")     # lnlq! counts one more than its passes
         ws = kb.krylov_workspace(solver, m, n, np.float64, device="cuda")
