@@ -39,6 +39,7 @@ struct CsrAny {
 struct Handle {
   int solver = 0, dtype = 1, device_kind = 0;
   bool block = false;                  // ws is a BlockWorkspace (krylov_block_* entry points)
+  const SolverInfo* info = nullptr;    // single-RHS handles: the solver's row (kb_internal.h)
   int p = 0;
   void* ws = nullptr;
   std::shared_ptr<CsrAny> csr;
@@ -76,13 +77,6 @@ int fail(const char* where, const char* msg) {
   return -1;
 }
 
-bool supported_solver(int s) {
-  return s == S_CG || s == S_MINRES || s == S_GMRES || s == S_BICGSTAB || s == S_FOM || s == S_FGMRES || s == S_CGS ||
-         s == S_CG_LANCZOS || s == S_CR || s == S_DIOM || s == S_DQGMRES || s == S_LSQR || s == S_LSMR ||
-         s == S_LSLQ || s == S_CGLS || s == S_CRLS || s == S_BILQ || s == S_QMR || s == S_CAR || s == S_MINARES ||
-         s == S_BILQR || s == S_TRILQR || s == S_CRAIG || s == S_CRAIGMR || s == S_LNLQ || s == S_CGNE || s == S_CRMR;
-}
-
 int pick_device() {
   int cnt = 0;
   if (cudaGetDeviceCount(&cnt) != cudaSuccess || cnt <= 0) {
@@ -114,10 +108,6 @@ int m_of(Handle* h) {
   if (h->block) return n_of(h);
   return h->dtype == KRYLOV_FLOAT64 ? W<double>(h)->m : W<float>(h)->m;
 }
-bool is_ls(const Handle* h) { return !h->block && is_ls_kind(h->solver); }
-bool is_cg_ls(int s) { return s == S_CGLS || s == S_CRLS; }     // CGLS / CRLS: M on the residual space, no N
-bool is_biorth(int s) { return s == S_BILQ || s == S_QMR; }      // BiLQ / QMR: square, apply A and its adjoint
-bool is_adjoint(const Handle* h) { return !h->block && is_adjoint_kind(h->solver); }   // BiLQR / TriLQR: x and y
 template <class T> Csr<T>& csr_of(CsrAny& a);
 template <> Csr<double>& csr_of<double>(CsrAny& a) { return a.d; }
 template <> Csr<float>& csr_of<float>(CsrAny& a) { return a.f; }
@@ -141,12 +131,12 @@ template <class T> void destroy_handle(Handle* h) {
   delete h;
 }
 
-// Bring a caller vector of length m (b; c of the square solvers) into a device buffer (host or device, per device_kind).
-template <class T> const T* stage_in(Handle* h, Workspace<T>* ws, const void* src, T*& buf) {
+// Bring a caller vector of len entries (b, c) into a device buffer (host or device, per device_kind).
+template <class T> const T* stage_in(Handle* h, Workspace<T>* ws, const void* src, T*& buf, int len) {
   if (!src) return nullptr;
   if (h->device_kind == KRYLOV_CUDA) return (const T*)src;
-  if (!buf) buf = dev_alloc<T>((size_t)ws->m);
-  KB_CUDA(cudaMemcpyAsync(buf, src, sizeof(T) * (size_t)ws->m, cudaMemcpyHostToDevice, ws->ctx.stream));
+  if (!buf) buf = dev_alloc<T>((size_t)len);
+  KB_CUDA(cudaMemcpyAsync(buf, src, sizeof(T) * (size_t)len, cudaMemcpyHostToDevice, ws->ctx.stream));
   return buf;
 }
 
@@ -167,8 +157,8 @@ template <class T> LinOp<T> make_cb_op(Handle* h, Workspace<T>* ws, KrylovMatvec
 }
 
 // _opts_kw + per-family kwargs (interfaces/src/c_stores.jl:255-260, 288-300 CG,
-// 303-315 MINRES, 334-354 BiCGSTAB, 377-398 GMRES)
-SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
+// 303-315 MINRES, 334-354 BiCGSTAB, 377-398 GMRES): `fields` are the OptField bits the solver takes
+SolveOpts map_opts(const Handle* h, unsigned fields, const KrylovOptions* o) {
   SolveOpts s;
   KrylovOptions d = krylov_default_options();
   if (!o) o = &d;
@@ -177,23 +167,17 @@ SolveOpts map_opts(const Handle* h, const KrylovOptions* o) {
   s.itmax = o->itmax;
   s.verbose = o->verbose;
   s.timemax = std::isnan(o->timemax) ? INFINITY : o->timemax;
-  if (h->solver == S_CG || h->solver == S_CR) { s.radius = o->radius; s.linesearch = o->linesearch != 0; }   // _typed_solve_cg!
-  if (h->solver == S_DIOM || h->solver == S_DQGMRES) s.reorthogonalization = o->reorthogonalization != 0;      // _typed_solve_mn_reorth!
+  if (fields & O_RADIUS) s.radius = o->radius;
+  if (fields & O_LINESEARCH) s.linesearch = o->linesearch != 0;
+  if (fields & O_LAMBDA) s.lambda = o->lambda;
+  if (fields & O_RESTART) s.restart = o->restart != 0;
+  if (fields & O_REORTH) s.reorthogonalization = o->reorthogonalization != 0;
   s.cr_gamma = std::isnan(h->ext.cr_gamma) ? -1 : h->ext.cr_gamma;
-  if (h->solver == S_MINRES) { s.lambda = o->lambda; s.linesearch = o->linesearch != 0; }
-  if (h->solver == S_MINARES) s.lambda = o->lambda;   // _typed_solve_sym_lambda! (CAR: _typed_solve!, M only)
-  if (is_ls_kind(h->solver)) { s.lambda = o->lambda; s.radius = o->radius; }   // _typed_solve_ls_mn_radius! (c_stores.jl:403-423)
-  if (h->solver == S_LSLQ || is_leastnorm_kind(h->solver)) s.radius = 0;   // _typed_solve_ls_mn!: λ and no trust region
-  if (is_normal_ln_kind(h->solver)) s.radius = 0;                          // CGNE / CRMR: λ and N (c_stores.jl:460)
   s.sigma = std::isnan(h->ext.sigma) ? 0 : h->ext.sigma;
   s.utol = std::isnan(h->ext.utol) ? -1 : h->ext.utol;
   s.transfer_to_lsqr = h->ext.transfer_to_lsqr != 0;
   s.transfer_to_bicg = h->ext.transfer_to_bicg != 0;
   s.transfer_to_usymcg = h->ext.transfer_to_bicg != 0;   // TriLQR's kwarg travels in the same field
-  // _typed_solve_gmres! serves GMRES, FGMRES and FOM (c_stores.jl:376-398)
-  if (h->solver == S_GMRES || h->solver == S_FGMRES || h->solver == S_FOM) {
-    s.restart = o->restart != 0; s.reorthogonalization = o->reorthogonalization != 0;
-  }
   s.check_curvature = h->ext.check_curvature != 0;
   s.history = h->ext.history != 0;
   s.ldiv = h->ext.ldiv != 0;
@@ -226,65 +210,91 @@ std::shared_ptr<CsrAny> transpose_any(Ctx& c, CsrAny& src, int rows = 0) {
   return a;
 }
 
-// A^T of the handle's CSR operator, formed once per attached operator and kept on the handle until it changes
-// TriLQR's has max(m, n) rows: its fused T2 pass finishes every row of q (m entries) in the launch over A^T's rows.
+// A^T of the handle's CSR operator, formed once per attached operator and kept on the handle until it changes.
+// For the adjoint pairs (c required) it has max(m, n) rows: TriLQR's fused T2 pass finishes every row of q (m entries)
+// in the launch over A^T's rows.
 template <class T> const Csr<T>* adjoint_csr(Handle* h, Workspace<T>* ws) {
   if (!h->csrT || h->csrT_for != h->csr.get()) {
     h->csrT.reset();
-    h->csrT = transpose_any(ws->ctx, *h->csr, h->solver == S_TRILQR ? std::max(ws->m, ws->n) : 0);
+    h->csrT = transpose_any(ws->ctx, *h->csr, h->info->c == C_REQUIRED_N ? std::max(ws->m, ws->n) : 0);
     h->csrT_for = h->csr.get();
   }
   return &csr_of<T>(*h->csrT);
 }
 
-// lsqr! / lsmr! (c_stores.jl:403-423), cgls! / crls! (_typed_solve_ls_m_radius!): b has m entries, x has n; A maps
-// n -> m and needs its adjoint
+// One solve path for every solver, read from its row S.  The faults are checked in one order: the operator (A, and A^T
+// when the solver applies it), then M and N, then b and c.
 template <class T>
-int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, void* ud,
-                const KrylovOptions* opts) {
+int do_solve(Handle* h, const SolverInfo& S, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN,
+             const void* b, const void* c, void* ud, const KrylovOptions* opts) {
   Workspace<T>* ws = W<T>(h);
   KB_CUDA(cudaSetDevice(ws->ctx.device));
-  SolveOpts so = map_opts(h, opts);
+  SolveOpts so = map_opts(h, S.opts, opts);
   const int m = ws->m, n = ws->n;
-  LinOp<T> A, At;
+  LinOp<T> A, At;              // A maps n -> m, A^T m -> n
   if (fA) {
-    if (!fAt)
-      throw std::runtime_error(is_cg_ls(h->solver)      ? "cgls and crls apply the adjoint of A: matvec_At must be given with matvec_A"
-                             : h->solver == S_LSLQ ? "lslq applies the adjoint of A: matvec_At must be given with matvec_A"
-                             : h->solver == S_CRAIG ? "craig applies the adjoint of A: matvec_At must be given with matvec_A"
-                             : h->solver == S_CRAIGMR ? "craigmr applies the adjoint of A: matvec_At must be given with matvec_A"
-                             : h->solver == S_LNLQ ? "lnlq applies the adjoint of A: matvec_At must be given with matvec_A"
-                             : h->solver == S_CGNE ? "cgne applies the adjoint of A: matvec_At must be given with matvec_A"
-                             : h->solver == S_CRMR ? "crmr applies the adjoint of A: matvec_At must be given with matvec_A"
-                                                   : "lsqr and lsmr apply the adjoint of A: matvec_At must be given with matvec_A");
-    A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
-    At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
+    if (S.adjoint && !fAt)
+      throw std::runtime_error(std::string(S.name) + " applies the adjoint of A: matvec_At must be given with matvec_A");
+    A = make_cb_op<T>(h, ws, fA, ud); A.n = m;
+    if (S.adjoint) { At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; }
+    if (S.rect) { A.nin = n; At.nin = m; }
   } else if (h->csr) {
     const Csr<T>& C = csr_of<T>(*h->csr);
-    if (C.n != m || C.max_col >= n)
-      throw std::runtime_error("CSR operator: size inconsistent with the workspace ((m, n) = (" + std::to_string(m) + ", " +
-                               std::to_string(n) + "), operator rows = " + std::to_string(C.n) + ", largest column = " +
-                               std::to_string(C.max_col) + ")");
+    // columns: n, plus the halo entries of a row-partitioned operator -- anything beyond is an out-of-bounds gather
+    const long long ncols = (long long)n + (ws->dist.world > 1 ? ws->dist.halo.nhalo : 0);
+    if (C.n != m || C.max_col >= ncols)
+      throw std::runtime_error("CSR operator: size or column index inconsistent with the workspace ((m, n) = (" + std::to_string(m) +
+                               ", " + std::to_string(n) + "), operator rows = " + std::to_string(C.n) +
+                               ", largest column = " + std::to_string(C.max_col) + ")");
     A.kind = LinOp<T>::CSR; A.csr = &C; A.n = m;
-    At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = n;
+    if (!S.rect) A.dict = &dict_of<T>(*h->csr);
+    if (S.adjoint) { At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = At.csr->n; }
   } else {
-    throw std::runtime_error("no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr");
+    throw std::runtime_error(S.adjoint ? "no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr"
+                                       : "no operator: pass matvec_A or attach one with krylov_b200_set_operator_csr");
   }
-  LinOp<T> M = make_cb_op<T>(h, ws, fM, ud), N = make_cb_op<T>(h, ws, fN, ud);
-  M.n = m; N.n = n;                      // M acts on the m-dimensional data space, N on the n-dimensional solution space
-  if (is_normal_ln_kind(h->solver)) N.n = m;   // CGNE / CRMR: N acts on the m-dimensional residual space
-  if (!fM && h->Mdiag) { M.kind = LinOp<T>::DIAG; M.diag = (const T*)h->Mdiag; }
-  if (!fN && h->Ndiag) { N.kind = LinOp<T>::DIAG; N.diag = (const T*)h->Ndiag; }
-  // The reference's C layer drops N for CGLS / CRLS; a caller passing one expects it to act, so it is refused.
-  if (is_cg_ls(h->solver) && !N.is_identity())
-    throw std::runtime_error("cgls and crls take no right preconditioner N (M acts on the m-dimensional residual space)");
-  // The reference's C layer drops M for CGNE / CRMR in the same way; N is their only preconditioner.
-  if (is_normal_ln_kind(h->solver) && !M.is_identity())
-    throw std::runtime_error(std::string(h->solver == S_CGNE ? "cgne" : "crmr") +
-                             " takes no preconditioner M: N (on the m-dimensional residual space) is its only preconditioner");
+  // M (which = 0) and N (1) on the spaces the row names: a callback, else an attached diagonal, else block-Jacobi blocks
+  LinOp<T> P[2];
+  for (int w = 0; w < 2; w++) {
+    const PrecondSlot& slot = w == 0 ? S.M : S.N;
+    const KrylovMatvec f = w == 0 ? fM : fN;
+    void* diag = w == 0 ? h->Mdiag : h->Ndiag;
+    if (slot.use == P_REFUSED && (f || diag || h->Pblk[w])) throw std::runtime_error(slot.refusal);
+    P[w] = make_cb_op<T>(h, ws, f, ud);
+    P[w].n = precond_len(S, w, m, n);
+    if (f) continue;
+    if (diag) { P[w].kind = LinOp<T>::DIAG; P[w].diag = (const T*)diag; }
+    else if (h->Pblk[w]) {
+      P[w].kind = LinOp<T>::BDIAG; P[w].blocks = (const T*)h->Pblk[w]; P[w].blocks_inv = (const T*)h->Pblk_inv[w]; P[w].bs = h->Pbs[w];
+    }
+  }
+  const LinOp<T>& M = P[0];
+  const LinOp<T>& N = P[1];
+  if (S.bdiag == BD_REFUSED_AT_SOLVE && (M.kind == LinOp<T>::BDIAG || N.kind == LinOp<T>::BDIAG))
+    throw std::runtime_error(S.bdiag_refusal);
   if (!b) throw std::runtime_error("b is NULL");
-  const T* bd = stage_in<T>(h, ws, b, ws->bbuf);
+  if (S.c == C_REQUIRED_N && !c) throw std::runtime_error(std::string(S.name) + " solves A^T y = c as well: c must be given");
+  const T* bd = stage_in<T>(h, ws, b, ws->bbuf, m);
+  const T* cd = S.c == C_NONE ? nullptr : stage_in<T>(h, ws, c, ws->cbuf, S.c == C_REQUIRED_N ? n : m);
+  dist_check_alive(ws->ctx);             // row-partitioned: refuse to start on a dead communicator
   switch (h->solver) {
+    case S_CG: cg_solve<T>(*ws, A, bd, M, so); break;
+    case S_MINRES: minres_solve<T>(*ws, A, bd, M, so); break;
+    case S_GMRES: gmres_solve<T>(*ws, A, bd, M, N, so); break;
+    case S_FOM: fom_solve<T>(*ws, A, bd, M, N, so); break;
+    case S_FGMRES: fgmres_solve<T>(*ws, A, bd, M, N, so); break;
+    case S_CG_LANCZOS: cg_lanczos_solve<T>(*ws, A, bd, M, so); break;
+    case S_CR: cr_solve<T>(*ws, A, bd, M, so); break;
+    case S_CAR: car_solve<T>(*ws, A, bd, M, so); break;
+    case S_MINARES: minares_solve<T>(*ws, A, bd, M, so); break;
+    case S_DQGMRES: dqgmres_solve<T>(*ws, A, bd, M, N, so); break;
+    case S_DIOM: diom_solve<T>(*ws, A, bd, M, N, so); break;
+    case S_CGS: cgs_solve<T>(*ws, A, bd, cd, M, N, so); break;
+    case S_BICGSTAB: bicgstab_solve<T>(*ws, A, bd, cd, M, N, so); break;
+    case S_BILQ: bilq_solve<T>(*ws, A, At, bd, cd, M, N, so); break;
+    case S_QMR: qmr_solve<T>(*ws, A, At, bd, cd, M, N, so); break;
+    case S_BILQR: bilqr_solve<T>(*ws, A, At, bd, cd, so); break;
+    case S_TRILQR: trilqr_solve<T>(*ws, A, At, bd, cd, so); break;
     case S_LSQR: lsqr_solve<T>(*ws, A, At, bd, M, N, so); break;
     case S_LSMR: lsmr_solve<T>(*ws, A, At, bd, M, N, so); break;
     case S_LSLQ: lslq_solve<T>(*ws, A, At, bd, M, N, so); break;
@@ -296,124 +306,7 @@ int do_solve_ls(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, K
     case S_CGNE: cgne_solve<T>(*ws, A, At, bd, N, so); break;
     case S_CRMR: crmr_solve<T>(*ws, A, At, bd, N, so); break;
   }
-  return 0;
-}
-
-template <class T>
-int do_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, const void* c,
-             void* ud, const KrylovOptions* opts) {
-  Workspace<T>* ws = W<T>(h);
-  KB_CUDA(cudaSetDevice(ws->ctx.device));
-  SolveOpts so = map_opts(h, opts);
-  LinOp<T> A;
-  if (fA) A = make_cb_op<T>(h, ws, fA, ud);
-  else if (h->csr) {
-    A.kind = LinOp<T>::CSR; A.csr = &csr_of<T>(*h->csr); A.dict = &dict_of<T>(*h->csr); A.n = ws->n;
-    // columns: n local ones plus, row-partitioned, the halo entries -- anything beyond is an out-of-bounds gather
-    const long long ncols = (long long)ws->n + (ws->dist.world > 1 ? ws->dist.halo.nhalo : 0);
-    if (A.csr->n != ws->n || A.csr->max_col >= ncols)
-      throw std::runtime_error("CSR operator: size or column index inconsistent with the workspace (n = " + std::to_string(ws->n) +
-                               ", operator rows = " + std::to_string(A.csr->n) + ", largest column = " + std::to_string(A.csr->max_col) + ")");
-  }
-  else throw std::runtime_error("no operator: pass matvec_A or attach one with krylov_b200_set_operator_csr");
-  if (A.kind == LinOp<T>::CSR && A.csr->n != ws->n) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
-  LinOp<T> M = make_cb_op<T>(h, ws, fM, ud), N = make_cb_op<T>(h, ws, fN, ud);
-  if (!fM && h->Mdiag) { M.kind = LinOp<T>::DIAG; M.diag = (const T*)h->Mdiag; }
-  if (!fN && h->Ndiag) { N.kind = LinOp<T>::DIAG; N.diag = (const T*)h->Ndiag; }
-  if (!fM && !h->Mdiag && h->Pblk[0]) { M.kind = LinOp<T>::BDIAG; M.blocks = (const T*)h->Pblk[0]; M.blocks_inv = (const T*)h->Pblk_inv[0]; M.bs = h->Pbs[0]; M.n = ws->n; }
-  if (!fN && !h->Ndiag && h->Pblk[1]) { N.kind = LinOp<T>::BDIAG; N.blocks = (const T*)h->Pblk[1]; N.blocks_inv = (const T*)h->Pblk_inv[1]; N.bs = h->Pbs[1]; N.n = ws->n; }
-  if (!b) throw std::runtime_error("b is NULL");
-  const T* bd = stage_in<T>(h, ws, b, ws->bbuf);
-  dist_check_alive(ws->ctx);             // row-partitioned: refuse to start on a dead communicator
-  switch (h->solver) {
-    case S_CG: cg_solve<T>(*ws, A, bd, M, so); break;
-    case S_MINRES: minres_solve<T>(*ws, A, bd, M, so); break;
-    case S_GMRES: gmres_solve<T>(*ws, A, bd, M, N, so); break;
-    case S_FOM: fom_solve<T>(*ws, A, bd, M, N, so); break;
-    case S_FGMRES: fgmres_solve<T>(*ws, A, bd, M, N, so); break;
-    case S_CG_LANCZOS: cg_lanczos_solve<T>(*ws, A, bd, M, so); break;
-    case S_CR: cr_solve<T>(*ws, A, bd, M, so); break;
-    case S_CAR: case S_MINARES:
-      // the reference's C layer drops N for both; a caller passing one expects it to act, so it is refused
-      if (!N.is_identity())
-        throw std::runtime_error("car and minares take no right preconditioner N (matvec_N): only M, and for minares none");
-      if (h->solver == S_CAR) car_solve<T>(*ws, A, bd, M, so);
-      else minares_solve<T>(*ws, A, bd, M, so);
-      break;
-    case S_DQGMRES: dqgmres_solve<T>(*ws, A, bd, M, N, so); break;
-    case S_DIOM: diom_solve<T>(*ws, A, bd, M, N, so); break;
-    case S_CGS: {
-      const T* cd = stage_in<T>(h, ws, c, ws->cbuf);
-      cgs_solve<T>(*ws, A, bd, cd, M, N, so);
-      break;
-    }
-    case S_BICGSTAB: {
-      // the reference's C layer never forwards `c` for BiCGSTAB (c = b); we accept it when given
-      const T* cd = stage_in<T>(h, ws, c, ws->cbuf);
-      bicgstab_solve<T>(*ws, A, bd, cd, M, N, so);
-      break;
-    }
-    case S_BILQ: case S_QMR: {
-      // the adjoint: matvec_At with matvec_A, else the cached transpose of the CSR operator
-      LinOp<T> At;
-      if (fA) {
-        if (!fAt) throw std::runtime_error("bilq and qmr apply the adjoint of A: matvec_At must be given with matvec_A");
-        At = make_cb_op<T>(h, ws, fAt, ud);
-      } else {
-        At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = ws->n;
-      }
-      if (M.kind == LinOp<T>::BDIAG || N.kind == LinOp<T>::BDIAG)
-        throw std::runtime_error("bilq and qmr apply M^H and N^H: block-Jacobi preconditioners are not available for them");
-      // like BiCGSTAB's, `c` is accepted when given (the reference's C layer never forwards it: c = b)
-      const T* cd = stage_in<T>(h, ws, c, ws->cbuf);
-      if (h->solver == S_BILQ) bilq_solve<T>(*ws, A, At, bd, cd, M, N, so);
-      else qmr_solve<T>(*ws, A, At, bd, cd, M, N, so);
-      break;
-    }
-  }
   dist_check_alive(ws->ctx);             // a reduction timed out during the solve: raise instead of returning NaNs
-  return 0;
-}
-
-// bilqr! / trilqr!: x (n entries) solves A x = b and y (m entries) solves A^T y = c; b has m entries, c has n.  A maps
-// n -> m (square for BiLQR) and needs its adjoint.  Neither solver takes a preconditioner.
-template <class T>
-int do_solve_adjoint(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, KrylovMatvec fN, const void* b, const void* c,
-                     void* ud, const KrylovOptions* opts) {
-  Workspace<T>* ws = W<T>(h);
-  const char* name = h->solver == S_BILQR ? "bilqr" : "trilqr";
-  if (fM || fN || h->Mdiag || h->Ndiag || h->Pblk[0] || h->Pblk[1])
-    throw std::runtime_error(std::string(name) + " takes no preconditioner (matvec_M, matvec_N or an attached M / N)");
-  if (!b) throw std::runtime_error("b is NULL");
-  if (!c) throw std::runtime_error(std::string(name) + " solves A^T y = c as well: c must be given");
-  KB_CUDA(cudaSetDevice(ws->ctx.device));
-  SolveOpts so = map_opts(h, opts);
-  const int m = ws->m, n = ws->n;
-  LinOp<T> A, At;
-  if (fA) {
-    if (!fAt) throw std::runtime_error(std::string(name) + " applies the adjoint of A: matvec_At must be given with matvec_A");
-    A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
-    At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m;
-  } else if (h->csr) {
-    const Csr<T>& C = csr_of<T>(*h->csr);
-    if (C.n != m || C.max_col >= n)
-      throw std::runtime_error("CSR operator: size inconsistent with the workspace ((m, n) = (" + std::to_string(m) + ", " +
-                               std::to_string(n) + "), operator rows = " + std::to_string(C.n) + ", largest column = " +
-                               std::to_string(C.max_col) + ")");
-    A.kind = LinOp<T>::CSR; A.csr = &C; A.n = m;
-    At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = At.csr->n;
-  } else {
-    throw std::runtime_error("no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr");
-  }
-  const T* bd = stage_in<T>(h, ws, b, ws->bbuf);                 // m entries
-  const T* cd = (const T*)c;                                     // n entries
-  if (h->device_kind != KRYLOV_CUDA) {
-    if (!ws->cbuf) ws->cbuf = dev_alloc<T>((size_t)n);
-    KB_CUDA(cudaMemcpyAsync(ws->cbuf, c, sizeof(T) * (size_t)n, cudaMemcpyHostToDevice, ws->ctx.stream));
-    cd = ws->cbuf;
-  }
-  if (h->solver == S_BILQR) bilqr_solve<T>(*ws, A, At, bd, cd, so);
-  else trilqr_solve<T>(*ws, A, At, bd, cd, so);
   return 0;
 }
 
@@ -461,18 +354,10 @@ template <class T> int do_get_x(Handle* h, void* x, int n) {
 
 template <class T> int do_warm_start(Handle* h, const void* x0, int n) {
   Workspace<T>* ws = W<T>(h);
-  if (is_adjoint_kind(h->solver))
-    throw std::runtime_error(std::string(h->solver == S_BILQR ? "bilqr" : "trilqr") +
-                             " solves two systems: warm-start it with krylov_warm_start2 (x0 and y0)");
-  if (is_ls_kind(h->solver))
-    throw std::runtime_error(is_cg_ls(h->solver)      ? "cgls and crls do not support warm-start (they take no x0)"
-                             : h->solver == S_LSLQ ? "lslq does not support warm-start (it takes no x0)"
-                             : h->solver == S_CRAIG ? "craig does not support warm-start (it takes no x0)"
-                             : h->solver == S_CRAIGMR ? "craigmr does not support warm-start (it takes no x0)"
-                             : h->solver == S_LNLQ ? "lnlq does not support warm-start (it takes no x0)"
-                             : h->solver == S_CGNE ? "cgne does not support warm-start (it takes no x0)"
-                             : h->solver == S_CRMR ? "crmr does not support warm-start (it takes no x0)"
-                                                 : "lsqr and lsmr do not support warm-start (they take no x0)");
+  if (h->info->warm == WARM_X0_Y0)
+    throw std::runtime_error(std::string(h->info->name) + " solves two systems: warm-start it with krylov_warm_start2 (x0 and y0)");
+  if (h->info->warm == WARM_NONE)
+    throw std::runtime_error(std::string(h->info->name) + " does not support warm-start (it takes no x0)");
   if (n != ws->n) throw std::runtime_error("x0 should have size n");
   KB_CUDA(cudaSetDevice(ws->ctx.device));
   // c_stores.jl:218-229: allocate dx if empty, copy, set the flag
@@ -508,8 +393,9 @@ template <class T> void* vec_by_name(Workspace<T>* ws, const char* nm) {
   if (ws->kind == S_CGNE && !strcmp(nm, "Aᴴz")) return ws->Ar;   // CgneWorkspace (the fused path leaves Aᴴz and q unwritten)
   if (ws->kind == S_CRMR && !strcmp(nm, "Aᴴr")) return ws->Ar;   // CrmrWorkspace
   if (ws->kind == S_CRMR && !strcmp(nm, "Nq")) return ws->z;
-  if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ || is_adjoint_kind(ws->kind) ? ws->w : nullptr;
-  if (is_adjoint_kind(ws->kind)) {                 // BilqrWorkspace / TrilqrWorkspace (w_{k-3} / w_{k-2} rotate by pointer)
+  const bool pair = ws->kind == S_BILQR || ws->kind == S_TRILQR;
+  if (!strcmp(nm, "d̅") || !strcmp(nm, "dbar")) return ws->kind == S_BILQ || pair ? ws->w : nullptr;
+  if (pair) {                 // BilqrWorkspace / TrilqrWorkspace (w_{k-3} / w_{k-2} rotate by pointer)
     if (!strcmp(nm, "y") || !strcmp(nm, "t")) return ws->y;
     if (!strcmp(nm, "Δx")) return ws->dx;
     if (!strcmp(nm, "Δy") || !strcmp(nm, "dy")) return ws->dy;
@@ -538,14 +424,15 @@ extern "C" {
 int krylov_workspace_create(KrylovSolverType solver, int m, int n, KrylovDataType dtype, KrylovDeviceType device,
                             const KrylovWorkspaceOptions* wopts, void** ws_out) {
   try {
-    if (!supported_solver((int)solver) || (dtype != KRYLOV_FLOAT32 && dtype != KRYLOV_FLOAT64)) return -2;
+    const SolverInfo* info = solver_info((int)solver);
+    if (!info || (dtype != KRYLOV_FLOAT32 && dtype != KRYLOV_FLOAT64)) return -2;
     if (device != KRYLOV_CPU && device != KRYLOV_CUDA) return fail("krylov_workspace_create", "unknown device");
     if (!ws_out) return fail("krylov_workspace_create", "ws_out is NULL");
     if (m < 0 || n < 0) return fail("krylov_workspace_create", "negative dimension");
     const int dev = pick_device();
     const int memory = wopts ? wopts->memory : 0, window = wopts ? wopts->window : 0;   // 0 -> 20 / 5 (c_stores.jl:1799-1800)
     Handle* h = new Handle();
-    h->solver = (int)solver; h->dtype = (int)dtype; h->device_kind = (int)device;
+    h->solver = (int)solver; h->info = info; h->dtype = (int)dtype; h->device_kind = (int)device;
     h->ext = krylov_b200_default_options();
     try {
       if (dtype == KRYLOV_FLOAT64) h->ws = ws_create<double>((SolverKind)solver, m, n, memory, window, dev);
@@ -580,14 +467,8 @@ int krylov_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, Krylov
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_solve", "unknown workspace handle");
-    if (is_adjoint(h))
-      return h->dtype == KRYLOV_FLOAT64 ? do_solve_adjoint<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts)
-                                        : do_solve_adjoint<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts);
-    if (is_ls(h))                    // the square solvers never apply the adjoint
-      return h->dtype == KRYLOV_FLOAT64 ? do_solve_ls<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts)
-                                        : do_solve_ls<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, userdata, opts);
-    return h->dtype == KRYLOV_FLOAT64 ? do_solve<double>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts)
-                                      : do_solve<float>(h, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts);
+    return h->dtype == KRYLOV_FLOAT64 ? do_solve<double>(h, *h->info, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts)
+                                      : do_solve<float>(h, *h->info, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts);
   } catch (const std::exception& e) { return fail("krylov_solve", e); }
 }
 
@@ -603,8 +484,7 @@ int krylov_get_y(void* ws, void* y, int m) {
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_get_y", "unknown workspace handle");
-    // solution_count (c_stores.jl:211-216) is 2 for BiLQR, TriLQR, CRAIG, CRAIGMR and LNLQ only
-    if (!is_adjoint(h) && !is_leastnorm_kind(h->solver)) return -2;
+    if (h->info->nsol != 2) return -2;   // solution_count (c_stores.jl:211-216)
     if (!y) return fail("krylov_get_y", "y is NULL");
     return h->dtype == KRYLOV_FLOAT64 ? do_get_y<double>(h, y, m) : do_get_y<float>(h, y, m);
   } catch (const std::exception& e) { return fail("krylov_get_y", e); }
@@ -626,7 +506,7 @@ int krylov_warm_start2(void* ws, const void* x0, const void* y0, int nx, int ny)
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_warm_start2", "unknown workspace handle");
-    if (!is_adjoint(h)) return -2;
+    if (h->info->warm != WARM_X0_Y0) return -2;
     return h->dtype == KRYLOV_FLOAT64 ? do_warm_start2<double>(h, x0, y0, nx, ny) : do_warm_start2<float>(h, x0, y0, nx, ny);
   } catch (const std::exception& e) { return fail("krylov_warm_start2", e); }
 }
@@ -717,10 +597,7 @@ template <class T> int do_block_solve(Handle* h, KrylovBlockMatvec fA, KrylovBlo
                                       void* ud, const KrylovOptions* opts) {
   BlockWorkspace<T>* ws = BW<T>(h);
   KB_CUDA(cudaSetDevice(ws->ctx.device));
-  SolveOpts so = map_opts(h, opts);
-  KrylovOptions d = krylov_default_options();
-  const KrylovOptions* o = opts ? opts : &d;
-  so.restart = o->restart != 0; so.reorthogonalization = o->reorthogonalization != 0;
+  SolveOpts so = map_opts(h, O_RESTART | O_REORTH, opts);
   BlockOp<T> A = make_block_cb<T>(h, fA, ud);
   if (!fA) {
     if (!h->csr) throw std::runtime_error("no operator: pass matvec_A or attach one with krylov_b200_set_operator_csr");
@@ -820,7 +697,7 @@ int krylov_b200_set_operator_csr(void* ws, int n, long long nnz, const void* row
     KB_CUDA(cudaSetDevice(cx.device));
     // n: number of rows (m of a least-squares workspace, whose operator has the workspace's n columns)
     if (n != m_of(h)) throw std::runtime_error("(workspace.m, workspace.n) is inconsistent with size(A)");
-    const int ncols = is_ls(h) || (!h->block && h->solver == S_TRILQR) ? n_of(h) : -1;
+    const int ncols = h->info && h->info->rect ? n_of(h) : -1;
     if (h->dtype == KRYLOV_FLOAT64)
       csr_upload<double>(cx, a->d, n, nnz, rowptr, colind, (const double*)values, index_base, index_bytes, location != 0, ncols, &a->dd);
     else
@@ -857,8 +734,7 @@ int krylov_b200_set_preconditioner_diag(void* ws, int which, const void* d, int 
     void*& slot = which == 0 ? h->Mdiag : h->Ndiag;
     if (!d) { dev_free(slot); slot = nullptr; return 0; }
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
-    // least squares: M has m entries, N has n; CGNE / CRMR: N acts on the residual space and has m entries
-    const int n = which == 0 || (!h->block && is_normal_ln_kind(h->solver)) ? m_of(h) : n_of(h);
+    const int n = h->info ? precond_len(*h->info, which, m_of(h), n_of(h)) : n_of(h);
     KB_CUDA(cudaSetDevice(ctx_of(h).device));
     if (!slot) slot = dev_alloc<char>(esz * (size_t)n);
     KB_CUDA(cudaMemcpy(slot, d, esz * (size_t)n, location ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
@@ -876,7 +752,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
     h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0;
     if (!blocks) return 0;
-    if (is_ls(h)) return fail("krylov_b200_set_preconditioner_blockdiag", "not available on least-squares (LSQR, LSMR, CGLS, CRLS) or least-norm (CRAIG, CRAIGMR, LNLQ, CGNE, CRMR) workspaces");
+    if (h->info->bdiag == BD_REFUSED_AT_ATTACH) return fail("krylov_b200_set_preconditioner_blockdiag", h->info->bdiag_refusal);
     if (bs < 2 || bs > 8) return fail("krylov_b200_set_preconditioner_blockdiag", "block size must be in 2..8");
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
     const int n = n_of(h);
@@ -1103,12 +979,7 @@ int krylov_b200_dist_init(void* ws, int rank, int world, int nhalo, const int* h
   try {
     Handle* h = lookup(ws);
     if (!h) return fail("krylov_b200_dist_init", "unknown workspace handle");
-    if (is_ls(h)) return fail("krylov_b200_dist_init", "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) and least-norm (CRAIG, CRAIGMR, LNLQ, CGNE, CRMR) solves are not available");
-    if (is_biorth(h->solver))        // A^T of a row block needs the column halo of A, not its row halo
-      return fail("krylov_b200_dist_init", "row-partitioned BiLQ / QMR solves are not available");
-    if (h->solver == S_CAR || h->solver == S_MINARES)
-      return fail("krylov_b200_dist_init", "row-partitioned CAR / MINARES solves are not available");
-    if (is_adjoint(h)) return fail("krylov_b200_dist_init", "row-partitioned BiLQR / TriLQR solves are not available");
+    if (h->info->dist) return fail("krylov_b200_dist_init", h->info->dist);
     return h->dtype == KRYLOV_FLOAT64 ? dist_init_t<double>(h, rank, world, nhalo, halo_rank, halo_off)
                                       : dist_init_t<float>(h, rank, world, nhalo, halo_rank, halo_off);
   } catch (const std::exception& e) { return fail("krylov_b200_dist_init", e); }

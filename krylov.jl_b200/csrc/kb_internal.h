@@ -218,19 +218,110 @@ struct Stats {
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
                   S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_TRILQR = 18, S_BILQR = 19, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
                   S_CGNE = 26, S_CRMR = 27, S_CRAIG = 28, S_CRAIGMR = 29, S_LNLQ = 30, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
-// the least-squares and least-norm solvers: A is m x n, b has m entries and x has n
-inline bool is_ls_kind(int k) {
-  return k == S_LSLQ || k == S_LSQR || k == S_LSMR || k == S_CGLS || k == S_CRLS || k == S_CRAIG || k == S_CRAIGMR ||
-         k == S_LNLQ || k == S_CGNE || k == S_CRMR;
+// The interface facts of each solver the C ABI serves, one row per SolverKind (capi.cu reads them; ws_create `rect`).
+enum PrecondUse : unsigned char {
+  P_ON_N,        // takes the preconditioner on the n-dimensional space (the square solvers: n = m)
+  P_ON_M,        // takes it on the m-dimensional space
+  P_IGNORED,     // accepted and not applied, as the reference's C layer does
+  P_REFUSED      // refused with the row's text
+};
+struct PrecondSlot { PrecondUse use; const char* refusal; };
+enum BdiagRule : unsigned char { BD_TAKES, BD_REFUSED_AT_ATTACH, BD_REFUSED_AT_SOLVE };
+enum CRule : unsigned char {
+  C_NONE,            // c is ignored
+  C_OPTIONAL_M,      // c has m entries; nullptr: c = b
+  C_REQUIRED_N       // the adjoint system A^T y = c: c has n entries (and A^T, cached, max(m, n) rows)
+};
+enum WarmRule : unsigned char { WARM_X0, WARM_X0_Y0, WARM_NONE };
+// the KrylovOptions fields that reach SolveOpts
+enum OptField : unsigned { O_RADIUS = 1, O_LINESEARCH = 2, O_LAMBDA = 4, O_RESTART = 8, O_REORTH = 16 };
+struct SolverInfo {
+  const char* name;
+  bool rect;                 // A is m x n (b has m entries, x n); else m == n
+  bool adjoint;              // applies A^T: matvec_At, or the cached transpose of the CSR operator
+  PrecondSlot M, N;
+  BdiagRule bdiag;           // block-Jacobi M / N
+  const char* bdiag_refusal;
+  CRule c;
+  int nsol;                  // 2: krylov_get_y returns y (m entries)
+  WarmRule warm;
+  const char* dist;          // nullptr: row-partitioned solves are available; else the refusal of krylov_b200_dist_init
+  unsigned opts;             // OptField bits
+};
+
+constexpr PrecondSlot kOnN{P_ON_N, nullptr}, kOnM{P_ON_M, nullptr}, kIgnored{P_IGNORED, nullptr};
+constexpr const char* kLsqBdiag =
+    "not available on least-squares (LSQR, LSMR, CGLS, CRLS) or least-norm (CRAIG, CRAIGMR, LNLQ, CGNE, CRMR) workspaces";
+constexpr const char* kLsqDist = "row-partitioned least-squares (LSQR, LSMR, CGLS, CRLS) and least-norm (CRAIG, CRAIGMR, "
+                                 "LNLQ, CGNE, CRMR) solves are not available";
+constexpr PrecondSlot kNoNLs{P_REFUSED, "cgls and crls take no right preconditioner N (M acts on the m-dimensional residual space)"};
+constexpr PrecondSlot kNoNCar{P_REFUSED, "car and minares take no right preconditioner N (matvec_N): only M, and for minares none"};
+constexpr const char* kCarDist = "row-partitioned CAR / MINARES solves are not available";
+constexpr const char* kBiorthBdiag = "bilq and qmr apply M^H and N^H: block-Jacobi preconditioners are not available for them";
+constexpr const char* kBiorthDist = "row-partitioned BiLQ / QMR solves are not available";
+constexpr const char* kAdjointDist = "row-partitioned BiLQR / TriLQR solves are not available";
+constexpr const char* kNoPBilqr = "bilqr takes no preconditioner (matvec_M, matvec_N or an attached M / N)";
+constexpr const char* kNoPTrilqr = "trilqr takes no preconditioner (matvec_M, matvec_N or an attached M / N)";
+constexpr const char* kNoMCgne = "cgne takes no preconditioner M: N (on the m-dimensional residual space) is its only preconditioner";
+constexpr const char* kNoMCrmr = "crmr takes no preconditioner M: N (on the m-dimensional residual space) is its only preconditioner";
+
+// Indexed by SolverKind; the last row is S_CG_LANCZOS.  Rows without a name: ids the library does not serve.
+inline constexpr SolverInfo kSolvers[] = {
+  // name, rect, adjoint, M, N, bdiag, bdiag_refusal, c, nsol, warm, dist, opts
+  {"cg",         false, false, kOnN,    kIgnored, BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_RADIUS | O_LINESEARCH},
+  {"cr",         false, false, kOnN,    kIgnored, BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_RADIUS | O_LINESEARCH},
+  {},                                                                                                  // 2 SYMMLQ
+  {"minres",     false, false, kOnN,    kIgnored, BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_LAMBDA | O_LINESEARCH},
+  {},                                                                                                  // 4 MINRES-QLP
+  {"diom",       false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_REORTH},
+  {"dqgmres",    false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_REORTH},
+  {"fom",        false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_RESTART | O_REORTH},
+  {"gmres",      false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_RESTART | O_REORTH},
+  {"fgmres",     false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, O_RESTART | O_REORTH},
+  // BiCGSTAB, CGS, BiLQ and QMR accept c when given; the reference's C layer never forwards it (c = b)
+  {"bicgstab",   false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_OPTIONAL_M, 1, WARM_X0, nullptr, 0},
+  {"cgs",        false, false, kOnN,    kOnN,     BD_TAKES, nullptr, C_OPTIONAL_M, 1, WARM_X0, nullptr, 0},
+  // A^T of a row block needs the column halo of A, not its row halo
+  {"bilq",       false, true,  kOnN,    kOnN,     BD_REFUSED_AT_SOLVE, kBiorthBdiag, C_OPTIONAL_M, 1, WARM_X0, kBiorthDist, 0},
+  {"qmr",        false, true,  kOnN,    kOnN,     BD_REFUSED_AT_SOLVE, kBiorthBdiag, C_OPTIONAL_M, 1, WARM_X0, kBiorthDist, 0},
+  {}, {}, {}, {},                                                                                      // 14-17 USYMLQ, USYMQR, TriCG, TriMR
+  {"trilqr",     true,  true,  {P_REFUSED, kNoPTrilqr}, {P_REFUSED, kNoPTrilqr}, BD_REFUSED_AT_SOLVE, kNoPTrilqr,
+                 C_REQUIRED_N, 2, WARM_X0_Y0, kAdjointDist, 0},
+  {"bilqr",      false, true,  {P_REFUSED, kNoPBilqr}, {P_REFUSED, kNoPBilqr}, BD_REFUSED_AT_SOLVE, kNoPBilqr,
+                 C_REQUIRED_N, 2, WARM_X0_Y0, kAdjointDist, 0},
+  {"lslq",       true,  true,  kOnM,    kOnN,     BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA},
+  {"lsqr",       true,  true,  kOnM,    kOnN,     BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA | O_RADIUS},
+  {"lsmr",       true,  true,  kOnM,    kOnN,     BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA | O_RADIUS},
+  {},                                                                                                  // 23 USYMLQR
+  // the reference's C layer drops N for CGLS / CRLS; a caller passing one expects it to act, so it is refused
+  {"cgls",       true,  true,  kOnM,    kNoNLs,   BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA | O_RADIUS},
+  {"crls",       true,  true,  kOnM,    kNoNLs,   BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA | O_RADIUS},
+  // CGNE / CRMR: CG and CR on A A^T y = b with x = A^T y; the C layer drops M in the same way, N (on the m-dimensional
+  // residual space) is their only preconditioner
+  {"cgne",       true,  true,  {P_REFUSED, kNoMCgne}, kOnM, BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA},
+  {"crmr",       true,  true,  {P_REFUSED, kNoMCrmr}, kOnM, BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 1, WARM_NONE, kLsqDist, O_LAMBDA},
+  // the least-norm solvers: min ||x|| subject to A x = b, x = A^T y; they return the multipliers y too
+  {"craig",      true,  true,  kOnM,    kOnN,     BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 2, WARM_NONE, kLsqDist, O_LAMBDA},
+  {"craigmr",    true,  true,  kOnM,    kOnN,     BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 2, WARM_NONE, kLsqDist, O_LAMBDA},
+  {"lnlq",       true,  true,  kOnM,    kOnN,     BD_REFUSED_AT_ATTACH, kLsqBdiag, C_NONE, 2, WARM_NONE, kLsqDist, O_LAMBDA},
+  {},                                                                                                  // 31 GPMR
+  // the reference's C layer drops N for CAR and MINARES; it is refused as for CGLS.  MINARES's driver refuses M.
+  {"car",        false, false, kOnN,    kNoNCar,  BD_TAKES, nullptr, C_NONE, 1, WARM_X0, kCarDist, 0},
+  {"minares",    false, false, kOnN,    kNoNCar,  BD_TAKES, nullptr, C_NONE, 1, WARM_X0, kCarDist, O_LAMBDA},
+  {"cg_lanczos", false, false, kOnN,    kIgnored, BD_TAKES, nullptr, C_NONE, 1, WARM_X0, nullptr, 0},
+};
+constexpr int kSolverRows = sizeof(kSolvers) / sizeof(kSolvers[0]);
+static_assert(kSolverRows == S_MINARES + 2, "one row per id up to S_MINARES, then S_CG_LANCZOS");
+// the row of `kind`, nullptr for ids the library does not serve
+inline const SolverInfo* solver_info(int kind) {
+  if (kind == S_CG_LANCZOS) return &kSolvers[kSolverRows - 1];
+  return kind >= 0 && kind < kSolverRows - 1 && kSolvers[kind].name ? &kSolvers[kind] : nullptr;
 }
-// CGNE / CRMR: CG and CR on A A^T y = b with x = A^T y; they return x only and take one preconditioner, N, on the
-// m-dimensional residual space
-inline bool is_normal_ln_kind(int k) { return k == S_CGNE || k == S_CRMR; }
-// the least-norm solvers: min ||x|| subject to A x = b, with x = A^T y; they return the multipliers y (m entries) too
-inline bool is_leastnorm_kind(int k) { return k == S_CRAIG || k == S_CRAIGMR || k == S_LNLQ; }
-// the adjoint-pair solvers: two solutions, x (A x = b) and y (A^T y = c).  TriLQR: A is m x n, b and y have m entries,
-// c and x have n; BiLQR: square
-inline bool is_adjoint_kind(int k) { return k == S_BILQR || k == S_TRILQR; }
+// entries of an attached diagonal: a refused or ignored M has m, N n
+inline int precond_len(const SolverInfo& s, int which, int m, int n) {
+  const PrecondUse u = which == 0 ? s.M.use : s.N.use;
+  return u == P_ON_M || (u != P_ON_N && which == 0) ? m : n;
+}
 
 // One workspace per (solver, dtype): owns every device vector of the solver
 // (src/krylov_workspaces.jl; SURVEY.md appendix B for fields and aliasing).

@@ -19,7 +19,8 @@ namespace kb {
 // ---------------------------------------------------------------------------
 template <class T> Workspace<T>* ws_create(SolverKind kind, int m, int n, int memory, int window, int device) {
   const double t0 = now_seconds();
-  if (m != n && !is_ls_kind(kind) && kind != S_TRILQR) throw std::runtime_error("System must be square");
+  const SolverInfo* info = solver_info(kind);
+  if (m != n && !(info && info->rect)) throw std::runtime_error("System must be square");
   Workspace<T>* ws = new Workspace<T>();
   try {
     ws->kind = kind; ws->m = m; ws->n = n;

@@ -110,6 +110,29 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p), a
 
 
+def _float(v):
+    return None if v is None else float(v)
+
+
+def _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=(), ext=()):
+    """The KrylovOptions / KrylovB200Options pair of one solve: the keywords every solver takes, then the solver's own
+    fields (`opts` into KrylovOptions, `ext` into KrylovB200Options; a None value keeps the default)."""
+    o = lib().krylov_default_options()
+    if atol is not None:
+        o.atol = float(atol)
+    if rtol is not None:
+        o.rtol = float(rtol)
+    o.itmax, o.verbose = int(itmax), int(verbose)
+    o.timemax = math.nan if math.isinf(timemax) else float(timemax)
+    e = lib().krylov_b200_default_options()
+    e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+    for struct, fields in ((o, opts), (e, ext)):
+        for name, val in dict(fields).items():
+            if val is not None:
+                setattr(struct, name, val)
+    return o, e
+
+
 class CsrOperator:
     """A CSR operator resident in HBM, independent of any workspace (SURVEY.md 8f-4):
 
@@ -376,42 +399,13 @@ class KrylovWorkspace:
         """solver!(ws, A, b; kwargs...)  -- kwargs as in cg.jl:100-111, gmres.jl:96-108,
         bicgstab.jl:105-116, minres.jl:138-151.  M / N: None (identity), a 1-D array
         (Diagonal preconditioner) or a host callable."""
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        o.radius, o.linesearch, o.lambda_ = float(radius), int(linesearch), float(lambda_)
-        o.restart, o.reorthogonalization = int(restart), int(reorthogonalization)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused, e.batch = int(history), int(ldiv), int(fused), int(batch)
-        e.time_kernels = int(time_kernels)
-        e.check_curvature = int(check_curvature)
-        if gamma is not None:
-            e.cr_gamma = float(gamma)
-        if etol is not None:
-            e.etol = float(etol)
-        if conlim is not None:
-            e.conlim = float(conlim)
-        if artol is not None:
-            e.axtol = float(artol)   # MINARES's Artol travels in the axtol field
-        keep = []
-        if callback is not None:
-            wsref = self
-
-            def cb_tramp(_ws, _user):
-                r = callback(wsref)
-                if not isinstance(r, (bool, np.bool_)):
-                    wsref._cb_error = TypeError(f"callback must return Bool, got {type(r).__name__}")   # cg.jl:264
-                    return 1
-                return int(r)
-            e.callback = _lib.CALLBACK(cb_tramp)
-            keep.append(e.callback)
-        self._cb_error = None
-        lib().krylov_b200_set_options(self._h, C.byref(e))
-
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
+                        opts=dict(radius=float(radius), linesearch=int(linesearch), lambda_=float(lambda_),
+                                  restart=int(restart), reorthogonalization=int(reorthogonalization)),
+                        ext=dict(batch=int(batch), time_kernels=int(time_kernels), check_curvature=int(check_curvature),
+                                 cr_gamma=_float(gamma), etol=_float(etol), conlim=_float(conlim),
+                                 axtol=_float(artol)))   # MINARES's Artol travels in the axtol field
+        keep = [self._set_options(e, callback)]
         fA = None
         if callable(A) and not hasattr(A, "shape"):
             fA, k = self._wrap_matvec(A)
@@ -432,22 +426,45 @@ class KrylovWorkspace:
                 self._set_diag(which, None)
             else:
                 self._set_diag(which, P)
+        return self._solve_staged(o, fA, None, fM, fN, b, c, self.m)
+
+    def _set_options(self, e, callback):
+        """Install the KrylovB200Options of one solve, `callback` behind a trampoline; returns what must outlive the
+        solve."""
+        if callback is not None:
+            wsref = self
+
+            def cb_tramp(_ws, _user):
+                r = callback(wsref)
+                if not isinstance(r, (bool, np.bool_)):
+                    wsref._cb_error = TypeError(f"callback must return Bool, got {type(r).__name__}")   # cg.jl:264
+                    return 1
+                return int(r)
+            e.callback = _lib.CALLBACK(cb_tramp)
+        self._cb_error = None
+        lib().krylov_b200_set_options(self._h, C.byref(e))
+        return e.callback
+
+    def _solve_staged(self, o, fA, fAt, fM, fN, b, c, c_len):
+        """Stage b (m entries) and c (c_len entries), call krylov_solve and raise what it or the callback reported."""
         if not _is_torch(b):
             b = np.ascontiguousarray(b, dtype=self.dtype)
             if self.device == "cuda":
                 raise B200Error("ktypeof(b) must be a device vector for a device workspace")
         elif self.device != "cuda":
             raise B200Error("ktypeof(b) must be a host vector for a host workspace")
-        if b.shape[0] != self.n:
+        if b.shape[0] != self.m:
             raise B200Error("Inconsistent problem size")
-        pb, kb = _ptr(b)
-        if c is not None and not _is_torch(c):
-            c = np.ascontiguousarray(c, dtype=self.dtype)
+        pb, kb_ = _ptr(b)
+        if c is not None:
+            if not _is_torch(c):
+                c = np.ascontiguousarray(c, dtype=self.dtype)
+            if c.shape[0] != c_len:
+                raise B200Error("Inconsistent problem size")
         pc, kc = _ptr(c)
-        self._order_after(kb, kc)
+        self._order_after(kb_, kc)
         null = _lib.MATVEC()
-        rc = lib().krylov_solve(self._h, fA or null, null, fM or null, fN or null, pb, pc, None, C.byref(o))
-        del keep
+        rc = lib().krylov_solve(self._h, fA or null, fAt or null, fM or null, fN or null, pb, pc, None, C.byref(o))
         if self._cb_error is not None:
             raise self._cb_error
         if rc != 0:
@@ -769,9 +786,6 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
     b has m entries, x has n.  `window` (default 5) sizes the forward-error window."""
     _N_on_residual_space = False    # CGNE / CRMR: N acts on the m-dimensional residual space
 
-    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, window: int = 0, device: str = "host", memory: int = 0):
-        super().__init__(m_or_A, n_or_b, dtype, memory=memory, window=window, device=device)
-
     def _wrap_rect(self, f, nin, nout):
         """Host callback y = f(x) with len(x) = nin and len(y) = nout (staged through pinned memory)."""
         if self.device == "cuda":
@@ -797,39 +811,17 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
             raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
         if sqd:
             lambda_ = 1.0
-        o = lib().krylov_default_options()
-        o.atol, o.rtol = float(atol), float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        o.radius, o.lambda_ = float(radius), float(lambda_)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
-        for name, val in (("etol", etol), ("axtol", axtol), ("btol", btol), ("conlim", conlim)):
-            if val is not None:
-                setattr(e, name, float(val))
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
+                        opts=dict(radius=float(radius), lambda_=float(lambda_)),
+                        ext=dict(etol=_float(etol), axtol=_float(axtol), btol=_float(btol), conlim=_float(conlim)))
         return self._run(A, b, M, N, o, e, callback)
 
     def _run(self, A, b, M, N, o, e, callback, c=None, c_len=None):
         """Set the options, the operator pair and the preconditioners, stage b (and c, of c_len entries, default m) and
         call krylov_solve."""
         m, n = self.m, self.n
-        keep = []
-        if callback is not None:
-            wsref = self
-
-            def cb_tramp(_ws, _user):
-                r = callback(wsref)
-                if not isinstance(r, (bool, np.bool_)):
-                    wsref._cb_error = TypeError(f"callback must return Bool, got {type(r).__name__}")
-                    return 1
-                return int(r)
-            e.callback = _lib.CALLBACK(cb_tramp)
-            keep.append(e.callback)
-        self._cb_error = None
-        lib().krylov_b200_set_options(self._h, C.byref(e))
-
-        null = _lib.MATVEC()
-        fA = fAt = null
+        keep = [self._set_options(e, callback)]
+        fA = fAt = None
         if hasattr(A, "matvec") and hasattr(A, "rmatvec") and not isinstance(A, CsrOperator):   # LinearOperator
             fA, fAt = self._wrap_rect(A.matvec, n, m), self._wrap_rect(A.rmatvec, m, n)
         elif isinstance(A, tuple) and len(A) == 2 and all(callable(f) for f in A):
@@ -837,7 +829,7 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
         elif A is not None:
             self.set_operator(A)
         keep += [fA, fAt]
-        fP = [null, null]
+        fP = [None, None]
         for which, (P, ln) in enumerate(((M, m), (N, m if self._N_on_residual_space else n))):
             if P is not None and callable(P) and not hasattr(P, "shape"):
                 fP[which] = self._wrap_rect(P, ln, ln)
@@ -847,29 +839,7 @@ class _LeastSquaresWorkspace(KrylovWorkspace):
                 if P is not None and getattr(P, "ndim", 1) != 1:
                     raise B200Error(f"{self.solver} takes diagonal preconditioners (1-D arrays) or host callables")
                 self._set_diag(which, P)
-        if not _is_torch(b):
-            b = np.ascontiguousarray(b, dtype=self.dtype)
-            if self.device == "cuda":
-                raise B200Error("ktypeof(b) must be a device vector for a device workspace")
-        elif self.device != "cuda":
-            raise B200Error("ktypeof(b) must be a host vector for a host workspace")
-        if b.shape[0] != m:
-            raise B200Error("Inconsistent problem size")
-        pb, kb_ = _ptr(b)
-        if c is not None:
-            if not _is_torch(c):
-                c = np.ascontiguousarray(c, dtype=self.dtype)
-            if c.shape[0] != (m if c_len is None else c_len):
-                raise B200Error("Inconsistent problem size")
-        pc, kc = _ptr(c)
-        self._order_after(kb_, kc)
-        rc = lib().krylov_solve(self._h, fA, fAt, fP[0], fP[1], pb, pc, None, C.byref(o))
-        del keep
-        if self._cb_error is not None:
-            raise self._cb_error
-        if rc != 0:
-            raise B200Error(_lib.last_error())
-        return self
+        return self._solve_staged(o, fA, fAt, fP[0], fP[1], b, c, m if c_len is None else c_len)
 
 
 class LsqrWorkspace(_LeastSquaresWorkspace):
@@ -897,20 +867,9 @@ class LslqWorkspace(_LeastSquaresWorkspace):
             raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
         if sqd:
             lambda_ = 1.0
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        o.lambda_ = float(lambda_)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
-        e.sigma, e.transfer_to_lsqr = float(sigma), int(transfer_to_lsqr)
-        for name, val in (("etol", etol), ("utol", utol), ("btol", btol), ("conlim", conlim)):
-            if val is not None:
-                setattr(e, name, float(val))
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=dict(lambda_=float(lambda_)),
+                        ext=dict(sigma=float(sigma), transfer_to_lsqr=int(transfer_to_lsqr), etol=_float(etol),
+                                 utol=_float(utol), btol=_float(btol), conlim=_float(conlim)))
         return self._run(A, b, M, N, o, e, callback)
 
 
@@ -925,16 +884,8 @@ class _NormalEquationsWorkspace(_LeastSquaresWorkspace):
         space: None, the diagonal of a Diagonal preconditioner, or a host callable.  There is no N."""
         if unknown:
             raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        o.radius, o.lambda_ = float(radius), float(lambda_)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
+                        opts=dict(radius=float(radius), lambda_=float(lambda_)))
         return self._run(A, b, M, None, o, e, callback)
 
 
@@ -952,23 +903,12 @@ class _BiorthWorkspace(_LeastSquaresWorkspace):
     scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables."""
     nA = 2
 
-    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
-        super().__init__(m_or_A, n_or_b, dtype, device=device)
-
     def _solve(self, A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown,
                transfer_to_bicg=True):
         if unknown:
             raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
-        e.transfer_to_bicg = int(transfer_to_bicg)
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
+                        ext=dict(transfer_to_bicg=int(transfer_to_bicg)))
         return self._run(A, b, M, N, o, e, callback, c)
 
 
@@ -999,24 +939,13 @@ class _AdjointWorkspace(_LeastSquaresWorkspace):
     scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables.  Neither takes a preconditioner."""
     nA = 2
 
-    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
-        super().__init__(m_or_A, n_or_b, dtype, device=device)
-
     def _solve(self, A, b, c, transfer, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown):
         if unknown:
             raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
         if c is None:
             raise B200Error(f"{self.solver}! solves A^T y = c as well: c must be given")
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        e = lib().krylov_b200_default_options()
-        e.history, e.fused = int(history), int(fused)
-        e.transfer_to_bicg = int(transfer)           # TriLQR's transfer_to_usymcg travels in the same field
+        # TriLQR's transfer_to_usymcg travels in the transfer_to_bicg field
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, False, fused, ext=dict(transfer_to_bicg=int(transfer)))
         return self._run(A, b, None, None, o, e, callback, c, c_len=self.n)
 
     def warm_start(self, x0, y0):
@@ -1089,9 +1018,6 @@ class _LeastNormWorkspace(_LeastSquaresWorkspace):
     callables.  M (m entries) and N (n entries): None, the diagonal of a Diagonal preconditioner, or a host callable."""
     nA = 2
 
-    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
-        super().__init__(m_or_A, n_or_b, dtype, device=device)
-
     def _solve(self, A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
                unknown, transfer_to_lsqr=False, btol=None, conlim=None, ext=None):
         if unknown:
@@ -1100,22 +1026,9 @@ class _LeastNormWorkspace(_LeastSquaresWorkspace):
             raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
         if sqd:
             lambda_ = 1.0
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        o.lambda_ = float(lambda_)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
-        e.transfer_to_lsqr = int(transfer_to_lsqr)
-        for name, val in (("btol", btol), ("conlim", conlim)):
-            if val is not None:
-                setattr(e, name, float(val))
-        for name, val in (ext or {}).items():
-            setattr(e, name, val)
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=dict(lambda_=float(lambda_)),
+                        ext=dict(dict(transfer_to_lsqr=int(transfer_to_lsqr), btol=_float(btol), conlim=_float(conlim)),
+                                 **(ext or {})))
         return self._run(A, b, M, N, o, e, callback)
 
     y = _AdjointWorkspace.y
@@ -1170,25 +1083,13 @@ class _NormalLeastNormWorkspace(_LeastSquaresWorkspace):
     nA = 2
     _N_on_residual_space = True
 
-    def __init__(self, m_or_A, n_or_b=None, dtype=None, *, device: str = "host", memory: int = 0, window: int = 0):
-        super().__init__(m_or_A, n_or_b, dtype, device=device)
-
     def solve(self, A, b, *, N=None, ldiv=False, lambda_=0.0, atol=None, rtol=None, itmax=0, timemax=math.inf,
               verbose=0, history=False, callback=None, fused=True, **unknown):
         """cgne!(ws, A, b; kwargs...) / crmr!(ws, A, b; kwargs...)  -- kwargs as in cgne.jl:116-126 and
         crmr.jl:114-124: atol and rtol default to sqrt(eps), itmax = 0 means m + n, λ (`lambda_`) >= 0."""
         if unknown:
             raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        o = lib().krylov_default_options()
-        if atol is not None:
-            o.atol = float(atol)
-        if rtol is not None:
-            o.rtol = float(rtol)
-        o.itmax, o.verbose = int(itmax), int(verbose)
-        o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-        o.lambda_ = float(lambda_)
-        e = lib().krylov_b200_default_options()
-        e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
+        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=dict(lambda_=float(lambda_)))
         return self._run(A, b, None, N, o, e, callback)
 
 
@@ -1200,28 +1101,40 @@ class CrmrWorkspace(_NormalLeastNormWorkspace):
     solver = "crmr"
 
 
+def _one_shot(name, b, n, run, **ws_kw):
+    """Create the workspace of `name` (m = len(b) rows, n columns) for b's element type and place, return run(ws) and
+    free it.  The element type of a torch b is read without copying it to the host."""
+    if _is_torch(b):
+        import torch
+        dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
+    else:
+        dt = np.asarray(b).dtype
+    if dt not in (np.float32, np.float64):
+        dt = np.float64
+    ws = _WS[name](b.shape[0], int(n), dt, device="cuda" if _is_torch(b) else "host", **ws_kw)
+    try:
+        return run(ws)
+    finally:
+        ws.free()
+
+
+def _columns(name, A, n):
+    if n is None:
+        if not hasattr(A, "shape"):
+            raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
+        n = A.shape[1]
+    return n
+
+
 def _make_least_norm(name):
     def f(A, b, x0=None, *, n=None, **kw):
         if x0 is not None:
             raise B200Error(f"{name} does not support warm-start (it takes no x0)")
-        m = b.shape[0]
-        if n is None:
-            if not hasattr(A, "shape"):
-                raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
-            n = A.shape[1]
-        if _is_torch(b):                      # the element type, without copying a device b to the host
-            import torch
-            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
-        else:
-            dt = np.asarray(b).dtype
-        if dt not in (np.float32, np.float64):
-            dt = np.float64
-        ws = _WS[name](m, int(n), dt, device="cuda" if _is_torch(b) else "host")
-        try:
+
+        def run(ws):
             ws.solve(A, b, **kw)
             return ws.x, ws.y, ws.stats
-        finally:
-            ws.free()
+        return _one_shot(name, b, _columns(name, A, n), run)
     f.__name__ = name
     f.__doc__ = f"(x, y, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
     return f
@@ -1231,24 +1144,11 @@ def _make_normal_least_norm(name):
     def f(A, b, x0=None, *, n=None, **kw):
         if x0 is not None:
             raise B200Error(f"{name} does not support warm-start (it takes no x0)")
-        m = b.shape[0]
-        if n is None:
-            if not hasattr(A, "shape"):
-                raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
-            n = A.shape[1]
-        if _is_torch(b):                      # the element type, without copying a device b to the host
-            import torch
-            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
-        else:
-            dt = np.asarray(b).dtype
-        if dt not in (np.float32, np.float64):
-            dt = np.float64
-        ws = _WS[name](m, int(n), dt, device="cuda" if _is_torch(b) else "host")
-        try:
+
+        def run(ws):
             ws.solve(A, b, **kw)
             return ws.x, ws.stats
-        finally:
-            ws.free()
+        return _one_shot(name, b, _columns(name, A, n), run)
     f.__name__ = name
     f.__doc__ = f"(x, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
     return f
@@ -1256,24 +1156,14 @@ def _make_normal_least_norm(name):
 
 def _make_adjoint(name):
     def f(A, b, c, x0=None, y0=None, **kw):
-        m, n = b.shape[0], c.shape[0]
-        if _is_torch(b):                      # the element type, without copying a device b to the host
-            import torch
-            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
-        else:
-            dt = np.asarray(b).dtype
-        if dt not in (np.float32, np.float64):
-            dt = np.float64
-        ws = _WS[name](m, n, dt, device="cuda" if _is_torch(b) else "host")
-        try:
+        def run(ws):
             if (x0 is None) != (y0 is None):
                 raise B200Error(f"{name}: pass both x0 and y0, or neither")
             if x0 is not None:
                 ws.warm_start(x0, y0)
             ws.solve(A, b, c, **kw)
             return ws.x, ws.y, ws.stats
-        finally:
-            ws.free()
+        return _one_shot(name, b, c.shape[0], run)
     f.__name__ = name
     f.__doc__ = f"(x, y, stats) = {name}(A, b, c[, x0, y0]; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, c n"
     return f
@@ -1295,20 +1185,10 @@ def _make_adjoint_inplace(name):
 
 def _make_least_squares(name):
     def f(A, b, *, n=None, window=0, **kw):
-        m = b.shape[0]
-        if n is None:
-            if not hasattr(A, "shape"):
-                raise B200Error(f"{name}: pass n= (number of columns) with a tuple operator")
-            n = A.shape[1]
-        dt = b.cpu().numpy().dtype if _is_torch(b) else np.asarray(b).dtype
-        if dt not in (np.float32, np.float64):
-            dt = np.float64
-        ws = _WS[name](m, int(n), dt, window=window, device="cuda" if _is_torch(b) else "host")
-        try:
+        def run(ws):
             ws.solve(A, b, **kw)
             return ws.x, ws.stats
-        finally:
-            ws.free()
+        return _one_shot(name, b, _columns(name, A, n), run, window=window)
     f.__name__ = name
     f.__doc__ = f"(x, stats) = {name}(A, b; window=5, kwargs...)  (src/{name}.jl); A is m x n, b has m entries"
     return f
@@ -1349,16 +1229,10 @@ def _make_inplace(name):
 
 def _make_outofplace(name):
     def f(A, b, x0=None, *, memory=0, window=0, **kw):
-        n = b.shape[0]
-        dt = b.cpu().numpy().dtype if _is_torch(b) else np.asarray(b).dtype
-        if dt not in (np.float32, np.float64):
-            dt = np.float64
-        ws = _WS[name](n, n, dt, memory=memory, window=window, device="cuda" if _is_torch(b) else "host")
-        try:
+        def run(ws):
             krylov_solve_(ws, A, b, x0, **kw)
             return ws.x, ws.stats
-        finally:
-            ws.free()
+        return _one_shot(name, b, b.shape[0], run, memory=memory, window=window)
     f.__name__ = name
     f.__doc__ = f"(x, stats) = {name}(A, b[, x0]; kwargs...)"
     return f

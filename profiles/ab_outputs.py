@@ -11,9 +11,11 @@ right-hand-side solvers with the fused paths on and off: diagonal M and N, ldiv,
 `memory`, reorthogonalization, b = 0, itmax = 3, a callback exit, timemax = 0, the solver-specific exits and Float32,
 and CG on a constant-coefficient operator (the path of the CsrDict encoding, M = I and a diagonal M, both types), CG's
 two-launch kernels (fused = 2), a block-Jacobi M and the in-kernel phase timing (time_kernels).  LSQR and LSMR get the
-same treatment; LSLQ, CGLS, CRLS, CRAIG, CRAIGMR, BiLQ, QMR, BiLQR, TriLQR, CAR and MINARES run compactly (defaults,
-Float32, itmax = 3 and a callback exit, fused and not).  For the two-solution solvers y and the dual history are
-compared too.
+same treatment; LSLQ, CGLS, CRLS, CRAIG, CRAIGMR, LNLQ, CGNE, CRMR, BiLQ, QMR, BiLQR, TriLQR, CAR and MINARES run
+compactly (defaults, Float32, itmax = 3 and a callback exit, fused and not), and each rectangular one once more per
+preconditioner it takes (M on the m-space, N on the n-space, CGNE / CRMR's N on the m-space) and per option field it
+forwards (λ; the trust-region radius of CGLS / CRLS).  CG, CR, MINRES and CG-Lanczos also run with an N they ignore.
+For the two-solution solvers y and the dual history are compared too.
 """
 import json
 import os
@@ -30,8 +32,13 @@ SQUARE = {"cg": "lap", "cr": "lap", "minres": "lap", "cg_lanczos": "lap", "bicgs
 TAKES_N = {"bicgstab", "cgs", "gmres", "fom", "fgmres", "dqgmres", "diom"}
 ARNOLDI = {"gmres", "fom", "fgmres"}
 COMPACT = {"lslq": "grad", "cgls": "grad", "crls": "grad", "craig": "div", "craigmr": "div", "bilq": "kron",
-           "qmr": "kron", "bilqr": "kron", "trilqr": "grad", "car": "lap", "minares": "lap"}
+           "qmr": "kron", "bilqr": "kron", "trilqr": "grad", "car": "lap", "minares": "lap", "lnlq": "div", "cgne": "div",
+          "crmr": "div"}
 ADJOINT = {"bilqr", "trilqr"}
+# the rectangular solvers beyond LSQR / LSMR: the preconditioners they take and whether they forward the radius
+RECT = {"lslq": ("M", "N"), "cgls": ("M",), "crls": ("M",), "craig": ("M", "N"), "craigmr": ("M", "N"),
+        "lnlq": ("M", "N"), "cgne": ("N",), "crmr": ("N",)}
+N_ON_M = {"cgne", "crmr"}
 CHUNK = 12
 
 
@@ -92,6 +99,8 @@ def configs():
         add(s, p, callback=3, atol=0.0, rtol=0.0)
         add(s, p, timemax=0.0)
         add(s, p, dtype="float32")
+        if s not in TAKES_N:
+            add(s, p, N="d")                                          # an N the solver ignores
         if s in ARNOLDI:
             add(s, p, restart=True, memory=5)
             add(s, p, restart=True, memory=5, x0=True)
@@ -151,6 +160,12 @@ def configs():
         add(s, p, dtype="float32", **c)
         add(s, p, itmax=3, **c)
         add(s, p, callback=3, **c)
+    for s, slots in RECT.items():
+        for which in slots:
+            add(s, COMPACT[s], **{which: "pos"})
+        add(s, COMPACT[s], lambda_=0.1)
+        if s in ("cgls", "crls"):
+            add(s, COMPACT[s], radius=0.5)
     return out
 
 
@@ -175,7 +190,7 @@ def run_chunk(lo, hi, path):
         vec = {"d": lambda: 1.0 / diag, "sd": lambda: 1.0 / np.sqrt(diag),
                "pos": lambda ln: np.linspace(0.5, 2.0, ln),
                "bj4": lambda: np.linalg.inv(np.stack([A[k:k + 4, k:k + 4].toarray() for k in range(0, n, 4)]))}
-        for which, ln in (("M", m), ("N", n)):
+        for which, ln in (("M", m), ("N", m if cfg["solver"] in N_ON_M else n)):
             if which in kw:
                 kw[which] = vec["pos"](ln) if kw[which] == "pos" else vec[kw[which]]()
         c = kw.pop("c", None)
