@@ -351,6 +351,32 @@ int kb200_csr_plan(void *csr, long long *out7);
  * mask byte per row; built when the operator is created unless KB200_CSR_DICT=0): 1 if encoded (*npairs = number of
  * pairs), 0 if not (*npairs = 0), -1 on a NULL object.  Fused CG runs its persistent kernel on the encoding. */
 int kb200_csr_dict(void *csr, int *npairs);
+/* Kernels launched so far through a flat-API context (kb200_ctx_create); -1 for NULL. */
+long long kb200_ctx_launch_count(void *ctx);
+
+/* ---- Krylov processes (src/krylov_processes.jl): the basis and the projected matrix of k steps ----
+ * csr: the operator A (m x n; square for the Lanczos processes and Arnoldi).  csrT: A^T as a CSR object (n x m), or
+ * NULL to have the call form it with kb200_csr_transpose and free it afterwards.  b (and c): device vectors in dtype,
+ * which must be the CSR object's.  V, U: caller-allocated device outputs, column-major, k+1 columns, leading dimension
+ * = the vector's length.  beta, gamma: host scalars; T, TH, L: host arrays of the reference's SparseMatrixCSC nzval
+ * (3k-1 entries for T and TH, 2k+1 for L); H: host, dense (k+1) x k column-major.  flags: bit 0 allow_breakdown, bit 1
+ * reorthogonalization (hermitian_lanczos: local, arnoldi: full; ignored by the others).
+ * All k steps are enqueued on the context's stream with the coefficients kept on the device; the call reads them back
+ * once and returns after synchronising the stream.  With csrT = NULL the call first forms A^T through the host (the
+ * operator is copied down, transposed and uploaded again), so pass csrT to repeat calls on one operator at one
+ * read-back each.  The coefficient block and scratch vectors are kept in the context between calls (grown on demand).  0 on success; -1 with krylov_b200_last_error on an exact breakdown
+ * without allow_breakdown (the reference's message), k < 1, a shape or dtype mismatch, or a row-partitioned context;
+ * -2 for a complex dtype.  With allow_breakdown, the column after a breakdown is zero, as kfill! leaves it; when
+ * nonhermitian_lanczos meets c^T b == 0 its first columns V[:,1], U[:,1] are zero too (the reference leaves them
+ * undefined). */
+int kb200_hermitian_lanczos(void *ctx, void *csr, int k, int dtype, const void *b, void *V, double *beta, double *T, int flags);
+int kb200_arnoldi(void *ctx, void *csr, int k, int dtype, const void *b, void *V, double *beta, double *H, int flags);
+int kb200_golub_kahan(void *ctx, void *csr, void *csrT, int k, int dtype, const void *b, void *V, void *U, double *beta, double *L,
+                      int flags);
+int kb200_nonhermitian_lanczos(void *ctx, void *csr, void *csrT, int k, int dtype, const void *b, const void *c, void *V, void *U,
+                               double *beta, double *gamma, double *T, double *TH, int flags);
+int kb200_saunders_simon_yip(void *ctx, void *csr, void *csrT, int k, int dtype, const void *b, const void *c, void *V, void *U,
+                             double *beta, double *gamma, double *T, double *TH, int flags);
 
 #ifdef __cplusplus
 }

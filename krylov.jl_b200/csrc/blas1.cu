@@ -52,8 +52,10 @@ void Ctx::destroy() {
   if (tickets) cudaFree(tickets);
   if (dscal) cudaFree(dscal);
   if (hscal) cudaFreeHost(hscal);
+  if (proc_scratch) cudaFree(proc_scratch);
   if (own_stream && stream) cudaStreamDestroy(stream);
   partials = nullptr; tickets = nullptr; dscal = nullptr; hscal = nullptr; stream = nullptr;
+  proc_scratch = nullptr; proc_scratch_bytes = 0;
 }
 
 template <class T> T* dev_alloc(size_t n) {

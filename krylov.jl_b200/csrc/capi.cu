@@ -11,6 +11,7 @@
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 
 #include "../../include/krylov_b200.h"
@@ -1304,6 +1305,95 @@ int kb200_csr_plan(void* csr, long long* out) {
     out[0] = A.ntiles; out[1] = A.tile_cap; out[2] = A.max_row; out[3] = A.tma_ok; out[4] = A.stages; out[5] = A.grid; out[6] = (long long)A.smem_bytes;
   }
   return 0;
+}
+
+long long kb200_ctx_launch_count(void* ctx) { return ctx ? ((Ctx*)ctx)->launches : -1; }
+
+}  // extern "C"
+
+// ---- Krylov processes (processes.cu) ------------------------------------------------------------------------------
+namespace {
+// Common checks of the process entry points, then body(ctx, A, At) with At formed here (and freed) when not given.
+template <class F>
+int proc_entry(const char* name, void* ctx, void* csr, void* csrT, int k, int dtype, bool square, bool adjoint, F body) {
+  try {
+    if (dtype == KRYLOV_COMPLEX32 || dtype == KRYLOV_COMPLEX64) return -2;
+    if (!ctx || !csr) throw std::runtime_error("ctx and the CSR object are required");
+    if (dtype != KRYLOV_FLOAT32 && dtype != KRYLOV_FLOAT64) throw std::runtime_error("unknown dtype " + std::to_string(dtype));
+    Ctx& c = *(Ctx*)ctx;
+    if (c.dcomm) throw std::runtime_error("the processes do not run on row-partitioned contexts");
+    CsrAny* a = (CsrAny*)csr;
+    if (a->dtype != dtype) throw std::runtime_error("dtype differs from the CSR object's");
+    if (k < 1) throw std::runtime_error("k must be at least 1 (got " + std::to_string(k) + ")");
+    int m = 0, n = 0;
+    kb200_csr_shape(a, &m, &n, nullptr);
+    const int max_col = dtype == KRYLOV_FLOAT64 ? a->d.max_col : a->f.max_col;
+    if (max_col >= n) throw std::runtime_error("column index outside the operator's columns");
+    if (m < 1 || n < 1) throw std::runtime_error("the operator is empty");
+    if (square && m != n) throw std::runtime_error("the operator must be square (got " + std::to_string(m) + " x " + std::to_string(n) + ")");
+    std::unique_ptr<CsrAny> own;
+    CsrAny* at = nullptr;
+    if (adjoint) {
+      at = (CsrAny*)csrT;
+      if (!at) {
+        own.reset((CsrAny*)kb200_csr_transpose(ctx, csr));
+        if (!own) throw std::runtime_error(g_last_error);
+        at = own.get();
+      }
+      int tm = 0, tn = 0;
+      kb200_csr_shape(at, &tm, &tn, nullptr);
+      if (at->dtype != dtype) throw std::runtime_error("dtype of At differs from the CSR object's");
+      if (tm != n || tn != m)
+        throw std::runtime_error("At must be " + std::to_string(n) + " x " + std::to_string(m) + " (got " + std::to_string(tm) + " x " +
+                                 std::to_string(tn) + ")");
+    }
+    KB_CUDA(cudaSetDevice(c.device));
+    if (dtype == KRYLOV_FLOAT64) body(c, a->d, at ? &at->d : nullptr, (double*)nullptr);
+    else body(c, a->f, at ? &at->f : nullptr, (float*)nullptr);
+    return 0;
+  } catch (const std::exception& e) { return fail(name, e); }
+}
+}  // namespace
+
+extern "C" {
+
+int kb200_hermitian_lanczos(void* ctx, void* csr, int k, int dtype, const void* b, void* V, double* beta, double* T, int flags) {
+  return proc_entry("kb200_hermitian_lanczos", ctx, csr, nullptr, k, dtype, true, false, [&](Ctx& c, auto& A, auto*, auto* tag) {
+    typedef std::remove_pointer_t<decltype(tag)> R;
+    if (!b || !V || !beta || !T) throw std::runtime_error("b, V, beta and T are required");
+    hermitian_lanczos_run<R>(c, A, k, (const R*)b, (R*)V, beta, T, flags);
+  });
+}
+int kb200_arnoldi(void* ctx, void* csr, int k, int dtype, const void* b, void* V, double* beta, double* H, int flags) {
+  return proc_entry("kb200_arnoldi", ctx, csr, nullptr, k, dtype, true, false, [&](Ctx& c, auto& A, auto*, auto* tag) {
+    typedef std::remove_pointer_t<decltype(tag)> R;
+    if (!b || !V || !beta || !H) throw std::runtime_error("b, V, beta and H are required");
+    arnoldi_run<R>(c, A, k, (const R*)b, (R*)V, beta, H, flags);
+  });
+}
+int kb200_golub_kahan(void* ctx, void* csr, void* csrT, int k, int dtype, const void* b, void* V, void* U, double* beta, double* L,
+                      int flags) {
+  return proc_entry("kb200_golub_kahan", ctx, csr, csrT, k, dtype, false, true, [&](Ctx& c, auto& A, auto* At, auto* tag) {
+    typedef std::remove_pointer_t<decltype(tag)> R;
+    if (!b || !V || !U || !beta || !L) throw std::runtime_error("b, V, U, beta and L are required");
+    golub_kahan_run<R>(c, A, *At, k, (const R*)b, (R*)V, (R*)U, beta, L, flags);
+  });
+}
+int kb200_nonhermitian_lanczos(void* ctx, void* csr, void* csrT, int k, int dtype, const void* b, const void* cv, void* V, void* U,
+                               double* beta, double* gamma, double* T, double* TH, int flags) {
+  return proc_entry("kb200_nonhermitian_lanczos", ctx, csr, csrT, k, dtype, true, true, [&](Ctx& c, auto& A, auto* At, auto* tag) {
+    typedef std::remove_pointer_t<decltype(tag)> R;
+    if (!b || !cv || !V || !U || !beta || !gamma || !T || !TH) throw std::runtime_error("b, c, V, U, beta, gamma, T and Tᴴ are required");
+    nonhermitian_lanczos_run<R>(c, A, *At, k, (const R*)b, (const R*)cv, (R*)V, (R*)U, beta, gamma, T, TH, flags);
+  });
+}
+int kb200_saunders_simon_yip(void* ctx, void* csr, void* csrT, int k, int dtype, const void* b, const void* cv, void* V, void* U,
+                             double* beta, double* gamma, double* T, double* TH, int flags) {
+  return proc_entry("kb200_saunders_simon_yip", ctx, csr, csrT, k, dtype, false, true, [&](Ctx& c, auto& A, auto* At, auto* tag) {
+    typedef std::remove_pointer_t<decltype(tag)> R;
+    if (!b || !cv || !V || !U || !beta || !gamma || !T || !TH) throw std::runtime_error("b, c, V, U, beta, gamma, T and Tᴴ are required");
+    saunders_simon_yip_run<R>(c, A, *At, k, (const R*)b, (const R*)cv, (R*)V, (R*)U, beta, gamma, T, TH, flags);
+  });
 }
 
 int kb200_csr_dict(void* csr, int* npairs) {

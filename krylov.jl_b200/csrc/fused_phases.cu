@@ -1679,6 +1679,21 @@ void crmr_fused_iteration(Workspace<T>& ws, const Csr<T>& A, const Csr<T>& At, b
   *rr = h.rr; *gamma_out = h.gamma;
 }
 
+// ===========================================================================
+// Krylov processes  (src/krylov_processes.jl; drivers in processes.cu, functors Proc* in kb_internal.h)
+// ===========================================================================
+// No read-back here: every scalar a pass needs is in the call's device block, and the driver reads it once at the end.
+template <class T> void proc_spmv(Ctx& c, const Csr<T>& A, const T* x, const T* x_s, const ProcEpi<T>& epi, const ProcFin<T>& fin) {
+  if (A.n <= 0) return;
+  launch_spmv_epi_g<T, 1>(c, A, ProcXDiv<T>{x, x_s, T(0)}, epi, fin);
+}
+template <class T> void proc_stream(Ctx& c, int n, const ProcUpdBody<T>& body, const ProcFin<T>& fin) {
+  launch_stream<T, 1>(c, n, body, fin);
+}
+template <class T> void proc_divide(Ctx& c, const ProcDivBody<T>& body) {
+  launch_stream<T, 0>(c, std::max(body.n1, body.out2 ? body.n2 : 0), body, NoFin());
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1723,7 +1738,10 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void lnlq_fused_flush<T>(Workspace<T>&, T, T, T, T, T);                                                  \
   template void lnlq_fused_xup<T>(Workspace<T>&, T, T);                                                           \
   template void cgne_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T, T*, T*);          \
-  template void crmr_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T*, T*);
+  template void crmr_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T*, T*);          \
+  template void proc_spmv<T>(Ctx&, const Csr<T>&, const T*, const T*, const ProcEpi<T>&, const ProcFin<T>&);       \
+  template void proc_stream<T>(Ctx&, int, const ProcUpdBody<T>&, const ProcFin<T>&);                                \
+  template void proc_divide<T>(Ctx&, const ProcDivBody<T>&);
 INST(double)
 INST(float)
 #undef INST

@@ -42,6 +42,8 @@ struct Ctx {
                                  // slot 1 the SpMV's, slot 15 k_dist_sum (the fused passes use ws.fused_state)
   void* hscal = nullptr;         // pinned mirror of dscal
   long long launches = 0;        // kernels launched through this context (bench: gpu_launches)
+  void* proc_scratch = nullptr;  // the Krylov processes' coefficient block and scratch vectors (processes.cu), kept
+  size_t proc_scratch_bytes = 0; // from one call to the next and grown on demand; freed by destroy()
   DistComm* dcomm = nullptr;     // device-resident communicator of a row-partitioned solve (nullptr: single GPU)
   DistExchange* dex = nullptr;   // host-side plan of the general x-halo exchange (nullptr: single GPU)
 
@@ -617,6 +619,126 @@ template <class T> void bilq_solve(Workspace<T>& ws, const LinOp<T>& A, const Li
                                    const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
 template <class T> void qmr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const T* c,
                                   const LinOp<T>& M, const LinOp<T>& N, const SolveOpts& o);
+
+// ---------------------------------------------------------------------------
+// Krylov processes (src/krylov_processes.jl): drivers in processes.cu, passes in fused_phases.cu.  A call enqueues
+// every pass of its k steps back to back; the coefficients live in a per-call device block laid out like the
+// reference's nzval, the passes read their scalars from it, and the host reads the block back once at the end.
+// ---------------------------------------------------------------------------
+template <class T> struct ProcHead {       // start of the per-call device block
+  int brk_kind, brk_iter;                  // first exact breakdown (kind 0: none), recorded in stream order
+  T one, tmp;                              // 1 (the divisor of a stored column) and a reorthogonalization coefficient
+  T beta1, gamma1;                         // β₁ and γ₁ (γ₁ᴴ) of the two-sided processes
+};
+
+template <class T> __device__ __forceinline__ T proc_div(T x, T s) { return s == T(0) ? T(0) : div_rn(x, s); }
+
+// Gather of an SpMV that applies a pending division: x[j] / *scale_src, 0 when the divisor is 0 (kdivcopy! on a
+// column that kfill! zeroes after a breakdown).  gather_for_cta (spmv_tiles.cuh) loads the divisor once per CTA.
+template <class T> struct ProcXDiv {
+  const T* __restrict__ x;
+  const T* scale_src;
+  T scale;
+  __device__ __forceinline__ T operator()(int j) const { return proc_div(__ldg(&x[j]), scale); }
+};
+
+// SpMV epilogue of every process.  For its own row: own = src / *src_s stored in vout (the column the pending
+// division produces, never the gathered one); q = acc - *s1 w1 - *s2 w2 (a null w stands for own, a null s skips the
+// term); qout = q; with src2: own2 = src2 / *src2_s stored in vout2; with r: r -= *rs rx.  Accumulates one dot:
+// dot 0 <own, q>, 1 <q, q>, 2 <own2, q>, 3 <y, q>, 4 <q, r>.
+template <class T> struct ProcEpi {
+  const T* src; const T* src_s; T* vout;
+  const T* src2; const T* src2_s; T* vout2;
+  const T* w1; const T* s1;
+  const T* w2; const T* s2;
+  T* qout;
+  T* r; const T* rx; const T* rs;
+  const T* y;
+  int dot;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const {
+    const T own = src ? proc_div(src[row], *src_s) : T(0);
+    if (vout) vout[row] = own;
+    T q = acc;
+    if (s1) q = add_rn(q, mul_rn(-*s1, w1 ? w1[row] : own));
+    if (s2) q = add_rn(q, mul_rn(-*s2, w2 ? w2[row] : own));
+    qout[row] = q;
+    T own2 = T(0);
+    if (src2) { own2 = proc_div(src2[row], *src2_s); vout2[row] = own2; }
+    T rv = T(0);
+    if (r) { rv = add_rn(r[row], mul_rn(-*rs, rx[row])); r[row] = rv; }
+    const T a = dot == 0 ? own : dot == 1 ? q : dot == 2 ? own2 : dot == 3 ? y[row] : rv;
+    d[0] += a * q;
+  }
+};
+
+// Streaming pass: q -= *s x (x null: q is only read), then <y, q> (y null: <q, q>).
+template <class T> struct ProcUpdBody {
+  T* q; const T* x; const T* s; const T* y;
+  __device__ __forceinline__ void operator()(int i, T* d) const {
+    T v = q[i];
+    if (x) { v = add_rn(v, mul_rn(-*s, x[i])); q[i] = v; }
+    d[0] += (y ? y[i] : v) * v;
+  }
+};
+
+// Final normalisation: out1 = src1 / *s1 over n1 entries and out2 = src2 / *s2 over n2 (0 when the divisor is 0).
+template <class T> struct ProcDivBody {
+  T* out1; const T* src1; const T* s1; int n1;
+  T* out2; const T* src2; const T* s2; int n2;
+  __device__ __forceinline__ void operator()(int i, T*) const {
+    if (i < n1) out1[i] = proc_div(src1[i], *s1);
+    if (out2 && i < n2) out2[i] = proc_div(src2[i], *s2);
+  }
+};
+
+// What the CTA that completes a pass's reduction does with the total t (one thread, in stream order).
+//   SET:    dst[0..3] = t; then *copy_dst = *copy_src (Lanczos: Tᵢ₋₁.ᵢ = Tᵢ.ᵢ₋₁).
+//   NORM:   v = sqrt(t) into dst[0..3]; v == 0 records breakdown (kind, iter).
+//   ACC:    *tmp = t; dst[k] += t (reorthogonalization).
+//   BIORTH: t = pᴴq (or cᴴb); 0 records breakdown and gives β = γ = 0, else β = sqrt(|t|), γ = t / β;
+//           dst[0] = β, dst[1] = γ, dst[2] = γ, dst[3] = β.
+template <class T> struct ProcFin {
+  enum { SET, NORM, ACC, BIORTH };
+  ProcHead<T>* h;
+  T* dst[4];
+  const T* copy_src; T* copy_dst;
+  int mode, kind, iter;
+  __device__ void operator()(const T* tot) const {
+    T v = tot[0], w = v;
+    if (mode == NORM) { v = w = sqrt_rn(tot[0]); }
+    if (mode == ACC) h->tmp = v;
+    if (mode == BIORTH) {
+      if (v == T(0)) { v = w = T(0); }
+      else { const T b = sqrt_rn(fabs(tot[0])); w = div_rn(tot[0], b); v = b; }
+    }
+    if ((mode == NORM || mode == BIORTH) && v == T(0) && h->brk_kind == 0) { h->brk_kind = kind; h->brk_iter = iter; }
+    for (int k = 0; k < 4; k++) {
+      if (!dst[k]) continue;
+      const T val = (mode == BIORTH && (k == 1 || k == 2)) ? w : v;
+      *dst[k] = mode == ACC ? add_rn(*dst[k], val) : val;
+    }
+    if (copy_dst) *copy_dst = *copy_src;
+  }
+};
+
+// The launches (fused_phases.cu): an SpMV on A whose gather divides by a device scalar, a streaming update / dot pass
+// and the final normalisation pass.
+template <class T> void proc_spmv(Ctx& c, const Csr<T>& A, const T* x, const T* x_s, const ProcEpi<T>& epi, const ProcFin<T>& fin);
+template <class T> void proc_stream(Ctx& c, int n, const ProcUpdBody<T>& body, const ProcFin<T>& fin);
+template <class T> void proc_divide(Ctx& c, const ProcDivBody<T>& body);
+
+// The processes (processes.cu).  V / U: caller's device outputs, column-major with leading dimension = the vector's
+// length.  coef (and coefH): host outputs in the reference's nzval order (dense column-major (k+1) x k for H).
+// Exact breakdown without allow_breakdown throws the reference's message.  flags: bit 0 allow_breakdown, bit 1
+// reorthogonalization.
+template <class T> void hermitian_lanczos_run(Ctx& c, const Csr<T>& A, int k, const T* b, T* V, double* beta, double* coef, int flags);
+template <class T> void arnoldi_run(Ctx& c, const Csr<T>& A, int k, const T* b, T* V, double* beta, double* H, int flags);
+template <class T> void golub_kahan_run(Ctx& c, const Csr<T>& A, const Csr<T>& At, int k, const T* b, T* V, T* U, double* beta,
+                                        double* coef, int flags);
+template <class T> void nonhermitian_lanczos_run(Ctx& c, const Csr<T>& A, const Csr<T>& At, int k, const T* b, const T* cv, T* V,
+                                                 T* U, double* beta, double* gamma, double* coefT, double* coefTH, int flags);
+template <class T> void saunders_simon_yip_run(Ctx& c, const Csr<T>& A, const Csr<T>& At, int k, const T* b, const T* cv, T* V,
+                                               T* U, double* beta, double* gamma, double* coefT, double* coefTH, int flags);
 
 double now_seconds();
 

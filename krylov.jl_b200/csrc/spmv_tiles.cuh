@@ -89,6 +89,12 @@ __device__ __forceinline__ XScaled<T> gather_for_cta(const XScaled<T>& g) {
   out.scale = *g.scale_src;
   return out;
 }
+template <class T>
+__device__ __forceinline__ ProcXDiv<T> gather_for_cta(const ProcXDiv<T>& g) {    // the processes' divided gather
+  ProcXDiv<T> out = g;
+  out.scale = *g.scale_src;
+  return out;
+}
 
 // Row-partitioned operators: column j >= nloc is halo entry j - nloc of the local halo buffer (filled by
 // k_halo_exchange); the source is chosen by a pointer select, not a branch, so the batch of gathers stays a

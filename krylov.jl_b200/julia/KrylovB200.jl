@@ -699,4 +699,126 @@ function Krylov.block_gmres!(ws::Krylov.BlockGmresWorkspace{T,T,B200Vector{T},B2
   Krylov.block_gmres!(ws, A, B; kw...)
 end
 
+# ---- Krylov processes (src/krylov_processes.jl): one kb200_<process> call each, every step enqueued on the GPU with the
+# coefficients kept on the device and read back once (DESIGN.md §3i).  Bases come back as B200Matrix{T} (column-major,
+# k + 1 columns), T / Tᴴ / L as SparseMatrixCSC{T,Int} with the reference's colptr / rowval, H as a dense Matrix{T}.
+# Aᵀ (golub_kahan, nonhermitian_lanczos, saunders_simon_yip) is formed by the library for the call, through the host:
+# those three copy the operator down once more before their single coefficient read-back.
+proc_flags(allow_breakdown::Bool, reorthogonalization::Bool = false) = Cint(allow_breakdown) | (reorthogonalization ? Cint(2) : Cint(0))
+# error(...) with the reference's message (the library prefixes its entry point's name)
+proc_check(rc, name::String) = rc == 0 ? nothing :
+  error(replace(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())), "kb200_$name: " => ""; count = 1))
+
+function tridiagonal_pattern(k::Int)            # krylov_processes.jl:35-51: (k+1) x k, 3k-1 stored entries
+  colptr = zeros(Int, k+1); rowval = zeros(Int, 3k-1)
+  colptr[1] = 1
+  for i = 1:k
+    pos = colptr[i]
+    colptr[i+1] = 3i
+    if i == 1
+      rowval[pos] = i; rowval[pos+1] = i+1
+    else
+      rowval[pos] = i-1; rowval[pos+1] = i; rowval[pos+2] = i+1
+    end
+  end
+  colptr, rowval
+end
+
+function bidiagonal_pattern(k::Int)             # krylov_processes.jl:331-346: (k+1) x (k+1), 2k+1 stored entries
+  colptr = zeros(Int, k+2); rowval = zeros(Int, 2k+1)
+  colptr[1] = 1
+  for i = 1:k+1
+    pos = colptr[i]
+    if i ≤ k
+      colptr[i+1] = pos + 2; rowval[pos] = i; rowval[pos+1] = i+1
+    else
+      colptr[i+1] = pos + 1; rowval[pos] = i
+    end
+  end
+  colptr, rowval
+end
+
+function Krylov.hermitian_lanczos(A::B200CSR{T}, b::B200Vector{T}, k::Int;
+                                  allow_breakdown::Bool=false, reorthogonalization::Bool=false) where T<:BlasT
+  A.m == A.n || error("A must be square")
+  length(b) == A.n || error("Inconsistent problem size")
+  k ≥ 1 || error("k must be at least 1")
+  V = B200Matrix{T}(undef, A.n, k+1)
+  β = Ref{Cdouble}(0)
+  nz = zeros(Cdouble, 3k-1)
+  proc_check(ccall((:kb200_hermitian_lanczos, lib), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ref{Cdouble}, Ptr{Cdouble}, Cint),
+                   ctx(), A.handle, k, dtype_id(T), b.ptr, V.ptr, β, nz, proc_flags(allow_breakdown, reorthogonalization)),
+             "hermitian_lanczos")
+  colptr, rowval = tridiagonal_pattern(k)
+  return V, T(β[]), SparseMatrixCSC(k+1, k, colptr, rowval, T.(nz))
+end
+
+function Krylov.arnoldi(A::B200CSR{T}, b::B200Vector{T}, k::Int;
+                        allow_breakdown::Bool=false, reorthogonalization::Bool=false) where T<:BlasT
+  A.m == A.n || error("A must be square")
+  length(b) == A.n || error("Inconsistent problem size")
+  k ≥ 1 || error("k must be at least 1")
+  V = B200Matrix{T}(undef, A.n, k+1)
+  β = Ref{Cdouble}(0)
+  H = zeros(Cdouble, k+1, k)
+  proc_check(ccall((:kb200_arnoldi, lib), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ref{Cdouble}, Ptr{Cdouble}, Cint),
+                   ctx(), A.handle, k, dtype_id(T), b.ptr, V.ptr, β, H, proc_flags(allow_breakdown, reorthogonalization)),
+             "arnoldi")
+  return V, T(β[]), T.(H)
+end
+
+function Krylov.golub_kahan(A::B200CSR{T}, b::B200Vector{T}, k::Int; allow_breakdown::Bool=false) where T<:BlasT
+  length(b) == A.m || error("Inconsistent problem size")
+  k ≥ 1 || error("k must be at least 1")
+  V = B200Matrix{T}(undef, A.n, k+1)
+  U = B200Matrix{T}(undef, A.m, k+1)
+  β = Ref{Cdouble}(0)
+  nz = zeros(Cdouble, 2k+1)
+  proc_check(ccall((:kb200_golub_kahan, lib), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{Cdouble}, Ptr{Cdouble}, Cint),
+                   ctx(), A.handle, C_NULL, k, dtype_id(T), b.ptr, V.ptr, U.ptr, β, nz, proc_flags(allow_breakdown)),
+             "golub_kahan")
+  colptr, rowval = bidiagonal_pattern(k)
+  return V, U, T(β[]), SparseMatrixCSC(k+1, k+1, colptr, rowval, T.(nz))
+end
+
+function Krylov.nonhermitian_lanczos(A::B200CSR{T}, b::B200Vector{T}, c::B200Vector{T}, k::Int;
+                                     allow_breakdown::Bool=false) where T<:BlasT
+  A.m == A.n || error("A must be square")
+  length(b) == length(c) == A.n || error("Inconsistent problem size")
+  k ≥ 1 || error("k must be at least 1")
+  V = B200Matrix{T}(undef, A.n, k+1)
+  U = B200Matrix{T}(undef, A.n, k+1)
+  β = Ref{Cdouble}(0); γ = Ref{Cdouble}(0)
+  nzT = zeros(Cdouble, 3k-1); nzTᴴ = zeros(Cdouble, 3k-1)
+  proc_check(ccall((:kb200_nonhermitian_lanczos, lib), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{Cdouble},
+                    Ref{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint),
+                   ctx(), A.handle, C_NULL, k, dtype_id(T), b.ptr, c.ptr, V.ptr, U.ptr, β, γ, nzT, nzTᴴ, proc_flags(allow_breakdown)),
+             "nonhermitian_lanczos")
+  colptr, rowval = tridiagonal_pattern(k)
+  return V, T(β[]), SparseMatrixCSC(k+1, k, colptr, rowval, T.(nzT)), U, T(γ[]),
+         SparseMatrixCSC(k+1, k, copy(colptr), copy(rowval), T.(nzTᴴ))
+end
+
+function Krylov.saunders_simon_yip(A::B200CSR{T}, b::B200Vector{T}, c::B200Vector{T}, k::Int;
+                                   allow_breakdown::Bool=false) where T<:BlasT
+  length(b) == A.m && length(c) == A.n || error("Inconsistent problem size")
+  k ≥ 1 || error("k must be at least 1")
+  V = B200Matrix{T}(undef, A.m, k+1)
+  U = B200Matrix{T}(undef, A.n, k+1)
+  β = Ref{Cdouble}(0); γ = Ref{Cdouble}(0)
+  nzT = zeros(Cdouble, 3k-1); nzTᴴ = zeros(Cdouble, 3k-1)
+  proc_check(ccall((:kb200_saunders_simon_yip, lib), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{Cdouble},
+                    Ref{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Cint),
+                   ctx(), A.handle, C_NULL, k, dtype_id(T), b.ptr, c.ptr, V.ptr, U.ptr, β, γ, nzT, nzTᴴ, proc_flags(allow_breakdown)),
+             "saunders_simon_yip")
+  colptr, rowval = tridiagonal_pattern(k)
+  return V, T(β[]), SparseMatrixCSC(k+1, k, colptr, rowval, T.(nzT)), U, T(γ[]),
+         SparseMatrixCSC(k+1, k, copy(colptr), copy(rowval), T.(nzTᴴ))
+end
+
 end # module

@@ -1277,3 +1277,221 @@ def iteration_count(ws): return int(lib().krylov_niter(ws._h))
 def elapsed_time(ws): return float(lib().krylov_elapsed_time(ws._h))
 def Aprod_count(ws): return ws.nA * iteration_count(ws)
 def warm_start_(ws, x0): return ws.warm_start(x0)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Krylov processes (src/krylov_processes.jl): the basis and the projected matrix of k steps, on the GPU
+# ---------------------------------------------------------------------------------------------------------------------
+def _tridiag_structure(k):
+    """colptr / rowval (0-based) of the reference's (k+1) x k tridiagonal T: 3k-1 stored entries."""
+    colptr = np.zeros(k + 1, np.int64)
+    rowval = np.zeros(3 * k - 1, np.int64)
+    for i in range(1, k + 1):
+        pos = colptr[i - 1]
+        colptr[i] = 3 * i - 1
+        rows = (i, i + 1) if i == 1 else (i - 1, i, i + 1)
+        rowval[pos:pos + len(rows)] = np.array(rows) - 1
+    return colptr, rowval
+
+
+def _bidiag_structure(k):
+    """colptr / rowval (0-based) of golub_kahan's (k+1) x (k+1) lower bidiagonal L: 2k+1 stored entries."""
+    colptr = np.zeros(k + 2, np.int64)
+    rowval = np.zeros(2 * k + 1, np.int64)
+    for i in range(1, k + 2):
+        pos = colptr[i - 1]
+        rows = (i, i + 1) if i <= k else (i,)
+        colptr[i] = pos + len(rows)
+        rowval[pos:pos + len(rows)] = np.array(rows) - 1
+    return colptr, rowval
+
+
+def _csc(nzval, structure, shape):
+    import scipy.sparse as sp
+    colptr, rowval = structure
+    return sp.csc_matrix((nzval, rowval, colptr), shape=shape)
+
+
+class _ProcessCall:
+    """Operators and device vectors of one process call: A (and Aᵀ) as CSR objects, b / c and the outputs V / U on the
+    device, NumPy inputs staged in and out, torch inputs used in place."""
+
+    def __init__(self, name, A, vecs, At, adjoint):
+        import scipy.sparse as sp
+        self.name, self._free = name, []
+        self.torch = any(_is_torch(v) for v in vecs)
+        first = vecs[0]
+        if self.torch:
+            if not all(_is_torch(v) and v.is_cuda for v in vecs):
+                raise B200Error(f"{name}: pass b and c both as torch CUDA tensors or both as NumPy arrays")
+            self.dtype = np.dtype(str(first.dtype).replace("torch.", ""))
+        else:
+            self.dtype = np.asarray(first).dtype
+            if self.dtype.kind in "iub":
+                self.dtype = np.dtype(np.float64)
+        self.dt = _dtype_id(self.dtype)                 # complex and other types are refused here
+        if isinstance(A, CsrOperator):
+            self.A = A
+        elif sp.issparse(A):
+            self.A = CsrOperator.from_scipy(A, dtype=self.dtype)
+            self._free.append(self.A)
+        else:
+            raise B200Error(f"{name} needs a CSR operator (a SciPy sparse matrix or a CsrOperator); matrix-free operators "
+                            "and callbacks are not supported")
+        if self.A.dtype != self.dtype:
+            raise B200Error(f"{name}: the operator is {self.A.dtype}, b is {self.dtype}")
+        self.m, self.n = self.A.shape
+        self.At = None
+        if adjoint:
+            if At is None:                               # formed once per call
+                At = A.T if sp.issparse(A) else None
+            if isinstance(At, CsrOperator):
+                self.At = At
+            elif At is not None:
+                if not sp.issparse(At):
+                    raise B200Error(f"{name}: At must be a SciPy sparse matrix or a CsrOperator")
+                if At.shape != (self.n, self.m):
+                    raise B200Error(f"{name}: At must be {self.n} x {self.m}, got {At.shape[0]} x {At.shape[1]}")
+                self.At = CsrOperator.from_scipy(At, dtype=self.dtype)
+                self._free.append(self.At)
+
+    def vec_in(self, v, length, label):
+        if int(v.shape[0]) != length or len(v.shape) != 1:
+            raise B200Error(f"{self.name}: {label} must have {length} entries, got shape {tuple(v.shape)}")
+        if self.torch:
+            import torch
+            if v.dtype != getattr(torch, self.dtype.name):
+                raise B200Error(f"{self.name}: {label} must be {self.dtype}")
+            v = v.contiguous()
+            self._free.append(v)
+            return C.c_void_p(v.data_ptr())
+        v = np.ascontiguousarray(v, dtype=self.dtype)
+        d = lib().kb200_alloc(max(v.nbytes, 1))
+        self._free.append(d)
+        if lib().kb200_h2d(d, v.ctypes.data_as(C.c_void_p), v.nbytes) != 0:
+            raise B200Error(_lib.last_error())
+        return C.c_void_p(d)
+
+    def basis(self, rows, k):
+        """Device storage of an output basis, rows x (k+1) column-major."""
+        if self.torch:
+            import torch
+            V = torch.empty((k + 1, rows), dtype=getattr(torch, self.dtype.name), device="cuda").t()
+            return V, C.c_void_p(V.data_ptr())
+        d = lib().kb200_alloc(rows * (k + 1) * self.dtype.itemsize)
+        self._free.append(d)
+        return d, C.c_void_p(d)
+
+    def out(self, V, rows, k):
+        if self.torch:
+            return V
+        h = np.empty((rows, k + 1), self.dtype, order="F")
+        if lib().kb200_d2h(h.ctypes.data_as(C.c_void_p), C.c_void_p(V), h.nbytes) != 0:
+            raise B200Error(_lib.last_error())
+        return h
+
+    def run(self, *args):
+        if self.torch:
+            import torch
+            torch.cuda.current_stream().synchronize()    # b / c complete before the library's stream reads them
+        rc = getattr(lib(), f"kb200_{self.name}")(self.A._ctx, self.A._csr, *args)
+        if rc != 0:
+            msg = _lib.last_error() if rc == -1 else f"{self.name}: unsupported element type"
+            raise B200Error(msg.split(f"kb200_{self.name}: ", 1)[-1])
+
+    def close(self):
+        for f in self._free:
+            if isinstance(f, CsrOperator):
+                f.free()
+            elif isinstance(f, int):
+                lib().kb200_free(C.c_void_p(f))
+        self._free = []
+
+
+def _flags(allow_breakdown, reorthogonalization=False):
+    return int(bool(allow_breakdown)) | (2 if reorthogonalization else 0)
+
+
+def hermitian_lanczos(A, b, k: int, *, allow_breakdown: bool = False, reorthogonalization: bool = False):
+    """V, β, T = hermitian_lanczos(A, b, k) (src/krylov_processes.jl:28-103): V is n x (k+1), βv₁ = b and T the
+    (k+1) x k tridiagonal matrix with A V[:, :k] = V T, as a scipy.sparse.csc_matrix with the reference's structure.
+    A: a symmetric SciPy sparse matrix or CsrOperator; b: NumPy array or torch CUDA tensor (then V is a torch tensor with
+    column-major strides and nothing is copied to the host but the coefficients)."""
+    P = _ProcessCall("hermitian_lanczos", A, [b], None, False)
+    try:
+        pb = P.vec_in(b, P.n, "b")
+        V, pV = P.basis(P.n, k)
+        beta, nz = C.c_double(), np.zeros(max(3 * k - 1, 0), np.float64)
+        P.run(int(k), P.dt, pb, pV, C.byref(beta), nz.ctypes.data_as(C.POINTER(C.c_double)),
+              _flags(allow_breakdown, reorthogonalization))
+        return P.out(V, P.n, k), beta.value, _csc(nz.astype(P.dtype), _tridiag_structure(k), (k + 1, k))
+    finally:
+        P.close()
+
+
+def arnoldi(A, b, k: int, *, allow_breakdown: bool = False, reorthogonalization: bool = False):
+    """V, β, H = arnoldi(A, b, k) (src/krylov_processes.jl:250-296): V is n x (k+1), βv₁ = b and H the dense
+    (k+1) x k upper Hessenberg matrix with A V[:, :k] = V H (modified Gram-Schmidt; reorthogonalization: a second pass
+    against every previous vector)."""
+    P = _ProcessCall("arnoldi", A, [b], None, False)
+    try:
+        pb = P.vec_in(b, P.n, "b")
+        V, pV = P.basis(P.n, k)
+        beta, H = C.c_double(), np.zeros((max(k, 0) + 1, max(k, 0)), np.float64, order="F")
+        P.run(int(k), P.dt, pb, pV, C.byref(beta), H.ctypes.data_as(C.POINTER(C.c_double)),
+              _flags(allow_breakdown, reorthogonalization))
+        return P.out(V, P.n, k), beta.value, np.asfortranarray(H.astype(P.dtype))
+    finally:
+        P.close()
+
+
+def golub_kahan(A, b, k: int, *, allow_breakdown: bool = False, At=None):
+    """V, U, β, L = golub_kahan(A, b, k) (src/krylov_processes.jl:323-402): A is m x n, V n x (k+1), U m x (k+1),
+    βu₁ = b and L the (k+1) x (k+1) lower bidiagonal matrix with A V[:, :k] = U L[:, :k] and Aᵀ U = V Lᵀ.
+    At: Aᵀ (SciPy or CsrOperator); by default it is formed once for the call."""
+    P = _ProcessCall("golub_kahan", A, [b], At, True)
+    try:
+        pb = P.vec_in(b, P.m, "b")
+        V, pV = P.basis(P.n, k)
+        U, pU = P.basis(P.m, k)
+        beta, nz = C.c_double(), np.zeros(max(2 * k + 1, 0), np.float64)
+        P.run(P.At._csr if P.At else None, int(k), P.dt, pb, pV, pU, C.byref(beta),
+              nz.ctypes.data_as(C.POINTER(C.c_double)), _flags(allow_breakdown))
+        return (P.out(V, P.n, k), P.out(U, P.m, k), beta.value,
+                _csc(nz.astype(P.dtype), _bidiag_structure(k), (k + 1, k + 1)))
+    finally:
+        P.close()
+
+
+def _two_sided(name, A, b, c, k, allow_breakdown, At, lb, lc):
+    P = _ProcessCall(name, A, [b, c], At, True)
+    try:
+        rows_v, rows_u = (P.n, P.n) if name == "nonhermitian_lanczos" else (P.m, P.n)
+        pb, pc = P.vec_in(b, lb(P), "b"), P.vec_in(c, lc(P), "c")
+        V, pV = P.basis(rows_v, k)
+        U, pU = P.basis(rows_u, k)
+        beta, gamma = C.c_double(), C.c_double()
+        nzT, nzH = np.zeros(max(3 * k - 1, 0), np.float64), np.zeros(max(3 * k - 1, 0), np.float64)
+        P.run(P.At._csr if P.At else None, int(k), P.dt, pb, pc, pV, pU, C.byref(beta), C.byref(gamma),
+              nzT.ctypes.data_as(C.POINTER(C.c_double)), nzH.ctypes.data_as(C.POINTER(C.c_double)), _flags(allow_breakdown))
+        s = _tridiag_structure(k)
+        return (P.out(V, rows_v, k), beta.value, _csc(nzT.astype(P.dtype), s, (k + 1, k)), P.out(U, rows_u, k), gamma.value,
+                _csc(nzH.astype(P.dtype), s, (k + 1, k)))
+    finally:
+        P.close()
+
+
+def nonhermitian_lanczos(A, b, c, k: int, *, allow_breakdown: bool = False, At=None):
+    """V, β, T, U, γᴴ, Tᴴ = nonhermitian_lanczos(A, b, c, k) (src/krylov_processes.jl:133-224): square A, βv₁ = b,
+    γᴴu₁ = c, A V[:, :k] = V T and Aᵀ U[:, :k] = U Tᴴ with Uᵀ V = I.  When cᵀb == 0 (allow_breakdown) V[:, 0] and U[:, 0]
+    are zero, where the reference leaves them undefined."""
+    return _two_sided("nonhermitian_lanczos", A, b, c, k, allow_breakdown, At, lambda P: P.n, lambda P: P.n)
+
+
+def saunders_simon_yip(A, b, c, k: int, *, allow_breakdown: bool = False, At=None):
+    """V, β, T, U, γᴴ, Tᴴ = saunders_simon_yip(A, b, c, k) (src/krylov_processes.jl:431-524): A is m x n, V m x (k+1),
+    U n x (k+1), βv₁ = b, γᴴu₁ = c, A U[:, :k] = V T and Aᵀ V[:, :k] = U Tᴴ."""
+    return _two_sided("saunders_simon_yip", A, b, c, k, allow_breakdown, At, lambda P: P.m, lambda P: P.n)
+
+
+__all__ += ["hermitian_lanczos", "arnoldi", "golub_kahan", "nonhermitian_lanczos", "saunders_simon_yip"]

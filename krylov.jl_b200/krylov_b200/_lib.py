@@ -140,6 +140,12 @@ SIGNATURES = {
     "kb200_csr_dict": (_I, [_P, C.POINTER(_I)]),
     "kb200_spmm_csr": (_I, [_P, _P, _I, _P, _P, _I]),
     "krylov_b200_block_panel_op": (_I, [_P, _I, _I, _I, _D, _P, _P, _D, _P, _P, _P]),
+    "kb200_ctx_launch_count": (_LL, [_P]),
+    "kb200_hermitian_lanczos": (_I, [_P, _P, _I, _I, _P, _P, C.POINTER(_D), C.POINTER(_D), _I]),
+    "kb200_arnoldi": (_I, [_P, _P, _I, _I, _P, _P, C.POINTER(_D), C.POINTER(_D), _I]),
+    "kb200_golub_kahan": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, C.POINTER(_D), C.POINTER(_D), _I]),
+    "kb200_nonhermitian_lanczos": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P] + [C.POINTER(_D)] * 4 + [_I]),
+    "kb200_saunders_simon_yip": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P] + [C.POINTER(_D)] * 4 + [_I]),
 }
 
 _LIB = None
