@@ -1,9 +1,8 @@
 """ctypes front-end of the CPU restatement of bilqr! / trilqr! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_adjoint.h, built with the shared BLAS-1 wrappers of krylov_oracle_impl.h by adjoint.mk into a library
-that links against the shared oracle library and uses its test knobs: oracle.dot_mode (re-exported here) switches the
-dot products of these solvers as of every other family.  The adjoint problem
+krylov_oracle_adjoint.h, built into the oracle library that oracle.py builds and loads, so oracle.dot_mode
+(re-exported here) switches the dot products of these solvers as of every other family.  The adjoint problem
 generators of test/test_utils.jl:212-283 (and the ODE / PDE discretizations of test/get_div_grad.jl:27-138 they use)
 are restated here.  Parity pinning: tests/test_oracle_adjoint.py and tests/golden/oracle_adjoint.json (frozen
 histories).
@@ -12,39 +11,12 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle import oracle as _shared
 from oracle.oracle import (_ITER_CB, Stats, _csr, _opts, _p, _suf, _vec, bc_breakdown, dot_mode,  # noqa: F401
-                           kron_unsymmetric)
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_SOURCES = ("krylov_oracle_adjoint.c", "krylov_oracle_adjoint.h", "krylov_oracle_impl.h", "adjoint.mk",
-            "libkrylov_oracle.so")
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_adjoint.so with adjoint.mk (when missing or older than its sources), after the
-    shared oracle library it links against."""
-    _shared.build()
-    so = os.path.join(_HERE, "libkrylov_oracle_adjoint.so")
-    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "adjoint.mk"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _shared.lib()                 # the shared library first: this one resolves the test knobs against it
-        _LIB = C.CDLL(build())
-    return _LIB
+                           kron_unsymmetric, lib)
 
 
 def _adjoint(tri, A, b, c, x0, y0, transfer, timemax, callback, dtype, kw):

@@ -1,49 +1,23 @@
 """ctypes front-end of the CPU restatement of cgne! and crmr! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_cgne.h, built with the shared BLAS-1 wrappers of krylov_oracle_impl.h by cgne.mk into a library that links
-against the shared oracle library and uses its test knobs: oracle.dot_mode (re-exported here) switches the dot products
-of these solvers as of every other family.  The generators of test/test_utils.jl that the reference's test/test_cgne.jl
-and test/test_crmr.jl use are re-exported from leastnorm_oracle.py and oracle.py.
+krylov_oracle_cgne.h, built into the oracle library that oracle.py builds and loads, so oracle.dot_mode (re-exported
+here) switches the dot products of these solvers as of every other family.  The generators of test/test_utils.jl
+that the reference's test/test_cgne.jl and test/test_crmr.jl use are re-exported from leastnorm_oracle.py and
+oracle.py.
 Parity pinning: tests/test_oracle_cgne_crmr.py and tests/golden/oracle_cgne_crmr.json (frozen histories).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle import oracle as _shared
 from oracle.leastnorm_oracle import (over_consistent, over_inconsistent, small_sp, square_consistent,  # noqa: F401
                                      square_inconsistent, under_consistent, under_inconsistent, zero_rhs)
-from oracle.oracle import _ITER_CB, Stats, _csr, _p, _suf, _vec, dot_mode, square_preconditioned  # noqa: F401
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_SOURCES = ("krylov_oracle_cgne.c", "krylov_oracle_cgne.h", "krylov_oracle_impl.h", "cgne.mk", "libkrylov_oracle.so")
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_cgne.so with cgne.mk (when missing or older than its sources), after the shared
-    oracle library it links against."""
-    _shared.build()
-    so = os.path.join(_HERE, "libkrylov_oracle_cgne.so")
-    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "cgne.mk"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _shared.lib()                 # the shared library first: this one resolves the test knobs against it
-        _LIB = C.CDLL(build())
-    return _LIB
+from oracle.oracle import _ITER_CB, Stats, _csr, _p, _suf, _vec, dot_mode, lib, square_preconditioned  # noqa: F401
 
 
 class CgneOpts(C.Structure):

@@ -34,6 +34,11 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #include "krylov_oracle_lslq.h"
 #include "krylov_oracle_biorth.h"
 #include "krylov_oracle_ares.h"
+#include "krylov_oracle_adjoint.h"
+#include "krylov_oracle_leastnorm.h"
+#include "krylov_oracle_lnlq.h"
+#include "krylov_oracle_cgne.h"
+#include "krylov_oracle_processes.h"
 #undef REAL
 #undef SUF
 #undef SQRT
@@ -60,6 +65,11 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #include "krylov_oracle_lslq.h"
 #include "krylov_oracle_biorth.h"
 #include "krylov_oracle_ares.h"
+#include "krylov_oracle_adjoint.h"
+#include "krylov_oracle_leastnorm.h"
+#include "krylov_oracle_lnlq.h"
+#include "krylov_oracle_cgne.h"
+#include "krylov_oracle_processes.h"
 
 
 /* ---------------------------------------------------------------------------

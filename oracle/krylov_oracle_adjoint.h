@@ -1,7 +1,7 @@
 /*
  * krylov_oracle_adjoint.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included
  * first).  Literal restatement of bilqr! (src/bilqr.jl:115-484) and trilqr! (src/trilqr.jl:114-461) on the BLAS-1
- * wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle_adjoint.c and loaded by oracle/adjoint_oracle.py.
+ * wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle.c and loaded by oracle/adjoint_oracle.py.
  * Parity pinning: tests/test_oracle_adjoint.py (the reference's assertions of test/test_bilqr.jl and
  * test/test_trilqr.jl) and tests/golden/oracle_adjoint.json (frozen histories).
  */

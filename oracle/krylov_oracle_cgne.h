@@ -2,7 +2,7 @@
  * krylov_oracle_cgne.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included first).
  * Restatement of cgne! (src/cgne.jl:134-252) and crmr! (src/crmr.jl:132-244), CG and CR on A A^T y = b with
  * x = A^T y: the least-norm solution of A x = b on an m x n CSR matrix.  Written from the algorithm on the BLAS-1
- * wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle_cgne.c and loaded by oracle/cgne_oracle.py.  A^T is
+ * wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle.c and loaded by oracle/cgne_oracle.py.  A^T is
  * passed as its own CSR (n rows, ascending row indices of A in each row).  N (m entries, on the residual space) is a
  * diagonal or NULL; lambda >= 0 regularizes through the m-vector s.
  * Parity pinning: tests/test_oracle_cgne_crmr.py (the reference's assertions of test/test_cgne.jl and

@@ -3,7 +3,7 @@
  * first).  Restatement of the least-norm solvers, min ||x|| subject to A x = b with x = A^T y, on an m x n CSR matrix:
  *   craig!    src/craig.jl:174-405   (CG on A A^T y = b)
  *   craigmr!  src/craigmr.jl:161-396 (MINRES on A A^T y = b)
- * written from the algorithm on the BLAS-1 wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle_leastnorm.c
+ * written from the algorithm on the BLAS-1 wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle.c
  * and loaded by oracle/leastnorm_oracle.py.  A^T is passed as its own CSR (n rows, ascending row indices of A in each
  * row).  M (m entries) and N (n entries) are diagonals or NULL.
  * Parity pinning: tests/test_oracle_leastnorm.py (the reference's assertions of test/test_craig.jl and

@@ -2,7 +2,7 @@
  * krylov_oracle_lnlq.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included first).
  * Restatement of lnlq! (src/lnlq.jl:168-568), SYMMLQ on A A^T y = b with x = A^T y: the least-norm solution of
  * A x = b on an m x n CSR matrix, with the sigma-based upper bounds on ||x - x*|| and ||y - y*||.  Written from the
- * algorithm on the BLAS-1 wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle_lnlq.c and loaded by
+ * algorithm on the BLAS-1 wrappers of krylov_oracle_impl.h, instantiated by krylov_oracle.c and loaded by
  * oracle/lnlq_oracle.py.  A^T is passed as its own CSR (n rows, ascending row indices of A in each row).  M (m entries)
  * and N (n entries) are diagonals or NULL.
  * Parity pinning: tests/test_oracle_lnlq.py (the reference's assertions of test/test_lnlq.jl) and

@@ -2,7 +2,7 @@
  * krylov_oracle_processes.h -- TEST INFRASTRUCTURE ONLY (same status as krylov_oracle_impl.h, which must be included
  * first).  Restatement of the Krylov processes of src/krylov_processes.jl (hermitian_lanczos, arnoldi, golub_kahan,
  * nonhermitian_lanczos, saunders_simon_yip), real case, written from the algorithms on the BLAS-1 wrappers of
- * krylov_oracle_impl.h.  Instantiated by krylov_oracle_processes.c and loaded by oracle/processes_oracle.py.
+ * krylov_oracle_impl.h.  Instantiated by krylov_oracle.c and loaded by oracle/processes_oracle.py.
  * V and U are column-major with leading dimension = the vector's length.  T, Th and L are the nzval arrays of the
  * reference's SparseMatrixCSC outputs (zeroed here first, like zeros(R, ...)); H is dense (k+1) x k column-major.
  * A^T is passed as its own CSR.  Return value: 0, or the breakdown kind (1-based, in the order the reference checks)

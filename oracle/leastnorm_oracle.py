@@ -1,50 +1,23 @@
 """ctypes front-end of the CPU restatement of craig! / craigmr! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
-krylov_oracle_leastnorm.h, built with the shared BLAS-1 wrappers of krylov_oracle_impl.h by leastnorm.mk into a library
-that links against the shared oracle library and uses its test knobs: oracle.dot_mode (re-exported here) switches the
-dot products of these solvers as of every other family.  The generators of test/test_utils.jl that the reference's
-test/test_craig.jl and test/test_craigmr.jl use are restated here, or re-exported from oracle.py and lsq_oracle.py.
+krylov_oracle_leastnorm.h, built into the oracle library that oracle.py builds and loads, so oracle.dot_mode
+(re-exported here) switches the dot products of these solvers as of every other family.  The generators of
+test/test_utils.jl that the reference's test/test_craig.jl and test/test_craigmr.jl use are restated here, or
+re-exported from oracle.py and lsq_oracle.py.
 Parity pinning: tests/test_oracle_leastnorm.py and tests/golden/oracle_leastnorm.json (frozen histories).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle import oracle as _shared
 from oracle.lsq_oracle import regularization, saddle_point, sqd  # noqa: F401
-from oracle.oracle import (_ITER_CB, Stats, _csr, _p, _suf, _vec, dot_mode, square_inconsistent,  # noqa: F401
-                           two_preconditioners, zero_rhs)
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_SOURCES = ("krylov_oracle_leastnorm.c", "krylov_oracle_leastnorm.h", "krylov_oracle_impl.h", "leastnorm.mk",
-            "libkrylov_oracle.so")
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_leastnorm.so with leastnorm.mk (when missing or older than its sources), after the
-    shared oracle library it links against."""
-    _shared.build()
-    so = os.path.join(_HERE, "libkrylov_oracle_leastnorm.so")
-    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "leastnorm.mk"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _shared.lib()                 # the shared library first: this one resolves the test knobs against it
-        _LIB = C.CDLL(build())
-    return _LIB
+from oracle.oracle import (_ITER_CB, Stats, _csr, _p, _suf, _vec, dot_mode, lib,  # noqa: F401
+                           square_inconsistent, two_preconditioners, zero_rhs)
 
 
 class LnOpts(C.Structure):

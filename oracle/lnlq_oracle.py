@@ -1,50 +1,24 @@
 """ctypes front-end of the CPU restatement of lnlq! -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solver lives in
-krylov_oracle_lnlq.h, built with the shared BLAS-1 wrappers of krylov_oracle_impl.h by lnlq.mk into a library that links
-against the shared oracle library and uses its test knobs: oracle.dot_mode (re-exported here) switches the dot products
-of this solver as of every other family.  The generators of test/test_utils.jl that the reference's test/test_lnlq.jl
-uses are re-exported from leastnorm_oracle.py, which restates them for CRAIG and CRAIGMR.
+krylov_oracle_lnlq.h, built into the oracle library that oracle.py builds and loads, so oracle.dot_mode (re-exported
+here) switches the dot products of this solver as of every other family.  The generators of test/test_utils.jl
+that the reference's test/test_lnlq.jl uses are re-exported from leastnorm_oracle.py, which restates them for CRAIG
+and CRAIGMR.
 Parity pinning: tests/test_oracle_lnlq.py and tests/golden/oracle_lnlq.json (frozen histories).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle import oracle as _shared
 from oracle.leastnorm_oracle import (over_consistent, regularization, saddle_point, small_ln, small_sp,  # noqa: F401
                                      small_sqd, sqd, square_consistent, two_preconditioners, under_consistent,
                                      zero_rhs)
-from oracle.oracle import _ITER_CB, Stats, _csr, _p, _suf, _vec, dot_mode  # noqa: F401
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_SOURCES = ("krylov_oracle_lnlq.c", "krylov_oracle_lnlq.h", "krylov_oracle_impl.h", "lnlq.mk", "libkrylov_oracle.so")
-
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_lnlq.so with lnlq.mk (when missing or older than its sources), after the shared
-    oracle library it links against."""
-    _shared.build()
-    so = os.path.join(_HERE, "libkrylov_oracle_lnlq.so")
-    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "lnlq.mk"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _shared.lib()                 # the shared library first: this one resolves the test knobs against it
-        _LIB = C.CDLL(build())
-    return _LIB
+from oracle.oracle import _ITER_CB, Stats, _csr, _p, _suf, _vec, dot_mode, lib  # noqa: F401
 
 
 class LnlqOpts(C.Structure):

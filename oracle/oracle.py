@@ -13,6 +13,7 @@ residual histories on the benchmark configs: parity unpinned (no Julia here).
 from __future__ import annotations
 
 import ctypes as C
+import glob
 import math
 import os
 import subprocess
@@ -22,9 +23,7 @@ import scipy.sparse as sp
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
-_SOURCES = ("krylov_oracle.c", "krylov_oracle_impl.h", "krylov_oracle_siblings.h", "krylov_oracle_block.h",
-            "krylov_oracle_lsq.h", "krylov_oracle_cgls.h", "krylov_oracle_lslq.h", "krylov_oracle_biorth.h",
-            "krylov_oracle_ares.h", "Makefile")
+_SOURCES = "krylov_oracle*.[ch]", "Makefile"    # the one translation unit, every family's header, the recipe
 _ITER_CB = C.CFUNCTYPE(C.c_int, C.c_int, C.c_void_p)    # oracle_iter_cb: nonzero stops the solve
 
 
@@ -46,7 +45,7 @@ def build(force: bool = False) -> str:
     """Compile oracle/libkrylov_oracle.so, every solver family's oracle, with the committed Makefile (when missing or
     older than its sources)."""
     so = os.path.join(_HERE, "libkrylov_oracle.so")
-    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
+    srcs = [f for pattern in _SOURCES for f in glob.glob(os.path.join(_HERE, pattern))]
     if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["make", "-C", _HERE, "-s"])
     return so

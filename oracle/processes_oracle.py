@@ -1,8 +1,8 @@
 """ctypes front-end of the CPU restatement of the Krylov processes -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The processes live in
-krylov_oracle_processes.h, built with the shared BLAS-1 wrappers of krylov_oracle_impl.h by processes.mk into a library
-that links against the shared oracle library, so oracle.dot_mode (re-exported here) switches their dot products too.
+krylov_oracle_processes.h, built into the oracle library that oracle.py builds and loads, so oracle.dot_mode
+(re-exported here) switches their dot products too.
 Each function returns the reference's outputs with the coefficient matrices as their nzval arrays (dense H for
 arnoldi); an exact breakdown without allow_breakdown raises ProcessBreakdown with the reference's message.
 Parity pinning: tests/test_oracle_processes.py and tests/golden/oracle_processes.json.
@@ -10,19 +10,11 @@ Parity pinning: tests/test_oracle_processes.py and tests/golden/oracle_processes
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle import oracle as _shared
-from oracle.oracle import _csr, _p, _suf, _vec, dot_mode  # noqa: F401
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-_SOURCES = ("krylov_oracle_processes.c", "krylov_oracle_processes.h", "krylov_oracle_impl.h", "processes.mk",
-            "libkrylov_oracle.so")
+from oracle.oracle import _csr, _p, _suf, _vec, dot_mode, lib  # noqa: F401
 
 # the reference's messages, in the order each process checks them (kind 1, 2, ...)
 MESSAGES = {
@@ -39,24 +31,6 @@ MESSAGES = {
 class ProcessBreakdown(RuntimeError):
     """The reference's ErrorException on an exact breakdown with allow_breakdown = false."""
 
-
-def build(force: bool = False) -> str:
-    """Compile oracle/libkrylov_oracle_processes.so with processes.mk (when missing or older than its sources), after the
-    shared oracle library it links against."""
-    _shared.build()
-    so = os.path.join(_HERE, "libkrylov_oracle_processes.so")
-    srcs = [os.path.join(_HERE, f) for f in _SOURCES]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "processes.mk"])
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _shared.lib()
-        _LIB = C.CDLL(build())
-    return _LIB
 
 
 def _call(name, dtype, args):

@@ -1,9 +1,13 @@
-"""The parity bar of the GPU solver tests against the CPU oracle, shared by the solver families' GPU tests.
+"""The parity bar of the GPU solver tests against the CPU oracle, and the other helpers shared by the solver families'
+tests: the golden-case generators, the gradient operators and their untiled twins, launch counting and the ring-depth
+sweep.
 
 A GPU history must follow the oracle's within TOL relative at every iteration, or within 10x the oracle's own change
 under a few-ulp perturbation of b where that is larger: the device's tree-ordered dot products differ from the oracle's
 sequential sums by a few roundings, so the oracle's sensitivity to such a change is the measured width of the bar."""
 import functools
+import importlib.util
+import os
 
 import numpy as np
 import scipy.sparse as sp
@@ -123,10 +127,69 @@ def shapes():
     b60, A60, *_ = lsq_oracle.lsq_test(60, 30, 3, 3, 0)
     Aw = sp.csr_matrix(A60.T)                                   # 30 x 60: m < n
     D = sp.csr_matrix(lsq_oracle.ddx(50))                       # 50 x 51
-    rp, ci, va = P.grad_csr(7)
-    G = sp.csr_matrix((va, ci, rp), shape=(len(rp) - 1, 7 ** 3))
+    G = grad(7)
     R1, R2 = rect_with_gaps(300, 120, 1), rect_with_gaps(90, 200, 2)
     Sq = sp.csr_matrix(sp.random(200, 200, density=0.05, random_state=3) + 4 * sp.identity(200))
     return {"square": (Sq, rng.standard_normal(200)), "tall_lstp": (A60, b60), "wide_lstp": (Aw, rng.standard_normal(30)),
             "ddx": (D, rng.standard_normal(50)), "grad7": (G, rng.standard_normal(G.shape[0])),
             "tall_gaps": (R1, rng.standard_normal(300)), "wide_gaps": (R2, rng.standard_normal(90))}
+
+
+def golden_module(name):
+    """tests/golden/gen_golden_<name>.py loaded as a module: the generator of a family's frozen oracle cases."""
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", f"gen_golden_{name}.py")
+    spec = importlib.util.spec_from_file_location(f"gen_golden_{name}", path)
+    module = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(module)
+    return module
+
+
+def grad(N):
+    """The gradient of the N³ grid (problems.grad_csr) as a SciPy CSR matrix: one row per grid edge, N³ columns."""
+    rp, ci, va = P.grad_csr(N)
+    return sp.csr_matrix((va, ci, rp), shape=(len(rp) - 1, N ** 3))
+
+
+def dense_line(A, row):
+    """A plus a dense row (row=True) or column: long enough that its tile, or the tile of Aᵀ, is untiled."""
+    A = sp.lil_matrix(A)
+    line = 1.0 + np.arange(A.shape[1 if row else 0]) / A.shape[1 if row else 0]
+    if row:
+        A[0, :] = line
+    else:
+        A[:, 0] = line.reshape(-1, 1)
+    return sp.csr_matrix(A)
+
+
+def launches_per_iteration(kb, solver, A, b, fused=True, *, extra_iter=0, **solve_kw):
+    """The kernel launches one more iteration costs: the difference between solves of 12 and 6 iterations, over 6.
+    solve_kw must make the solve run to itmax, where it reports itmax + extra_iter iterations (LNLQ counts the
+    terminal pass too)."""
+    def launches(itmax):
+        ws = kb.krylov_workspace(solver, A.shape[0], A.shape[1], np.float64)
+        try:
+            ws.solve(A, b, fused=fused, itmax=itmax, **solve_kw)
+            assert ws.stats.niter == itmax + extra_iter, ws.stats.status
+            return ws.launches
+        finally:
+            ws.free()
+    return (launches(12) - launches(6)) / 6
+
+
+def assert_ring_depth_changes_no_bit(monkeypatch, run):
+    """run() solves and returns its outcome as a tuple of bytes and scalars.  At 3, 2 and 1 CTAs per SM, every ring
+    depth from 1 to 4 must give the same tuple (KB200_CTAS_PER_SM / KB200_STAGES are read when an operator is planned).
+    The CTA count sets the grid, and with it the order of the grid-wide sums, so the comparison is within one CTA
+    count; the default plan must equal one of the forced ones."""
+    monkeypatch.delenv("KB200_STAGES", raising=False)
+    monkeypatch.delenv("KB200_CTAS_PER_SM", raising=False)
+    default = run()
+    ref, default_forced = {}, False
+    for cps in (3, 2, 1):
+        for stages in (1, 2, 3, 4):
+            monkeypatch.setenv("KB200_CTAS_PER_SM", str(cps))
+            monkeypatch.setenv("KB200_STAGES", str(stages))
+            out = run()
+            default_forced = default_forced or out == default
+            assert out == ref.setdefault(cps, out), (cps, stages)
+    assert default_forced

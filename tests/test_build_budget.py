@@ -60,7 +60,10 @@ def test_staged_spmv_family_register_budget():
 
 
 # The fused passes of each solver family (fused_phases.cu): family -> [(filter on the demangled kernel name,
-# {kernel template: instantiations it matches, Float32 and Float64 together})].
+# {kernel template: instantiations it matches, Float32 and Float64 together}[, foreign])].  The optional foreign field
+# is a pair (names set aside or None, pattern): the pattern must not match what remains of any kernel name the filter
+# matches, so those kernels carry no other family's functor.
+_NOT_LSQ_FUNCTORS = (None, r"kb::(Craig|Cgls|Crls|Lnlq|Car|Minares|Lsq)")
 PHASE_KERNELS = {
     "lsq": [(r"kb::(LsqP|LsqrP3|LsmrP3)", {"spmv_epi_tma": 6,        # P1, P2 (LSQR), P2 (LSMR) x Float32 / Float64
                                            "stream_epi": 4})],       # the LSQR and LSMR P3 passes x 2
@@ -83,19 +86,36 @@ PHASE_KERNELS = {
     "leastnorm": [(r"kb::Craig", {"spmv_epi_tma": 8,                 # CRAIG C1, C2 and CRAIGMR R1, R2 x 2
                                   "spmv_epi_rows": 8,
                                   "stream_epi": 4})],                # CRAIG's x flush and CRAIGMR's R3 x 2
+    # L1 on A and L2 on Aᵀ (staged and untiled), the y / w̄ flush and the terminal x pass, x Float32 / Float64
+    "lnlq": [(r"kb::Lnlq", {"spmv_epi_tma": 4, "spmv_epi_rows": 4, "stream_epi": 4})],
+    "cgne": [(r"kb::Cgne", {"spmv_epi_tma": 4,                       # E1 on A, E2 on Aᵀ, staged and untiled, x 2
+                            "spmv_epi_rows": 4,
+                            "stream_epi": 0}, _NOT_LSQ_FUNCTORS)],
+    "crmr": [(r"kb::Crmr", {"spmv_epi_tma": 4,                       # R1, R3 and the streaming R2, R4, x 2
+                            "spmv_epi_rows": 4,
+                            "stream_epi": 4}, _NOT_LSQ_FUNCTORS)],
+    # one SpMV epilogue on a divided gather (staged and untiled), the streaming update / dot pass and the final
+    # normalisation pass, x Float32 / Float64; besides their own Proc* functors the kernels name only shared types
+    "processes": [(r"kb::Proc", {"spmv_epi_tma": 2, "spmv_epi_rows": 2, "stream_epi": 4},
+                   (r"kb::Proc\w+|kb::NoFin|kb::Csr\b|kb::DistComm", r"kb::[A-Z]"))],
 }
+
+
+def _phase_kernels(pat):
+    """(demangled name, registers, spill bytes) of every fused_phases.cu kernel whose name matches pat."""
+    ents = _entries("fused_phases")
+    if not shutil.which("c++filt"):
+        pytest.skip("c++filt not available")
+    dm = _demangle([e[0] for e in ents])
+    return [(dm[n], r, s) for n, r, s in ents if re.search(pat, dm[n])]
 
 
 @pytest.mark.parametrize("family", sorted(PHASE_KERNELS))
 def test_phase_kernels_fit_three_ctas_per_sm(family):
     """The fused passes keep the 3-CTA/SM budget of the staged SpMV family: every spmv_epi_tma instantiation uses at
     most 72 registers (288 threads x 72 x 3 CTAs fill the 64K register file), and no kernel of the family spills."""
-    ents = _entries("fused_phases")
-    if not shutil.which("c++filt"):
-        pytest.skip("c++filt not available")
-    dm = _demangle([e[0] for e in ents])
-    for pat, counts in PHASE_KERNELS[family]:
-        hit = [(dm[n], r, s) for n, r, s in ents if re.search(pat, dm[n])]
+    for pat, counts, *_ in PHASE_KERNELS[family]:
+        hit = _phase_kernels(pat)
         for tmpl, count in counts.items():
             assert len([e for e in hit if e[0].startswith(f"void kb::{tmpl}<")]) == count, (pat, tmpl, hit)
         f32 = sorted(e[0].replace("float", "double") for e in hit if "<float" in e[0])
@@ -104,6 +124,16 @@ def test_phase_kernels_fit_three_ctas_per_sm(family):
             assert spill == 0, (name, regs, spill)
             if "spmv_epi_tma<" in name:
                 assert regs <= 72, (name, regs)
+
+
+@pytest.mark.parametrize("family", sorted(f for f, rows in PHASE_KERNELS.items() if any(len(r) > 2 for r in rows)))
+def test_phase_kernels_carry_no_foreign_functor(family):
+    """The kernels of a row with a foreign field carry no other family's functor, so the instantiation counts that
+    other rows pin by name stay theirs."""
+    for pat, _, *foreign in PHASE_KERNELS[family]:
+        for own, other in foreign:
+            for name, _, _ in _phase_kernels(pat):
+                assert not re.search(other, re.sub(own, "", name) if own else name), (pat, name)
 
 
 def test_block_fast_kernels_do_not_spill():

@@ -3,7 +3,6 @@ count, status, solved_primal and solved_dual; both residual histories within par
 10x the oracle's own sensitivity to a few-ulp change of b and c, where that is larger); x and y within 1e-6 relative.
 Both paths: the fused one (3 launches per iteration) and fused = 0.  Float32 within the measured dot-rounding envelope."""
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -19,9 +18,7 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOLVERS = ["bilqr", "trilqr"]
 KEYS = ("residuals_primal", "residuals_dual")
-_spec = importlib.util.spec_from_file_location("gen_golden_adjoint", os.path.join(HERE, "golden", "gen_golden_adjoint.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = parity.golden_module("adjoint")
 
 
 @pytest.fixture(scope="module")

@@ -3,7 +3,6 @@ same iteration count, `solved` and status; residual histories within 1e-6 relati
 oracle's own sensitivity to a few-ulp change of b, where that is larger); x within the same bar.  Float32 within the
 measured dot-rounding envelope (DESIGN.md §5).  The fused path (3 launches per iteration) against the primitive one."""
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -18,9 +17,7 @@ from parity import TOL
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOLVERS = ["bilq", "qmr"]
-_spec = importlib.util.spec_from_file_location("gen_golden_bilq_qmr", os.path.join(HERE, "golden", "gen_golden_bilq_qmr.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = parity.golden_module("bilq_qmr")
 
 
 @pytest.fixture(scope="module")

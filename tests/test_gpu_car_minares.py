@@ -4,7 +4,6 @@ iteration (or 10x the oracle's own sensitivity to a few-ulp change of b, where t
 Float32 within the measured dot-rounding envelope (DESIGN.md §5).  The fused path (3 launches per iteration) against
 the primitive one."""
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -19,9 +18,7 @@ from parity import TOL
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOLVERS = ["car", "minares"]
-_spec = importlib.util.spec_from_file_location("gen_golden_car_minares", os.path.join(HERE, "golden", "gen_golden_car_minares.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = parity.golden_module("car_minares")
 KAT = [(s, name) for s, cs in G.cases().items() for name in sorted(cs)]
 
 

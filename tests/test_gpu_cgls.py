@@ -3,7 +3,6 @@ same iteration count, status and `inconsistent`; residual and Aᴴ-residual hist
 iteration (or 10x the oracle's own sensitivity to a few-ulp change of b, where that is larger); x within 1e-6."""
 import ctypes as C
 import functools
-import importlib.util
 import os
 
 import numpy as np
@@ -18,9 +17,7 @@ from parity import TOL
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOLVERS = ["cgls", "crls"]
-_spec = importlib.util.spec_from_file_location("gen_golden_cgls", os.path.join(HERE, "golden", "gen_golden_cgls.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = parity.golden_module("cgls")
 
 
 @pytest.fixture(scope="module")

@@ -4,7 +4,6 @@ every iteration (or 10x the oracle's own sensitivity to a few-ulp change of b, w
 relative where the counts are steady.  Both paths: the fused one (2 launches per CGNE iteration, 4 per CRMR iteration)
 and fused = 0."""
 import ctypes as C
-import importlib.util
 import json
 import os
 
@@ -14,7 +13,6 @@ import scipy.sparse as sp
 
 import parity
 from krylov_b200 import _lib
-from krylov_b200 import problems as P
 from parity import TOL
 
 pytestmark = pytest.mark.gpu
@@ -49,19 +47,11 @@ def compare(O, kb, solver, A, b, **kw):
                           **kw)
 
 
-def golden_cases():
-    spec = importlib.util.spec_from_file_location("gen_golden_cgne_crmr",
-                                                  os.path.join(HERE, "golden", "gen_golden_cgne_crmr.py"))
-    G = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(G)
-    return G.cases()
-
-
 @pytest.mark.parametrize("fused", [True, False])
 @pytest.mark.parametrize("case", sorted(GOLD))
 def test_oracle_cases(O, kb, case, fused):
     """The problems of test_cgne.jl / test_crmr.jl; those with N or λ > 0 run the primitive path whatever `fused`."""
-    solver, A, b, kw = golden_cases()[case]
+    solver, A, b, kw = parity.golden_module("cgne_crmr").cases()[case]
     # small_sp runs a 5-iteration CGNE to itmax on an inconsistent system: its last steps work on rounding noise
     compare(O, kb, solver, A, b, fused=fused, xtol=None if "small_sp" in case else TOL, **kw)
 
@@ -119,93 +109,36 @@ def test_callback_preconditioner_matches_its_diagonal(O, kb, solver):
     assert np.linalg.norm(x - xo) <= TOL * np.linalg.norm(xo)
 
 
-def _launches(kb, solver, A, b, fused, itmax):
-    ws = kb.krylov_workspace(solver, A.shape[0], A.shape[1], np.float64)
-    try:
-        ws.solve(A, b, fused=fused, itmax=itmax, **ZERO_TOL)
-        assert ws.stats.niter == itmax, ws.stats.status
-        return ws.launches
-    finally:
-        ws.free()
-
-
-def launches_per_iteration(kb, solver, A, b, fused=True):
-    return (_launches(kb, solver, A, b, fused, 12) - _launches(kb, solver, A, b, fused, 6)) / 6
-
-
-def _grad(N):
-    rp, ci, va = P.grad_csr(N)
-    return sp.csr_matrix((va, ci, rp), shape=(len(rp) - 1, N ** 3))
-
-
-def _div(N):
-    return sp.csr_matrix(_grad(N).T)
-
-
-def _dense_line(A, row):
-    """A plus a dense row (row=True) or column: long enough that its tile, or the tile of Aᵀ, is untiled."""
-    A = sp.lil_matrix(A)
-    line = 1.0 + np.arange(A.shape[1 if row else 0]) / A.shape[1 if row else 0]
-    if row:
-        A[0, :] = line
-    else:
-        A[:, 0] = line.reshape(-1, 1)
-    return sp.csr_matrix(A)
-
-
 @pytest.mark.parametrize("solver,want", [("cgne", 2), ("crmr", 4)])
 def test_fused_path_runs_and_untiled_twin_matches(O, kb, solver, want):
     """2 (CGNE) and 4 (CRMR) launches per iteration on a staged operator (the divergence of the 24³ grid, m < n), and
     as many on its untiled twins (with a dense row: A untiled; with a dense column: Aᵀ untiled), whose first three
     iterations match the oracle.  From the fourth on, the dense line's outlying singular value makes both solvers'
     histories depend on the order of the sums (a NumPy restatement departs from the oracle there too)."""
-    D = _div(24)
+    D = sp.csr_matrix(parity.grad(24).T)
     rng = np.random.default_rng(3)
     b = D @ rng.standard_normal(D.shape[1])
-    assert launches_per_iteration(kb, solver, D, b) == want
-    assert launches_per_iteration(kb, solver, D, b, fused=False) > want
+    assert parity.launches_per_iteration(kb, solver, D, b, **ZERO_TOL) == want
+    assert parity.launches_per_iteration(kb, solver, D, b, fused=False, **ZERO_TOL) > want
     for row in (True, False):
-        U = _dense_line(_div(24), row)
+        U = parity.dense_line(parity.grad(24).T, row)
         bu = U @ rng.standard_normal(U.shape[1])
-        assert launches_per_iteration(kb, solver, U, bu) == want
+        assert parity.launches_per_iteration(kb, solver, U, bu, **ZERO_TOL) == want
         compare(O, kb, solver, U, bu, fused=True, itmax=3, **ZERO_TOL)
 
 
-RING_ENV = ("KB200_STAGES", "KB200_CTAS_PER_SM")
-
-
 @pytest.mark.parametrize("solver", SOLVERS)
-def test_ring_depth_changes_no_bit(kb, solver):
+def test_ring_depth_changes_no_bit(kb, monkeypatch, solver):
     """On an operator of about 10⁶ columns, at 3, 2 and 1 CTAs per SM, every ring depth gives byte-identical x,
-    histories, niter and status; the default plan is compared with the same plan forced."""
-    A = _div(72)                                                # 373 248 rows, 1 119 744 columns
+    histories, niter and status (parity.assert_ring_depth_changes_no_bit)."""
+    A = sp.csr_matrix(parity.grad(72).T)                        # the divergence: 373 248 rows, 1 119 744 columns
     b = A @ np.cos(np.arange(A.shape[1], dtype=np.float64))
     kw = dict(itmax=20, history=True, **ZERO_TOL)
-    ref = {}
-    saved = {k: os.environ.get(k) for k in RING_ENV}
-    try:
-        for cps in (None, 3, 2, 1):
-            for stages in ((None,) if cps is None else (1, 2, 3, 4)):
-                for k in RING_ENV:
-                    os.environ.pop(k, None)
-                if cps is not None:
-                    os.environ["KB200_CTAS_PER_SM"], os.environ["KB200_STAGES"] = str(cps), str(stages)
-                x, st = getattr(kb, solver)(A, b, **kw)
-                out = (x.tobytes(), np.asarray(st.residuals).tobytes(), np.asarray(st.Aresiduals).tobytes(), st.niter,
-                       st.status)
-                if cps is None:
-                    ref["default"] = out
-                    continue
-                if out == ref["default"]:
-                    ref.setdefault("default_cps", cps)
-                assert out == ref.setdefault(cps, out), (cps, stages)
-        assert "default_cps" in ref
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+
+    def run():
+        x, st = getattr(kb, solver)(A, b, **kw)
+        return x.tobytes(), np.asarray(st.residuals).tobytes(), np.asarray(st.Aresiduals).tobytes(), st.niter, st.status
+    parity.assert_ring_depth_changes_no_bit(monkeypatch, run)
 
 
 @pytest.mark.parametrize("fused", [True, False])
@@ -308,20 +241,3 @@ def test_c_abi_contract(O, kb, solver, sid):
             assert L.krylov_b200_get_vector(ws._h, name.encode(), C.byref(p)) == 0 and p.value, name
     finally:
         ws.free()
-
-
-def test_reference_c_programs():
-    """The cgne and crmr rows of the reference's test_all_solvers.c (built into oracle/_ref/ by build()) pass, and so
-    does every row that passed before."""
-    import subprocess
-    exe = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "test_all_solvers")
-    if not os.path.exists(exe):
-        pytest.skip("oracle/_ref/test_all_solvers was not built (reference tree absent at build time)")
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
-    rows = {ln.split()[0].lower(): ln for ln in out.stdout.splitlines() if ln.split()}
-    for name in ("cgne", "crmr"):
-        assert name in rows and "PASS" in rows[name], out.stdout[-3000:]
-    for name in ("cg", "cr", "minres", "gmres", "fom", "fgmres", "bicgstab", "cgs", "bilq", "qmr", "lsqr", "lsmr", "lslq",
-                 "cgls", "crls", "car", "minares", "diom", "dqgmres", "bilqr", "trilqr", "craig", "craigmr", "lnlq"):
-        if name in rows:
-            assert "PASS" in rows[name], rows[name]

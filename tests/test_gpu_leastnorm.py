@@ -11,7 +11,6 @@ import scipy.sparse as sp
 
 import parity
 from krylov_b200 import _lib
-from krylov_b200 import problems as P
 from parity import TOL
 
 pytestmark = pytest.mark.gpu
@@ -119,91 +118,37 @@ def test_shapes(O, kb, solver, shape, fused):
     compare(O, kb, solver, A, b, fused=fused, itmax=10, xtol=None if "lstp" in shape else TOL, **zero_tol(solver))
 
 
-def _launches(kb, solver, A, b, fused, itmax):
-    ws = getattr(kb, solver.capitalize() + "Workspace")(A.shape[0], A.shape[1], np.float64)
-    try:
-        ws.solve(A, b, fused=fused, itmax=itmax, **zero_tol(solver))
-        assert ws.stats.niter == itmax, ws.stats.status
-        return ws.launches
-    finally:
-        ws.free()
-
-
-def launches_per_iteration(kb, solver, A, b, fused=True):
-    return (_launches(kb, solver, A, b, fused, 12) - _launches(kb, solver, A, b, fused, 6)) / 6
-
-
-def _grad(N):
-    rp, ci, va = P.grad_csr(N)
-    return sp.csr_matrix((va, ci, rp), shape=(len(rp) - 1, N ** 3))
-
-
-def _dense_line(A, row):
-    """A plus a dense row (row=True) or column: long enough that its tile, or the tile of Aᵀ, is untiled."""
-    A = sp.lil_matrix(A)
-    line = 1.0 + np.arange(A.shape[1 if row else 0]) / A.shape[1 if row else 0]
-    if row:
-        A[0, :] = line
-    else:
-        A[:, 0] = line.reshape(-1, 1)
-    return sp.csr_matrix(A)
-
-
 @pytest.mark.parametrize("solver", SOLVERS)
 def test_fused_path_runs_and_untiled_twin_matches(O, kb, solver):
     """At most 3 launches per iteration on a staged operator (CRAIG 2, CRAIGMR 3), and as many on its untiled twin,
     the gradient with a dense row (A untiled) or a dense column (Aᵀ untiled), whose results match the oracle."""
-    G = _grad(24)
+    G = parity.grad(24)
     rng = np.random.default_rng(3)
     b = G @ rng.standard_normal(G.shape[1])
     want = {"craig": 2, "craigmr": 3}[solver]
-    assert launches_per_iteration(kb, solver, G, b) == want
-    assert launches_per_iteration(kb, solver, G, b, fused=False) > want
+    assert parity.launches_per_iteration(kb, solver, G, b, **zero_tol(solver)) == want
+    assert parity.launches_per_iteration(kb, solver, G, b, fused=False, **zero_tol(solver)) > want
     for row in (True, False):
-        U = _dense_line(_grad(24), row)
+        U = parity.dense_line(parity.grad(24), row)
         bu = U @ rng.standard_normal(U.shape[1])
-        assert launches_per_iteration(kb, solver, U, bu) == want
+        assert parity.launches_per_iteration(kb, solver, U, bu, **zero_tol(solver)) == want
         compare(O, kb, solver, U, bu, fused=True, itmax=40, xtol=None, **zero_tol(solver))
 
 
-RING_ENV = ("KB200_STAGES", "KB200_CTAS_PER_SM")
-
-
 @pytest.mark.parametrize("solver", SOLVERS)
-def test_ring_depth_changes_no_bit(kb, solver):
+def test_ring_depth_changes_no_bit(kb, monkeypatch, solver):
     """On an operator of about 10⁶ rows, at 3, 2 and 1 CTAs per SM, every ring depth gives byte-identical x, y,
-    histories, niter and status (KB200_STAGES / KB200_CTAS_PER_SM are read when an operator is planned).  The CTA count
-    sets the grid, and with it the order of the grid-wide sums, so the comparison is within one CTA count; the default
-    plan is compared with the same plan forced."""
-    G = _grad(72)                                               # 1 119 744 rows, 373 248 columns
+    histories, niter and status (parity.assert_ring_depth_changes_no_bit)."""
+    G = parity.grad(72)                                         # 1 119 744 rows, 373 248 columns
     A = sp.csr_matrix(G.T) if solver == "craig" else G          # both orientations of the gradient pair
     b = A @ np.cos(np.arange(A.shape[1], dtype=np.float64))
     kw = dict(itmax=20, history=True, **zero_tol(solver))
-    ref = {}
-    saved = {k: os.environ.get(k) for k in RING_ENV}
-    try:
-        for cps in (None, 3, 2, 1):
-            for stages in ((None,) if cps is None else (1, 2, 3, 4)):
-                for k in RING_ENV:
-                    os.environ.pop(k, None)
-                if cps is not None:
-                    os.environ["KB200_CTAS_PER_SM"], os.environ["KB200_STAGES"] = str(cps), str(stages)
-                x, y, st = getattr(kb, solver)(A, b, **kw)
-                out = (x.tobytes(), y.tobytes(), np.asarray(st.residuals).tobytes(), np.asarray(st.Aresiduals).tobytes(),
-                       st.niter, st.status)
-                if cps is None:
-                    ref["default"] = out
-                    continue
-                if out == ref["default"]:
-                    ref.setdefault("default_cps", cps)
-                assert out == ref.setdefault(cps, out), (cps, stages)
-        assert "default_cps" in ref                             # the default plan is one of the forced ones
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+
+    def run():
+        x, y, st = getattr(kb, solver)(A, b, **kw)
+        return (x.tobytes(), y.tobytes(), np.asarray(st.residuals).tobytes(), np.asarray(st.Aresiduals).tobytes(),
+                st.niter, st.status)
+    parity.assert_ring_depth_changes_no_bit(monkeypatch, run)
 
 
 @pytest.mark.parametrize("solver", SOLVERS)
@@ -311,15 +256,15 @@ def test_sqd_with_lambda_raises(kb):
 
 
 def test_reference_c_programs():
-    """The craig and craigmr rows of the reference's test_all_solvers.c (built into oracle/_ref/ by build()) pass,
-    and so does every row that passed before."""
+    """The rows of the least-norm solvers (craig, craigmr, lnlq, cgne, crmr) in the reference's test_all_solvers.c
+    (built into oracle/_ref/ by build()) pass, and so does every row that passed before."""
     import subprocess
     exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "test_all_solvers")
     if not os.path.exists(exe):
         pytest.skip("oracle/_ref/test_all_solvers was not built (reference tree absent at build time)")
     out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
     rows = {ln.split()[0].lower(): ln for ln in out.stdout.splitlines() if ln.split()}
-    for name in ("craig", "craigmr"):
+    for name in ("craig", "craigmr", "lnlq", "cgne", "crmr"):
         assert name in rows and "PASS" in rows[name], out.stdout[-3000:]
     for name in ("cg", "cr", "minres", "gmres", "fom", "fgmres", "bicgstab", "cgs", "bilq", "qmr", "lsqr", "lsmr", "lslq",
                  "cgls", "crls", "car", "minares", "diom", "dqgmres", "bilqr", "trilqr"):

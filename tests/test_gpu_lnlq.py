@@ -11,7 +11,6 @@ import scipy.sparse as sp
 
 import parity
 from krylov_b200 import _lib
-from krylov_b200 import problems as P
 from parity import TOL
 
 pytestmark = pytest.mark.gpu
@@ -59,13 +58,8 @@ def compare(O, kb, A, b, *, bounds=False, xtol=TOL, **kw):
 def oracle_cases(O):
     """name -> (A, b, kwargs, has bounds): the problems of the reference's test_lnlq.jl (tests/golden/gen_golden_lnlq.py,
     without the NaN-producing small_ln LNLQ point)."""
-    import importlib.util
-    here = os.path.dirname(os.path.abspath(__file__))
-    spec = importlib.util.spec_from_file_location("gen_golden_lnlq", os.path.join(here, "golden", "gen_golden_lnlq.py"))
-    G = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(G)
     out = {}
-    for name, (A, b, kw) in G.cases().items():
+    for name, (A, b, kw) in parity.golden_module("lnlq").cases().items():
         if name == "small_ln_lq":
             continue
         bounds = kw.get("sigma", 0.0) > 0 or kw.get("lambda_", 0.0) > 0 or kw.get("sqd", False)
@@ -147,84 +141,32 @@ def test_shapes_with_bounds(O, kb, fused):
     compare(O, kb, A, b, fused=fused, itmax=10, sigma=1e-3, bounds=True, atol=0.0, rtol=0.0)
 
 
-def _launches(kb, A, b, fused, itmax):
-    ws = kb.LnlqWorkspace(A.shape[0], A.shape[1], np.float64)
-    try:
-        ws.solve(A, b, fused=fused, itmax=itmax, **ZERO_TOL)
-        assert ws.stats.niter == itmax + 1, ws.stats.status
-        return ws.launches
-    finally:
-        ws.free()
-
-
-def launches_per_pass(kb, A, b, fused=True):
-    return (_launches(kb, A, b, fused, 12) - _launches(kb, A, b, fused, 6)) / 6
-
-
-def _grad(N):
-    rp, ci, va = P.grad_csr(N)
-    return sp.csr_matrix((va, ci, rp), shape=(len(rp) - 1, N ** 3))
-
-
-def _dense_line(A, row):
-    """A plus a dense row (row=True) or column: long enough that its tile, or the tile of Aᵀ, is untiled."""
-    A = sp.lil_matrix(A)
-    line = 1.0 + np.arange(A.shape[1 if row else 0]) / A.shape[1 if row else 0]
-    if row:
-        A[0, :] = line
-    else:
-        A[:, 0] = line.reshape(-1, 1)
-    return sp.csr_matrix(A)
-
-
 def test_fused_path_runs_and_untiled_twin_matches(O, kb):
     """2 launches per pass on a staged operator, and as many on its untiled twins (the gradient with a dense row: A
     untiled; with a dense column: Aᵀ untiled), whose results match the oracle."""
-    G = _grad(24)
+    G = parity.grad(24)
     rng = np.random.default_rng(3)
     b = G @ rng.standard_normal(G.shape[1])
-    assert launches_per_pass(kb, G, b) == 2
-    assert launches_per_pass(kb, G, b, fused=False) > 2
+    assert parity.launches_per_iteration(kb, "lnlq", G, b, extra_iter=1, **ZERO_TOL) == 2
+    assert parity.launches_per_iteration(kb, "lnlq", G, b, fused=False, extra_iter=1, **ZERO_TOL) > 2
     for row in (True, False):
-        U = _dense_line(_grad(24), row)
+        U = parity.dense_line(parity.grad(24), row)
         bu = U @ rng.standard_normal(U.shape[1])
-        assert launches_per_pass(kb, U, bu) == 2
+        assert parity.launches_per_iteration(kb, "lnlq", U, bu, extra_iter=1, **ZERO_TOL) == 2
         compare(O, kb, U, bu, fused=True, itmax=40, xtol=None, **ZERO_TOL)
 
 
-RING_ENV = ("KB200_STAGES", "KB200_CTAS_PER_SM")
-
-
-def test_ring_depth_changes_no_bit(kb):
+def test_ring_depth_changes_no_bit(kb, monkeypatch):
     """On an operator of about 10⁶ rows, at 3, 2 and 1 CTAs per SM, every ring depth gives byte-identical x, y,
-    histories, niter and status; the default plan is compared with the same plan forced."""
-    A = _grad(72)                                               # 1 119 744 rows, 373 248 columns
+    histories, niter and status (parity.assert_ring_depth_changes_no_bit)."""
+    A = parity.grad(72)                                         # 1 119 744 rows, 373 248 columns
     b = A @ np.cos(np.arange(A.shape[1], dtype=np.float64))
     kw = dict(itmax=20, history=True, **ZERO_TOL)
-    ref = {}
-    saved = {k: os.environ.get(k) for k in RING_ENV}
-    try:
-        for cps in (None, 3, 2, 1):
-            for stages in ((None,) if cps is None else (1, 2, 3, 4)):
-                for k in RING_ENV:
-                    os.environ.pop(k, None)
-                if cps is not None:
-                    os.environ["KB200_CTAS_PER_SM"], os.environ["KB200_STAGES"] = str(cps), str(stages)
-                x, y, st = kb.lnlq(A, b, **kw)
-                out = (x.tobytes(), y.tobytes(), np.asarray(st.residuals).tobytes(), st.niter, st.status)
-                if cps is None:
-                    ref["default"] = out
-                    continue
-                if out == ref["default"]:
-                    ref.setdefault("default_cps", cps)
-                assert out == ref.setdefault(cps, out), (cps, stages)
-        assert "default_cps" in ref
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+
+    def run():
+        x, y, st = kb.lnlq(A, b, **kw)
+        return x.tobytes(), y.tobytes(), np.asarray(st.residuals).tobytes(), st.niter, st.status
+    parity.assert_ring_depth_changes_no_bit(monkeypatch, run)
 
 
 def test_options_against_oracle(O, kb):
@@ -363,19 +305,3 @@ def test_c_abi_contract(O, kb):
 def test_sqd_with_lambda_raises(kb):
     with pytest.raises(kb.B200Error, match="sqd cannot be set to true if λ ≠ 0 !"):
         kb.lnlq(sp.csr_matrix(np.eye(2)), np.ones(2), sqd=True, lambda_=1.0)
-
-
-def test_reference_c_programs():
-    """The lnlq row of the reference's test_all_solvers.c (built into oracle/_ref/ by build()) passes, and so does
-    every row that passed before."""
-    import subprocess
-    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "test_all_solvers")
-    if not os.path.exists(exe):
-        pytest.skip("oracle/_ref/test_all_solvers was not built (reference tree absent at build time)")
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
-    rows = {ln.split()[0].lower(): ln for ln in out.stdout.splitlines() if ln.split()}
-    assert "lnlq" in rows and "PASS" in rows["lnlq"], out.stdout[-3000:]
-    for name in ("cg", "cr", "minres", "gmres", "fom", "fgmres", "bicgstab", "cgs", "bilq", "qmr", "lsqr", "lsmr", "lslq",
-                 "cgls", "crls", "car", "minares", "diom", "dqgmres", "bilqr", "trilqr", "craig", "craigmr"):
-        if name in rows:
-            assert "PASS" in rows[name], rows[name]

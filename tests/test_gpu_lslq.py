@@ -3,7 +3,6 @@ of tests/test_gpu_cgls.py: same iteration count, status and `inconsistent`; resi
 histories within 1e-6 relative (or 10x the oracle's own sensitivity to a few-ulp change of b); x within 1e-6."""
 import ctypes as C
 import functools
-import importlib.util
 import os
 
 import numpy as np
@@ -17,9 +16,7 @@ from parity import TOL
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
-_spec = importlib.util.spec_from_file_location("gen_golden_lslq", os.path.join(HERE, "golden", "gen_golden_lslq.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = parity.golden_module("lslq")
 BOUNDS = ("err_lbnds", "err_ubnds_lq", "err_ubnds_cg")
 
 

@@ -1,7 +1,6 @@
 """The CPU oracle's bilqr and trilqr (oracle/krylov_oracle_adjoint.h) against the reference's own known-answer tests
 (test/test_bilqr.jl, test/test_trilqr.jl, real case, same assertions and tolerance), and against the frozen histories
 of tests/golden/oracle_adjoint.json (tests/golden/gen_golden_adjoint.py)."""
-import importlib.util
 import json
 import os
 
@@ -9,12 +8,11 @@ import numpy as np
 import pytest
 
 from oracle import adjoint_oracle as O
+from parity import golden_module
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-6                                                         # bilqr_tol / trilqr_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_adjoint", os.path.join(HERE, "golden", "gen_golden_adjoint.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("adjoint")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_adjoint.json")))
 
 

@@ -1,7 +1,6 @@
 """The CPU oracle's bilq and qmr (oracle/krylov_oracle_biorth.h) against the reference's own known-answer tests
 (test/test_bilq.jl, test/test_qmr.jl, real case, same assertions and tolerance), and against the frozen histories of
 tests/golden/oracle_bilq_qmr.json (tests/golden/gen_golden_bilq_qmr.py)."""
-import importlib.util
 import json
 import os
 
@@ -9,12 +8,11 @@ import numpy as np
 import pytest
 
 from oracle import biorth_oracle as O
+from parity import golden_module
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-6                                                         # bilq_tol / qmr_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_bilq_qmr", os.path.join(HERE, "golden", "gen_golden_bilq_qmr.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("bilq_qmr")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_bilq_qmr.json")))
 SOLVERS = ("bilq", "qmr")
 SOLVED = {"bilq": ("solution xᴸ good enough given atol and rtol", "solution xᶜ good enough given atol and rtol"),

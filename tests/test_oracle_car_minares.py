@@ -1,7 +1,6 @@
 """The CPU oracle's car and minares (oracle/krylov_oracle_ares.h) against the reference's own known-answer tests
 (test/test_car.jl, test/test_minares.jl, real case, same assertions and tolerance), and against the frozen histories of
 tests/golden/oracle_car_minares.json (tests/golden/gen_golden_car_minares.py)."""
-import importlib.util
 import json
 import os
 
@@ -9,12 +8,11 @@ import numpy as np
 import pytest
 
 from oracle import ares_oracle as O
+from parity import golden_module
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-6                                                         # car_tol / minares_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_car_minares", os.path.join(HERE, "golden", "gen_golden_car_minares.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("car_minares")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_car_minares.json")))
 
 

@@ -1,18 +1,17 @@
 """The CPU oracle's cgls / crls (oracle/krylov_oracle_cgls.h) against the reference's own known-answer tests
 (test/test_cgls.jl, test/test_crls.jl, real case, same assertions and tolerance), and against the frozen histories of
 tests/golden/oracle_cgls.json (tests/golden/gen_golden_cgls.py)."""
-import importlib.util
 import json
 import os
 
 import numpy as np
 import pytest
 
+from parity import golden_module
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-5                                                         # cgls_tol / crls_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_cgls", os.path.join(HERE, "golden", "gen_golden_cgls.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("cgls")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_cgls.json")))
 SOLVERS = ["cgls", "crls"]
 

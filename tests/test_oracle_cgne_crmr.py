@@ -2,7 +2,6 @@
 (test/test_cgne.jl and test/test_crmr.jl, real case, same tolerance), against a dense restatement of both recurrences,
 against the frozen histories of tests/golden/oracle_cgne_crmr.json (tests/golden/gen_golden_cgne_crmr.py), and on the
 reference's quirks the GPU must repeat."""
-import importlib.util
 import json
 import os
 
@@ -11,13 +10,11 @@ import pytest
 import scipy.sparse as sp
 
 from oracle import cgne_oracle as O
+from parity import golden_module
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-6                                                         # cgne_tol, crmr_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_cgne_crmr",
-                                               os.path.join(HERE, "golden", "gen_golden_cgne_crmr.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("cgne_crmr")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_cgne_crmr.json")))
 SOLVERS = ["cgne", "crmr"]
 

@@ -1,7 +1,6 @@
 """The CPU oracle's craig and craigmr (oracle/krylov_oracle_leastnorm.h) against the reference's own assertions
 (test/test_craig.jl, test/test_craigmr.jl, real case, same tolerance), and against the frozen histories of
 tests/golden/oracle_leastnorm.json (tests/golden/gen_golden_leastnorm.py)."""
-import importlib.util
 import json
 import os
 
@@ -9,12 +8,11 @@ import numpy as np
 import pytest
 
 from oracle import leastnorm_oracle as O
+from parity import golden_module
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-6                                                         # craig_tol / craigmr_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_leastnorm", os.path.join(HERE, "golden", "gen_golden_leastnorm.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("leastnorm")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_leastnorm.json")))
 SOLVERS = ["craig", "craigmr"]
 

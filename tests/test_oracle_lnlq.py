@@ -1,7 +1,6 @@
 """The CPU oracle's lnlq (oracle/krylov_oracle_lnlq.h) against the reference's own assertions (test/test_lnlq.jl,
 real case, same tolerance, transfer_to_craig false and true), against the frozen histories of
 tests/golden/oracle_lnlq.json (tests/golden/gen_golden_lnlq.py), and on the reference's quirks the GPU must repeat."""
-import importlib.util
 import json
 import os
 
@@ -9,12 +8,11 @@ import numpy as np
 import pytest
 
 from oracle import lnlq_oracle as O
+from parity import golden_module
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-6                                                         # lnlq_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_lnlq", os.path.join(HERE, "golden", "gen_golden_lnlq.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("lnlq")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_lnlq.json")))
 TRANSFER = [False, True]
 

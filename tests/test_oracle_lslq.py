@@ -1,18 +1,17 @@
 """The CPU oracle's lslq (oracle/krylov_oracle_lslq.h) against the reference's own known-answer tests
 (test/test_lslq.jl, real case, same assertions and tolerance), and against the frozen histories of
 tests/golden/oracle_lslq.json (tests/golden/gen_golden_lslq.py)."""
-import importlib.util
 import json
 import os
 
 import numpy as np
 import pytest
 
+from parity import golden_module
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-5                                                         # lslq_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_lslq", os.path.join(HERE, "golden", "gen_golden_lslq.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("lslq")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_lslq.json")))
 
 

@@ -1,7 +1,6 @@
 """The CPU oracle's lsqr / lsmr (oracle/krylov_oracle_lsq.h) against the reference's own known-answer tests
 (test/test_lsqr.jl, test/test_lsmr.jl, real case, same assertions and tolerance), and against the frozen histories of
 tests/golden/oracle_lsq.json (tests/golden/gen_golden_lsq.py)."""
-import importlib.util
 import json
 import os
 
@@ -9,11 +8,11 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+from parity import golden_module
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 1.0e-4                                                         # lsqr_tol / lsmr_tol
-_spec = importlib.util.spec_from_file_location("gen_golden_lsq", os.path.join(HERE, "golden", "gen_golden_lsq.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
+G = golden_module("lsq")
 GOLD = json.load(open(os.path.join(HERE, "golden", "oracle_lsq.json")))
 SOLVERS = ["lsqr", "lsmr"]
 
