@@ -170,7 +170,9 @@ int krylov_b200_set_preconditioner_diag(void *ws, int which, const void *d, int 
  * its leading part) of the operator the solver applies (P^-1 with the default ldiv = false; with ldiv = true the
  * blocks are P and their inverses, formed once here, are applied).  cg! with M block-diagonal runs the persistent
  * fused kernel (z = M r formed block by block in the r-update phase); every other solver applies it as one extra
- * kernel per product.  A diagonal set with krylov_b200_set_preconditioner_diag takes precedence.  NULL detaches. */
+ * kernel per product.  A diagonal set with krylov_b200_set_preconditioner_diag takes precedence.  NULL detaches.
+ * A singular block is accepted (ldiv = false applies the blocks as given), but a solve with ldiv = true then returns
+ * -1 and names the first singular block in krylov_b200_last_error, as the reference's factorization raises. */
 int krylov_b200_set_preconditioner_blockdiag(void *ws, int which, int bs, const void *blocks, int location);
 
 /* cg_lanczos! (src/cg_lanczos.jl) has no slot in the reference's KrylovSolverType; this value selects it in
@@ -303,6 +305,13 @@ int kb200_copy(void *ctx, int dtype, int n, void *y, const void *x);
 int kb200_scalcopy(void *ctx, int dtype, int n, void *y, double s, const void *x);
 int kb200_divcopy(void *ctx, int dtype, int n, void *y, const void *x, double s);
 int kb200_fill(void *ctx, int dtype, int n, void *x, double v);
+/* The block-Jacobi kernels behind krylov_b200_set_preconditioner_blockdiag, on ceil(n / bs) dense bs x bs row-major
+ * blocks (2 <= bs <= 8; a last block of n % bs rows uses its leading part).  blockdiag_mul: y = blockdiag(B_k) x,
+ * each row summed left to right with every product rounded.  blockdiag_invert: inv[k] = B_k^-1 (Gauss-Jordan with
+ * partial pivoting; the padding of the last block is zero); a singular block gets a zero inverse and sets *singular
+ * (a device int) to 1, which is never cleared here. */
+int kb200_blockdiag_mul(void *ctx, int dtype, int n, int bs, const void *blocks, const void *x, void *y);
+int kb200_blockdiag_invert(void *ctx, int dtype, int n, int bs, const void *blocks, void *inv, int *singular);
 /* CSR operator objects for the flat API (same arguments as set_operator_csr). */
 void *kb200_csr_create(void *ctx, int dtype, int n, long long nnz, const void *rowptr, const void *colind,
                        const void *values, int index_base, int index_bytes, int location);

@@ -13,6 +13,7 @@
 #include <mutex>
 #include <type_traits>
 #include <unordered_map>
+#include <vector>
 
 #include "../../include/krylov_b200.h"
 #include "kb_internal.h"
@@ -51,6 +52,7 @@ struct Handle {
   void* Pblk[2] = {nullptr, nullptr};      // block-Jacobi M / N: dense diagonal blocks (device) ...
   void* Pblk_inv[2] = {nullptr, nullptr};  // ... and their inverses (ldiv = true)
   int Pbs[2] = {0, 0};
+  int Psing[2] = {-1, -1};                 // first singular block of M / N (-1: none): ldiv = true refuses to solve
   KrylovB200Options ext;
   void *hx = nullptr, *hy = nullptr;   // pinned staging for host callbacks
 };
@@ -273,6 +275,12 @@ int do_solve(Handle* h, const SolverInfo& S, KrylovMatvec fA, KrylovMatvec fAt, 
   const LinOp<T>& N = P[1];
   if (S.bdiag == BD_REFUSED_AT_SOLVE && (M.kind == LinOp<T>::BDIAG || N.kind == LinOp<T>::BDIAG))
     throw std::runtime_error(S.bdiag_refusal);
+  // ldiv = true solves with each block, as the reference's factorization does; it raises on a singular one
+  for (int w = 0; w < 2; w++)
+    if (so.ldiv && P[w].kind == LinOp<T>::BDIAG && (w == 0 ? S.M : S.N).use != P_IGNORED && h->Psing[w] >= 0)
+      throw std::runtime_error(std::string("block-Jacobi ") + (w == 0 ? "M" : "N") + " with ldiv = true: diagonal block " +
+                               std::to_string(h->Psing[w]) + " (rows " + std::to_string(h->Psing[w] * P[w].bs) +
+                               " onwards, 0-based) is singular");
   if (!b) throw std::runtime_error("b is NULL");
   if (S.c == C_REQUIRED_N && !c) throw std::runtime_error(std::string(S.name) + " solves A^T y = c as well: c must be given");
   const T* bd = stage_in<T>(h, ws, b, ws->bbuf, m);
@@ -751,7 +759,7 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     if (!h) return fail("krylov_b200_set_preconditioner_blockdiag", "unknown (single right-hand side) workspace handle");
     if (which != 0 && which != 1) return fail("krylov_b200_set_preconditioner_blockdiag", "which must be 0 (M) or 1 (N)");
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
-    h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0;
+    h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0; h->Psing[which] = -1;
     if (!blocks) return 0;
     if (h->info->bdiag == BD_REFUSED_AT_ATTACH) return fail("krylov_b200_set_preconditioner_blockdiag", h->info->bdiag_refusal);
     if (bs < 2 || bs > 8) return fail("krylov_b200_set_preconditioner_blockdiag", "block size must be in 2..8");
@@ -773,7 +781,17 @@ int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const 
     KB_CUDA(cudaMemcpyAsync(&sing, dsing, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     c.sync();
     cudaFree(dsing);
-    if (sing) fprintf(stderr, "[krylov_b200] warning: a diagonal block of the block-Jacobi preconditioner is singular (its inverse, used by ldiv = true, is zero)\n");
+    if (sing) {
+      // the kernel zeroes the inverse of exactly the singular blocks (an invertible block's inverse is never zero):
+      // the first all-zero inverse names the block a solve with ldiv = true refuses
+      std::vector<unsigned char> inv(esz * cnt);
+      KB_CUDA(cudaMemcpyAsync(inv.data(), h->Pblk_inv[which], esz * cnt, cudaMemcpyDeviceToHost, c.stream));
+      c.sync();
+      const size_t per = esz * bs * bs;
+      for (size_t k = 0; k * per < inv.size() && h->Psing[which] < 0; k++)
+        if (std::all_of(inv.begin() + k * per, inv.begin() + (k + 1) * per, [](unsigned char v) { return v == 0; }))
+          h->Psing[which] = (int)k;
+    }
     return 0;
   } catch (const std::exception& e) { return fail("krylov_b200_set_preconditioner_blockdiag", e); }
 }
@@ -1108,6 +1126,16 @@ int kb200_divcopy(void* ctx, int dtype, int n, void* y, const void* x, double s)
 }
 int kb200_fill(void* ctx, int dtype, int n, void* x, double v) {
   FLAT("kb200_fill", k_fill<T>(c, n, (T*)x, (T)v), k_fill<T>(c, n, (T*)x, (T)v))
+}
+int kb200_blockdiag_mul(void* ctx, int dtype, int n, int bs, const void* blocks, const void* x, void* y) {
+  if (bs < 2 || bs > 8) return fail("kb200_blockdiag_mul", "block size must be in 2..8");
+  FLAT("kb200_blockdiag_mul", k_blockdiag_mul<T>(c, n, bs, (const T*)blocks, (const T*)x, (T*)y),
+       k_blockdiag_mul<T>(c, n, bs, (const T*)blocks, (const T*)x, (T*)y))
+}
+int kb200_blockdiag_invert(void* ctx, int dtype, int n, int bs, const void* blocks, void* inv, int* singular) {
+  if (bs < 2 || bs > 8) return fail("kb200_blockdiag_invert", "block size must be in 2..8");
+  FLAT("kb200_blockdiag_invert", k_blockdiag_invert<T>(c, n, bs, (const T*)blocks, (T*)inv, singular),
+       k_blockdiag_invert<T>(c, n, bs, (const T*)blocks, (T*)inv, singular))
 }
 
 void* kb200_csr_create(void* ctx, int dtype, int n, long long nnz, const void* rowptr, const void* colind, const void* values,

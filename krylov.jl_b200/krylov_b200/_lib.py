@@ -123,6 +123,8 @@ SIGNATURES = {
     "kb200_scalcopy": (_I, [_P, _I, _I, _P, _D, _P]),
     "kb200_divcopy": (_I, [_P, _I, _I, _P, _P, _D]),
     "kb200_fill": (_I, [_P, _I, _I, _P, _D]),
+    "kb200_blockdiag_mul": (_I, [_P, _I, _I, _I, _P, _P, _P]),
+    "kb200_blockdiag_invert": (_I, [_P, _I, _I, _I, _P, _P, _P]),
     "kb200_csr_create": (_P, [_P, _I, _I, _LL, _P, _P, _P, _I, _I, _I]),
     "kb200_csr_create_rect": (_P, [_P, _I, _I, _I, _LL, _P, _P, _P, _I, _I, _I]),
     "kb200_csr_destroy": (None, [_P]),
