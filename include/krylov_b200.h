@@ -305,6 +305,13 @@ int kb200_copy(void *ctx, int dtype, int n, void *y, const void *x);
 int kb200_scalcopy(void *ctx, int dtype, int n, void *y, double s, const void *x);
 int kb200_divcopy(void *ctx, int dtype, int n, void *y, const void *x, double s);
 int kb200_fill(void *ctx, int dtype, int n, void *x, double v);
+/* The fused primitives of the solvers' unfused path, for testing them directly.  dot2: *r1 = <a, b> and
+ * *r2 = <u, v> in one pass (bicgstab's omega).  cg_prologue: x = 0, r = p = b and *gamma = <b, b> in one pass (cg with
+ * x0 = 0 and M = I).  diagmul: y = d .* x, or y = x ./ d when ldiv is non-zero (a diagonal preconditioner). */
+int kb200_dot2(void *ctx, int dtype, int n, const void *a, const void *b, const void *u, const void *v, double *r1,
+               double *r2);
+int kb200_cg_prologue(void *ctx, int dtype, int n, const void *b, void *x, void *r, void *p, double *gamma);
+int kb200_diagmul(void *ctx, int dtype, int n, void *y, const void *d, const void *x, int ldiv);
 /* The block-Jacobi kernels behind krylov_b200_set_preconditioner_blockdiag, on ceil(n / bs) dense bs x bs row-major
  * blocks (2 <= bs <= 8; a last block of n % bs rows uses its leading part).  blockdiag_mul: y = blockdiag(B_k) x,
  * each row summed left to right with every product rounded.  blockdiag_invert: inv[k] = B_k^-1 (Gauss-Jordan with

@@ -7,6 +7,8 @@
 // Element updates use non-contracted mul/add so they agree bit-for-bit with
 // the reference's `y[i] += s*x[i]` (Julia does not fuse); reductions are
 // deterministic two-stage tree sums finalised by the last CTA on the device.
+#include <cmath>
+#include <limits>
 #include <mutex>
 #include <set>
 #include <utility>
@@ -74,23 +76,27 @@ template char* dev_alloc<char>(size_t);
 // ---------------------------------------------------------------------------
 enum EwOp { EW_AXPY, EW_AXPBY, EW_SCAL, EW_COPY, EW_SCALCOPY, EW_DIVCOPY, EW_FILL, EW_DIAGMUL, EW_DIAGDIV };
 
+// The grid-stride loops here count in unsigned 32-bit: n <= INT_MAX and stride <= kMaxPartials * kBlock = 2^19, so
+// i + 3 * stride and every step stay below n + 4 * stride < 2^32.  In int they overflow once n is within 4 strides
+// of INT_MAX (an 8 GiB Float32 vector fits on one GPU).  A negative n counts as 0 (un), as it did in int: the
+// reductions still launch one CTA for n <= 0 to write their result.
 template <class T, int OP>
 __global__ void __launch_bounds__(kBlock) ew_kernel(int n, T s, T t, const T* x, const T* d, T* y) {
-  const int stride = gridDim.x * blockDim.x;
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned stride = gridDim.x * blockDim.x, un = n > 0 ? n : 0;
+  unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
   // 4 independent elements per trip keep enough loads in flight per thread.
-  for (; i + 3 * stride < n; i += 4 * stride) {
+  for (; i + 3 * stride < un; i += 4 * stride) {
     T xv[4], yv[4];
 #pragma unroll
     for (int u = 0; u < 4; u++) {
-      const int j = i + u * stride;
+      const unsigned j = i + u * stride;
       if (OP != EW_FILL && OP != EW_SCAL) xv[u] = x[j];
       if (OP == EW_AXPY || OP == EW_AXPBY || OP == EW_SCAL) yv[u] = y[j];
       if (OP == EW_DIAGMUL || OP == EW_DIAGDIV) yv[u] = d[j];
     }
 #pragma unroll
     for (int u = 0; u < 4; u++) {
-      const int j = i + u * stride;
+      const unsigned j = i + u * stride;
       T r;
       if (OP == EW_AXPY) r = add_rn(yv[u], mul_rn(s, xv[u]));
       else if (OP == EW_AXPBY) r = add_rn(mul_rn(s, xv[u]), mul_rn(t, yv[u]));
@@ -104,7 +110,7 @@ __global__ void __launch_bounds__(kBlock) ew_kernel(int n, T s, T t, const T* x,
       y[j] = r;
     }
   }
-  for (; i < n; i += stride) {
+  for (; i < un; i += stride) {
     T r;
     if (OP == EW_AXPY) r = add_rn(y[i], mul_rn(s, x[i]));
     else if (OP == EW_AXPBY) r = add_rn(mul_rn(s, x[i]), mul_rn(t, y[i]));
@@ -138,7 +144,7 @@ template <class T> void k_scalcopy(Ctx& c, int n, T* y, T s, const T* x) { ew_la
 template <class T> void k_divcopy(Ctx& c, int n, T* y, const T* x, T s) { ew_launch<T, EW_DIVCOPY>(c, n, s, T(0), x, nullptr, y); }
 template <class T> void k_fill(Ctx& c, int n, T* x, T v) {
   if (n <= 0) return;
-  if (v == T(0)) { KB_CUDA(cudaMemsetAsync(x, 0, sizeof(T) * (size_t)n, c.stream)); return; }
+  if (v == T(0) && !std::signbit(v)) { KB_CUDA(cudaMemsetAsync(x, 0, sizeof(T) * (size_t)n, c.stream)); return; }   // -0.0 is not all-zero bits
   ew_launch<T, EW_FILL>(c, n, v, T(0), nullptr, nullptr, x);
 }
 template <class T> void k_diagmul(Ctx& c, int n, T* y, const T* d, const T* x, bool ldiv) {
@@ -212,31 +218,69 @@ template <class T> void k_blockdiag_invert(Ctx& c, int n, int bs, const T* block
 // ---------------------------------------------------------------------------
 // Reductions
 // ---------------------------------------------------------------------------
-template <class T, int K>
+// DOT_SUM: out[k] = <a, b> (k = 0) and <u, v> (k = 1 when K = 2).  The two modes of k_nrm2 read only a:
+// DOT_NRM2 sums a_i^2 and also leaves max|a_i| in out[1]; DOT_NRM2_SCALED sums (a_i 2^-e)^2, where 2^e <= max|a_i| < 2^(e+1)
+// is taken from that out[1], and returns 2^e sqrt(sum).  do_sqrt: out[k] = sqrt(sum) instead of the sum.
+enum DotMode { DOT_SUM, DOT_NRM2, DOT_NRM2_SCALED };
+
+__device__ __forceinline__ double scale2(double v, int e) { return scalbn(v, e); }   // v 2^e, one rounding
+__device__ __forceinline__ float scale2(float v, int e) { return scalbnf(v, e); }
+__device__ __forceinline__ int exponent_of(double v) { return ilogb(v); }
+__device__ __forceinline__ int exponent_of(float v) { return ilogbf(v); }
+
+// Like block_sum, for the maximum (NaNs are ignored: fmax).  All threads of the CTA must call; valid in thread 0.
+template <class T>
+__device__ __forceinline__ T block_max(T v, T* smem) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if (lane == 0) smem[w] = v;
+  __syncthreads();
+  T r = T(0);
+  if (w == 0) {
+    r = lane < nw ? smem[lane] : T(0);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) r = fmax(r, __shfl_xor_sync(0xffffffffu, r, o));
+  }
+  __syncthreads();
+  return r;
+}
+
+template <class T, int K, int MODE = DOT_SUM>
 __global__ void __launch_bounds__(kBlock) dot_kernel(int n, const T* __restrict__ a, const T* __restrict__ b,
                                                      const T* __restrict__ u, const T* __restrict__ v, T* part,
                                                      unsigned* ticket, T* out, int do_sqrt, DistComm* dc) {
+  static_assert(MODE == DOT_SUM || K == 1, "the nrm2 modes reduce one vector");
   __shared__ T sm[32];
-  const int stride = gridDim.x * blockDim.x;
-  T acc[K];
+  const unsigned stride = gridDim.x * blockDim.x, un = n > 0 ? n : 0;   // unsigned: see ew_kernel
+  const int sh = MODE == DOT_NRM2_SCALED ? -exponent_of(out[1]) : 0;
+  T acc[K], mx = T(0);
 #pragma unroll
   for (int k = 0; k < K; k++) acc[k] = T(0);
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  for (; i + 3 * stride < n; i += 4 * stride) {
+  unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (; i + 3 * stride < un; i += 4 * stride) {
     T av[4], bv[4], uv[4], vv[4];
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      av[q] = a[i + q * stride]; bv[q] = b[i + q * stride];
+      av[q] = a[i + q * stride];
+      if (MODE == DOT_NRM2_SCALED) av[q] = scale2(av[q], sh);
+      bv[q] = MODE == DOT_SUM ? b[i + q * stride] : av[q];
       if (K > 1) { uv[q] = u[i + q * stride]; vv[q] = v[i + q * stride]; }
     }
 #pragma unroll
     for (int q = 0; q < 4; q++) {
       acc[0] += av[q] * bv[q];
       if (K > 1) acc[K - 1] += uv[q] * vv[q];
+      if (MODE == DOT_NRM2) mx = fmax(mx, fabs(av[q]));
     }
   }
-  for (; i < n; i += stride) {
-    acc[0] += a[i] * b[i];
+  for (; i < un; i += stride) {
+    if (MODE == DOT_SUM) acc[0] += a[i] * b[i];
+    else {
+      const T ai = MODE == DOT_NRM2_SCALED ? scale2(a[i], sh) : a[i];
+      acc[0] += ai * ai;
+      if (MODE == DOT_NRM2) mx = fmax(mx, fabs(ai));
+    }
     if (K > 1) acc[K - 1] += u[i] * v[i];
   }
   T mine[K], tot[K];
@@ -244,13 +288,24 @@ __global__ void __launch_bounds__(kBlock) dot_kernel(int n, const T* __restrict_
   for (int k = 0; k < K; k++) {
     mine[k] = block_sum(acc[k], sm);
   }
+  if (MODE == DOT_NRM2) {
+    const T m = block_max(mx, sm);
+    if (threadIdx.x == 0) part[gridDim.x + blockIdx.x] = m;   // after the sums' partials; grid_sum_last's fence covers it
+  }
   if (grid_sum_last<T, K>(mine, part, ticket, sm, tot)) {
+    T gmax = T(0);
+    if (MODE == DOT_NRM2) {
+      for (int j = threadIdx.x; j < (int)gridDim.x; j += blockDim.x) gmax = fmax(gmax, __ldcg(&part[gridDim.x + j]));
+      gmax = block_max(gmax, sm);
+    }
     if (threadIdx.x == 0) {
 #pragma unroll
       for (int k = 0; k < K; k++) {
         const T g = dist_reduce(dc, tot[k]);       // row-partitioned solve: sum over ranks
-        out[k] = do_sqrt ? sqrt_rn(g) : g;
+        const T r = do_sqrt ? sqrt_rn(g) : g;
+        out[k] = MODE == DOT_NRM2_SCALED ? scale2(r, -sh) : r;
       }
+      if (MODE == DOT_NRM2) out[1] = gmax;
     }
   }
 }
@@ -281,8 +336,41 @@ template <class T> T k_dot(Ctx& c, int n, const T* x, const T* y) {
   dot_launch<T>(c, n, x, y, 0, 0);
   return read_slot<T>(c, 0);
 }
+template <class T, int MODE>
+static void nrm2_launch(Ctx& c, int n, const T* x) {
+  const int grid = n > 0 ? stream_grid(n, 4, 4) : 1;
+  dot_kernel<T, 1, MODE><<<grid, kBlock, 0, c.stream>>>(n, x, x, nullptr, nullptr, (T*)c.partials, c.tickets, slot_ptr<T>(c, 0), 1, nullptr);
+  KB_CUDA(cudaGetLastError());
+  c.launches++;
+}
+
+// knorm = BLAS nrm2 (src/krylov_utils.jl:316): finite and accurate whenever ||x|| itself is.  One pass forms
+// sqrt(sum x_i^2) and max|x_i|; the result stands unless the sum overflowed (Inf while max|x_i| is finite) or is so
+// small that squares below the normal range may have moved it.  In that case one more pass sums the squares of x
+// scaled by a power of two that brings max|x_i| into [1, 2), and scales the root back.
+//
+// Threshold: a rounding whose result is below realmin (the smallest normal number, 2^emin) errs by at most half the
+// subnormal spacing, 2^(emin - p) = realmin * eps / 2 (p = 53 / 24 bits).  The sum makes fewer than n such roundings,
+// so they move it by less than n * realmin * eps / 2, which is at most one ulp of the sum (ulp(S) > S * eps / 2)
+// whenever S >= n * realmin.  Hence: rescale when sqrt(S) < sqrt(n * realmin).  A zero vector (max|x_i| = 0) never
+// does, so it still costs one launch; nor does a NaN, which the first pass already returns.
+//
+// A row-partitioned solve (c.dcomm) keeps the plain sqrt(sum x_i^2): every rank sees the same reduced sum, but a
+// rescaled pass would need a max over the ranks as well.
 template <class T> T k_nrm2(Ctx& c, int n, const T* x) {
-  dot_launch<T>(c, n, x, x, 0, 1);
+  if (c.dcomm) {
+    dot_launch<T>(c, n, x, x, 0, 1);
+    return read_slot<T>(c, 0);
+  }
+  nrm2_launch<T, DOT_NRM2>(c, n, x);
+  KB_CUDA(cudaMemcpyAsync(c.hscal, c.dscal, 2 * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+  c.sync();
+  const T nrm = reinterpret_cast<T*>(c.hscal)[0], xmax = reinterpret_cast<T*>(c.hscal)[1];
+  const T small = (T)std::sqrt((double)n * (double)std::numeric_limits<T>::min());
+  const bool overflowed = std::isinf(nrm) && std::isfinite(xmax);
+  const bool underflowed = xmax > T(0) && nrm < small;
+  if (!overflowed && !underflowed) return nrm;
+  nrm2_launch<T, DOT_NRM2_SCALED>(c, n, x);
   return read_slot<T>(c, 0);
 }
 template <class T> void k_dot2(Ctx& c, int n, const T* a, const T* b, const T* u, const T* v, T* r1, T* r2) {
@@ -344,8 +432,20 @@ __global__ void __launch_bounds__(kBlock) cg_prologue_kernel(int n, const T* __r
                                                              T* __restrict__ p, T* part, unsigned* ticket, T* out, DistComm* dc) {
   __shared__ T sm[32];
   T acc = T(0);
-  const int stride = gridDim.x * blockDim.x;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+  const unsigned stride = gridDim.x * blockDim.x, un = n > 0 ? n : 0;   // unsigned: see ew_kernel
+  unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (; i + 3 * stride < un; i += 4 * stride) {    // 4 loads in flight per thread, summed in the same order as one by one
+    T v[4];
+#pragma unroll
+    for (int q = 0; q < 4; q++) v[q] = b[i + q * stride];
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const unsigned j = i + q * stride;
+      x[j] = T(0); r[j] = v[q]; p[j] = v[q];
+      acc += v[q] * v[q];
+    }
+  }
+  for (; i < un; i += stride) {
     const T v = b[i];
     x[i] = T(0); r[i] = v; p[i] = v;
     acc += v * v;

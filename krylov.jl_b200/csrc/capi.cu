@@ -1127,6 +1127,20 @@ int kb200_divcopy(void* ctx, int dtype, int n, void* y, const void* x, double s)
 int kb200_fill(void* ctx, int dtype, int n, void* x, double v) {
   FLAT("kb200_fill", k_fill<T>(c, n, (T*)x, (T)v), k_fill<T>(c, n, (T*)x, (T)v))
 }
+int kb200_dot2(void* ctx, int dtype, int n, const void* a, const void* b, const void* u, const void* v, double* r1,
+               double* r2) {
+  FLAT("kb200_dot2",
+       { T s1; T s2; k_dot2<T>(c, n, (const T*)a, (const T*)b, (const T*)u, (const T*)v, &s1, &s2); *r1 = s1; *r2 = s2; },
+       { T s1; T s2; k_dot2<T>(c, n, (const T*)a, (const T*)b, (const T*)u, (const T*)v, &s1, &s2); *r1 = s1; *r2 = s2; })
+}
+int kb200_cg_prologue(void* ctx, int dtype, int n, const void* b, void* x, void* r, void* p, double* gamma) {
+  FLAT("kb200_cg_prologue", *gamma = k_cg_prologue<T>(c, n, (const T*)b, (T*)x, (T*)r, (T*)p),
+       *gamma = k_cg_prologue<T>(c, n, (const T*)b, (T*)x, (T*)r, (T*)p))
+}
+int kb200_diagmul(void* ctx, int dtype, int n, void* y, const void* d, const void* x, int ldiv) {
+  FLAT("kb200_diagmul", k_diagmul<T>(c, n, (T*)y, (const T*)d, (const T*)x, ldiv != 0),
+       k_diagmul<T>(c, n, (T*)y, (const T*)d, (const T*)x, ldiv != 0))
+}
 int kb200_blockdiag_mul(void* ctx, int dtype, int n, int bs, const void* blocks, const void* x, void* y) {
   if (bs < 2 || bs > 8) return fail("kb200_blockdiag_mul", "block size must be in 2..8");
   FLAT("kb200_blockdiag_mul", k_blockdiag_mul<T>(c, n, bs, (const T*)blocks, (const T*)x, (T*)y),

@@ -123,6 +123,9 @@ SIGNATURES = {
     "kb200_scalcopy": (_I, [_P, _I, _I, _P, _D, _P]),
     "kb200_divcopy": (_I, [_P, _I, _I, _P, _P, _D]),
     "kb200_fill": (_I, [_P, _I, _I, _P, _D]),
+    "kb200_dot2": (_I, [_P, _I, _I, _P, _P, _P, _P, C.POINTER(_D), C.POINTER(_D)]),
+    "kb200_cg_prologue": (_I, [_P, _I, _I, _P, _P, _P, _P, C.POINTER(_D)]),
+    "kb200_diagmul": (_I, [_P, _I, _I, _P, _P, _P, _I]),
     "kb200_blockdiag_mul": (_I, [_P, _I, _I, _I, _P, _P, _P]),
     "kb200_blockdiag_invert": (_I, [_P, _I, _I, _I, _P, _P, _P]),
     "kb200_csr_create": (_P, [_P, _I, _I, _LL, _P, _P, _P, _I, _I, _I]),

@@ -31,11 +31,12 @@ def test_header_symbols_are_exported_and_bound():
 
 def test_signature_argument_counts_match_header():
     """Each ctypes signature takes as many arguments as the header's prototype (the kernel test entry points
-    kb200_spmm_csr, krylov_b200_block_panel_op and the block-Jacobi kernels among them)."""
+    kb200_spmm_csr, krylov_b200_block_panel_op, the block-Jacobi kernels and the fused vector primitives among
+    them)."""
     src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "krylov_b200.h")).read(), flags=re.S)
     protos = dict(re.findall(r"\b((?:krylov|kb200)_[a-z0-9_A-Z]+)\s*\(([^()]*)\)\s*;", src))
     for name in ("kb200_spmm_csr", "krylov_b200_block_panel_op", "kb200_spmv_csr", "kb200_blockdiag_mul",
-                 "kb200_blockdiag_invert"):
+                 "kb200_blockdiag_invert", "kb200_dot2", "kb200_cg_prologue", "kb200_diagmul"):
         assert name in protos
     for name, params in protos.items():
         params = params.strip()
