@@ -22,7 +22,7 @@ import ctypes as C
 import math
 import os
 from dataclasses import dataclass, field
-from typing import Callable, Optional
+from typing import Optional
 
 import numpy as np
 
@@ -30,20 +30,10 @@ from . import _lib
 from ._lib import (KRYLOV_CPU, KRYLOV_CUDA, KRYLOV_FLOAT32, KRYLOV_FLOAT64, SOLVER_IDS, KrylovB200Options,
                    KrylovB200Stats, KrylovOptions, KrylovWorkspaceOptions, lib)
 
-__all__ = ["CgWorkspace", "GmresWorkspace", "BicgstabWorkspace", "MinresWorkspace", "KrylovWorkspace", "SimpleStats",
-           "cg", "cg_", "gmres", "gmres_", "bicgstab", "bicgstab_", "minres", "minres_", "krylov_workspace",
-           "krylov_solve", "krylov_solve_", "solution", "statistics", "results", "issolved", "iteration_count",
-           "elapsed_time", "Aprod_count", "warm_start_", "device_count", "B200Error",
-           "FomWorkspace", "FgmresWorkspace", "CgsWorkspace", "CgLanczosWorkspace", "fom", "fom_", "fgmres", "fgmres_",
-           "cgs", "cgs_", "cg_lanczos", "cg_lanczos_", "CrWorkspace", "DiomWorkspace", "DqgmresWorkspace", "cr", "cr_", "diom",
-           "diom_", "dqgmres", "dqgmres_", "BlockGmresWorkspace", "block_gmres", "block_gmres_", "CsrOperator",
-           "LsqrWorkspace", "LsmrWorkspace", "lsqr", "lsqr_", "lsmr", "lsmr_",
-           "CglsWorkspace", "CrlsWorkspace", "cgls", "cgls_", "crls", "crls_", "LslqWorkspace", "lslq", "lslq_",
-           "BilqWorkspace", "QmrWorkspace", "bilq", "bilq_", "qmr", "qmr_",
-           "CarWorkspace", "MinaresWorkspace", "car", "car_", "minares", "minares_",
-           "AdjointStats", "BilqrWorkspace", "TrilqrWorkspace", "bilqr", "bilqr_", "trilqr", "trilqr_",
-           "CraigWorkspace", "CraigmrWorkspace", "craig", "craig_", "craigmr", "craigmr_", "LnlqWorkspace", "lnlq", "lnlq_",
-           "CgneWorkspace", "CrmrWorkspace", "cgne", "cgne_", "crmr", "crmr_"]
+__all__ = ["KrylovWorkspace", "SimpleStats", "AdjointStats", "B200Error", "CsrOperator", "BlockGmresWorkspace",
+           "block_gmres", "block_gmres_", "krylov_workspace", "krylov_solve", "krylov_solve_", "solution", "statistics",
+           "results", "issolved", "iteration_count", "elapsed_time", "Aprod_count", "warm_start_", "device_count"]
+# the workspace class, solver! and solver of every row of _SOLVERS are added where they are made
 
 
 class B200Error(RuntimeError):
@@ -110,26 +100,31 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p), a
 
 
-def _float(v):
-    return None if v is None else float(v)
+_KEYWORDS = {   # solve keyword -> (the option struct it travels in, its field there, conversion)
+    **{k: (KrylovOptions, k, float) for k in ("atol", "rtol", "lambda_", "radius")},
+    **{k: (KrylovOptions, k, int) for k in ("itmax", "verbose", "restart", "reorthogonalization", "linesearch")},
+    "timemax": (KrylovOptions, "timemax", lambda t: math.nan if math.isinf(t) else float(t)),
+    **{k: (KrylovB200Options, k, float) for k in ("etol", "conlim", "axtol", "btol", "sigma", "utol")},
+    **{k: (KrylovB200Options, k, int) for k in ("history", "ldiv", "fused", "batch", "time_kernels", "check_curvature",
+                                                "transfer_to_lsqr", "transfer_to_bicg")},
+    "gamma": (KrylovB200Options, "cr_gamma", float),
+    "artol": (KrylovB200Options, "axtol", float),                  # MINARES's Artol
+    "utolx": (KrylovB200Options, "utol", float),                   # LNLQ's tolerances on its error bounds
+    "utoly": (KrylovB200Options, "etol", float),
+    "transfer_to_craig": (KrylovB200Options, "transfer_to_bicg", int),     # LNLQ
+    "transfer_to_usymcg": (KrylovB200Options, "transfer_to_bicg", int),    # TriLQR
+}
 
 
-def _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=(), ext=()):
-    """The KrylovOptions / KrylovB200Options pair of one solve: the keywords every solver takes, then the solver's own
-    fields (`opts` into KrylovOptions, `ext` into KrylovB200Options; a None value keeps the default)."""
-    o = lib().krylov_default_options()
-    if atol is not None:
-        o.atol = float(atol)
-    if rtol is not None:
-        o.rtol = float(rtol)
-    o.itmax, o.verbose = int(itmax), int(verbose)
-    o.timemax = math.nan if math.isinf(timemax) else float(timemax)
-    e = lib().krylov_b200_default_options()
-    e.history, e.ldiv, e.fused = int(history), int(ldiv), int(fused)
-    for struct, fields in ((o, opts), (e, ext)):
-        for name, val in dict(fields).items():
-            if val is not None:
-                setattr(struct, name, val)
+def _options(kw, defaults):
+    """The KrylovOptions / KrylovB200Options pair of one solve from its option keywords.  None keeps the library's
+    default for atol, rtol and the keywords whose default is None."""
+    o, e = lib().krylov_default_options(), lib().krylov_b200_default_options()
+    for name, val in kw.items():
+        if val is None and (name in ("atol", "rtol") or defaults.get(name) is None):
+            continue
+        struct, field_, conv = _KEYWORDS[name]
+        setattr(o if struct is KrylovOptions else e, field_, conv(val))
     return o, e
 
 
@@ -378,55 +373,69 @@ class KrylovWorkspace:
             raise B200Error(_lib.last_error())
 
     # -- solve --------------------------------------------------------------
-    def _wrap_matvec(self, f: Optional[Callable]):
-        if f is None:
-            return _lib.MATVEC(), None
-        n, dt = self.n, self.dtype
+    def _wrap(self, f, nin, nout):
+        """Host callback y = f(x) with len(x) = nin and len(y) = nout (staged through pinned memory)."""
         if self.device == "cuda":
             raise B200Error("Python callables are host operators; create the workspace with device='host'")
+        dt = self.dtype
 
         def tramp(xp, yp, _ud):
-            x = np.ctypeslib.as_array(C.cast(xp, C.POINTER(C.c_byte)), shape=(n * dt.itemsize,)).view(dt)
-            y = np.ctypeslib.as_array(C.cast(yp, C.POINTER(C.c_byte)), shape=(n * dt.itemsize,)).view(dt)
+            x = np.ctypeslib.as_array(C.cast(xp, C.POINTER(C.c_byte)), shape=(nin * dt.itemsize,)).view(dt)
+            y = np.ctypeslib.as_array(C.cast(yp, C.POINTER(C.c_byte)), shape=(nout * dt.itemsize,)).view(dt)
             y[:] = f(x)
-        cb = _lib.MATVEC(tramp)
-        return cb, cb
+        return _lib.MATVEC(tramp)
 
-    def solve(self, A, b, *, c=None, M=None, N=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
-              history=False, callback=None, radius=0.0, linesearch=False, lambda_=0.0, etol=None, conlim=None,
-              restart=False, reorthogonalization=False, ldiv=False, fused=True, batch=0, time_kernels=False,
-              check_curvature=False, gamma=None, artol=None):
-        """solver!(ws, A, b; kwargs...)  -- kwargs as in cg.jl:100-111, gmres.jl:96-108,
-        bicgstab.jl:105-116, minres.jl:138-151.  M / N: None (identity), a 1-D array
-        (Diagonal preconditioner) or a host callable."""
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
-                        opts=dict(radius=float(radius), linesearch=int(linesearch), lambda_=float(lambda_),
-                                  restart=int(restart), reorthogonalization=int(reorthogonalization)),
-                        ext=dict(batch=int(batch), time_kernels=int(time_kernels), check_curvature=int(check_curvature),
-                                 cr_gamma=_float(gamma), etol=_float(etol), conlim=_float(conlim),
-                                 axtol=_float(artol)))   # MINARES's Artol travels in the axtol field
+    @property
+    def _row(self) -> Optional["_Solver"]:
+        return _SOLVERS.get(self.solver)
+
+    def solve(self, A, b, *args, **kw):
+        """solver!(ws, A, b; kwargs...), and bilqr! / trilqr!(ws, A, b, c; kwargs...): the keywords and defaults are
+        listed in help() of the workspace class.  A: a SciPy matrix, a CsrOperator or a (rowptr, colind, values)
+        tuple (uploaded as a CSR operator); or host callables: A itself for the solvers that do not apply A^T, a
+        scipy.sparse.linalg.LinearOperator or a (matvec, rmatvec) pair for those that do.  M / N: None (identity), a
+        1-D array (Diagonal preconditioner), a host callable, or, for the solvers that do not apply A^T, the
+        (nblocks, bs, bs) diagonal blocks of a block-Jacobi preconditioner."""
+        row, name = self._row, self.solver
+        if args:
+            if row.c != "n" or len(args) > 1 or "c" in kw:
+                raise TypeError(f"{name}!: the arguments after the workspace are A, b{', c' if row.c == 'n' else ''}")
+            kw["c"] = args[0]
+        if kw.keys() - row.kw.keys():
+            raise B200Error(f"{name}!: unsupported keyword argument(s) {', '.join(sorted(kw.keys() - row.kw.keys()))}")
+        kw = {**row.kw, **row.fixed, **kw}
+        c, M, N, callback = (kw.pop(k, None) for k in ("c", "M", "N", "callback"))
+        if row.c == "n" and c is None:
+            raise B200Error(f"{name}! solves A^T y = c as well: c must be given")
+        if kw.pop("sqd", False):
+            if kw["lambda_"] != 0:
+                raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
+            kw["lambda_"] = 1.0
+        o, e = _options(kw, row.kw)
         keep = [self._set_options(e, callback)]
-        fA = None
-        if callable(A) and not hasattr(A, "shape"):
-            fA, k = self._wrap_matvec(A)
-            keep.append(k)
-        elif A is not None:
+        m, n = self.m, self.n
+        fA = fAt = None
+        if row.At:
+            if hasattr(A, "matvec") and hasattr(A, "rmatvec") and not isinstance(A, CsrOperator):   # LinearOperator
+                A = (A.matvec, A.rmatvec)
+            if isinstance(A, tuple) and len(A) == 2 and all(callable(f) for f in A):
+                fA, fAt = self._wrap(A[0], n, m), self._wrap(A[1], m, n)
+        elif callable(A) and not hasattr(A, "shape"):
+            fA = self._wrap(A, n, n)
+        if fA is None and A is not None:
             self.set_operator(A)
-        fM = fN = None
-        for which, P in ((0, M), (1, N)):
-            if P is None:
-                self._set_diag(which, None)
-            elif callable(P) and not hasattr(P, "shape"):
-                f, k = self._wrap_matvec(P)
-                keep.append(k)
-                if which == 0:
-                    fM = f
-                else:
-                    fN = f
+        fP = []
+        for which, (P, space) in enumerate(((M, row.M), (N, row.N))):
+            if callable(P) and not hasattr(P, "shape"):
+                fP.append(self._wrap(P, *[m if space == "m" else n] * 2))
                 self._set_diag(which, None)
             else:
+                if row.At and getattr(P, "ndim", 1) != 1:
+                    raise B200Error(f"{name} takes diagonal preconditioners (1-D arrays) or host callables")
+                fP.append(None)
                 self._set_diag(which, P)
-        return self._solve_staged(o, fA, None, fM, fN, b, c, self.m)
+        keep += [fA, fAt] + fP
+        return self._solve_staged(o, fA, fAt, *fP, b, c, n if row.c == "n" else m)
 
     def _set_options(self, e, callback):
         """Install the KrylovB200Options of one solve, `callback` behind a trampoline; returns what must outlive the
@@ -471,9 +480,21 @@ class KrylovWorkspace:
             raise B200Error(_lib.last_error())
         return self
 
-    def warm_start(self, x0):
+    def warm_start(self, x0, y0=None):
+        """warm_start!(workspace, x0), and warm_start!(workspace, x0, y0) for BiLQR / TriLQR: x0 has n entries, y0 m."""
+        if (y0 is not None) != (self._row.c == "n"):
+            raise TypeError(f"{self.solver} warm-starts from {'x0 and y0' if self._row.c == 'n' else 'x0 alone'}")
         if not _is_torch(x0):
             x0 = np.ascontiguousarray(x0, dtype=self.dtype)
+        if y0 is not None:
+            if not _is_torch(y0):
+                y0 = np.ascontiguousarray(y0, dtype=self.dtype)
+            px, kx = _ptr(x0)
+            py, ky = _ptr(y0)
+            self._order_after(kx, ky)
+            if lib().krylov_warm_start2(self._h, px, py, int(x0.shape[0]), int(y0.shape[0])) != 0:
+                raise B200Error(_lib.last_error())
+            return self
         if x0.shape[0] != self.n:
             raise B200Error(f"x0 should have size {self.n}")
         p, k = _ptr(x0)
@@ -507,7 +528,25 @@ class KrylovWorkspace:
         return out
 
     @property
-    def stats(self) -> SimpleStats:
+    def y(self):
+        """The second solution, m entries (x = A^T y of CRAIG, CRAIGMR and LNLQ; A^T y = c of BiLQR and TriLQR): a
+        host copy (or a torch CUDA tensor for device workspaces)."""
+        if not getattr(self._row, "y", False):
+            raise AttributeError(f"{self.solver} has no second solution y")
+        if self.device == "cuda":
+            import torch
+            out = torch.empty(self.m, dtype=torch.float64 if self.dtype == np.float64 else torch.float32, device="cuda")
+            if lib().krylov_get_y(self._h, C.c_void_p(out.data_ptr()), self.m) != 0:
+                raise B200Error(_lib.last_error())
+            return out
+        out = np.empty(self.m, dtype=self.dtype)
+        if lib().krylov_get_y(self._h, out.ctypes.data_as(C.c_void_p), self.m) != 0:
+            raise B200Error(_lib.last_error())
+        return out
+
+    @property
+    def stats(self):
+        """SimpleStats, with the error-bound histories of LSLQ and LNLQ; AdjointStats for BiLQR and TriLQR."""
         s = KrylovB200Stats()
         if lib().krylov_b200_get_stats(self._h, C.byref(s)) != 0:
             raise B200Error(_lib.last_error())
@@ -516,15 +555,17 @@ class KrylovWorkspace:
             buf = (C.c_double * max(cnt, 1))()
             k = lib().krylov_b200_get_history(self._h, which, buf, cnt)
             return list(buf[:max(k, 0)])
+        if getattr(self._row, "c", None) == "n":
+            return AdjointStats(s.niter, bool(s.solved_primal), bool(s.solved_dual), hist(0, s.nresiduals),
+                                hist(6, s.nresiduals_dual), s.timer, s.status.decode("utf-8"))
         out = SimpleStats(s.niter, bool(s.solved), bool(s.inconsistent), bool(s.indefinite), s.npcCount,
                           hist(0, s.nresiduals), hist(1, s.nAresiduals), hist(2, s.nAcond), s.allocation_timer, s.timer,
                           s.status.decode("utf-8"))
         out.Anorm = s.Anorm          # LanczosStats.Anorm (cg_lanczos!), NaN otherwise
-        if self.solver == "lslq":    # LSLQStats (src/krylov_stats.jl:352-365)
-            out.err_lbnds, out.err_ubnds_lq = hist(3, s.nerr_lbnds), hist(4, s.nerr_ubnds_lq)
-            out.err_ubnds_cg, out.error_with_bnd = hist(5, s.nerr_ubnds_cg), bool(s.error_with_bnd)
-        elif self.solver == "lnlq":  # LNLQStats (src/krylov_stats.jl): the bounds travel in LSLQ's history slots 3 and 4
-            out.error_bnd_x, out.error_bnd_y = hist(3, s.nerr_lbnds), hist(4, s.nerr_ubnds_lq)
+        bounds = getattr(self._row, "bounds", ())
+        for attr, slot, count in bounds:
+            setattr(out, attr, hist(slot, getattr(s, count)))
+        if bounds:
             out.error_with_bnd = bool(s.error_with_bnd)
         return out
 
@@ -542,79 +583,6 @@ class KrylovWorkspace:
     @property
     def npc_dir(self):
         return self.vector("npc_dir")
-
-
-class CgWorkspace(KrylovWorkspace):
-    solver = "cg"
-
-
-class MinresWorkspace(KrylovWorkspace):
-    solver = "minres"
-
-
-class GmresWorkspace(KrylovWorkspace):
-    solver = "gmres"
-
-
-class BicgstabWorkspace(KrylovWorkspace):
-    solver = "bicgstab"
-    nA = 2
-
-
-# sibling solvers on the same kernels (SURVEY.md 8f-3)
-class FomWorkspace(KrylovWorkspace):
-    solver = "fom"
-
-
-class FgmresWorkspace(KrylovWorkspace):
-    solver = "fgmres"
-
-
-class CgsWorkspace(KrylovWorkspace):
-    solver = "cgs"
-    nA = 2
-
-
-class CgLanczosWorkspace(KrylovWorkspace):
-    solver = "cg_lanczos"
-
-
-class CrWorkspace(KrylovWorkspace):
-    solver = "cr"
-
-
-class DiomWorkspace(KrylovWorkspace):
-    solver = "diom"
-
-
-class DqgmresWorkspace(KrylovWorkspace):
-    solver = "dqgmres"
-
-
-class CarWorkspace(KrylovWorkspace):
-    solver = "car"
-
-    def solve(self, A, b, *, M=None, ldiv=False, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
-              history=False, callback=None, fused=True, **unknown):
-        """car!(ws, A, b; kwargs...)  -- kwargs as in car.jl:90-99: atol and rtol default to sqrt(eps), itmax = 0
-        means 2n.  M: None, the diagonal of a Diagonal preconditioner, or a host callable."""
-        if unknown:
-            raise B200Error(f"car!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        return super().solve(A, b, M=M, ldiv=ldiv, atol=atol, rtol=rtol, itmax=itmax, timemax=timemax, verbose=verbose,
-                             history=history, callback=callback, fused=fused)
-
-
-class MinaresWorkspace(KrylovWorkspace):
-    solver = "minares"
-
-    def solve(self, A, b, *, M=None, ldiv=False, lambda_=0.0, atol=None, rtol=None, artol=None, itmax=0,
-              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
-        """minares!(ws, A, b; kwargs...)  -- kwargs as in minares.jl:93-104 (λ is lambda_, Artol is artol; atol, rtol
-        and artol default to sqrt(eps)).  M must be None: the reference does not support preconditioners yet."""
-        if unknown:
-            raise B200Error(f"minares!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        return super().solve(A, b, M=M, ldiv=ldiv, lambda_=lambda_, atol=atol, rtol=rtol, artol=artol, itmax=itmax,
-                             timemax=timemax, verbose=verbose, history=history, callback=callback, fused=fused)
 
 
 class BlockGmresWorkspace(KrylovWorkspace):
@@ -781,341 +749,97 @@ def block_gmres_(ws: BlockGmresWorkspace, A, B, X0=None, **kw):
     return ws.solve(A, B, **kw)
 
 
-class _LeastSquaresWorkspace(KrylovWorkspace):
-    """Workspace of lsqr! / lsmr! on an m x n operator (src/krylov_workspaces.jl LsqrWorkspace / LsmrWorkspace):
-    b has m entries, x has n.  `window` (default 5) sizes the forward-error window."""
-    _N_on_residual_space = False    # CGNE / CRMR: N acts on the m-dimensional residual space
-
-    def _wrap_rect(self, f, nin, nout):
-        """Host callback y = f(x) with len(x) = nin and len(y) = nout (staged through pinned memory)."""
-        if self.device == "cuda":
-            raise B200Error("Python callables are host operators; create the workspace with device='host'")
-        dt = self.dtype
-
-        def tramp(xp, yp, _ud):
-            x = np.ctypeslib.as_array(C.cast(xp, C.POINTER(C.c_byte)), shape=(nin * dt.itemsize,)).view(dt)
-            y = np.ctypeslib.as_array(C.cast(yp, C.POINTER(C.c_byte)), shape=(nout * dt.itemsize,)).view(dt)
-            y[:] = f(x)
-        return _lib.MATVEC(tramp)
-
-    def solve(self, A, b, *, M=None, N=None, ldiv=False, sqd=False, lambda_=0.0, radius=0.0, etol=None, axtol=None,
-              btol=None, conlim=None, atol=0.0, rtol=0.0, itmax=0, timemax=math.inf, verbose=0, history=False,
-              callback=None, fused=True):
-        """lsqr!(ws, A, b; kwargs...) / lsmr!(ws, A, b; kwargs...)  -- kwargs as in lsqr.jl:145-162 (atol and rtol
-        default to 0 as in Julia; etol, axtol, btol default to sqrt(eps), conlim to 1/sqrt(eps)).
-
-        A: a SciPy matrix, a CsrOperator or a (rowptr, colind, values) tuple (uploaded as a CSR operator), or a
-        scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables.  M (m entries) and N (n entries):
-        None, the diagonal of a Diagonal preconditioner, or a host callable."""
-        if sqd and lambda_ != 0:
-            raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
-        if sqd:
-            lambda_ = 1.0
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
-                        opts=dict(radius=float(radius), lambda_=float(lambda_)),
-                        ext=dict(etol=_float(etol), axtol=_float(axtol), btol=_float(btol), conlim=_float(conlim)))
-        return self._run(A, b, M, N, o, e, callback)
-
-    def _run(self, A, b, M, N, o, e, callback, c=None, c_len=None):
-        """Set the options, the operator pair and the preconditioners, stage b (and c, of c_len entries, default m) and
-        call krylov_solve."""
-        m, n = self.m, self.n
-        keep = [self._set_options(e, callback)]
-        fA = fAt = None
-        if hasattr(A, "matvec") and hasattr(A, "rmatvec") and not isinstance(A, CsrOperator):   # LinearOperator
-            fA, fAt = self._wrap_rect(A.matvec, n, m), self._wrap_rect(A.rmatvec, m, n)
-        elif isinstance(A, tuple) and len(A) == 2 and all(callable(f) for f in A):
-            fA, fAt = self._wrap_rect(A[0], n, m), self._wrap_rect(A[1], m, n)
-        elif A is not None:
-            self.set_operator(A)
-        keep += [fA, fAt]
-        fP = [None, None]
-        for which, (P, ln) in enumerate(((M, m), (N, m if self._N_on_residual_space else n))):
-            if P is not None and callable(P) and not hasattr(P, "shape"):
-                fP[which] = self._wrap_rect(P, ln, ln)
-                keep.append(fP[which])
-                self._set_diag(which, None)
-            else:
-                if P is not None and getattr(P, "ndim", 1) != 1:
-                    raise B200Error(f"{self.solver} takes diagonal preconditioners (1-D arrays) or host callables")
-                self._set_diag(which, P)
-        return self._solve_staged(o, fA, fAt, fP[0], fP[1], b, c, m if c_len is None else c_len)
+# ---------------------------------------------------------------------------------------------------------------------
+# The solvers: one row each.  The workspace class, solver! and solver of every row are made from it below.
+# ---------------------------------------------------------------------------------------------------------------------
+_COMMON = dict(atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False, callback=None, fused=True,
+               ldiv=False)
 
 
-class LsqrWorkspace(_LeastSquaresWorkspace):
-    solver = "lsqr"
+@dataclass
+class _Solver:
+    """What the binding needs to know of one solver; the library checks the rest.
+
+    cls, cite: the workspace class's name and where the reference documents the solver's keywords.
+    kw: the keywords it takes besides _COMMON, M, N and c, with their defaults (None keeps the library's default).
+    fixed: option keywords it does not take but sets to these values.
+    nA: operator products per iteration (workspace_accessors.jl:101-139).
+    M, N: the space a host-callable preconditioner acts on, "m" or "n"; None where the solver takes none.
+    c: None; "m": optional, m entries; "n": required, n entries, for the adjoint system A^T y = c solved along with
+       A x = b (the third positional argument, then x0 and y0 for a warm start; AdjointStats).
+    rect: A is m x n, so the out-of-place form takes n= with a tuple operator, and (unless c is "n") no x0.
+    At: A^T is applied: A is a CSR operator, a LinearOperator or a (matvec, rmatvec) pair, and M, N are 1-D.
+    y: there is a second solution y, m entries.
+    bounds: (stats attribute, history slot, count field) of the error-bound histories in its statistics: LSLQStats
+      (src/krylov_stats.jl:352-365), and LNLQStats, whose two bounds travel in LSLQ's slots 3 and 4.
+    ws_kw: the workspace options the out-of-place form takes."""
+    cls: str
+    cite: str
+    kw: dict = field(default_factory=dict)
+    fixed: dict = field(default_factory=dict)
+    nA: int = 1
+    M: Optional[str] = None
+    N: Optional[str] = None
+    c: Optional[str] = None
+    rect: bool = False
+    At: bool = False
+    y: bool = False
+    bounds: tuple = ()
+    ws_kw: tuple = ()
+
+    def __post_init__(self):
+        taken = [k for k in ("M", "N", "c") if getattr(self, k)]
+        self.kw = {k: v for k, v in {**_COMMON, **dict.fromkeys(taken), **self.kw}.items() if k not in self.fixed}
 
 
-class LsmrWorkspace(_LeastSquaresWorkspace):
-    solver = "lsmr"
-
-
-class LslqWorkspace(_LeastSquaresWorkspace):
-    """Workspace of lslq! on an m x n operator (src/krylov_workspaces.jl LslqWorkspace): b has m entries, x has n;
-    `window` (default 5) sizes the forward-error window."""
-    solver = "lslq"
-
-    def solve(self, A, b, *, M=None, N=None, ldiv=False, transfer_to_lsqr=False, sqd=False, lambda_=0.0, sigma=0.0,
-              etol=None, utol=None, btol=None, conlim=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
-              history=False, callback=None, fused=True, **unknown):
-        """lslq!(ws, A, b; kwargs...)  -- kwargs as in lslq.jl:178-196: etol, utol, btol, atol and rtol default to
-        sqrt(eps), conlim to 1/sqrt(eps); σ (`sigma`) > 0 turns on the Gauss-Radau error bounds.  M (m entries) and N
-        (n entries): None, the diagonal of a Diagonal preconditioner, or a host callable."""
-        if unknown:
-            raise B200Error(f"lslq!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        if sqd and lambda_ != 0:
-            raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
-        if sqd:
-            lambda_ = 1.0
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=dict(lambda_=float(lambda_)),
-                        ext=dict(sigma=float(sigma), transfer_to_lsqr=int(transfer_to_lsqr), etol=_float(etol),
-                                 utol=_float(utol), btol=_float(btol), conlim=_float(conlim)))
-        return self._run(A, b, M, N, o, e, callback)
-
-
-class _NormalEquationsWorkspace(_LeastSquaresWorkspace):
-    """Workspace of cgls! / crls! on an m x n operator (src/krylov_workspaces.jl CglsWorkspace / CrlsWorkspace):
-    b has m entries, x has n."""
-
-    def solve(self, A, b, *, M=None, ldiv=False, radius=0.0, lambda_=0.0, atol=None, rtol=None, itmax=0,
-              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
-        """cgls!(ws, A, b; kwargs...) / crls!(ws, A, b; kwargs...)  -- kwargs as in cgls.jl:110-121 and
-        crls.jl:101-112: atol and rtol default to sqrt(eps), itmax = 0 means m + n.  M (m entries) acts on the residual
-        space: None, the diagonal of a Diagonal preconditioner, or a host callable.  There is no N."""
-        if unknown:
-            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
-                        opts=dict(radius=float(radius), lambda_=float(lambda_)))
-        return self._run(A, b, M, None, o, e, callback)
-
-
-class CglsWorkspace(_NormalEquationsWorkspace):
-    solver = "cgls"
-
-
-class CrlsWorkspace(_NormalEquationsWorkspace):
-    solver = "crls"
-
-
-class _BiorthWorkspace(_LeastSquaresWorkspace):
-    """Workspace of bilq! / qmr! on a square operator (src/krylov_workspaces.jl BilqWorkspace / QmrWorkspace).  Both
-    apply A and its adjoint: a CSR operator (its transpose is formed once and cached), or a
-    scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables."""
-    nA = 2
-
-    def _solve(self, A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown,
-               transfer_to_bicg=True):
-        if unknown:
-            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused,
-                        ext=dict(transfer_to_bicg=int(transfer_to_bicg)))
-        return self._run(A, b, M, N, o, e, callback, c)
-
-
-class BilqWorkspace(_BiorthWorkspace):
-    solver = "bilq"
-
-    def solve(self, A, b, *, c=None, transfer_to_bicg=True, M=None, N=None, ldiv=False, atol=None, rtol=None, itmax=0,
-              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
-        """bilq!(ws, A, b; kwargs...)  -- kwargs as in bilq.jl:97-109: c defaults to b, atol and rtol to sqrt(eps),
-        itmax = 0 means 2n.  M, N: None, the diagonal of a Diagonal preconditioner, or a self-adjoint host callable."""
-        return self._solve(A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown,
-                           transfer_to_bicg)
-
-
-class QmrWorkspace(_BiorthWorkspace):
-    solver = "qmr"
-
-    def solve(self, A, b, *, c=None, M=None, N=None, ldiv=False, atol=None, rtol=None, itmax=0, timemax=math.inf,
-              verbose=0, history=False, callback=None, fused=True, **unknown):
-        """qmr!(ws, A, b; kwargs...)  -- kwargs as in qmr.jl:104-115 (defaults as for bilq!)."""
-        return self._solve(A, b, c, M, N, ldiv, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown)
-
-
-class _AdjointWorkspace(_LeastSquaresWorkspace):
-    """Workspace of bilqr! / trilqr! (src/krylov_workspaces.jl BilqrWorkspace / TrilqrWorkspace): the primal system
-    A x = b and the adjoint system A^T y = c, solved together.  A is m x n (square for BiLQR): b and y have m entries,
-    c and x have n.  Both apply A and its adjoint: a CSR operator (its transpose is formed once and cached), or a
-    scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host callables.  Neither takes a preconditioner."""
-    nA = 2
-
-    def _solve(self, A, b, c, transfer, atol, rtol, itmax, timemax, verbose, history, callback, fused, unknown):
-        if unknown:
-            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        if c is None:
-            raise B200Error(f"{self.solver}! solves A^T y = c as well: c must be given")
-        # TriLQR's transfer_to_usymcg travels in the transfer_to_bicg field
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, False, fused, ext=dict(transfer_to_bicg=int(transfer)))
-        return self._run(A, b, None, None, o, e, callback, c, c_len=self.n)
-
-    def warm_start(self, x0, y0):
-        """warm_start!(workspace, x0, y0): x0 has n entries, y0 m."""
-        if not _is_torch(x0):
-            x0 = np.ascontiguousarray(x0, dtype=self.dtype)
-        if not _is_torch(y0):
-            y0 = np.ascontiguousarray(y0, dtype=self.dtype)
-        px, kx = _ptr(x0)
-        py, ky = _ptr(y0)
-        self._order_after(kx, ky)
-        if lib().krylov_warm_start2(self._h, px, py, int(x0.shape[0]), int(y0.shape[0])) != 0:
-            raise B200Error(_lib.last_error())
-        return self
-
-    @property
-    def y(self):
-        """The solution of A^T y = c: a host copy (or a torch CUDA tensor for device workspaces)."""
-        if self.device == "cuda":
-            import torch
-            out = torch.empty(self.m, dtype=torch.float64 if self.dtype == np.float64 else torch.float32, device="cuda")
-            if lib().krylov_get_y(self._h, C.c_void_p(out.data_ptr()), self.m) != 0:
-                raise B200Error(_lib.last_error())
-            return out
-        out = np.empty(self.m, dtype=self.dtype)
-        if lib().krylov_get_y(self._h, out.ctypes.data_as(C.c_void_p), self.m) != 0:
-            raise B200Error(_lib.last_error())
-        return out
-
-    @property
-    def stats(self) -> AdjointStats:
-        s = KrylovB200Stats()
-        if lib().krylov_b200_get_stats(self._h, C.byref(s)) != 0:
-            raise B200Error(_lib.last_error())
-
-        def hist(which, cnt):
-            buf = (C.c_double * max(cnt, 1))()
-            k = lib().krylov_b200_get_history(self._h, which, buf, cnt)
-            return list(buf[:max(k, 0)])
-        return AdjointStats(s.niter, bool(s.solved_primal), bool(s.solved_dual), hist(0, s.nresiduals),
-                            hist(6, s.nresiduals_dual), s.timer, s.status.decode("utf-8"))
-
-
-class BilqrWorkspace(_AdjointWorkspace):
-    solver = "bilqr"
-
-    def solve(self, A, b, c, *, transfer_to_bicg=True, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
-              history=False, callback=None, fused=True, **unknown):
-        """bilqr!(ws, A, b, c; kwargs...)  -- kwargs as in bilqr.jl:99-107: atol and rtol default to sqrt(eps),
-        itmax = 0 means 2n."""
-        return self._solve(A, b, c, transfer_to_bicg, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-                           unknown)
-
-
-class TrilqrWorkspace(_AdjointWorkspace):
-    solver = "trilqr"
-
-    def solve(self, A, b, c, *, transfer_to_usymcg=True, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0,
-              history=False, callback=None, fused=True, **unknown):
-        """trilqr!(ws, A, b, c; kwargs...)  -- kwargs as in trilqr.jl: atol and rtol default to sqrt(eps), itmax = 0
-        means m + n.  A is m x n, b has m entries and c n."""
-        return self._solve(A, b, c, transfer_to_usymcg, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-                           unknown)
-
-
-class _LeastNormWorkspace(_LeastSquaresWorkspace):
-    """Workspace of craig! / craigmr! on an m x n operator (src/krylov_workspaces.jl CraigWorkspace / CraigmrWorkspace):
-    the least-norm solution of A x = b, x = A^T y.  b and y have m entries, x has n.  A and its adjoint: a CSR operator
-    (its transpose is formed once and cached), or a scipy.sparse.linalg.LinearOperator / (matvec, rmatvec) pair of host
-    callables.  M (m entries) and N (n entries): None, the diagonal of a Diagonal preconditioner, or a host callable."""
-    nA = 2
-
-    def _solve(self, A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-               unknown, transfer_to_lsqr=False, btol=None, conlim=None, ext=None):
-        if unknown:
-            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        if sqd and lambda_ != 0:
-            raise B200Error("sqd cannot be set to true if λ ≠ 0 !")
-        if sqd:
-            lambda_ = 1.0
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=dict(lambda_=float(lambda_)),
-                        ext=dict(dict(transfer_to_lsqr=int(transfer_to_lsqr), btol=_float(btol), conlim=_float(conlim)),
-                                 **(ext or {})))
-        return self._run(A, b, M, N, o, e, callback)
-
-    y = _AdjointWorkspace.y
-
-
-class CraigWorkspace(_LeastNormWorkspace):
-    solver = "craig"
-
-    def solve(self, A, b, *, M=None, N=None, ldiv=False, transfer_to_lsqr=False, sqd=False, lambda_=0.0, btol=None,
-              conlim=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False, callback=None,
-              fused=True, **unknown):
-        """craig!(ws, A, b; kwargs...)  -- kwargs as in craig.jl:151-166: btol, atol and rtol default to sqrt(eps),
-        conlim to 1/sqrt(eps), itmax = 0 means m + n; transfer_to_lsqr acts when λ > 0."""
-        return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-                           unknown, transfer_to_lsqr, btol, conlim)
-
-
-class CraigmrWorkspace(_LeastNormWorkspace):
-    solver = "craigmr"
-
-    def solve(self, A, b, *, M=None, N=None, ldiv=False, sqd=False, lambda_=0.0, atol=None, rtol=None, itmax=0,
-              timemax=math.inf, verbose=0, history=False, callback=None, fused=True, **unknown):
-        """craigmr!(ws, A, b; kwargs...)  -- kwargs as in craigmr.jl:141-153: atol and rtol default to sqrt(eps),
-        itmax = 0 means m + n."""
-        return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-                           unknown)
-
-
-class LnlqWorkspace(_LeastNormWorkspace):
-    solver = "lnlq"
-
-    def solve(self, A, b, *, M=None, N=None, ldiv=False, transfer_to_craig=True, sqd=False, lambda_=0.0, sigma=0.0,
-              utolx=None, utoly=None, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False,
-              callback=None, fused=True, **unknown):
-        """lnlq!(ws, A, b; kwargs...)  -- kwargs as in lnlq.jl:144-160: utolx, utoly, atol and rtol default to sqrt(eps),
-        itmax = 0 means m + n; σ (`sigma`) > 0, or λ > 0, turns on the upper bounds on ‖x - x*‖ and ‖y - y*‖
-        (stats.error_bnd_x / error_bnd_y)."""
-        ext = {"sigma": float(sigma), "transfer_to_bicg": int(transfer_to_craig)}
-        for name, val in (("utol", utolx), ("etol", utoly)):          # the C ABI carries utolx in utol, utoly in etol
-            if val is not None:
-                ext[name] = float(val)
-        return self._solve(A, b, M, N, ldiv, sqd, lambda_, atol, rtol, itmax, timemax, verbose, history, callback, fused,
-                           unknown, ext=ext)
-
-
-class _NormalLeastNormWorkspace(_LeastSquaresWorkspace):
-    """Workspace of cgne! / crmr! on an m x n operator (src/krylov_workspaces.jl CgneWorkspace / CrmrWorkspace): the
-    least-norm solution of A x = b by CG / CR on A A^T y = b, x = A^T y.  b has m entries, x has n; only x is returned.
-    A and its adjoint: a CSR operator (its transpose is formed once and cached), or a scipy.sparse.linalg.LinearOperator
-    / (matvec, rmatvec) pair of host callables.  N (m entries) acts on the residual space: None, the diagonal of a
-    Diagonal preconditioner, or a host callable.  There is no M."""
-    nA = 2
-    _N_on_residual_space = True
-
-    def solve(self, A, b, *, N=None, ldiv=False, lambda_=0.0, atol=None, rtol=None, itmax=0, timemax=math.inf,
-              verbose=0, history=False, callback=None, fused=True, **unknown):
-        """cgne!(ws, A, b; kwargs...) / crmr!(ws, A, b; kwargs...)  -- kwargs as in cgne.jl:116-126 and
-        crmr.jl:114-124: atol and rtol default to sqrt(eps), itmax = 0 means m + n, λ (`lambda_`) >= 0."""
-        if unknown:
-            raise B200Error(f"{self.solver}!: unsupported keyword argument(s) {', '.join(sorted(unknown))}")
-        o, e = _options(atol, rtol, itmax, timemax, verbose, history, ldiv, fused, opts=dict(lambda_=float(lambda_)))
-        return self._run(A, b, None, N, o, e, callback)
-
-
-class CgneWorkspace(_NormalLeastNormWorkspace):
-    solver = "cgne"
-
-
-class CrmrWorkspace(_NormalLeastNormWorkspace):
-    solver = "crmr"
-
-
-def _one_shot(name, b, n, run, **ws_kw):
-    """Create the workspace of `name` (m = len(b) rows, n columns) for b's element type and place, return run(ws) and
-    free it.  The element type of a torch b is read without copying it to the host."""
-    if _is_torch(b):
-        import torch
-        dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
-    else:
-        dt = np.asarray(b).dtype
-    if dt not in (np.float32, np.float64):
-        dt = np.float64
-    ws = _WS[name](b.shape[0], int(n), dt, device="cuda" if _is_torch(b) else "host", **ws_kw)
-    try:
-        return run(ws)
-    finally:
-        ws.free()
+_SQUARE = dict(kw=dict(radius=0.0, linesearch=False, lambda_=0.0, etol=None, conlim=None, restart=False,
+                       reorthogonalization=False, batch=0, time_kernels=False, check_curvature=False, gamma=None,
+                       artol=None), M="n", N="n", c="m", ws_kw=("memory", "window"))
+_LSQ = dict(M="m", N="n", rect=True, At=True, ws_kw=("window",))
+_LN = dict(nA=2, M="m", N="n", rect=True, At=True, y=True)
+_SQD = dict(sqd=False, lambda_=0.0)
+_SOLVERS = {
+    "cg": _Solver("CgWorkspace", "cg.jl:100-111", **_SQUARE),
+    "cr": _Solver("CrWorkspace", "cr.jl", **_SQUARE),
+    "minres": _Solver("MinresWorkspace", "minres.jl:138-151", **_SQUARE),
+    "diom": _Solver("DiomWorkspace", "diom.jl", **_SQUARE),
+    "fom": _Solver("FomWorkspace", "fom.jl", **_SQUARE),
+    "dqgmres": _Solver("DqgmresWorkspace", "dqgmres.jl", **_SQUARE),
+    "gmres": _Solver("GmresWorkspace", "gmres.jl:96-108", **_SQUARE),
+    "fgmres": _Solver("FgmresWorkspace", "fgmres.jl", **_SQUARE),
+    "bicgstab": _Solver("BicgstabWorkspace", "bicgstab.jl:105-116", nA=2, **_SQUARE),
+    "cgs": _Solver("CgsWorkspace", "cgs.jl", nA=2, **_SQUARE),
+    "cg_lanczos": _Solver("CgLanczosWorkspace", "cg_lanczos.jl", **_SQUARE),
+    "car": _Solver("CarWorkspace", "car.jl:90-99", M="n", ws_kw=("memory", "window")),
+    "minares": _Solver("MinaresWorkspace", "minares.jl:93-104", dict(lambda_=0.0, artol=None), M="n",
+                       ws_kw=("memory", "window")),
+    "lsqr": _Solver("LsqrWorkspace", "lsqr.jl:145-162", dict(_SQD, radius=0.0, etol=None, axtol=None, btol=None,
+                                                              conlim=None, atol=0.0, rtol=0.0), **_LSQ),
+    "lsmr": _Solver("LsmrWorkspace", "lsmr.jl", dict(_SQD, radius=0.0, etol=None, axtol=None, btol=None, conlim=None,
+                                                     atol=0.0, rtol=0.0), **_LSQ),
+    "lslq": _Solver("LslqWorkspace", "lslq.jl:178-196", dict(_SQD, transfer_to_lsqr=False, sigma=0.0, etol=None,
+                                                              utol=None, btol=None, conlim=None),
+                    bounds=(("err_lbnds", 3, "nerr_lbnds"), ("err_ubnds_lq", 4, "nerr_ubnds_lq"),
+                            ("err_ubnds_cg", 5, "nerr_ubnds_cg")), **_LSQ),
+    "cgls": _Solver("CglsWorkspace", "cgls.jl:110-121", dict(radius=0.0, lambda_=0.0), **dict(_LSQ, N=None)),
+    "crls": _Solver("CrlsWorkspace", "crls.jl:101-112", dict(radius=0.0, lambda_=0.0), **dict(_LSQ, N=None)),
+    "bilq": _Solver("BilqWorkspace", "bilq.jl:97-109", dict(transfer_to_bicg=True), nA=2, M="m", N="n", c="m", At=True,
+                    ws_kw=("memory", "window")),
+    "qmr": _Solver("QmrWorkspace", "qmr.jl:104-115", fixed=dict(transfer_to_bicg=True), nA=2, M="m", N="n", c="m",
+                   At=True, ws_kw=("memory", "window")),
+    "bilqr": _Solver("BilqrWorkspace", "bilqr.jl:99-107", dict(transfer_to_bicg=True), dict(ldiv=False), nA=2, c="n",
+                     At=True, y=True),
+    "trilqr": _Solver("TrilqrWorkspace", "trilqr.jl", dict(transfer_to_usymcg=True), dict(ldiv=False), nA=2, c="n",
+                      rect=True, At=True, y=True),
+    "craig": _Solver("CraigWorkspace", "craig.jl:151-166", dict(_SQD, transfer_to_lsqr=False, btol=None, conlim=None),
+                     **_LN),
+    "craigmr": _Solver("CraigmrWorkspace", "craigmr.jl:141-153", _SQD, **_LN),
+    "lnlq": _Solver("LnlqWorkspace", "lnlq.jl:144-160", dict(_SQD, transfer_to_craig=True, sigma=0.0, utolx=None,
+                                                              utoly=None),
+                    bounds=(("error_bnd_x", 3, "nerr_lbnds"), ("error_bnd_y", 4, "nerr_ubnds_lq")), **_LN),
+    "cgne": _Solver("CgneWorkspace", "cgne.jl:116-126", dict(lambda_=0.0), **dict(_LN, M=None, N="m", y=False)),
+    "crmr": _Solver("CrmrWorkspace", "crmr.jl:114-124", dict(lambda_=0.0), **dict(_LN, M=None, N="m", y=False)),
+}
 
 
 def _columns(name, A, n):
@@ -1126,88 +850,87 @@ def _columns(name, A, n):
     return n
 
 
-def _make_least_norm(name):
-    def f(A, b, x0=None, *, n=None, **kw):
-        if x0 is not None:
-            raise B200Error(f"{name} does not support warm-start (it takes no x0)")
-
-        def run(ws):
-            ws.solve(A, b, **kw)
-            return ws.x, ws.y, ws.stats
-        return _one_shot(name, b, _columns(name, A, n), run)
-    f.__name__ = name
-    f.__doc__ = f"(x, y, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
-    return f
-
-
-def _make_normal_least_norm(name):
-    def f(A, b, x0=None, *, n=None, **kw):
-        if x0 is not None:
-            raise B200Error(f"{name} does not support warm-start (it takes no x0)")
-
-        def run(ws):
-            ws.solve(A, b, **kw)
-            return ws.x, ws.stats
-        return _one_shot(name, b, _columns(name, A, n), run)
-    f.__name__ = name
-    f.__doc__ = f"(x, stats) = {name}(A, b; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, x = A^T y"
-    return f
+def _positional(who, row, args, kw):
+    """Move the arguments after b into kw -- c, x0 and y0 for the solvers that require c, x0 for the others -- and
+    return the warm start (x0, y0)."""
+    names = ("c", "x0", "y0") if row.c == "n" else ("x0",)
+    if len(args) > len(names):
+        raise TypeError(f"{who}: the arguments after b are {', '.join(names)}")
+    for k, v in zip(names, args):
+        if k in kw:
+            raise TypeError(f"{who}: {k} is given twice")
+        kw[k] = v
+    return kw.pop("x0", None), kw.pop("y0", None) if row.c == "n" else None
 
 
-def _make_adjoint(name):
-    def f(A, b, c, x0=None, y0=None, **kw):
-        def run(ws):
-            if (x0 is None) != (y0 is None):
-                raise B200Error(f"{name}: pass both x0 and y0, or neither")
-            if x0 is not None:
-                ws.warm_start(x0, y0)
-            ws.solve(A, b, c, **kw)
-            return ws.x, ws.y, ws.stats
-        return _one_shot(name, b, c.shape[0], run)
-    f.__name__ = name
-    f.__doc__ = f"(x, y, stats) = {name}(A, b, c[, x0, y0]; kwargs...)  (src/{name}.jl); A is m x n, b has m entries, c n"
-    return f
-
-
-def _make_adjoint_inplace(name):
-    def f(ws, A, b, c, x0=None, y0=None, **kw):
-        if ws.solver != name:
-            raise B200Error(f"{name}! needs a {_WS[name].__name__}")
+def _warm_start(who, row, ws, x0, y0):
+    if row.c == "n":
         if (x0 is None) != (y0 is None):
-            raise B200Error(f"{name}!: pass both x0 and y0, or neither")
+            raise B200Error(f"{who}: pass both x0 and y0, or neither")
         if x0 is not None:
             ws.warm_start(x0, y0)
-        return ws.solve(A, b, c, **kw)
+    elif x0 is not None:
+        ws.warm_start(x0)
+
+
+def _make_inplace(name, row):
+    def f(ws, A, b, *args, **kw):
+        if ws.solver != name:
+            raise B200Error(f"{name}! needs a {row.cls}")
+        _warm_start(name + "!", row, ws, *_positional(name + "!", row, args, kw))
+        return ws.solve(A, b, **kw)
     f.__name__ = name + "_"
-    f.__doc__ = f"{name}!(workspace, A, b, c[, x0, y0]; kwargs...)"
+    f.__doc__ = f"{name}!(workspace, A, b{', c[, x0, y0]' if row.c == 'n' else '[, x0]'}; kwargs...)"
     return f
 
 
-def _make_least_squares(name):
-    def f(A, b, *, n=None, window=0, **kw):
-        def run(ws):
+def _make_outofplace(name, row):
+    def f(A, b, *args, **kw):
+        x0, y0 = _positional(name, row, args, kw)
+        if row.c == "n":
+            if kw.get("c") is None:
+                raise B200Error(f"{name}! solves A^T y = c as well: c must be given")
+            n = kw["c"].shape[0]
+        elif row.rect:
+            if x0 is not None:
+                raise B200Error(f"{name} does not support warm-start (it takes no x0)")
+            n = _columns(name, A, kw.pop("n", None))
+        else:
+            n = b.shape[0]
+        if _is_torch(b):       # the element type of a torch b is read without copying it to the host
+            import torch
+            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
+        else:
+            dt = np.asarray(b).dtype
+        if dt not in (np.float32, np.float64):
+            dt = np.float64
+        ws_kw = {k: kw.pop(k) for k in row.ws_kw if k in kw}
+        ws = globals()[row.cls](b.shape[0], int(n), dt, device="cuda" if _is_torch(b) else "host", **ws_kw)
+        try:
+            _warm_start(name, row, ws, x0, y0)
             ws.solve(A, b, **kw)
-            return ws.x, ws.stats
-        return _one_shot(name, b, _columns(name, A, n), run, window=window)
+            return (ws.x, ws.y, ws.stats) if row.y else (ws.x, ws.stats)
+        finally:
+            ws.free()
     f.__name__ = name
-    f.__doc__ = f"(x, stats) = {name}(A, b; window=5, kwargs...)  (src/{name}.jl); A is m x n, b has m entries"
+    f.__doc__ = (f"({'x, y' if row.y else 'x'}, stats) = {name}(A, b{', c[, x0, y0]' if row.c == 'n' else '' if row.rect else '[, x0]'}; "
+                 f"kwargs...)  (src/{row.cite})")
     return f
 
 
-_WS = {"cg": CgWorkspace, "minres": MinresWorkspace, "gmres": GmresWorkspace, "bicgstab": BicgstabWorkspace,
-       "fom": FomWorkspace, "fgmres": FgmresWorkspace, "cgs": CgsWorkspace, "cg_lanczos": CgLanczosWorkspace,
-       "cr": CrWorkspace, "diom": DiomWorkspace, "dqgmres": DqgmresWorkspace, "lsqr": LsqrWorkspace,
-       "lsmr": LsmrWorkspace, "cgls": CglsWorkspace, "crls": CrlsWorkspace,
-       "lslq": LslqWorkspace, "bilq": BilqWorkspace, "qmr": QmrWorkspace, "car": CarWorkspace,
-       "minares": MinaresWorkspace, "bilqr": BilqrWorkspace, "trilqr": TrilqrWorkspace, "craig": CraigWorkspace,
-       "craigmr": CraigmrWorkspace, "lnlq": LnlqWorkspace, "cgne": CgneWorkspace, "crmr": CrmrWorkspace}
+for _name, _row in _SOLVERS.items():
+    globals()[_row.cls] = type(_row.cls, (KrylovWorkspace,), dict(
+        solver=_name, nA=_row.nA, __doc__=f"Workspace of {_name}! (src/{_row.cite}); solve keywords and defaults: "
+                                          + ", ".join(f"{k}={v!r}" for k, v in _row.kw.items()) + "."))
+    globals()[_name + "_"], globals()[_name] = _make_inplace(_name, _row), _make_outofplace(_name, _row)
+    __all__ += [_row.cls, _name, _name + "_"]
 
 
 def krylov_workspace(method: str, *args, **kw) -> KrylovWorkspace:
     """krylov_workspace(Val(method), ...)  (src/interface.jl:248-348)"""
-    if method not in _WS:
-        raise B200Error(f"method {method!r} is outside the GPU path ({', '.join(sorted(_WS))})")
-    return _WS[method](*args, **kw)
+    if method not in _SOLVERS:
+        raise B200Error(f"method {method!r} is outside the GPU path ({', '.join(sorted(_SOLVERS))})")
+    return globals()[_SOLVERS[method].cls](*args, **kw)
 
 
 def krylov_solve_(ws: KrylovWorkspace, A, b, x0=None, **kw) -> KrylovWorkspace:
@@ -1217,55 +940,12 @@ def krylov_solve_(ws: KrylovWorkspace, A, b, x0=None, **kw) -> KrylovWorkspace:
     return ws.solve(A, b, **kw)
 
 
-def _make_inplace(name):
-    def f(ws, A, b, x0=None, **kw):
-        if ws.solver != name:
-            raise B200Error(f"{name}! needs a {_WS[name].__name__}")
-        return krylov_solve_(ws, A, b, x0, **kw)
-    f.__name__ = name + "_"
-    f.__doc__ = f"{name}!(workspace, A, b[, x0]; kwargs...)"
-    return f
-
-
-def _make_outofplace(name):
-    def f(A, b, x0=None, *, memory=0, window=0, **kw):
-        def run(ws):
-            krylov_solve_(ws, A, b, x0, **kw)
-            return ws.x, ws.stats
-        return _one_shot(name, b, b.shape[0], run, memory=memory, window=window)
-    f.__name__ = name
-    f.__doc__ = f"(x, stats) = {name}(A, b[, x0]; kwargs...)"
-    return f
-
-
-cg_, gmres_, bicgstab_, minres_ = (_make_inplace(s) for s in ("cg", "gmres", "bicgstab", "minres"))
-cg, gmres, bicgstab, minres = (_make_outofplace(s) for s in ("cg", "gmres", "bicgstab", "minres"))
-fom_, fgmres_, cgs_, cg_lanczos_ = (_make_inplace(s) for s in ("fom", "fgmres", "cgs", "cg_lanczos"))
-fom, fgmres, cgs, cg_lanczos = (_make_outofplace(s) for s in ("fom", "fgmres", "cgs", "cg_lanczos"))
-cr_, diom_, dqgmres_ = (_make_inplace(s) for s in ("cr", "diom", "dqgmres"))
-cr, diom, dqgmres = (_make_outofplace(s) for s in ("cr", "diom", "dqgmres"))
-lsqr_, lsmr_ = (_make_inplace(s) for s in ("lsqr", "lsmr"))
-lsqr, lsmr = (_make_least_squares(s) for s in ("lsqr", "lsmr"))
-cgls_, crls_, lslq_ = (_make_inplace(s) for s in ("cgls", "crls", "lslq"))
-cgls, crls, lslq = (_make_least_squares(s) for s in ("cgls", "crls", "lslq"))
-bilq_, qmr_ = (_make_inplace(s) for s in ("bilq", "qmr"))
-bilq, qmr = (_make_outofplace(s) for s in ("bilq", "qmr"))
-car_, minares_ = (_make_inplace(s) for s in ("car", "minares"))
-car, minares = (_make_outofplace(s) for s in ("car", "minares"))
-bilqr_, trilqr_ = (_make_adjoint_inplace(s) for s in ("bilqr", "trilqr"))
-bilqr, trilqr = (_make_adjoint(s) for s in ("bilqr", "trilqr"))
-craig_, craigmr_ = (_make_inplace(s) for s in ("craig", "craigmr"))
-craig, craigmr = (_make_least_norm(s) for s in ("craig", "craigmr"))
-lnlq_, lnlq = _make_inplace("lnlq"), _make_least_norm("lnlq")
-cgne_, crmr_ = (_make_inplace(s) for s in ("cgne", "crmr"))
-cgne, crmr = (_make_normal_least_norm(s) for s in ("cgne", "crmr"))
-
-
 def krylov_solve(method: str, A, b, x0=None, **kw):
-    return {"cg": cg, "gmres": gmres, "bicgstab": bicgstab, "minres": minres, "fom": fom, "fgmres": fgmres, "cgs": cgs,
-            "cg_lanczos": cg_lanczos, "cr": cr, "diom": diom, "dqgmres": dqgmres, "bilq": bilq,
-            "qmr": qmr, "car": car, "minares": minares, "craig": craig, "craigmr": craigmr,
-            "lnlq": lnlq, "cgne": cgne, "crmr": crmr}[method](A, b, x0, **kw)
+    """krylov_solve(method, A, b[, x0]; kwargs...): the out-of-place form of `method`.  BiLQR and TriLQR, which
+    take c as well, raise KeyError like a method outside the GPU path."""
+    if _SOLVERS[method].c == "n":
+        raise KeyError(method)
+    return globals()[method](A, b, x0, **kw)
 
 
 # workspace_accessors.jl:140-152
