@@ -390,31 +390,34 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   return t;
 }
 
-// Phase B with a block-Jacobi M (cg.jl:240-242): one thread per diagonal block updates r, forms z = M_blk r on the
-// spot (the block's rows are all in this thread's registers) and accumulates <r, z>.  BS = 0: run-time block size.
+// Phase B with a block-Jacobi M (cg.jl:240-242): one thread per row, as in the element loops, so that <r, z> has one
+// term per thread and sums in the same tree as every other reduction.  A CTA takes `chunk` rows per trip, a whole number
+// of blocks (kTileThreads rounded down to a multiple of bs, >= 256 for bs <= 8), so no block straddles two CTAs: each
+// thread updates its row of r, the CTA syncs, and each thread forms its row of z = M_blk r from the block's new r.
+// At n <= 256 and one CTA, row i is on thread i.  All threads of the CTA must call (uniform trip count per CTA).
+// BS = 0: run-time block size.
 template <class T, int BS>
-__device__ __forceinline__ T cg_phase_b_block(int n, int bs_rt, T nalpha, T* r, const T* Ap, T* z, const T* __restrict__ B, int first, int stride) {
+__device__ __forceinline__ T cg_phase_b_block(int n, int bs_rt, T nalpha, T* r, const T* Ap, T* z, const T* __restrict__ B) {
   const int bs = BS ? BS : bs_rt;
-  const int nb = (n + bs - 1) / bs;
+  const int chunk = kTileThreads - kTileThreads % bs, tid = threadIdx.x;
   T acc = T(0);
-  for (int blk = first; blk < nb; blk += stride) {
-    const int r0 = blk * bs, rows = min(bs, n - r0);
-    T rn[BS ? BS : 8];
+  for (int base = (int)blockIdx.x * chunk; base < n; base += (int)gridDim.x * chunk) {
+    const int i = base + tid;
+    const bool mine = tid < chunk && i < n;
+    T rn = T(0);
+    if (mine) { rn = add_rn(r[i], mul_rn(nalpha, Ap[i])); r[i] = rn; }
+    __syncthreads();                             // the block's new r is visible to all its rows (same CTA)
+    if (mine) {
+      const int r0 = i - i % bs, rows = min(bs, n - r0);
+      const T* Bi = B + (size_t)(r0 / bs) * bs * bs + (size_t)(i - r0) * bs;
+      T zi = T(0);
 #pragma unroll
-    for (int i = 0; i < (BS ? BS : 8); i++)
-      if (i < rows) { rn[i] = add_rn(r[r0 + i], mul_rn(nalpha, Ap[r0 + i])); r[r0 + i] = rn[i]; }
-    const T* Bk = B + (size_t)blk * bs * bs;
-#pragma unroll
-    for (int i = 0; i < (BS ? BS : 8); i++) {
-      if (i < rows) {
-        T zi = T(0);
-#pragma unroll
-        for (int j = 0; j < (BS ? BS : 8); j++)
-          if (j < rows) zi = add_rn(zi, mul_rn(__ldg(&Bk[i * bs + j]), rn[j]));
-        z[r0 + i] = zi;
-        acc += rn[i] * zi;
-      }
+      for (int j = 0; j < (BS ? BS : 8); j++)
+        if (j < rows) zi = add_rn(zi, mul_rn(__ldg(&Bi[j]), r[r0 + j]));
+      z[i] = zi;
+      acc += rn * zi;
     }
+    __syncthreads();                             // this trip's reads of r are done before the next trip's writes
   }
   return acc;
 }
@@ -502,10 +505,10 @@ __device__ __forceinline__ int cg_persist_iterations(int n, const CgPersistArgs<
     const int i = (int)blockIdx.x * kTileThreads + tid, stride = G * kTileThreads;
     T acc;
     if (MODE == kBlockJac) {
-      if (a.mbs == 4) acc = cg_phase_b_block<T, 4>(n, 4, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
-      else if (a.mbs == 2) acc = cg_phase_b_block<T, 2>(n, 2, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
-      else if (a.mbs == 8) acc = cg_phase_b_block<T, 8>(n, 8, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
-      else acc = cg_phase_b_block<T, 0>(n, a.mbs, nalpha, a.r, a.Ap, a.z, a.mblocks, i, stride);
+      if (a.mbs == 4) acc = cg_phase_b_block<T, 4>(n, 4, nalpha, a.r, a.Ap, a.z, a.mblocks);
+      else if (a.mbs == 2) acc = cg_phase_b_block<T, 2>(n, 2, nalpha, a.r, a.Ap, a.z, a.mblocks);
+      else if (a.mbs == 8) acc = cg_phase_b_block<T, 8>(n, 8, nalpha, a.r, a.Ap, a.z, a.mblocks);
+      else acc = cg_phase_b_block<T, 0>(n, a.mbs, nalpha, a.r, a.Ap, a.z, a.mblocks);
     } else {
       acc = cg_phase_b_elems<T, MODE>(n, nalpha, a.r, a.Ap, a.mdiag, i, stride);
     }

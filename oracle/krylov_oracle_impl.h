@@ -46,13 +46,29 @@ static void SUF(spmv)(const SUF(csr) *A, const REAL *x, REAL *y) {
 /* BLAS-1 wrappers, src/krylov_utils.jl:309-347 (sequential restatement). */
 /* Test knob (oracle_set_dot_mode): 0 = the restatement's sequential sum in REAL; 1 = the same terms accumulated in
  * double and rounded once.  Float32 parity tests run both and take the gap between the two histories as the
- * measured sensitivity of the iteration to the rounding of its dot products (tests/test_gpu_solvers.py). */
+ * measured sensitivity of the iteration to the rounding of its dot products (tests/test_gpu_solvers.py).
+ * 2 = the order of the device's reductions at one CTA of 256 threads (n <= 256; NaN beyond): term i is thread i's
+ * partial (REAL)0 + x[i]*y[i], each warp of 32 lanes folds in halves (lane l += lane l+16, +8, +4, +2, +1: what
+ * warp_sum's xor butterfly leaves in lane 0), and the 8 warp sums, padded to 32 with zeros, fold the same way
+ * (block_sum).  With it the oracle and the GPU must agree bit for bit (tests/test_gpu_exact_small.py). */
 extern int oracle_dot_mode;
+static REAL SUF(fold32)(REAL *v) {
+  for (int s = 16; s > 0; s >>= 1)
+    for (int l = 0; l < s; l++) v[l] = v[l] + v[l + s];
+  return v[0];
+}
 static REAL SUF(kdot)(int n, const REAL *x, const REAL *y) {
   if (oracle_dot_mode == 1) {
     double s = 0.0;
     for (int i = 0; i < n; i++) { double p = (double)x[i] * (double)y[i]; s = s + p; }
     return (REAL)s;
+  }
+  if (oracle_dot_mode == 2) {
+    if (n > 256) return (REAL)NAN;
+    REAL lane[256], warp[32];
+    for (int i = 0; i < 256; i++) { REAL p = i < n ? x[i] * y[i] : (REAL)0; lane[i] = (REAL)0 + p; }
+    for (int w = 0; w < 32; w++) warp[w] = w < 8 ? SUF(fold32)(lane + 32 * w) : (REAL)0;
+    return SUF(fold32)(warp);
   }
   REAL s = (REAL)0;
   for (int i = 0; i < n; i++) { REAL p = x[i] * y[i]; s = s + p; }
@@ -60,6 +76,13 @@ static REAL SUF(kdot)(int n, const REAL *x, const REAL *y) {
 }
 static REAL SUF(knorm)(int n, const REAL *x) { return SQRT(SUF(kdot)(n, x, x)); }
 static void SUF(kscal)(int n, REAL s, REAL *x) { for (int i = 0; i < n; i++) x[i] = s * x[i]; }
+/* The norm of a solver's window of error estimates: a few scalars the product keeps on the host and sums there in
+ * order, so a plain sequential sum whatever the dot mode. */
+static REAL SUF(err_norm)(int w, const REAL *e) {
+  REAL s = 0;
+  for (int i = 0; i < w; i++) s += e[i] * e[i];
+  return SQRT(s);
+}
 /* kdiv!(n,x,s) = kscal!(n, one/s, x)  (krylov_utils.jl:325) */
 static void SUF(kdiv)(int n, REAL *x, REAL s) { SUF(kscal)(n, (REAL)1 / s, x); }
 static void SUF(kcopy)(int n, REAL *y, const REAL *x) { memcpy(y, x, sizeof(REAL) * (size_t)n); }
@@ -744,7 +767,7 @@ int SUF(oracle_minres)(int n, const int *rowptr, const int *colind, const REAL *
     xENorm2 = xENorm2 + phi * phi;
     if (iter >= 2) { REAL *tmp = wa; wa = wb; wb = tmp; }
     err_vec[iter % window] = phi;
-    if (iter >= window) err_lbnd = SUF(knorm)(window, err_vec);
+    if (iter >= window) err_lbnd = SUF(err_norm)(window, err_vec);
     gmax = gmax > gamma ? gmax : gamma;
     gmin = gmin < gamma ? gmin : gamma;
     REAL zeta = rhs1 / gamma;

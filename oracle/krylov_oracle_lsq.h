@@ -38,11 +38,6 @@ static void SUF(spmv_rect)(int m, const int *rowptr, const int *colind, const RE
 static REAL SUF(knorm_ell)(int n, const REAL *x, const REAL *y) {
   return x == y ? SUF(knorm)(n, x) : SQRT(SUF(kdot)(n, x, y));
 }
-static REAL SUF(err_norm)(int w, const REAL *e) {
-  REAL s = 0;
-  for (int i = 0; i < w; i++) s += e[i] * e[i];
-  return SQRT(s);
-}
 
 /* lsmr = 0: lsqr!, 1: lsmr!.  Returns 0, or where the reference raises: 10 + to_boundary's error code. */
 int SUF(oracle_lsq)(int lsmr, int m, int n, const int *rowptr, const int *colind, const REAL *val, const REAL *b,

@@ -118,7 +118,8 @@ def _result(st, x, res, extra=None):
 
 class dot_mode:
     """with dot_mode(1): ...  -- the oracle's dot products, in every solver family, accumulate in double and round once
-    (test knob, krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision."""
+    (test knob, krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision;
+    2 sums in the order of the device's one-CTA reduction tree (n <= 256, NaN beyond)."""
 
     def __init__(self, mode):
         self.mode = int(mode)
