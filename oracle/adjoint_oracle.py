@@ -1,4 +1,4 @@
-"""ctypes front-end of the CPU restatement of bilqr! / trilqr! -- TEST INFRASTRUCTURE ONLY.
+"""Problem generators of the CPU restatement of bilqr! / trilqr!, and its solver functions -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
 krylov_oracle_adjoint.h, built into the oracle library that oracle.py builds and loads, so oracle.dot_mode
@@ -9,53 +9,12 @@ histories).
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 
 import numpy as np
 import scipy.sparse as sp
 
-from oracle.oracle import (_ITER_CB, Stats, _csr, _opts, _p, _suf, _vec, bc_breakdown, dot_mode,  # noqa: F401
-                           kron_unsymmetric, lib)
-
-
-def _adjoint(tri, A, b, c, x0, y0, transfer, timemax, callback, dtype, kw):
-    suf, _ = _suf(dtype)
-    A = sp.csr_matrix(A)
-    m, n = A.shape
-    _, rp, ci, va = _csr(A, dtype)
-    _, trp, tci, tva = _csr(A.T, dtype)
-    b, c, x0, y0 = (_vec(v, dtype) for v in (b, c, x0, y0))
-    if (x0 is None) != (y0 is None):
-        raise ValueError("pass both x0 and y0, or neither")
-    o = _opts(n, kw, 1 << 22)
-    itmax = o.itmax if o.itmax > 0 else (m + n if tri else 2 * n)
-    o.hist_cap = min(itmax + 2, 1 << 22)
-    x, t = np.zeros(n, dtype), np.zeros(m, dtype)
-    rres, sres = np.zeros(o.hist_cap, dtype), np.zeros(o.hist_cap, dtype)
-    nsres, sp_, sd_ = C.c_int(0), C.c_int(0), C.c_int(0)
-    st = Stats()
-    cb = _ITER_CB(lambda it, _u: int(bool(callback(it)))) if callback is not None else _ITER_CB()
-    f = getattr(lib(), f"oracle_adjoint_{suf}")
-    f.argtypes = [C.c_int] * 3 + [C.c_void_p] * 10 + [C.c_int, C.c_double, _ITER_CB] + [C.c_void_p] * 9
-    f(int(tri), m, n, _p(rp), _p(ci), _p(va), _p(trp), _p(tci), _p(tva), _p(b), _p(c), _p(x0), _p(y0), int(transfer),
-      -1.0 if math.isinf(timemax) else float(timemax), cb, None, C.cast(C.byref(o), C.c_void_p), _p(x), _p(t), _p(rres),
-      _p(sres), C.cast(C.byref(nsres), C.c_void_p), C.cast(C.byref(sp_), C.c_void_p), C.cast(C.byref(sd_), C.c_void_p),
-      C.cast(C.byref(st), C.c_void_p))
-    stats = dict(niter=st.niter, solved=bool(st.solved), solved_primal=bool(sp_.value), solved_dual=bool(sd_.value),
-                 status=st.status.decode("utf-8"), residuals_primal=rres[:min(st.nres, o.hist_cap)].copy(),
-                 residuals_dual=sres[:min(nsres.value, o.hist_cap)].copy())
-    return x, t, stats
-
-
-def bilqr(A, b, c, x0=None, y0=None, transfer_to_bicg=True, timemax=math.inf, callback=None, dtype=np.float64, **kw):
-    """bilqr! (src/bilqr.jl:115-484) -> (x, y, stats).  callback(iter) -> bool stops the solve when true."""
-    return _adjoint(False, A, b, c, x0, y0, transfer_to_bicg, timemax, callback, dtype, kw)
-
-
-def trilqr(A, b, c, x0=None, y0=None, transfer_to_usymcg=True, timemax=math.inf, callback=None, dtype=np.float64, **kw):
-    """trilqr! (src/trilqr.jl:114-461) -> (x, y, stats); A is m x n, b has m entries, c n."""
-    return _adjoint(True, A, b, c, x0, y0, transfer_to_usymcg, timemax, callback, dtype, kw)
+from oracle.oracle import bc_breakdown, bilqr, dot_mode, kron_unsymmetric, lib, trilqr  # noqa: F401
 
 
 # ---- problem generators of test/test_utils.jl:212-283 (real case) -------------------------------------------------

@@ -39,6 +39,7 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #include "krylov_oracle_lnlq.h"
 #include "krylov_oracle_cgne.h"
 #include "krylov_oracle_processes.h"
+#include "krylov_oracle_solve.h"
 #undef REAL
 #undef SUF
 #undef SQRT
@@ -70,6 +71,7 @@ void oracle_set_precond_block(int bs) { oracle_precond_block = bs; }
 #include "krylov_oracle_lnlq.h"
 #include "krylov_oracle_cgne.h"
 #include "krylov_oracle_processes.h"
+#include "krylov_oracle_solve.h"
 
 
 /* ---------------------------------------------------------------------------
@@ -123,4 +125,4 @@ double oracle_cg_timed_f64(int n, const int *rowptr, const int *colind, const do
   return t1 - t0;
 }
 
-int oracle_abi_version(void) { return 4; }
+int oracle_abi_version(void) { return 5; }

@@ -8,17 +8,16 @@
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
 /* ============ bilqr! (src/bilqr.jl:115-484) and trilqr! (src/trilqr.jl:114-461) ============
- * tri != 0 selects TriLQR: A is m x n, b and y have m entries, c and x have n (BiLQR: m == n).  A^T is passed as its own
+ * Variant 1 selects TriLQR: A is m x n, b and y have m entries, c and x have n (BiLQR: m == n).  A^T is passed as its own
  * CSR (n rows, ascending row indices of A in each row).  x0 / y0: NULL (no warm start) or Δx / Δy.  The callback
  * (NULL: none) returns nonzero to stop; timemax < 0 means no limit.  Vectors are copied and swapped as written (kcopy!,
  * @kswap!).  Stats: solved = solved_primal && solved_dual; the dual solution goes to y, its history to sres. */
-int SUF(oracle_adjoint)(int tri, int m, int n, const int *rowptr, const int *colind, const REAL *val,
-                        const int *trowptr, const int *tcolind, const REAL *tval,
-                        const REAL *b, const REAL *c, const REAL *x0, const REAL *y0,
-                        int transfer, double timemax, oracle_iter_cb callback, void *cb_user,
-                        const oracle_opts *o, REAL *x, REAL *t, REAL *rres, REAL *sres, int *nsres,
-                        int *solved_primal_out, int *solved_dual_out, oracle_stats *st) {
-  SUF(csr) A = {m, rowptr, colind, val}, At = {n, trowptr, tcolind, tval};
+static int SUF(adjoint)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int tri = variant, m = P->m, n = P->n;
+  const REAL *b = P->b, *c = P->c, *x0 = P->x0, *y0 = P->y0;
+  REAL *x = out->x, *t = out->y, *rres = out->residuals, *sres = out->residuals_dual;
+  int *nsres = &out->n_residuals_dual, *solved_primal_out = &out->solved_primal, *solved_dual_out = &out->solved_dual;
+  SUF(csr) A = {m, P->rowptr, P->colind, P->val}, At = {n, P->trowptr, P->tcolind, P->tval};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   *nsres = 0;
@@ -151,7 +150,7 @@ int SUF(oracle_adjoint)(int tri, int m, int n, const int *rowptr, const int *col
         norm_vk = norm_vk1;
       }
       if (history) PUSH(rres, st->nres, rNorm_lq);
-      int cg_ok = transfer && (FABS(dbark) > EPS);
+      int cg_ok = o->transfer && (FABS(dbark) > EPS);
       if (cg_ok) {
         zetabar = etak / dbark;
         REAL rho = betak1 * (sk * zeta1 - ck * zetabar);
@@ -210,10 +209,10 @@ int SUF(oracle_adjoint)(int tri, int m, int n, const int *rowptr, const int *col
     if (iter >= 3) eps3 = epsk2;
     if (iter >= 2) lam2 = l1;
     dbar1 = dbark; ck1 = ck; sk1 = sk; gammak = gammak1; betak = betak1;
-    if (callback) user_exit = callback(iter, cb_user) != 0;
+    if (o->callback) user_exit = o->callback(iter, o->cb_user) != 0;
     tired = iter >= itmax;
     breakdown = !tri && !solved_lq && !solved_cg && (pq == 0);
-    overtimed = timemax >= 0 && (oracle_now() - start) > timemax;
+    overtimed = o->timemax >= 0 && (oracle_now() - start) > o->timemax;
   }
   if (solved_cg) SUF(kaxpy)(n, zetabar, dbar, x);
   if (tired) set_status(st, "maximum number of iterations exceeded");

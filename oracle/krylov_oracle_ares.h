@@ -11,10 +11,11 @@
 
 /* ============ car!  (src/car.jl:108-256) ============
  * Mdiag: NULL => M === I (then Mu aliases u), else M = Diagonal(Mdiag) applied with mul! or ldiv!. */
-int SUF(oracle_car)(int n, const int *rowptr, const int *colind, const REAL *val, const REAL *b, const REAL *x0,
-                    const REAL *Mdiag, double timemax, oracle_iter_cb callback, void *cb_user, const oracle_opts *o,
-                    REAL *x, REAL *residuals, REAL *Aresiduals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(car)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M;
+  REAL *x = out->x, *residuals = out->residuals, *Aresiduals = out->Aresiduals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
@@ -73,8 +74,8 @@ int SUF(oracle_car)(int n, const int *rowptr, const int *colind, const REAL *val
     }
     iter++;
     tired = iter >= itmax;
-    user_exit = callback ? (callback(iter, cb_user) != 0) : 0;
-    overtimed = timemax >= 0 && oracle_now() - start > timemax;
+    user_exit = o->callback ? (o->callback(iter, o->cb_user) != 0) : 0;
+    overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
   }
   if (solved) set_status(st, "solution good enough given atol and rtol");
   if (tired) set_status(st, "maximum number of iterations exceeded");
@@ -89,18 +90,19 @@ done:
 }
 
 /* ============ minares!  (src/minares.jl:113-595), M = I ============
- * o->lambda is the shift λ; artol is the kwarg Artol (NaN -> sqrt(eps)).  The reference refuses any M != I.
+ * o->lambda is the shift λ; o->artol is the kwarg Artol (NaN -> sqrt(eps)).  The reference refuses any M != I.
  * vₖ / vₖ₊₁, wₖ₋₂ / wₖ₋₁ and dₖ₋₂ / dₖ₋₁ are swapped as @kswap! does. */
-int SUF(oracle_minares)(int n, const int *rowptr, const int *colind, const REAL *val, const REAL *b, const REAL *x0,
-                        double artol, double timemax, oracle_iter_cb callback, void *cb_user, const oracle_opts *o,
-                        REAL *x, REAL *residuals, REAL *Aresiduals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(minares)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0;
+  REAL *x = out->x, *residuals = out->residuals, *Aresiduals = out->Aresiduals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, warm_start = (x0 != NULL);
   REAL lambda = (REAL)o->lambda;
-  REAL atol = SUF(tol)(o->atol), rtol = SUF(tol)(o->rtol), Artol = SUF(tol)(artol);
+  REAL atol = SUF(tol)(o->atol), rtol = SUF(tol)(o->rtol), Artol = SUF(tol)(o->artol);
   int itmax = o->itmax;
   size_t nb = sizeof(REAL) * (size_t)n;
   REAL *vk = malloc(nb), *vk1 = malloc(nb), *wk2 = malloc(nb), *wk1 = malloc(nb), *dk2 = malloc(nb), *dk1 = malloc(nb);
@@ -277,8 +279,8 @@ int SUF(oracle_minares)(int n, const int *rowptr, const int *colind, const REAL 
     breakdown = (double)betak1 <= btol;
     solved = (rNorm <= eps_) || (ArNorm <= kappa);
     tired = iter >= itmax;
-    overtimed = timemax >= 0 && oracle_now() - start > timemax;
-    user_exit = callback ? (callback(iter, cb_user) != 0) : 0;
+    overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
+    user_exit = o->callback ? (o->callback(iter, o->cb_user) != 0) : 0;
 
     tmp = vk; vk = vk1; vk1 = tmp;
     if (iter >= 2) {

@@ -9,16 +9,15 @@
 
 /* ============ bilq!  (src/bilq.jl:118-407) and qmr!  (src/qmr.jl:124-405) ============
  * Both run the same Lanczos biorthogonalization (bilq.jl:226-255 = qmr.jl:230-258); they differ in the factorization
- * of the tridiagonal kept on the host and in the direction / solution update.  qmr != 0 selects QMR.  A^T is passed
+ * of the tridiagonal kept on the host and in the direction / solution update.  Variant 1 selects QMR.  A^T is passed
  * as its own CSR (rows ascending in each column of A: the order of the reference's adjoint product).  The callback
  * (NULL: none) returns nonzero to stop; timemax < 0 means no limit.  Unlike the reference, v / u / w are copied and
  * swapped exactly as written (kcopy!, @kswap!). */
-int SUF(oracle_biorth)(int qmr, int n, const int *rowptr, const int *colind, const REAL *val,
-                       const int *trowptr, const int *tcolind, const REAL *tval,
-                       const REAL *b, const REAL *c_in, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,
-                       int transfer_to_bicg, double timemax, oracle_iter_cb callback, void *cb_user,
-                       const oracle_opts *o, REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val}, At = {n, trowptr, tcolind, tval};
+static int SUF(biorth)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int qmr = variant, n = P->n;
+  const REAL *b = P->b, *c_in = P->c, *x0 = P->x0, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val}, At = {n, P->trowptr, P->tcolind, P->tval};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
@@ -128,7 +127,7 @@ int SUF(oracle_biorth)(int qmr, int n, const int *rowptr, const int *colind, con
       if (iter >= 2) { REAL *tmp = w2; w2 = w1; w1 = tmp; }
       zetabar = zetabar1; betak = betak1; gammak = gammak1; tau = tau1;
       int resid_decrease_mach = (rNorm + (REAL)1 <= (REAL)1);
-      if (callback) user_exit = callback(iter, cb_user) != 0;
+      if (o->callback) user_exit = o->callback(iter, o->cb_user) != 0;
       solved = (rNorm <= eps_) || resid_decrease_mach;
       tired = iter >= itmax;
       breakdown = !solved && (pq == 0);
@@ -173,20 +172,20 @@ int SUF(oracle_biorth)(int qmr, int n, const int *rowptr, const int *colind, con
         rNorm = SQRT((mu * mu) * (norm_vk * norm_vk) + (om * om) * (norm_vk1 * norm_vk1) + 2 * th);
       }
       if (history) PUSH(residuals, st->nres, rNorm);
-      int bicg_ok = transfer_to_bicg && (FABS(dbark) > EPS);
+      int bicg_ok = o->transfer && (FABS(dbark) > EPS);
       if (bicg_ok) {                                              /* bilq.jl:351-355 */
         zetabar = etak / dbark;
         REAL rho = betak1 * (sk * zeta1 - ck * zetabar);
         rNorm_cg = FABS(rho) * norm_vk1;
       }
       sk1 = sk; ck1 = ck; eta1 = etak; gammak = gammak1; betak = betak1; dbar1 = dbark; norm_vk = norm_vk1;
-      if (callback) user_exit = callback(iter, cb_user) != 0;
+      if (o->callback) user_exit = o->callback(iter, o->cb_user) != 0;
       solved = rNorm <= eps_;
       solved_cg = bicg_ok && (rNorm_cg <= eps_);
       tired = iter >= itmax;
       breakdown = !solved && !solved_cg && (pq == 0);
     }
-    overtimed = timemax >= 0 && (oracle_now() - start) > timemax;
+    overtimed = o->timemax >= 0 && (oracle_now() - start) > o->timemax;
   }
   if (solved_cg) SUF(kaxpy)(n, zetabar, dbar, x);                 /* BiCG point (bilq.jl:380-382) */
   if (tired) set_status(st, "maximum number of iterations exceeded");

@@ -111,7 +111,7 @@ static void SUF(panel_nn)(int n, int p, REAL alpha, const REAL *V, const REAL *S
 /* B, X0, X: n x p column-major.  memory: 0 -> 5 (block_gmres.jl:99), clipped to div(n,p). */
 int SUF(oracle_block_gmres)(int n, int p, const int *rowptr, const int *colind, const REAL *val,
                             const REAL *B, const REAL *X0, const REAL *Mdiag, const REAL *Ndiag,
-                            const oracle_opts *o, REAL *X, REAL *residuals, oracle_stats *st) {
+                            const oracle_options *o, REAL *X, REAL *residuals, oracle_stats *st) {
   SUF(csr) A = {n, rowptr, colind, val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");

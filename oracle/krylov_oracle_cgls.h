@@ -8,24 +8,14 @@
  * krylov_oracle_lsq.h).  M (m entries, acting on the residual space) is a diagonal or NULL.
  * Parity pinning: the reference's own assertions of test/test_cgls.jl and test/test_crls.jl (tests/test_oracle_cgls.py).
  */
-#ifndef ORACLE_CGLS_OPTS_DEFINED
-#define ORACLE_CGLS_OPTS_DEFINED
-typedef struct {
-  double atol, rtol;            /* NaN -> sqrt(eps(T)) */
-  double lambda, radius;
-  int itmax;                    /* 0 -> m + n */
-  int history;
-  int ldiv;
-  int hist_cap;
-} oracle_cgls_opts;
-#endif
-
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
-/* crls = 0: cgls!, 1: crls!.  Returns 0, or where the reference raises: 10 + to_boundary's error code. */
-int SUF(oracle_cgls)(int crls, int m, int n, const int *rowptr, const int *colind, const REAL *val, const REAL *b,
-                     const REAL *Mdiag, const oracle_cgls_opts *o, REAL *x, REAL *residuals, REAL *Aresiduals,
-                     oracle_stats *st) {
+/* variant 0: cgls!, 1: crls!.  Returns 0, or where the reference raises: 10 + to_boundary's error code. */
+static int SUF(cgls)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int crls = variant, m = P->m, n = P->n;
+  const int *rowptr = P->rowptr, *colind = P->colind;
+  const REAL *val = P->val, *b = P->b, *Mdiag = P->M;
+  REAL *x = out->x, *residuals = out->residuals, *Aresiduals = out->Aresiduals;
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, rc = 0;

@@ -8,25 +8,14 @@
  * Parity pinning: tests/test_oracle_cgne_crmr.py (the reference's assertions of test/test_cgne.jl and
  * test/test_crmr.jl) and tests/golden/oracle_cgne_crmr.json (frozen histories).
  */
-#ifndef ORACLE_CGNE_OPTS_DEFINED
-#define ORACLE_CGNE_OPTS_DEFINED
-typedef struct {
-  double atol, rtol;                /* NaN -> sqrt(eps(T)) */
-  double lambda;
-  int itmax;                        /* 0 -> m + n */
-  int history;
-  int ldiv;
-  int hist_cap;
-} oracle_cgne_opts;
-#endif
-
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
 /* cgne! (src/cgne.jl:134-252).  res: ||b||, then sqrt(<r, z>) after every iteration. */
-int SUF(oracle_cgne)(int m, int n, const int *rowptr, const int *colind, const REAL *val, const int *trowptr,
-                     const int *tcolind, const REAL *tval, const REAL *b, const REAL *Ndiag, const oracle_cgne_opts *o,
-                     double timemax, oracle_iter_cb callback, void *cb_user, REAL *x, REAL *res, oracle_stats *st) {
-  SUF(csr) A = {m, rowptr, colind, val}, At = {n, trowptr, tcolind, tval};
+static int SUF(cgne)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int m = P->m, n = P->n;
+  const REAL *b = P->b, *Ndiag = P->N;
+  REAL *x = out->x, *res = out->residuals;
+  SUF(csr) A = {m, P->rowptr, P->colind, P->val}, At = {n, P->trowptr, P->tcolind, P->tval};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
@@ -77,12 +66,12 @@ int SUF(oracle_cgne)(int m, int n, const int *rowptr, const int *colind, const R
     if (history) PUSH(res, st->nres, rNorm);
     iter = iter + 1;
     const int resid_decrease_mach = rNorm + (REAL)1 <= (REAL)1;
-    user_exit = callback ? callback(iter, cb_user) != 0 : 0;
+    user_exit = o->callback ? o->callback(iter, o->cb_user) != 0 : 0;
     const int resid_decrease_lim = rNorm <= eps_c;
     solved = resid_decrease_lim || resid_decrease_mach;
     inconsistent = (rNorm > 100 * eps_c) && (pNorm <= eps_i);
     tired = iter >= itmax;
-    overtimed = timemax >= 0 && oracle_now() - start > timemax;
+    overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
   }
   {
     const char *sx = "unknown";
@@ -100,11 +89,11 @@ done:
 }
 
 /* crmr! (src/crmr.jl:132-244).  res: ||r|| (r = N (b - A x)); ares: ||A^T r|| (+ λ ||r||² under the root). */
-int SUF(oracle_crmr)(int m, int n, const int *rowptr, const int *colind, const REAL *val, const int *trowptr,
-                     const int *tcolind, const REAL *tval, const REAL *b, const REAL *Ndiag, const oracle_cgne_opts *o,
-                     double timemax, oracle_iter_cb callback, void *cb_user, REAL *x, REAL *res, REAL *ares,
-                     oracle_stats *st) {
-  SUF(csr) A = {m, rowptr, colind, val}, At = {n, trowptr, tcolind, tval};
+static int SUF(crmr)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int m = P->m, n = P->n;
+  const REAL *b = P->b, *Ndiag = P->N;
+  REAL *x = out->x, *res = out->residuals, *ares = out->Aresiduals;
+  SUF(csr) A = {m, P->rowptr, P->colind, P->val}, At = {n, P->trowptr, P->tcolind, P->tval};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
@@ -158,11 +147,11 @@ int SUF(oracle_crmr)(int m, int n, const int *rowptr, const int *colind, const R
     ArNorm = SQRT(gamma);
     if (history) { PUSH(res, st->nres, rNorm); PUSH(ares, st->nAres, ArNorm); }
     iter = iter + 1;
-    user_exit = callback ? callback(iter, cb_user) != 0 : 0;
+    user_exit = o->callback ? o->callback(iter, o->cb_user) != 0 : 0;
     solved = rNorm <= eps_c;
     inconsistent = (rNorm > 100 * eps_c) && (ArNorm <= eps_i);
     tired = iter >= itmax;
-    overtimed = timemax >= 0 && oracle_now() - start > timemax;
+    overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
   }
   {
     const char *sx = "unknown";

@@ -247,22 +247,6 @@ typedef struct {
   char status[96];
 } oracle_stats;
 
-typedef struct {
-  double atol, rtol;       /* NaN -> sqrt(eps(T)) */
-  int itmax;               /* 0 -> 2n */
-  int history;
-  double radius;           /* CG */
-  int linesearch;          /* CG, MINRES */
-  double lambda;           /* MINRES */
-  double etol, conlim;     /* MINRES: NaN -> sqrt(eps), 1/sqrt(eps) */
-  int window;              /* MINRES: 0 -> 5 */
-  int memory;              /* GMRES: 0 -> 20 */
-  int restart;             /* GMRES */
-  int reorthogonalization; /* GMRES */
-  int ldiv;                /* preconditioners applied with ldiv! instead of mul! */
-  int hist_cap;            /* capacity of the history arrays */
-} oracle_opts;
-
 static void set_status(oracle_stats *st, const char *s) {
   strncpy(st->status, s, sizeof(st->status) - 1);
   st->status[sizeof(st->status) - 1] = 0;
@@ -270,9 +254,56 @@ static void set_status(oracle_stats *st, const char *s) {
 
 /* Per-iteration callback of the solvers that take one (NULL: none): returns nonzero to stop. */
 typedef int (*oracle_iter_cb)(int iter, void *user);
+
+/* The keyword arguments of every solver; each reads the fields its reference signature has.  Scalars stay double
+ * here and each body rounds them to REAL where the reference converts them. */
+typedef struct {
+  double atol, rtol, etol, axtol, btol, utol, utolx, utoly; /* NaN -> sqrt(eps(T)) */
+  double conlim;                /* NaN -> 1/sqrt(eps(T)) */
+  double artol;                 /* MINARES' Artol: NaN -> sqrt(eps(T)) */
+  double lambda, sigma, radius;
+  double gamma;                 /* CR: NaN -> sqrt(eps(T)) */
+  int itmax;                    /* 0 -> the family's default (2n square, m + n rectangular) */
+  int history;
+  int window;                   /* 0 -> 5 */
+  int memory;                   /* 0 -> 20 (5 for block_gmres) */
+  int restart, reorthogonalization, linesearch;
+  int ldiv;                     /* preconditioners applied with ldiv! instead of mul! */
+  int check_curvature;          /* CG-Lanczos */
+  int transfer_to_lsqr, transfer_to_craig;
+  int transfer;                 /* BiLQ / BiLQR: transfer_to_bicg; TriLQR: transfer_to_usymcg */
+  double timemax;               /* seconds; < 0: no limit */
+  oracle_iter_cb callback;
+  void *cb_user;
+  int hist_cap;                 /* capacity of the history arrays */
+} oracle_options;
 /* Wall clock in seconds, for timemax. */
 static double oracle_now(void) { struct timespec ts; timespec_get(&ts, TIME_UTC); return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec; }
 #endif
+
+/* One solve's operands: A is m x n (square solvers: m = n); At, Aᵀ as its own CSR, is NULL for the solvers that
+ * do not apply it.  b, c, x0, y0 and the diagonals M, N are NULL where not given. */
+typedef struct {
+  int m, n;
+  const int *rowptr, *colind;
+  const REAL *val;
+  const int *trowptr, *tcolind;
+  const REAL *tval;
+  const REAL *b, *c, *x0, *y0, *M, *N;
+} SUF(problem);
+
+/* One solve's results.  A NULL history is not written; residuals counts its entries in stats.nres, Aresiduals and
+ * Acond in stats.nAres, every other history in its own n_ field (counts may exceed options.hist_cap, the entries
+ * stored). */
+typedef struct {
+  REAL *x, *y;
+  REAL *residuals, *Aresiduals, *Acond;
+  REAL *err_lbnds, *err_ubnds_lq, *err_ubnds_cg, *error_bnd_x, *error_bnd_y, *residuals_dual;
+  int n_err_lbnds, n_err_ubnds_lq, n_err_ubnds_cg, n_error_bnd_x, n_error_bnd_y, n_residuals_dual;
+  REAL *npc_dir;
+  REAL Anorm;
+  int error_with_bnd, solved_primal, solved_dual;
+} SUF(outputs);
 
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
@@ -281,10 +312,11 @@ static REAL SUF(tol)(double t) { return isnan(t) ? SQRT(EPS) : (REAL)t; }
 /* =========================== cg!  (src/cg.jl:120-291) =========================== */
 /* Mdiag: NULL => M === I, else M = Diagonal(Mdiag).  x0: NULL => no warm start.
  * npc_dir: optional output (length n) when linesearch || radius > 0. */
-int SUF(oracle_cg)(int n, const int *rowptr, const int *colind, const REAL *val,
-                   const REAL *b, const REAL *x0, const REAL *Mdiag, const oracle_opts *o,
-                   REAL *x, REAL *residuals, REAL *npc_dir_out, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(cg)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M;
+  REAL *x = out->x, *residuals = out->residuals, *npc_dir_out = out->npc_dir;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   REAL radius = (REAL)o->radius;
@@ -388,11 +420,11 @@ done:
 }
 
 /* ======================== bicgstab!  (src/bicgstab.jl:125-277) ======================== */
-int SUF(oracle_bicgstab)(int n, const int *rowptr, const int *colind, const REAL *val,
-                         const REAL *b, const REAL *c_in, const REAL *x0,
-                         const REAL *Mdiag, const REAL *Ndiag, const oracle_opts *o,
-                         REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(bicgstab)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *c_in = P->c, *x0 = P->x0, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL);
@@ -473,10 +505,11 @@ done:
 }
 
 /* ========================== gmres!  (src/gmres.jl:121-384) ========================== */
-int SUF(oracle_gmres)(int n, const int *rowptr, const int *colind, const REAL *val,
-                      const REAL *b, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,
-                      const oracle_opts *o, REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(gmres)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL);
@@ -633,11 +666,12 @@ done:
 }
 
 /* ========================== minres!  (src/minres.jl:164-485) ========================== */
-int SUF(oracle_minres)(int n, const int *rowptr, const int *colind, const REAL *val,
-                       const REAL *b, const REAL *x0, const REAL *Mdiag, const oracle_opts *o,
-                       REAL *x, REAL *residuals, REAL *Aresiduals, REAL *Aconds,
-                       REAL *npc_dir_out, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(minres)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M;
+  REAL *x = out->x, *residuals = out->residuals, *Aresiduals = out->Aresiduals, *Aconds = out->Acond;
+  REAL *npc_dir_out = out->npc_dir;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL), linesearch = o->linesearch;

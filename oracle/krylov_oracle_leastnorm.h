@@ -9,33 +9,18 @@
  * Parity pinning: tests/test_oracle_leastnorm.py (the reference's assertions of test/test_craig.jl and
  * test/test_craigmr.jl) and tests/golden/oracle_leastnorm.json (frozen histories).
  */
-#ifndef ORACLE_LN_OPTS_DEFINED
-#define ORACLE_LN_OPTS_DEFINED
-typedef struct {
-  double atol, rtol, btol;      /* NaN -> sqrt(eps(T)) */
-  double conlim;                /* NaN -> 1/sqrt(eps(T)) */
-  double lambda;
-  int itmax;                    /* 0 -> m + n */
-  int history;
-  int ldiv;
-  int transfer_to_lsqr;
-  int hist_cap;
-} oracle_ln_opts;
-#endif
-
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
 static REAL SUF(ln_knorm_ell)(int n, const REAL *x, const REAL *y) {   /* knorm_elliptic (krylov_utils.jl:319) */
   return x == y ? SUF(knorm)(n, x) : SQRT(SUF(kdot)(n, x, y));
 }
 
-/* mr = 0: craig!, 1: craigmr!.  The callback (NULL: none) returns nonzero to stop; timemax < 0 means no limit. */
-int SUF(oracle_leastnorm)(int mr, int m, int n, const int *rowptr, const int *colind, const REAL *val,
-                          const int *trowptr, const int *tcolind, const REAL *tval, const REAL *b,
-                          const REAL *Mdiag, const REAL *Ndiag, const oracle_ln_opts *o, double timemax,
-                          oracle_iter_cb callback, void *cb_user, REAL *x, REAL *y, REAL *res, REAL *ares,
-                          oracle_stats *st) {
-  SUF(csr) A = {m, rowptr, colind, val}, At = {n, trowptr, tcolind, tval};
+/* variant 0: craig!, 1: craigmr!.  The callback (NULL: none) returns nonzero to stop; timemax < 0 means no limit. */
+static int SUF(leastnorm)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int mr = variant, m = P->m, n = P->n;
+  const REAL *b = P->b, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *y = out->y, *res = out->residuals, *ares = out->Aresiduals;
+  SUF(csr) A = {m, P->rowptr, P->colind, P->val}, At = {n, P->trowptr, P->tcolind, P->tval};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
@@ -142,10 +127,10 @@ int SUF(oracle_leastnorm)(int mr, int m, int n, const int *rowptr, const int *co
       ill_cond_mach = (REAL)1 + (REAL)1 / Acond <= (REAL)1;
       ill_cond_lim = (REAL)1 / Acond <= ctol;
       ill_cond = ill_cond_mach || ill_cond_lim;
-      user_exit = callback ? callback(iter, cb_user) != 0 : 0;
+      user_exit = o->callback ? o->callback(iter, o->cb_user) != 0 : 0;
       inconsistent = 0;
       tired = iter >= itmax;
-      overtimed = timemax >= 0 && oracle_now() - start > timemax;
+      overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
     }
     if (lambda > 0 && o->transfer_to_lsqr) {
       xi *= -theta / delta;
@@ -260,11 +245,11 @@ int SUF(oracle_leastnorm)(int mr, int m, int n, const int *rowptr, const int *co
       }
       theta = s * alphahat;
       rhobar = -c * alphahat;
-      user_exit = callback ? callback(iter, cb_user) != 0 : 0;
+      user_exit = o->callback ? o->callback(iter, o->cb_user) != 0 : 0;
       solved = rNorm <= eps_c;
       inconsistent = (rNorm > 100 * eps_c) && (ArNorm <= eps_i);
       tired = iter >= itmax;
-      overtimed = timemax >= 0 && oracle_now() - start > timemax;
+      overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
     }
     const char *sts = "unknown";
     if (tired) sts = "maximum number of iterations exceeded";

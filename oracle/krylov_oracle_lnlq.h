@@ -8,36 +8,23 @@
  * Parity pinning: tests/test_oracle_lnlq.py (the reference's assertions of test/test_lnlq.jl) and
  * tests/golden/oracle_lnlq.json (frozen histories).
  */
-#ifndef ORACLE_LNLQ_OPTS_DEFINED
-#define ORACLE_LNLQ_OPTS_DEFINED
-typedef struct {
-  double atol, rtol, utolx, utoly;  /* NaN -> sqrt(eps(T)) */
-  double lambda, sigma;
-  int itmax;                        /* 0 -> m + n */
-  int history;
-  int ldiv;
-  int transfer_to_craig;
-  int hist_cap;
-} oracle_lnlq_opts;
-#endif
-
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
 static REAL SUF(lnlq_knorm_ell)(int n, const REAL *x, const REAL *y) {   /* knorm_elliptic (krylov_utils.jl:319) */
   return x == y ? SUF(knorm)(n, x) : SQRT(SUF(kdot)(n, x, y));
 }
 
-/* lnlq! (src/lnlq.jl:168-568).  errx / erry receive error_bnd_x / error_bnd_y; out[0], out[1] their lengths and out[2]
- * error_with_bnd.  `iter` is incremented before the loop and at the end of every pass: niter = passes + 1. */
-int SUF(oracle_lnlq)(int m, int n, const int *rowptr, const int *colind, const REAL *val, const int *trowptr,
-                     const int *tcolind, const REAL *tval, const REAL *b, const REAL *Mdiag, const REAL *Ndiag,
-                     const oracle_lnlq_opts *o, double timemax, oracle_iter_cb callback, void *cb_user, REAL *x, REAL *y,
-                     REAL *res, REAL *errx, REAL *erry, int *out, oracle_stats *st) {
-  SUF(csr) A = {m, rowptr, colind, val}, At = {n, trowptr, tcolind, tval};
+/* lnlq! (src/lnlq.jl:168-568).  Writes the histories residuals, error_bnd_x and error_bnd_y, and error_with_bnd.
+ * `iter` is incremented before the loop and at the end of every pass: niter = passes + 1. */
+static int SUF(lnlq)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int m = P->m, n = P->n;
+  const REAL *b = P->b, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *y = out->y, *res = out->residuals, *errx = out->error_bnd_x, *erry = out->error_bnd_y;
+  SUF(csr) A = {m, P->rowptr, P->colind, P->val}, At = {n, P->trowptr, P->tcolind, P->tval};
   const double start = oracle_now();
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
-  out[0] = out[1] = out[2] = 0;
+  out->n_error_bnd_x = out->n_error_bnd_y = out->error_with_bnd = 0;
   const int history = o->history, ldiv = o->ldiv, MisI = Mdiag == NULL, NisI = Ndiag == NULL;
   const int transfer = o->transfer_to_craig;
   const REAL lambda = (REAL)o->lambda, sigma = (REAL)o->sigma;
@@ -97,7 +84,7 @@ int SUF(oracle_lnlq)(int m, int n, const int *rowptr, const int *colind, const R
     err_x = tautilde;
     err_y = zetatilde;
     solved_lq = err_x <= utolx || err_y <= utoly;
-    if (history) { PUSH(errx, out[0], err_x); PUSH(erry, out[1], err_y); }
+    if (history) { PUSH(errx, out->n_error_bnd_x, err_x); PUSH(erry, out->n_error_bnd_y, err_y); }
     rhobar = -sigma_est;
     csig = -1;
   }
@@ -189,7 +176,7 @@ int SUF(oracle_lnlq)(int m, int n, const int *rowptr, const int *colind, const R
       } else {
         err_y = FABS(zetatilde);
       }
-      if (history) { PUSH(errx, out[0], err_x); PUSH(erry, out[1], err_y); }
+      if (history) { PUSH(errx, out->n_error_bnd_x, err_x); PUSH(erry, out->n_error_bnd_y, err_y); }
     }
     REAL rNorm_lq;
     if (iter == 1) {
@@ -200,7 +187,7 @@ int SUF(oracle_lnlq)(int m, int n, const int *rowptr, const int *colind, const R
     }
     if (history) PUSH(res, st->nres, rNorm_lq);
     const REAL rNorm_cg = transfer ? FABS(betahat * tau) : 0;
-    user_exit = callback ? callback(iter, cb_user) != 0 : 0;
+    user_exit = o->callback ? o->callback(iter, o->cb_user) != 0 : 0;
     tired = iter >= itmax;
     solved_lq = rNorm_lq <= eps_c;
     solved_cg = transfer && (FABS(zetabar) > EPS) && (rNorm_cg <= eps_c);
@@ -208,7 +195,7 @@ int SUF(oracle_lnlq)(int m, int n, const int *rowptr, const int *colind, const R
       solved_lq = solved_lq || err_x <= utolx || err_y <= utoly;
       solved_cg = transfer && (solved_cg || err_x <= utolx || err_y <= utoly);
     }
-    overtimed = timemax >= 0 && oracle_now() - start > timemax;
+    overtimed = o->timemax >= 0 && oracle_now() - start > o->timemax;
     sk = s_next;
     alpha = alpha_next;
     alphahat = alphahat_next;
@@ -248,7 +235,7 @@ int SUF(oracle_lnlq)(int m, int n, const int *rowptr, const int *colind, const R
     set_status(st, s);
   }
   st->niter = iter; st->solved = solved_lq || solved_cg; st->inconsistent = 0;
-  out[2] = complex_error_bnd;
+  out->error_with_bnd = complex_error_bnd;
 done:
   free(Mu); free(Av); free(wbar); free(ub); free(Nv); free(Atu); free(vb); free(q);
   return 0;

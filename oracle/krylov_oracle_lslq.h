@@ -5,27 +5,18 @@
  * and N (n entries) are diagonals or NULL.
  * Parity pinning: the reference's own assertions of test/test_lslq.jl (tests/test_oracle_cgls.py).
  */
-#ifndef ORACLE_LSLQ_OPTS_DEFINED
-#define ORACLE_LSLQ_OPTS_DEFINED
-typedef struct {
-  double atol, rtol, etol, utol, btol;   /* NaN -> sqrt(eps(T)) */
-  double conlim;                         /* NaN -> 1/sqrt(eps(T)) */
-  double lambda, sigma;
-  int itmax;                             /* 0 -> m + n */
-  int history, window, ldiv, transfer_to_lsqr, hist_cap;
-} oracle_lslq_opts;
-#endif
-
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
-/* hist: 5 arrays of hist_cap entries (residuals, Aresiduals, err_lbnds, err_ubnds_lq, err_ubnds_cg); counts: their
- * lengths; *error_with_bnd: stats.error_with_bnd. */
-int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const REAL *val, const REAL *b, const REAL *Mdiag,
-                     const REAL *Ndiag, const oracle_lslq_opts *o, REAL *x, REAL **hist, int *counts, int *error_with_bnd,
-                     oracle_stats *st) {
+/* Writes the histories residuals, Aresiduals, err_lbnds, err_ubnds_lq and err_ubnds_cg, and error_with_bnd. */
+static int SUF(lslq)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int m = P->m, n = P->n;
+  const int *rowptr = P->rowptr, *colind = P->colind;
+  const REAL *val = P->val, *b = P->b, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x;
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
-  for (int k = 0; k < 5; k++) counts[k] = 0;
+  out->n_err_lbnds = out->n_err_ubnds_lq = out->n_err_ubnds_cg = 0;
+  int *error_with_bnd = &out->error_with_bnd;
   *error_with_bnd = 0;
   int history = o->history, ldiv = o->ldiv;
   int MisI = (Mdiag == NULL), NisI = (Ndiag == NULL);
@@ -47,7 +38,7 @@ int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const R
   REAL beta1 = SUF(knorm_ell)(m, u, Mu);
   if (beta1 == 0) {
     st->niter = 0; st->solved = 1; st->inconsistent = 0;
-    if (history) { PUSH(hist[0], counts[0], 0); PUSH(hist[1], counts[1], 0); }
+    if (history) { PUSH(out->residuals, st->nres, 0); PUSH(out->Aresiduals, st->nAres, 0); }
     set_status(st, "x is a zero-residual solution");
     goto done;
   }
@@ -60,7 +51,7 @@ int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const R
   REAL alpha = SUF(knorm_ell)(n, v, Nv);
   if (alpha == 0) {
     st->niter = 0; st->solved = 1; st->inconsistent = 0;
-    if (history) { PUSH(hist[0], counts[0], beta1); PUSH(hist[1], counts[1], 0); }
+    if (history) { PUSH(out->residuals, st->nres, beta1); PUSH(out->Aresiduals, st->nAres, 0); }
     set_status(st, "x is a minimum least-squares solution");
     goto done;
   }
@@ -76,7 +67,7 @@ int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const R
     REAL alphaL = alpha, betaL = beta, rhobar = -sigma, gammabar = alpha, psi = beta1;
     REAL c = -1, s = 0, delta = -1, tau = alpha * beta1, zeta = 0, zetabar = 0, zetatilde = 0, csig = -1;
     REAL rNorm = beta1, ArNorm = alpha * beta;
-    if (history) { PUSH(hist[0], counts[0], rNorm); PUSH(hist[1], counts[1], ArNorm); }
+    if (history) { PUSH(out->residuals, st->nres, rNorm); PUSH(out->Aresiduals, st->nAres, ArNorm); }
     int iter = 0, itmax = o->itmax != 0 ? o->itmax : m + n;
     REAL eps = atol + rtol * beta1;
     int solved = rNorm <= eps, tired = iter >= itmax, ill_cond = 0, ill_cond_mach = 0, ill_cond_lim = 0;
@@ -133,10 +124,10 @@ int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const R
       zetabar = zeta / c;
       REAL ra = psi * cp - zetaold * eta, rb = psi * sp;
       rNorm = SQRT(ra * ra + rb * rb);
-      if (history) PUSH(hist[0], counts[0], rNorm);
+      if (history) PUSH(out->residuals, st->nres, rNorm);
       REAL aa = gamma * epsl * zeta, ab = delta * eta * zetaold;
       ArNorm = SQRT(aa * aa + ab * ab);
-      if (history) PUSH(hist[1], counts[1], ArNorm);
+      if (history) PUSH(out->Aresiduals, st->nAres, ArNorm);
       psi = psi * sp;
       xcgNorm2 = xlqNorm2 + zetabar * zetabar;
       if (sigma > 0 && iter > 0 && !complex_error_bnd) {
@@ -144,7 +135,7 @@ int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const R
         if (disc < 0) complex_error_bnd = 1;
         else {
           REAL ub = SQRT(disc);
-          if (history) PUSH(hist[4], counts[4], ub);
+          if (history) PUSH(out->err_ubnds_cg, out->n_err_ubnds_cg, ub);
           fwd_err_ubnd = ub <= utol * SQRT(xcgNorm2);
         }
       }
@@ -158,13 +149,13 @@ int SUF(oracle_lslq)(int m, int n, const int *rowptr, const int *colind, const R
       err_vec[iter % window] = zeta;
       if (iter >= window) {
         err_lbnd = SUF(err_norm)(window, err_vec);
-        if (history) PUSH(hist[2], counts[2], err_lbnd);
+        if (history) PUSH(out->err_lbnds, out->n_err_lbnds, err_lbnd);
         fwd_err_lbnd = err_lbnd <= etol * xlqNorm;
       }
       if (sigma > 0 && !complex_error_bnd) {
         REAL etatilde = omega * s, epstilde = -omega * c, tautilde = -tau * delta / omega;
         zetatilde = (tautilde - zeta * etatilde) / epstilde;
-        if (history) PUSH(hist[3], counts[3], FABS(zetatilde));
+        if (history) PUSH(out->err_ubnds_lq, out->n_err_ubnds_lq, FABS(zetatilde));
       }
       ill_cond_mach = ((REAL)1 + test3 <= (REAL)1);
       int solved_mach = ((REAL)1 + test2 <= (REAL)1), zero_resid_mach = ((REAL)1 + t1 <= (REAL)1);

@@ -7,21 +7,6 @@
  * sequential A' * u over the CSC storage of A does).  M (m entries) and N (n entries) are diagonals or NULL.
  * Parity pinning: the reference's own assertions of test/test_lsqr.jl and test/test_lsmr.jl (tests/test_oracle_lsq.py).
  */
-#ifndef ORACLE_LSQ_OPTS_DEFINED
-#define ORACLE_LSQ_OPTS_DEFINED
-typedef struct {
-  double atol, rtol;            /* NaN -> sqrt(eps(T)) */
-  double etol, axtol, btol;     /* NaN -> sqrt(eps(T)) */
-  double conlim;                /* NaN -> 1/sqrt(eps(T)) */
-  double lambda, radius;
-  int itmax;                    /* 0 -> m + n */
-  int history;
-  int window;                   /* 0 -> 5 */
-  int ldiv;
-  int hist_cap;
-} oracle_lsq_opts;
-#endif
-
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
 /* y = A^T x for an m x n CSR A: column sums in ascending row order */
@@ -39,10 +24,12 @@ static REAL SUF(knorm_ell)(int n, const REAL *x, const REAL *y) {
   return x == y ? SUF(knorm)(n, x) : SQRT(SUF(kdot)(n, x, y));
 }
 
-/* lsmr = 0: lsqr!, 1: lsmr!.  Returns 0, or where the reference raises: 10 + to_boundary's error code. */
-int SUF(oracle_lsq)(int lsmr, int m, int n, const int *rowptr, const int *colind, const REAL *val, const REAL *b,
-                    const REAL *Mdiag, const REAL *Ndiag, const oracle_lsq_opts *o, REAL *x, REAL *residuals,
-                    REAL *Aresiduals, REAL *Anorm_out, oracle_stats *st) {
+/* variant 0: lsqr!, 1: lsmr!.  Returns 0, or where the reference raises: 10 + to_boundary's error code. */
+static int SUF(lsq)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int lsmr = variant, m = P->m, n = P->n;
+  const int *rowptr = P->rowptr, *colind = P->colind;
+  const REAL *val = P->val, *b = P->b, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals, *Aresiduals = out->Aresiduals, *Anorm_out = &out->Anorm;
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, rc = 0;

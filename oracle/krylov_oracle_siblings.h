@@ -21,11 +21,11 @@
 #define PUSH(arr, cnt, v) do { if ((arr) && (cnt) < o->hist_cap) (arr)[(cnt)] = (v); (cnt)++; } while (0)
 
 /* ============================ cgs!  (src/cgs.jl:125-282) ============================ */
-int SUF(oracle_cgs)(int n, const int *rowptr, const int *colind, const REAL *val,
-                    const REAL *b, const REAL *c_in, const REAL *x0,
-                    const REAL *Mdiag, const REAL *Ndiag, const oracle_opts *o,
-                    REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(cgs)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *c_in = P->c, *x0 = P->x0, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL);
@@ -107,11 +107,12 @@ done:
 }
 
 /* ======================= cg_lanczos!  (src/cg_lanczos.jl:110-264) ======================= */
-/* LanczosStats: residuals, indefinite, Anorm (returned through *Anorm), Acond stays NaN. */
-int SUF(oracle_cg_lanczos)(int n, const int *rowptr, const int *colind, const REAL *val,
-                           const REAL *b, const REAL *x0, const REAL *Mdiag, int check_curvature,
-                           const oracle_opts *o, REAL *x, REAL *residuals, REAL *Anorm, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+/* LanczosStats: residuals, indefinite, Anorm (returned through out->Anorm), Acond stays NaN. */
+static int SUF(cg_lanczos)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n, check_curvature = o->check_curvature;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M;
+  REAL *x = out->x, *residuals = out->residuals, *Anorm = &out->Anorm;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL);
@@ -188,10 +189,11 @@ done:
 }
 
 /* ============================ fom!  (src/fom.jl:121-368) ============================ */
-int SUF(oracle_fom)(int n, const int *rowptr, const int *colind, const REAL *val,
-                    const REAL *b, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,
-                    const oracle_opts *o, REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(fom)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL);
@@ -338,10 +340,11 @@ done:
 
 /* ========================== fgmres!  (src/fgmres.jl:128-388) ========================== */
 /* Ndiag == NULL: N === I, and Z[k] <- V[k] by the unconditional mulorldiv! (fgmres.jl:262). */
-int SUF(oracle_fgmres)(int n, const int *rowptr, const int *colind, const REAL *val,
-                       const REAL *b, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,
-                       const oracle_opts *o, REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(fgmres)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M, *Ndiag = P->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL);
@@ -498,10 +501,11 @@ done:
 }
 
 /* ========================== dqgmres!  (src/dqgmres.jl:121-335) ========================== */
-int SUF(oracle_dqgmres)(int n, const int *rowptr, const int *colind, const REAL *val,
-                        const REAL *b, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,
-                        const oracle_opts *o, REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(dqgmres)(int variant, const SUF(problem) *prob, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = prob->n;
+  const REAL *b = prob->b, *x0 = prob->x0, *Mdiag = prob->M, *Ndiag = prob->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, prob->rowptr, prob->colind, prob->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL), reorth = o->reorthogonalization;
@@ -596,10 +600,11 @@ done:
 }
 
 /* ============================ diom!  (src/diom.jl:121-332) ============================ */
-int SUF(oracle_diom)(int n, const int *rowptr, const int *colind, const REAL *val,
-                     const REAL *b, const REAL *x0, const REAL *Mdiag, const REAL *Ndiag,
-                     const oracle_opts *o, REAL *x, REAL *residuals, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(diom)(int variant, const SUF(problem) *prob, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = prob->n;
+  const REAL *b = prob->b, *x0 = prob->x0, *Mdiag = prob->M, *Ndiag = prob->N;
+  REAL *x = out->x, *residuals = out->residuals;
+  SUF(csr) A = {n, prob->rowptr, prob->colind, prob->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL), reorth = o->reorthogonalization;
@@ -697,18 +702,19 @@ done:
 }
 
 /* ============================== cr!  (src/cr.jl:128-478) ============================== */
-/* gamma_in: NaN -> sqrt(eps(T)).  npc_dir: output (length n) when linesearch || radius > 0.
+/* o->gamma: NaN -> sqrt(eps(T)).  npc_dir: output (length n) when linesearch || radius > 0.
  * Aresiduals receives ||A r|| like stats.Aresiduals.  st->error: 1 linesearch&&radius>0, 2 warm_start&&linesearch,
  * 5 "Indefinite system and no trust region", 10+e to_boundary errors. */
-int SUF(oracle_cr)(int n, const int *rowptr, const int *colind, const REAL *val,
-                   const REAL *b, const REAL *x0, const REAL *Mdiag, double gamma_in, const oracle_opts *o,
-                   REAL *x, REAL *residuals, REAL *Aresiduals, REAL *npc_dir, oracle_stats *st) {
-  SUF(csr) A = {n, rowptr, colind, val};
+static int SUF(cr)(int variant, const SUF(problem) *P, const oracle_options *o, SUF(outputs) *out, oracle_stats *st) {
+  const int n = P->n;
+  const REAL *b = P->b, *x0 = P->x0, *Mdiag = P->M;
+  REAL *x = out->x, *residuals = out->residuals, *Aresiduals = out->Aresiduals, *npc_dir = out->npc_dir;
+  SUF(csr) A = {n, P->rowptr, P->colind, P->val};
   memset(st, 0, sizeof(*st));
   set_status(st, "unknown");
   int history = o->history, ldiv = o->ldiv, warm_start = (x0 != NULL), linesearch = o->linesearch;
   REAL radius = (REAL)o->radius;
-  REAL gam = isnan(gamma_in) ? SQRT(EPS) : (REAL)gamma_in;
+  REAL gam = isnan(o->gamma) ? SQRT(EPS) : (REAL)o->gamma;
   int MisI = (Mdiag == NULL);
   REAL atol = SUF(tol)(o->atol), rtol = SUF(tol)(o->rtol);
   int itmax = o->itmax;

@@ -1,4 +1,4 @@
-"""ctypes front-end of the CPU restatement of lsqr! / lsmr! -- TEST INFRASTRUCTURE ONLY.
+"""Problem generators of the CPU restatement of lsqr! / lsmr!, and its solver functions -- TEST INFRASTRUCTURE ONLY.
 
 Same status as oracle/oracle.py (only tests/ may import it; the product never does).  The solvers live in
 krylov_oracle_lsq.h, built into the oracle library that oracle.py builds and loads.  The problem generators restate test/gen_lsq.jl and the least-squares helpers of test/test_utils.jl; the square
@@ -8,70 +8,10 @@ test/test_lsmr.jl) and tests/golden/oracle_lsq.json (frozen histories).
 """
 from __future__ import annotations
 
-import ctypes as C
-import math
-
 import numpy as np
 import scipy.sparse as sp
 
-from oracle.oracle import Stats, _p, _result, _suf, _vec, ddx, lib, two_preconditioners, zero_rhs  # noqa: F401
-
-
-class LsqOpts(C.Structure):
-    _fields_ = [("atol", C.c_double), ("rtol", C.c_double), ("etol", C.c_double), ("axtol", C.c_double),
-                ("btol", C.c_double), ("conlim", C.c_double), ("lambda_", C.c_double), ("radius", C.c_double),
-                ("itmax", C.c_int), ("history", C.c_int), ("window", C.c_int), ("ldiv", C.c_int), ("hist_cap", C.c_int)]
-
-
-def _lsq(lsmr, A, b, M, N, dtype, kw):
-    suf, ct = _suf(dtype)
-    A = sp.csr_matrix(A)
-    A.sort_indices()
-    m, n = A.shape
-    rp, ci = np.ascontiguousarray(A.indptr, dtype=np.int32), np.ascontiguousarray(A.indices, dtype=np.int32)
-    va = np.ascontiguousarray(A.data, dtype=dtype)
-    b, M, N = _vec(b, dtype), _vec(M, dtype), _vec(N, dtype)
-    sqd = kw.pop("sqd", False)
-    o = LsqOpts()
-    o.lambda_ = kw.pop("lambda_", 0.0)
-    if sqd:
-        if o.lambda_ != 0:
-            raise ValueError("sqd cannot be set to true if λ ≠ 0 !")
-        o.lambda_ = 1.0
-    o.atol, o.rtol = kw.pop("atol", 0.0), kw.pop("rtol", 0.0)           # Julia's kwarg defaults (lsqr.jl:155-156)
-    o.etol, o.axtol, o.btol = kw.pop("etol", math.nan), kw.pop("axtol", math.nan), kw.pop("btol", math.nan)
-    o.conlim, o.radius = kw.pop("conlim", math.nan), kw.pop("radius", 0.0)
-    o.itmax, o.history = kw.pop("itmax", 0), int(kw.pop("history", True))
-    o.window, o.ldiv = kw.pop("window", 0), int(kw.pop("ldiv", False))
-    itmax = o.itmax if o.itmax > 0 else m + n
-    o.hist_cap = kw.pop("hist_cap", min(itmax + 2, 1 << 22))
-    if kw:
-        raise TypeError(f"unknown options {sorted(kw)}")
-    x = np.zeros(n, dtype)
-    res, ares = np.zeros(o.hist_cap, dtype), np.zeros(o.hist_cap, dtype)
-    anorm = ct(0)
-    st = Stats()
-    f = getattr(lib(), f"oracle_lsq_{suf}")
-    f.argtypes = [C.c_int] * 3 + [C.c_void_p] * 12
-    rc = f(int(lsmr), m, n, _p(rp), _p(ci), _p(va), _p(b), _p(M), _p(N), C.cast(C.byref(o), C.c_void_p), _p(x), _p(res),
-           _p(ares), C.cast(C.byref(anorm), C.c_void_p), C.cast(C.byref(st), C.c_void_p))
-    if rc:
-        raise ArithmeticError({12: "zero direction", 13: "outside of the trust region"}.get(rc, "no real roots"))
-    k = min(st.nAres, o.hist_cap)
-    return _result(st, x, res, dict(Aresiduals=ares[:k].copy(), Anorm=float(anorm.value)))
-
-
-def lsqr(A, b, M=None, N=None, dtype=np.float64, **kw):
-    """lsqr! (src/lsqr.jl:174-440) on an m x n matrix.  M (m) / N (n): None or the diagonal of a Diagonal operator.
-    kwargs: lambda_, sqd, radius, etol, axtol, btol, conlim, atol, rtol (default 0), itmax, window, ldiv, history.
-    Extra stats key: Aresiduals."""
-    return _lsq(0, A, b, M, N, dtype, kw)
-
-
-def lsmr(A, b, M=None, N=None, dtype=np.float64, **kw):
-    """lsmr! (src/lsmr.jl:178-455); same arguments as lsqr.  Extra stats keys: Aresiduals, Anorm (LsmrStats)."""
-    return _lsq(1, A, b, M, N, dtype, kw)
-
+from oracle.oracle import ddx, lib, lsmr, lsqr, two_preconditioners, zero_rhs  # noqa: F401
 
 
 # ---- least-squares problems of test/gen_lsq.jl and test/test_utils.jl (restated; dense ones returned as CSR) ------

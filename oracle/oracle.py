@@ -14,9 +14,11 @@ from __future__ import annotations
 
 import ctypes as C
 import glob
+import inspect
 import math
 import os
 import subprocess
+from typing import NamedTuple
 
 import numpy as np
 import scipy.sparse as sp
@@ -33,12 +35,43 @@ class Stats(C.Structure):
                 ("nAres", C.c_int), ("error", C.c_int), ("status", C.c_char * 96)]
 
 
-class Opts(C.Structure):
-    _fields_ = [("atol", C.c_double), ("rtol", C.c_double), ("itmax", C.c_int), ("history", C.c_int),
-                ("radius", C.c_double), ("linesearch", C.c_int), ("lambda_", C.c_double),
-                ("etol", C.c_double), ("conlim", C.c_double), ("window", C.c_int), ("memory", C.c_int),
-                ("restart", C.c_int), ("reorthogonalization", C.c_int), ("ldiv", C.c_int),
-                ("hist_cap", C.c_int)]
+_TOLERANCES = ("atol", "rtol", "etol", "axtol", "btol", "utol", "utolx", "utoly", "conlim", "artol")
+
+
+class Options(C.Structure):
+    """oracle_options (krylov_oracle_impl.h): the keyword arguments of every solver."""
+    _fields_ = ([(f, C.c_double) for f in _TOLERANCES + ("lambda_", "sigma", "radius", "gamma")]
+                + [(f, C.c_int) for f in ("itmax", "history", "window", "memory", "restart", "reorthogonalization",
+                                          "linesearch", "ldiv", "check_curvature", "transfer_to_lsqr",
+                                          "transfer_to_craig", "transfer")]
+                + [("timemax", C.c_double), ("callback", _ITER_CB), ("cb_user", C.c_void_p), ("hist_cap", C.c_int)])
+
+    def __init__(self):
+        super().__init__(**{f: math.nan for f in _TOLERANCES + ("gamma",)}, timemax=-1.0)
+
+
+class Problem(C.Structure):
+    """problem_f32 / problem_f64: A (m x n) and Aᵀ as CSR, and the vectors; NULL where not given."""
+    _fields_ = [("m", C.c_int), ("n", C.c_int)] + [(f, C.c_void_p) for f in (
+        "rowptr", "colind", "val", "trowptr", "tcolind", "tval", "b", "c", "x0", "y0", "M", "N")]
+
+
+_HISTORIES = ("residuals", "Aresiduals", "Acond", "err_lbnds", "err_ubnds_lq", "err_ubnds_cg", "error_bnd_x",
+              "error_bnd_y", "residuals_dual")
+
+
+def _outputs_type(ct):
+    """outputs_f32 / outputs_f64: the solutions, the histories (residuals counted in Stats.nres, Aresiduals and Acond
+    in Stats.nAres, the others in n_<name>), the npc direction and the scalar results."""
+    class Outputs(C.Structure):
+        _fields_ = ([(f, C.c_void_p) for f in ("x", "y") + _HISTORIES]
+                    + [("n_" + h, C.c_int) for h in _HISTORIES[3:]]
+                    + [("npc_dir", C.c_void_p), ("Anorm", ct), ("error_with_bnd", C.c_int),
+                       ("solved_primal", C.c_int), ("solved_dual", C.c_int)])
+    return Outputs
+
+
+_OUTPUTS = {C.c_double: _outputs_type(C.c_double), C.c_float: _outputs_type(C.c_float)}
 
 
 def build(force: bool = False) -> str:
@@ -84,38 +117,6 @@ def _vec(v, dtype):
     return None if v is None else np.ascontiguousarray(v, dtype=dtype)
 
 
-def _opts(n, kw, default_hist):
-    o = Opts()
-    o.atol = kw.pop("atol", math.nan)
-    o.rtol = kw.pop("rtol", math.nan)
-    o.itmax = kw.pop("itmax", 0)
-    o.history = int(kw.pop("history", True))
-    o.radius = kw.pop("radius", 0.0)
-    o.linesearch = int(kw.pop("linesearch", False))
-    o.lambda_ = kw.pop("lambda_", 0.0)
-    o.etol = kw.pop("etol", math.nan)
-    o.conlim = kw.pop("conlim", math.nan)
-    o.window = kw.pop("window", 0)
-    o.memory = kw.pop("memory", 0)
-    o.restart = int(kw.pop("restart", False))
-    o.reorthogonalization = int(kw.pop("reorthogonalization", False))
-    o.ldiv = int(kw.pop("ldiv", False))
-    itmax = o.itmax if o.itmax > 0 else 2 * n
-    o.hist_cap = kw.pop("hist_cap", min(itmax + 2, default_hist))
-    if kw:
-        raise TypeError(f"unknown options {sorted(kw)}")
-    return o
-
-
-def _result(st, x, res, extra=None):
-    out = dict(niter=st.niter, solved=bool(st.solved), inconsistent=bool(st.inconsistent),
-               indefinite=bool(st.indefinite), npcCount=st.npcCount, error=st.error,
-               status=st.status.decode("utf-8"), residuals=res[:min(st.nres, len(res))].copy())
-    if extra:
-        out.update(extra)
-    return x, out
-
-
 class dot_mode:
     """with dot_mode(1): ...  -- the oracle's dot products, in every solver family, accumulate in double and round once
     (test knob, krylov_oracle_impl.h: kdot); the default 0 is the restatement's sequential sum in the working precision;
@@ -146,149 +147,257 @@ class precond_block:
         lib().oracle_set_precond_block(0)
 
 
-def cg(A, b, x0=None, M=None, dtype=np.float64, **kw):
-    """cg! (src/cg.jl:120-291).  M: None or the diagonal of a Diagonal preconditioner."""
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, x0, M = _vec(b, dtype), _vec(x0, dtype), _vec(M, dtype)
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res = np.zeros(o.hist_cap, dtype)
-    npc = np.zeros(n, dtype)
-    st = Stats()
-    getattr(lib(), f"oracle_cg_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(x0), _p(M), C.byref(o),
-                                        _p(x), _p(res), _p(npc), C.byref(st))
-    return _result(st, x, res, dict(npc_dir=npc))
+# ---- the solvers: one row per solver, one solve path ----------------------------------------------------------------
+_REQUIRED = inspect.Parameter.empty
+_VECTORS = ("c", "x0", "y0", "M", "N")
+# The keyword arguments every square solver accepts (each reads those its reference signature has), hist_cap included.
+_SQUARE_KW = dict(atol=math.nan, rtol=math.nan, itmax=0, history=True, radius=0.0, linesearch=False, lambda_=0.0,
+                  etol=math.nan, conlim=math.nan, window=0, memory=0, restart=False, reorthogonalization=False,
+                  ldiv=False, hist_cap=None)
+_STOP = (("timemax", math.inf), ("callback", None))
+_SIMPLE = ("niter", "solved", "inconsistent", "indefinite", "npcCount", "error", "status", "residuals")  # SimpleStats
+_LEASTNORM = ("niter", "solved", "inconsistent", "status", "residuals")
+_ADJOINT = ("niter", "solved", "solved_primal", "solved_dual", "status", "residuals_primal", "residuals_dual")
 
 
-def bicgstab(A, b, c=None, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """bicgstab! (src/bicgstab.jl:125-277)."""
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, c, x0, M, N = (_vec(v, dtype) for v in (b, c, x0, M, N))
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res = np.zeros(o.hist_cap, dtype)
-    st = Stats()
-    getattr(lib(), f"oracle_bicgstab_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(c), _p(x0), _p(M), _p(N),
-                                              C.byref(o), _p(x), _p(res), C.byref(st))
-    return _result(st, x, res)
+def _trust_region_error(rc, st):
+    return rc and {12: "zero direction", 13: "outside of the trust region"}.get(rc, "no real roots")
 
 
-def gmres(A, b, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """gmres! (src/gmres.jl:121-384)."""
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, x0, M, N = (_vec(v, dtype) for v in (b, x0, M, N))
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res = np.zeros(o.hist_cap, dtype)
-    st = Stats()
-    getattr(lib(), f"oracle_gmres_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(x0), _p(M), _p(N),
-                                           C.byref(o), _p(x), _p(res), C.byref(st))
-    return _result(st, x, res)
+def _cr_error(rc, st):
+    return rc and {1: "'linesearch' set to 'true' but radius > 0", 2: "warm_start and linesearch cannot be used together",
+                   5: "Indefinite system and no trust region"}.get(rc, f"to_boundary error {rc - 10}")
 
 
-def minres(A, b, x0=None, M=None, dtype=np.float64, **kw):
-    """minres! (src/minres.jl:164-485)."""
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, x0, M = _vec(b, dtype), _vec(x0, dtype), _vec(M, dtype)
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res, ares, acond = (np.zeros(o.hist_cap, dtype) for _ in range(3))
-    npc = np.zeros(n, dtype)
-    st = Stats()
-    getattr(lib(), f"oracle_minres_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(x0), _p(M), C.byref(o),
-                                            _p(x), _p(res), _p(ares), _p(acond), _p(npc), C.byref(st))
-    k = min(st.nAres, o.hist_cap)
-    return _result(st, x, res, dict(Aresiduals=ares[:k].copy(), Acond=acond[:k].copy(), npc_dir=npc))
+def _status_error(rc, st):
+    return st["error"] and st["status"]
 
 
-def cgs(A, b, c=None, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """cgs! (src/cgs.jl:125-282)."""
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, c, x0, M, N = (_vec(v, dtype) for v in (b, c, x0, M, N))
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res = np.zeros(o.hist_cap, dtype)
-    st = Stats()
-    getattr(lib(), f"oracle_cgs_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(c), _p(x0), _p(M), _p(N),
-                                         C.byref(o), _p(x), _p(res), C.byref(st))
-    return _result(st, x, res)
+class _Solver(NamedTuple):
+    doc: str
+    params: tuple                # positional parameters after (A, b), in order, with their defaults
+    keywords: dict               # the further keyword arguments and their defaults; hist_cap=None: accepted
+    stats: tuple = _SIMPLE       # the stats keys, in order
+    rect: bool = False           # itmax defaults to m + n (else 2n) where the history capacity is sized
+    transpose: bool = False      # the body applies Aᵀ, passed as its own CSR
+    two: bool = False            # returns (x, y, stats)
+    hist_extra: int = 2          # hist_cap = min(itmax + hist_extra, 2^22)
+    fixed_cap: bool = False      # a hist_cap keyword is accepted and ignored
+    error: object = None         # (return code, stats) -> the ArithmeticError message, or a false value
 
 
-def cg_lanczos(A, b, x0=None, M=None, check_curvature=False, dtype=np.float64, **kw):
-    """cg_lanczos! (src/cg_lanczos.jl:110-264).  Extra stats key: Anorm (LanczosStats)."""
+_LSQ_KW = dict(sqd=False, lambda_=0.0, atol=0.0, rtol=0.0, etol=math.nan, axtol=math.nan, btol=math.nan,   # lsqr.jl:155
+               conlim=math.nan, radius=0.0, itmax=0, history=True, window=0, ldiv=False, hist_cap=None)
+_CGLS_KW = dict(atol=math.nan, rtol=math.nan, lambda_=0.0, radius=0.0, itmax=0, history=True, ldiv=False, hist_cap=None)
+_CRAIG_KW = dict(lambda_=0.0, sqd=False, atol=math.nan, rtol=math.nan, btol=math.nan, conlim=math.nan, itmax=0,
+                 history=True, ldiv=False, transfer_to_lsqr=False)
+_CGNE_KW = dict(lambda_=0.0, atol=math.nan, rtol=math.nan, itmax=0, history=True, ldiv=False)
+_XMN = (("x0", None), ("M", None), ("N", None))
+
+_SOLVERS = {
+    "cg": _Solver("cg! (src/cg.jl:120-291).  M: None or the diagonal of a Diagonal preconditioner.",
+                  (("x0", None), ("M", None)), _SQUARE_KW, _SIMPLE + ("npc_dir",)),
+    "bicgstab": _Solver("bicgstab! (src/bicgstab.jl:125-277).", (("c", None),) + _XMN, _SQUARE_KW),
+    "gmres": _Solver("gmres! (src/gmres.jl:121-384).", _XMN, _SQUARE_KW),
+    "minres": _Solver("minres! (src/minres.jl:164-485).", (("x0", None), ("M", None)), _SQUARE_KW,
+                      _SIMPLE + ("Aresiduals", "Acond", "npc_dir")),
+    "cgs": _Solver("cgs! (src/cgs.jl:125-282).", (("c", None),) + _XMN, _SQUARE_KW),
+    "cg_lanczos": _Solver("cg_lanczos! (src/cg_lanczos.jl:110-264).  Extra stats key: Anorm (LanczosStats).",
+                          (("x0", None), ("M", None), ("check_curvature", False)), _SQUARE_KW, _SIMPLE + ("Anorm",)),
+    "fom": _Solver("fom! (src/fom.jl:121-368).", _XMN, _SQUARE_KW),
+    "fgmres": _Solver("fgmres! (src/fgmres.jl:128-388); N: None or the diagonal of a fixed right preconditioner.",
+                      _XMN, _SQUARE_KW),
+    "dqgmres": _Solver("dqgmres! (src/dqgmres.jl:121-335).", _XMN, _SQUARE_KW),
+    "diom": _Solver("diom! (src/diom.jl:121-332).", _XMN, _SQUARE_KW, error=_status_error),
+    "cr": _Solver("cr! (src/cr.jl:128-478).  Extra stats keys: Aresiduals, npc_dir.",
+                  (("x0", None), ("M", None), ("gamma", math.nan)), _SQUARE_KW, _SIMPLE + ("Aresiduals", "npc_dir"),
+                  error=_cr_error),
+    "car": _Solver("car! (src/car.jl:108-256).  M: None or the diagonal of a Diagonal preconditioner (ldiv=True applies "
+                   "its inverse); callback(iter) -> bool stops the solve when true; timemax in seconds.  Extra stats key: "
+                   "Aresiduals.", (("x0", None), ("M", None)) + _STOP, _SQUARE_KW, _SIMPLE + ("Aresiduals",)),
+    "minares": _Solver("minares! (src/minares.jl:113-595), M = I.  lambda_: the shift λ; artol: the kwarg Artol (None -> "
+                       "sqrt(eps)).  Extra stats key: Aresiduals.",
+                       (("x0", None), ("lambda_", 0.0), ("artol", None)) + _STOP, _SQUARE_KW, _SIMPLE + ("Aresiduals",)),
+    "bilq": _Solver("bilq! (src/bilq.jl:118-407).  c: None (= b) or the shadow vector; M, N: None or the diagonal of a "
+                    "Diagonal preconditioner; callback(iter) -> bool stops the solve when true; timemax in seconds.",
+                    (("c", None),) + _XMN + (("transfer_to_bicg", True),) + _STOP, _SQUARE_KW, transpose=True),
+    "qmr": _Solver("qmr! (src/qmr.jl:124-405); arguments as for bilq.", (("c", None),) + _XMN + _STOP, _SQUARE_KW,
+                   transpose=True),
+    "bilqr": _Solver("bilqr! (src/bilqr.jl:115-484) -> (x, y, stats).  callback(iter) -> bool stops the solve when true.",
+                     (("c", _REQUIRED), ("x0", None), ("y0", None), ("transfer_to_bicg", True)) + _STOP, _SQUARE_KW,
+                     _ADJOINT, transpose=True, two=True, fixed_cap=True),
+    "trilqr": _Solver("trilqr! (src/trilqr.jl:114-461) -> (x, y, stats); A is m x n, b has m entries, c n.",
+                      (("c", _REQUIRED), ("x0", None), ("y0", None), ("transfer_to_usymcg", True)) + _STOP, _SQUARE_KW,
+                      _ADJOINT, rect=True, transpose=True, two=True, fixed_cap=True),
+    "lsqr": _Solver("lsqr! (src/lsqr.jl:174-440) on an m x n matrix.  M (m) / N (n): None or the diagonal of a Diagonal "
+                    "operator.\n    kwargs: lambda_, sqd, radius, etol, axtol, btol, conlim, atol, rtol (default 0), itmax, "
+                    "window, ldiv, history.\n    Extra stats key: Aresiduals.",
+                    (("M", None), ("N", None)), _LSQ_KW, _SIMPLE + ("Aresiduals", "Anorm"), rect=True,
+                    error=_trust_region_error),
+    "lsmr": _Solver("lsmr! (src/lsmr.jl:178-455); same arguments as lsqr.  Extra stats keys: Aresiduals, Anorm "
+                    "(LsmrStats).", (("M", None), ("N", None)), _LSQ_KW, _SIMPLE + ("Aresiduals", "Anorm"), rect=True,
+                    error=_trust_region_error),
+    "cgls": _Solver("cgls! (src/cgls.jl:129-243) on an m x n matrix.  M (m entries): None or the diagonal of a Diagonal "
+                    "operator.\n    kwargs: lambda_, radius, atol, rtol (default sqrt(eps)), itmax, ldiv, history.  Extra "
+                    "stats key: Aresiduals.", (("M", None),), _CGLS_KW, _SIMPLE + ("Aresiduals",), rect=True,
+                    error=_trust_region_error),
+    "crls": _Solver("crls! (src/crls.jl:120-268); same arguments as cgls.", (("M", None),), _CGLS_KW,
+                    _SIMPLE + ("Aresiduals",), rect=True, error=_trust_region_error),
+    "lslq": _Solver("lslq! (src/lslq.jl:201-520) on an m x n matrix.  M (m) / N (n): None or the diagonal of a Diagonal "
+                    "operator.\n    kwargs: lambda_, sqd, sigma, etol, utol, btol, conlim, atol, rtol (default "
+                    "sqrt(eps)), itmax, window, ldiv,\n    transfer_to_lsqr, history.  Extra stats keys: Aresiduals, "
+                    "err_lbnds, err_ubnds_lq, err_ubnds_cg, error_with_bnd.", (("M", None), ("N", None)),
+                    dict(lambda_=0.0, sqd=False, sigma=0.0, atol=math.nan, rtol=math.nan, etol=math.nan, utol=math.nan,
+                         btol=math.nan, conlim=math.nan, itmax=0, history=True, window=0, ldiv=False,
+                         transfer_to_lsqr=False, hist_cap=None),
+                    _SIMPLE + ("Aresiduals", "err_lbnds", "err_ubnds_lq", "err_ubnds_cg", "error_with_bnd"), rect=True),
+    "craig": _Solver("craig! (src/craig.jl:174-405) -> (x, y, stats).  M (m) / N (n): None or the diagonal of a Diagonal "
+                     "operator.\n    kwargs: lambda_, sqd, transfer_to_lsqr, btol, conlim, atol, rtol, itmax, ldiv, "
+                     "history.  callback(iter) -> bool.", (("M", None), ("N", None)) + _STOP, _CRAIG_KW, _LEASTNORM,
+                     rect=True, transpose=True, two=True),
+    "craigmr": _Solver("craigmr! (src/craigmr.jl:161-396) -> (x, y, stats); stats also has Aresiduals.  Same arguments as "
+                       "craig, without\n    transfer_to_lsqr, btol and conlim.", (("M", None), ("N", None)) + _STOP,
+                       _CRAIG_KW, _LEASTNORM + ("Aresiduals",), rect=True, transpose=True, two=True),
+    "lnlq": _Solver("lnlq! (src/lnlq.jl:168-568) -> (x, y, stats); stats also has error_bnd_x, error_bnd_y and "
+                    "error_with_bnd.\n    M (m) / N (n): None or the diagonal of a Diagonal operator.  kwargs: lambda_, "
+                    "sqd, sigma, transfer_to_craig\n    (default True), utolx, utoly, atol, rtol, itmax, ldiv, history.  "
+                    "callback(iter) -> bool.", (("M", None), ("N", None)) + _STOP,
+                    dict(lambda_=0.0, sqd=False, sigma=0.0, atol=math.nan, rtol=math.nan, utolx=math.nan,
+                         utoly=math.nan, itmax=0, history=True, ldiv=False, transfer_to_craig=True),
+                    _LEASTNORM + ("error_bnd_x", "error_bnd_y", "error_with_bnd"), rect=True, transpose=True, two=True,
+                    hist_extra=3),
+    "cgne": _Solver("cgne! (src/cgne.jl:134-252) -> (x, stats).  N (m entries): None or the diagonal of a Diagonal "
+                    "operator on the\n    residual space.  kwargs: lambda_, atol, rtol, itmax, ldiv, history.  "
+                    "callback(iter) -> bool.", (("N", None),) + _STOP, _CGNE_KW, _LEASTNORM, rect=True, transpose=True),
+    "crmr": _Solver("crmr! (src/crmr.jl:132-244) -> (x, stats); stats also has Aresiduals.  Same arguments as cgne.",
+                    (("N", None),) + _STOP, _CGNE_KW, _LEASTNORM + ("Aresiduals",), rect=True, transpose=True),
+}
+
+
+def _callback(f):
+    return _ITER_CB() if f is None else _ITER_CB(lambda it, _u: int(bool(f(it))))
+
+
+_CONVERT = dict({k: int for k in ("history", "linesearch", "restart", "reorthogonalization", "ldiv", "check_curvature",
+                                  "transfer_to_lsqr", "transfer_to_craig", "transfer_to_bicg", "transfer_to_usymcg")},
+                gamma=float, artol=lambda a: math.nan if a is None else float(a),
+                timemax=lambda t: -1.0 if math.isinf(t) else float(t), callback=_callback)
+_FIELD = {"transfer_to_bicg": "transfer", "transfer_to_usymcg": "transfer"}
+
+
+def _options(keywords, kw, default_itmax, hist_extra=2, fixed_cap=False):
+    """Pops the accepted keywords into an Options; whatever is left in kw raises TypeError."""
+    o = Options()
+    sqd = kw.pop("sqd", False) if "sqd" in keywords else False
+    for key, default in keywords.items():
+        if key not in ("sqd", "hist_cap"):
+            v = kw.pop(key, default)
+            setattr(o, _FIELD.get(key, key), _CONVERT[key](v) if key in _CONVERT else v)
+    if sqd:
+        if o.lambda_ != 0:
+            raise ValueError("sqd cannot be set to true if λ ≠ 0 !")
+        o.lambda_ = 1.0
+    itmax = o.itmax if o.itmax > 0 else default_itmax
+    o.hist_cap = min(itmax + hist_extra, 1 << 22)
+    if "hist_cap" in keywords:
+        cap = kw.pop("hist_cap", o.hist_cap)
+        if not fixed_cap:
+            o.hist_cap = cap
+    if kw:
+        raise TypeError(f"unknown options {sorted(kw)}")
+    return o
+
+
+def _stat(key, st, out, hist, cap):
+    if key in ("niter", "npcCount", "error"):
+        return getattr(st, key)
+    if key in ("solved", "inconsistent", "indefinite"):
+        return bool(getattr(st, key))
+    if key == "status":
+        return st.status.decode("utf-8")
+    if key in ("error_with_bnd", "solved_primal", "solved_dual"):
+        return bool(getattr(out, key))
+    if key == "Anorm":
+        return float(out.Anorm)
+    if key == "npc_dir":
+        return hist[key]
+    h = "residuals" if key == "residuals_primal" else key
+    k = st.nres if h == "residuals" else st.nAres if h in ("Aresiduals", "Acond") else getattr(out, "n_" + h)
+    return hist[h][:min(k, cap)].copy()
+
+
+def _solve(name, A, b, dtype, kw):
+    row = _SOLVERS[name]
     suf, ct = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, x0, M = _vec(b, dtype), _vec(x0, dtype), _vec(M, dtype)
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res = np.zeros(o.hist_cap, dtype)
-    anorm = ct(0)
+    A = sp.csr_matrix(A)
+    m, n = A.shape
+    P = Problem(m, n)
+    _, rp, ci, va = _csr(A, dtype)
+    P.rowptr, P.colind, P.val = _p(rp), _p(ci), _p(va)
+    if row.transpose:
+        _, trp, tci, tva = _csr(A.T, dtype)
+        P.trowptr, P.tcolind, P.tval = _p(trp), _p(tci), _p(tva)
+    params = dict(row.params)
+    vecs = dict(b=_vec(b, dtype))
+    for v in _VECTORS:
+        if v in params:
+            vecs[v] = _vec(kw.pop(v, None), dtype)
+            if vecs[v] is None and params[v] is _REQUIRED:
+                raise TypeError(f"{name}() missing required argument: '{v}'")
+            setattr(P, v, _p(vecs[v]))
+    P.b = _p(vecs["b"])
+    if "y0" in params and (vecs["x0"] is None) != (vecs["y0"] is None):
+        raise ValueError("pass both x0 and y0, or neither")
+    keywords = {**row.keywords, **{k: d for k, d in row.params if k not in _VECTORS}}
+    o = _options(keywords, kw, m + n if row.rect else 2 * n, row.hist_extra, row.fixed_cap)
+    out = _OUTPUTS[ct]()
+    x, y = np.zeros(n, dtype), (np.zeros(m, dtype) if row.two else None)
+    hist = {h: np.zeros(o.hist_cap, dtype) for h in _HISTORIES
+            if h in row.stats or (h == "residuals" and "residuals_primal" in row.stats)}
+    if "npc_dir" in row.stats:
+        hist["npc_dir"] = np.zeros(n, dtype)
+    out.x, out.y = _p(x), _p(y)
+    for h, buf in hist.items():
+        setattr(out, h, _p(buf))
     st = Stats()
-    getattr(lib(), f"oracle_cg_lanczos_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(x0), _p(M), int(check_curvature),
-                                                C.byref(o), _p(x), _p(res), C.byref(anorm), C.byref(st))
-    return _result(st, x, res, dict(Anorm=float(anorm.value)))
+    rc = getattr(lib(), f"oracle_solve_{suf}")(name.encode(), C.byref(P), C.byref(o), C.byref(out), C.byref(st))
+    stats = {k: _stat(k, st, out, hist, o.hist_cap) for k in row.stats}
+    msg = row.error and row.error(rc, stats)
+    if msg:
+        raise ArithmeticError(msg)
+    return x, y, stats
 
 
-def _arnoldi_family(name, A, b, x0, M, N, dtype, kw):
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, x0, M, N = (_vec(v, dtype) for v in (b, x0, M, N))
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res = np.zeros(o.hist_cap, dtype)
-    st = Stats()
-    getattr(lib(), f"oracle_{name}_{suf}")(n, _p(rp), _p(ci), _p(va), _p(b), _p(x0), _p(M), _p(N),
-                                            C.byref(o), _p(x), _p(res), C.byref(st))
-    return _result(st, x, res)
+def solve(name, A, b, *, c=None, x0=None, y0=None, M=None, N=None, dtype=np.float64, **kw):
+    """Runs the oracle solver `name` (a key of _SOLVERS) -> (x, y, stats), y None for the single-solution solvers.
+    The vectors a solver does not take must be None; kw are its keyword arguments (an unknown one raises TypeError)."""
+    given = {k: v for k, v in dict(c=c, x0=x0, y0=y0, M=M, N=N).items() if v is not None}
+    return _solve(name, A, b, dtype, {**given, **kw})
 
 
-def fom(A, b, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """fom! (src/fom.jl:121-368)."""
-    return _arnoldi_family("fom", A, b, x0, M, N, dtype, kw)
+def _named(name):
+    """The solver function `name`, with its reference signature and return shape."""
+    row = _SOLVERS[name]
+    K = inspect.Parameter.POSITIONAL_OR_KEYWORD
+    sig = inspect.Signature([inspect.Parameter("A", K), inspect.Parameter("b", K)]
+                            + [inspect.Parameter(k, K, default=d) for k, d in row.params]
+                            + [inspect.Parameter("dtype", K, default=np.float64),
+                               inspect.Parameter("kw", inspect.Parameter.VAR_KEYWORD)])
+
+    def f(*args, **kwargs):
+        bound = sig.bind(*args, **kwargs)
+        bound.apply_defaults()
+        a = bound.arguments
+        x, y, stats = _solve(name, a.pop("A"), a.pop("b"), a.pop("dtype"), {**a.pop("kw"), **a})
+        return (x, y, stats) if row.two else (x, stats)
+
+    f.__name__ = f.__qualname__ = name
+    f.__doc__, f.__signature__ = row.doc, sig
+    return f
 
 
-def fgmres(A, b, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """fgmres! (src/fgmres.jl:128-388); N: None or the diagonal of a fixed right preconditioner."""
-    return _arnoldi_family("fgmres", A, b, x0, M, N, dtype, kw)
-
-
-def dqgmres(A, b, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """dqgmres! (src/dqgmres.jl:121-335)."""
-    return _arnoldi_family("dqgmres", A, b, x0, M, N, dtype, kw)
-
-
-def diom(A, b, x0=None, M=None, N=None, dtype=np.float64, **kw):
-    """diom! (src/diom.jl:121-332)."""
-    x, st = _arnoldi_family("diom", A, b, x0, M, N, dtype, kw)
-    if st["error"]:
-        raise ArithmeticError(st["status"])
-    return x, st
-
-
-def cr(A, b, x0=None, M=None, gamma=math.nan, dtype=np.float64, **kw):
-    """cr! (src/cr.jl:128-478).  Extra stats keys: Aresiduals, npc_dir."""
-    suf, _ = _suf(dtype)
-    n, rp, ci, va = _csr(A, dtype)
-    b, x0, M = _vec(b, dtype), _vec(x0, dtype), _vec(M, dtype)
-    o = _opts(n, kw, 1 << 22)
-    x = np.zeros(n, dtype)
-    res, ares = np.zeros(o.hist_cap, dtype), np.zeros(o.hist_cap, dtype)
-    npc = np.zeros(n, dtype)
-    st = Stats()
-    f = getattr(lib(), f"oracle_cr_{suf}")
-    f.argtypes = [C.c_int] + [C.c_void_p] * 6 + [C.c_double] + [C.c_void_p] * 6
-    rc = f(n, _p(rp), _p(ci), _p(va), _p(b), _p(x0), _p(M), float(gamma), C.cast(C.byref(o), C.c_void_p), _p(x), _p(res), _p(ares),
-           _p(npc), C.cast(C.byref(st), C.c_void_p))
-    if rc:
-        raise ArithmeticError({1: "'linesearch' set to 'true' but radius > 0", 2: "warm_start and linesearch cannot be used together",
-                               5: "Indefinite system and no trust region"}.get(rc, f"to_boundary error {rc - 10}"))
-    k = min(st.nAres, o.hist_cap)
-    return _result(st, x, res, dict(Aresiduals=ares[:k].copy(), npc_dir=npc))
+for _name in _SOLVERS:
+    globals()[_name] = _named(_name)
 
 
 def block_gmres(A, B, X0=None, M=None, N=None, dtype=np.float64, **kw):
@@ -299,13 +408,13 @@ def block_gmres(A, B, X0=None, M=None, N=None, dtype=np.float64, **kw):
     p = B.shape[1]
     X0f = None if X0 is None else np.asfortranarray(X0, dtype=dtype)
     M, N = _vec(M, dtype), _vec(N, dtype)
-    o = _opts(n, kw, 1 << 22)
+    o = _options(_SQUARE_KW, kw, 2 * n)
     X = np.zeros((n, p), dtype, order="F")
-    res = np.zeros(o.hist_cap, dtype)
+    hist = dict(residuals=np.zeros(o.hist_cap, dtype))
     st = Stats()
     getattr(lib(), f"oracle_block_gmres_{suf}")(n, p, _p(rp), _p(ci), _p(va), _p(B), _p(X0f), _p(M), _p(N),
-                                                 C.byref(o), _p(X), _p(res), C.byref(st))
-    return _result(st, X, res)
+                                                 C.byref(o), _p(X), _p(hist["residuals"]), C.byref(st))
+    return X, {k: _stat(k, st, None, hist, o.hist_cap) for k in _SIMPLE}
 
 
 def householder(Q, compact=False, dtype=np.float64):

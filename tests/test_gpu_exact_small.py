@@ -20,8 +20,7 @@ import pytest
 import scipy.sparse as sp
 
 from krylov_b200 import _lib
-from oracle import adjoint_oracle, ares_oracle, biorth_oracle, cgls_oracle, cgne_oracle, leastnorm_oracle, lnlq_oracle
-from oracle import lsq_oracle, processes_oracle
+from oracle import processes_oracle
 from oracle import oracle as O
 from test_oracle_dot_tree import device_tree, operands
 
@@ -141,12 +140,6 @@ SYM = ["cg", "cr", "minres", "cg_lanczos", "car", "minares"]
 UNSYM = ["gmres", "fom", "fgmres", "dqgmres", "diom", "cgs", "bicgstab", "bilq", "qmr", "bilqr"]
 LSQ = ["lsqr", "lsmr", "lslq", "cgls", "crls"]
 LN = ["craig", "craigmr", "lnlq", "cgne", "crmr"]
-ORACLE = {**{s: O for s in ["cg", "cr", "minres", "cg_lanczos", "gmres", "fom", "fgmres", "dqgmres", "diom", "cgs",
-                            "bicgstab"]},
-          "car": ares_oracle, "minares": ares_oracle, "bilq": biorth_oracle, "qmr": biorth_oracle,
-          "bilqr": adjoint_oracle, "trilqr": adjoint_oracle, "lsqr": lsq_oracle, "lsmr": lsq_oracle,
-          "lslq": cgls_oracle, "cgls": cgls_oracle, "crls": cgls_oracle, "craig": leastnorm_oracle,
-          "craigmr": leastnorm_oracle, "lnlq": lnlq_oracle, "cgne": cgne_oracle, "crmr": cgne_oracle}
 # the preconditioners each takes, and in which space (m or n)
 TAKES_M = {**{s: "n" for s in SYM if s != "minares"}, **{s: "n" for s in UNSYM if s != "bilqr"},
            **{s: "m" for s in LSQ + ["craig", "craigmr", "lnlq"]}}
@@ -203,9 +196,9 @@ def normal_range_run(solver, A, b, c, dt, kw):
         with O.dot_mode(2):
             if oracle_blocks(kw) is not None:
                 with O.precond_block(oracle_blocks(kw)):
-                    xo, yo, so = run_oracle(solver, A, b, c, dt, dict(kw, M=kw["M"].reshape(-1)))
+                    xo, yo, so = O.solve(solver, A, b, c=c, dtype=dt, **dict(kw, M=kw["M"].reshape(-1)))
             else:
-                xo, yo, so = run_oracle(solver, A, b, c, dt, kw)
+                xo, yo, so = O.solve(solver, A, b, c=c, dtype=dt, **kw)
         k = first_below_normal(A, so, dt)
         if k is None:
             return kw, (xo, yo, so)
@@ -224,20 +217,6 @@ def oracle_keys(solver, so):
     """The stats both sides report: every key of the oracle's stats dict but its error code and the CG/MINRES npc
     direction (a workspace vector, not a statistic)."""
     return [k for k in so if k not in ("error", "npc_dir") and not (k == "Anorm" and solver != "cg_lanczos")]
-
-
-def run_oracle(solver, A, b, c, dt, kw):
-    kw = dict(kw)
-    f = getattr(ORACLE[solver], solver)
-    if solver in ("bilqr", "trilqr"):
-        x, y, so = f(A, b, c, dtype=dt, **kw)
-    elif solver in ("craig", "craigmr", "lnlq"):
-        x, y, so = f(A, b, dtype=dt, **kw)
-    else:
-        if c is not None:
-            kw["c"] = c
-        (x, so), y = f(A, b, dtype=dt, **kw), None
-    return x, y, so
 
 
 def run_gpu(kb, solver, A, b, c, dt, kw):
