@@ -179,6 +179,35 @@ int krylov_b200_set_preconditioner_blockdiag(void *ws, int which, int bs, const 
  * krylov_workspace_create.  Options: M, check_curvature (KrylovB200Options), the common tolerances. */
 #define KRYLOV_B200_CG_LANCZOS 100
 
+/* ---- shift solvers: one Lanczos process for p shifted systems, p solutions ----
+ * cg_lanczos_shift! (src/cg_lanczos_shift.jl): (A + σᵢ I) xᵢ = b, A square (symmetric), M on the n-space;
+ * cgls_lanczos_shift! (src/cgls_lanczos_shift.jl): (AᵀA + σᵢ I) xᵢ = Aᵀb, A m x n (b: m entries, xᵢ: n), no M.
+ * They have no slot in the reference's KrylovSolverType; these values select them in
+ * krylov_b200_shift_workspace_create (-2 for another solver or a complex dtype, -1 for nshifts <= 0 or, for
+ * CG-Lanczos-shift, m != n).  The handle is a third kind: krylov_b200_set_operator_csr, _attach_csr,
+ * _share_operator, _set_preconditioner_diag / _blockdiag (M only: which = 1 is refused; CGLS-Lanczos-shift refuses any M
+ * at solve time),
+ * _set_options (history, ldiv, fused, callback, check_curvature), _get_stats, _launch_count and _stream accept it;
+ * krylov_solve, krylov_get_x, krylov_get_y, the warm starts and row partitioning refuse it (-1, last_error).
+ * krylov_b200_shift_solve: matvec_A (and matvec_At for CGLS-Lanczos-shift) may be NULL once a CSR operator is
+ * attached; shifts[nshifts] (host doubles, rounded to the dtype).  Options: atol, rtol, itmax (0: 2n, or m + n for
+ * CGLS-Lanczos-shift), timemax, verbose of KrylovOptions.  `shift` arguments are 0-based.
+ * krylov_b200_shift_get_x copies x_shift (n entries) to host or device memory, following the workspace's device.
+ * krylov_b200_shift_get_stats: any pointer may be NULL; status gets at most status_cap - 1 characters;
+ * indefinite[nshifts] (CG-Lanczos-shift: γᵢ ≤ 0 met; 0 for CGLS-Lanczos-shift) and history_len[nshifts].
+ * krylov_b200_shift_get_history copies shift's residual history (<= cap entries) and returns the count, or -1. */
+#define KRYLOV_B200_CG_LANCZOS_SHIFT 101
+#define KRYLOV_B200_CGLS_LANCZOS_SHIFT 102
+int krylov_b200_shift_workspace_create(int solver, int m, int n, int nshifts, KrylovDataType dtype, KrylovDeviceType device,
+                                       void **ws_out);
+int krylov_b200_shift_workspace_free(void *ws); /* 0 | 1 if the handle is unknown */
+int krylov_b200_shift_solve(void *ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, KrylovMatvec matvec_M, const void *b,
+                            const double *shifts, void *userdata, const KrylovOptions *opts);
+int krylov_b200_shift_get_x(void *ws, int shift, void *x, int n);
+int krylov_b200_shift_get_stats(void *ws, int *niter, int *solved, double *timer, char *status, int status_cap,
+                                int *indefinite, int *history_len);
+int krylov_b200_shift_get_history(void *ws, int shift, double *out, int cap);
+
 /* Extra solve-time switches not present in KrylovOptions. */
 typedef struct {
   int history;        /* 1: record residual history (kwarg `history`)              */

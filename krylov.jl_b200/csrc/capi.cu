@@ -41,6 +41,7 @@ struct CsrAny {
 struct Handle {
   int solver = 0, dtype = 1, device_kind = 0;
   bool block = false;                  // ws is a BlockWorkspace (krylov_block_* entry points)
+  bool shift = false;                  // ws is a shift solver's Workspace (krylov_b200_shift_* entry points)
   const SolverInfo* info = nullptr;    // single-RHS handles: the solver's row (kb_internal.h)
   int p = 0;
   void* ws = nullptr;
@@ -65,9 +66,28 @@ Handle* lookup_any(void* p) {
   auto it = g_handles.find(p);
   return it == g_handles.end() ? nullptr : it->second;
 }
-// single-RHS entry points only accept single-RHS handles, block entry points only block handles
-Handle* lookup(void* p) { Handle* h = lookup_any(p); return (h && !h->block) ? h : nullptr; }
+// single-RHS entry points only accept single-RHS handles, block entry points only block handles, shift entry points
+// only shift handles
+Handle* lookup(void* p) { Handle* h = lookup_any(p); return (h && !h->block && !h->shift) ? h : nullptr; }
 Handle* lookup_block(void* p) { Handle* h = lookup_any(p); return (h && h->block) ? h : nullptr; }
+Handle* lookup_shift(void* p) { Handle* h = lookup_any(p); return (h && h->shift) ? h : nullptr; }
+// the refusal of a single-RHS entry point given another kind of handle
+const char* not_single(void* p) {
+  Handle* h = lookup_any(p);
+  return h && h->shift ? "a CG-Lanczos-shift / CGLS-Lanczos-shift workspace solves through krylov_b200_shift_solve and "
+                         "returns its solutions through krylov_b200_shift_get_x"
+                       : "unknown workspace handle";
+}
+
+// The interface facts of the shift solvers (krylov_b200_shift_workspace_create), read as the single-RHS rows are.
+constexpr const char* kNoMCglsShift = "Preconditioner `M` is not supported.";
+constexpr const char* kShiftDist = "row-partitioned shift solves are not available";
+constexpr const char* kShiftNoN = "the shift solvers take no right preconditioner N (which = 1): only M (which = 0)";
+inline constexpr SolverInfo kShiftSolvers[] = {
+  {"cg_lanczos_shift",   false, false, kOnN, kIgnored, BD_TAKES, nullptr, C_NONE, 1, WARM_NONE, kShiftDist, 0},
+  {"cgls_lanczos_shift", true,  true,  {P_REFUSED, kNoMCglsShift}, kIgnored, BD_REFUSED_AT_ATTACH, kNoMCglsShift, C_NONE, 1,
+                         WARM_NONE, kShiftDist, 0},
+};
 
 int fail(const char* where, const std::exception& e) {
   g_last_error = std::string(where) + ": " + e.what();
@@ -475,7 +495,7 @@ int krylov_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, Krylov
                  const void* b, const void* c, void* userdata, const KrylovOptions* opts) {
   try {
     Handle* h = lookup(ws);
-    if (!h) return fail("krylov_solve", "unknown workspace handle");
+    if (!h) return fail("krylov_solve", not_single(ws));
     return h->dtype == KRYLOV_FLOAT64 ? do_solve<double>(h, *h->info, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts)
                                       : do_solve<float>(h, *h->info, matvec_A, matvec_At, matvec_M, matvec_N, b, c, userdata, opts);
   } catch (const std::exception& e) { return fail("krylov_solve", e); }
@@ -484,7 +504,7 @@ int krylov_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, Krylov
 int krylov_get_x(void* ws, void* x, int n) {
   try {
     Handle* h = lookup(ws);
-    if (!h) return fail("krylov_get_x", "unknown workspace handle");
+    if (!h) return fail("krylov_get_x", not_single(ws));
     return h->dtype == KRYLOV_FLOAT64 ? do_get_x<double>(h, x, n) : do_get_x<float>(h, x, n);
   } catch (const std::exception& e) { return fail("krylov_get_x", e); }
 }
@@ -492,7 +512,7 @@ int krylov_get_x(void* ws, void* x, int n) {
 int krylov_get_y(void* ws, void* y, int m) {
   try {
     Handle* h = lookup(ws);
-    if (!h) return fail("krylov_get_y", "unknown workspace handle");
+    if (!h) return fail("krylov_get_y", not_single(ws));
     if (h->info->nsol != 2) return -2;   // solution_count (c_stores.jl:211-216)
     if (!y) return fail("krylov_get_y", "y is NULL");
     return h->dtype == KRYLOV_FLOAT64 ? do_get_y<double>(h, y, m) : do_get_y<float>(h, y, m);
@@ -506,7 +526,7 @@ double krylov_elapsed_time(void* ws) { Handle* h = lookup(ws); return h ? stats_
 int krylov_warm_start(void* ws, const void* x0, int n) {
   try {
     Handle* h = lookup(ws);
-    if (!h) return fail("krylov_warm_start", "unknown workspace handle");
+    if (!h) return fail("krylov_warm_start", not_single(ws));
     return h->dtype == KRYLOV_FLOAT64 ? do_warm_start<double>(h, x0, n) : do_warm_start<float>(h, x0, n);
   } catch (const std::exception& e) { return fail("krylov_warm_start", e); }
 }
@@ -514,7 +534,7 @@ int krylov_warm_start(void* ws, const void* x0, int n) {
 int krylov_warm_start2(void* ws, const void* x0, const void* y0, int nx, int ny) {
   try {
     Handle* h = lookup(ws);
-    if (!h) return fail("krylov_warm_start2", "unknown workspace handle");
+    if (!h) return fail("krylov_warm_start2", not_single(ws));
     if (h->info->warm != WARM_X0_Y0) return -2;
     return h->dtype == KRYLOV_FLOAT64 ? do_warm_start2<double>(h, x0, y0, nx, ny) : do_warm_start2<float>(h, x0, y0, nx, ny);
   } catch (const std::exception& e) { return fail("krylov_warm_start2", e); }
@@ -740,6 +760,7 @@ int krylov_b200_set_preconditioner_diag(void* ws, int which, const void* d, int 
   try {
     Handle* h = lookup_any(ws);
     if (!h) return fail("krylov_b200_set_preconditioner_diag", "unknown workspace handle");
+    if (h->shift && which != 0) return fail("krylov_b200_set_preconditioner_diag", kShiftNoN);
     void*& slot = which == 0 ? h->Mdiag : h->Ndiag;
     if (!d) { dev_free(slot); slot = nullptr; return 0; }
     const size_t esz = h->dtype == KRYLOV_FLOAT64 ? 8 : 4;
@@ -755,9 +776,10 @@ int krylov_b200_set_preconditioner_diag(void* ws, int which, const void* d, int 
 // row-major, ceil(n / bs) of them.  The inverses are formed once here so that ldiv = true is a product as well.
 int krylov_b200_set_preconditioner_blockdiag(void* ws, int which, int bs, const void* blocks, int location) {
   try {
-    Handle* h = lookup(ws);
-    if (!h) return fail("krylov_b200_set_preconditioner_blockdiag", "unknown (single right-hand side) workspace handle");
+    Handle* h = lookup_any(ws);
+    if (!h || h->block) return fail("krylov_b200_set_preconditioner_blockdiag", "unknown (single right-hand side) workspace handle");
     if (which != 0 && which != 1) return fail("krylov_b200_set_preconditioner_blockdiag", "which must be 0 (M) or 1 (N)");
+    if (h->shift && which != 0) return fail("krylov_b200_set_preconditioner_blockdiag", kShiftNoN);
     dev_free(h->Pblk[which]); dev_free(h->Pblk_inv[which]);
     h->Pblk[which] = h->Pblk_inv[which] = nullptr; h->Pbs[which] = 0; h->Psing[which] = -1;
     if (!blocks) return 0;
@@ -1444,6 +1466,164 @@ int kb200_csr_dict(void* csr, int* npairs) {
   const int np = a->dtype == KRYLOV_FLOAT64 ? a->dd.npairs : a->df.npairs;
   if (npairs) *npairs = np;
   return np > 0 ? 1 : 0;
+}
+
+}  // extern "C"
+
+// ------------------------------ shift solvers -----------------------------
+// CG-Lanczos-shift and CGLS-Lanczos-shift: a third handle kind, p solutions per solve.  The single-RHS setters (operator,
+// preconditioners, options) accept it; krylov_solve, krylov_get_x and the warm starts refuse it.
+namespace {
+template <class T> int do_shift_solve(Handle* h, KrylovMatvec fA, KrylovMatvec fAt, KrylovMatvec fM, const void* b,
+                                      const double* shifts, void* ud, const KrylovOptions* opts) {
+  Workspace<T>* ws = W<T>(h);
+  const SolverInfo& S = *h->info;
+  KB_CUDA(cudaSetDevice(ws->ctx.device));
+  SolveOpts so = map_opts(h, 0, opts);
+  const int m = ws->m, n = ws->n;
+  LinOp<T> A, At;              // A maps n -> m, A^T m -> n
+  if (fA) {
+    if (S.adjoint && !fAt)
+      throw std::runtime_error(std::string(S.name) + " applies the adjoint of A: matvec_At must be given with matvec_A");
+    A = make_cb_op<T>(h, ws, fA, ud); A.n = m; A.nin = n;
+    if (S.adjoint) { At = make_cb_op<T>(h, ws, fAt, ud); At.n = n; At.nin = m; }
+  } else if (h->csr) {
+    const Csr<T>& Cs = csr_of<T>(*h->csr);
+    if (Cs.n != m || Cs.max_col >= n)
+      throw std::runtime_error("CSR operator: size or column index inconsistent with the workspace ((m, n) = (" + std::to_string(m) +
+                               ", " + std::to_string(n) + "), operator rows = " + std::to_string(Cs.n) +
+                               ", largest column = " + std::to_string(Cs.max_col) + ")");
+    A.kind = LinOp<T>::CSR; A.csr = &Cs; A.n = m;
+    if (S.adjoint) { At.kind = LinOp<T>::CSR; At.csr = adjoint_csr<T>(h, ws); At.n = At.csr->n; }
+  } else {
+    throw std::runtime_error(S.adjoint ? "no operator: pass matvec_A and matvec_At or attach one with krylov_b200_set_operator_csr"
+                                       : "no operator: pass matvec_A or attach one with krylov_b200_set_operator_csr");
+  }
+  if (S.M.use == P_REFUSED && (fM || h->Mdiag || h->Pblk[0])) throw std::runtime_error(S.M.refusal);
+  LinOp<T> M = make_cb_op<T>(h, ws, fM, ud);
+  M.n = n;
+  if (!fM && h->Mdiag) { M.kind = LinOp<T>::DIAG; M.diag = (const T*)h->Mdiag; }
+  else if (!fM && h->Pblk[0]) {
+    M.kind = LinOp<T>::BDIAG; M.blocks = (const T*)h->Pblk[0]; M.blocks_inv = (const T*)h->Pblk_inv[0]; M.bs = h->Pbs[0];
+    if (so.ldiv && h->Psing[0] >= 0)
+      throw std::runtime_error("block-Jacobi M with ldiv = true: diagonal block " + std::to_string(h->Psing[0]) + " (rows " +
+                               std::to_string(h->Psing[0] * M.bs) + " onwards, 0-based) is singular");
+  }
+  if (!b) throw std::runtime_error("b is NULL");
+  if (!shifts) throw std::runtime_error("shifts is NULL");
+  std::vector<T> sh(ws->nshifts);
+  for (int i = 0; i < ws->nshifts; i++) sh[i] = (T)shifts[i];
+  const T* bd = stage_in<T>(h, ws, b, ws->bbuf, m);
+  if (h->solver == S_CG_LANCZOS_SHIFT) cg_lanczos_shift_solve<T>(*ws, A, bd, sh.data(), M, so);
+  else cgls_lanczos_shift_solve<T>(*ws, A, At, bd, sh.data(), so);
+  return 0;
+}
+template <class T> int do_shift_get_x(Handle* h, int shift, void* x, int n) {
+  Workspace<T>* ws = W<T>(h);
+  if (shift < 0 || shift >= ws->nshifts)
+    throw std::runtime_error("shift index " + std::to_string(shift) + " outside 0.." + std::to_string(ws->nshifts - 1));
+  if (n > ws->n) n = ws->n;
+  KB_CUDA(cudaSetDevice(ws->ctx.device));
+  KB_CUDA(cudaMemcpyAsync(x, ws->Xs + (size_t)shift * ws->n, sizeof(T) * (size_t)n,
+                          h->device_kind == KRYLOV_CUDA ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ws->ctx.stream));
+  ws->ctx.sync();
+  return 0;
+}
+int shift_count(Handle* h) { return h->dtype == KRYLOV_FLOAT64 ? W<double>(h)->nshifts : W<float>(h)->nshifts; }
+}  // namespace
+
+extern "C" {
+
+int krylov_b200_shift_workspace_create(int solver, int m, int n, int nshifts, KrylovDataType dtype, KrylovDeviceType device,
+                                       void** ws_out) {
+  try {
+    if ((solver != KRYLOV_B200_CG_LANCZOS_SHIFT && solver != KRYLOV_B200_CGLS_LANCZOS_SHIFT) ||
+        (dtype != KRYLOV_FLOAT32 && dtype != KRYLOV_FLOAT64))
+      return -2;
+    if (device != KRYLOV_CPU && device != KRYLOV_CUDA) return fail("krylov_b200_shift_workspace_create", "unknown device");
+    if (!ws_out) return fail("krylov_b200_shift_workspace_create", "ws_out is NULL");
+    if (m < 0 || n < 0) return fail("krylov_b200_shift_workspace_create", "negative dimension");
+    if (nshifts <= 0) return fail("krylov_b200_shift_workspace_create", "nshifts must be positive");
+    if (solver == KRYLOV_B200_CG_LANCZOS_SHIFT && m != n) return fail("krylov_b200_shift_workspace_create", "System must be square");
+    const int dev = pick_device();
+    Handle* h = new Handle();
+    h->shift = true; h->p = nshifts; h->solver = solver; h->dtype = (int)dtype; h->device_kind = (int)device;
+    h->info = &kShiftSolvers[solver == KRYLOV_B200_CG_LANCZOS_SHIFT ? 0 : 1];
+    h->ext = krylov_b200_default_options();
+    try {
+      if (dtype == KRYLOV_FLOAT64) h->ws = shift_ws_create<double>((SolverKind)solver, m, n, nshifts, dev);
+      else h->ws = shift_ws_create<float>((SolverKind)solver, m, n, nshifts, dev);
+    } catch (...) { delete h; throw; }
+    {
+      std::lock_guard<std::mutex> lk(g_mu);
+      g_handles[h] = h;
+    }
+    *ws_out = h;
+    return 0;
+  } catch (const std::exception& e) { return fail("krylov_b200_shift_workspace_create", e); }
+}
+
+int krylov_b200_shift_workspace_free(void* ws) {
+  Handle* h = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(g_mu);
+    auto it = g_handles.find(ws);
+    if (it == g_handles.end() || !it->second->shift) return 1;
+    h = it->second;
+    g_handles.erase(it);
+  }
+  try {
+    destroy_any(h);
+  } catch (const std::exception& e) { fail("krylov_b200_shift_workspace_free", e); }
+  return 0;
+}
+
+int krylov_b200_shift_solve(void* ws, KrylovMatvec matvec_A, KrylovMatvec matvec_At, KrylovMatvec matvec_M, const void* b,
+                            const double* shifts, void* userdata, const KrylovOptions* opts) {
+  try {
+    Handle* h = lookup_shift(ws);
+    if (!h) return fail("krylov_b200_shift_solve", "unknown shift workspace handle");
+    return h->dtype == KRYLOV_FLOAT64 ? do_shift_solve<double>(h, matvec_A, matvec_At, matvec_M, b, shifts, userdata, opts)
+                                      : do_shift_solve<float>(h, matvec_A, matvec_At, matvec_M, b, shifts, userdata, opts);
+  } catch (const std::exception& e) { return fail("krylov_b200_shift_solve", e); }
+}
+
+int krylov_b200_shift_get_x(void* ws, int shift, void* x, int n) {
+  try {
+    Handle* h = lookup_shift(ws);
+    if (!h || !x) return fail("krylov_b200_shift_get_x", "unknown shift workspace handle or x is NULL");
+    return h->dtype == KRYLOV_FLOAT64 ? do_shift_get_x<double>(h, shift, x, n) : do_shift_get_x<float>(h, shift, x, n);
+  } catch (const std::exception& e) { return fail("krylov_b200_shift_get_x", e); }
+}
+
+int krylov_b200_shift_get_stats(void* ws, int* niter, int* solved, double* timer, char* status, int status_cap,
+                                int* indefinite, int* history_len) {
+  Handle* h = lookup_shift(ws);
+  if (!h) return fail("krylov_b200_shift_get_stats", "unknown shift workspace handle");
+  const Stats& s = stats_any(h);
+  if (niter) *niter = s.niter;
+  if (solved) *solved = s.solved;
+  if (timer) *timer = s.timer;
+  if (status && status_cap > 0) { strncpy(status, s.status.c_str(), (size_t)status_cap - 1); status[status_cap - 1] = 0; }
+  const int p = shift_count(h);
+  for (int i = 0; i < p; i++) {
+    if (indefinite) indefinite[i] = i < (int)s.shift_indefinite.size() ? s.shift_indefinite[i] : 0;
+    if (history_len) history_len[i] = i < (int)s.shift_residuals.size() ? (int)s.shift_residuals[i].size() : 0;
+  }
+  return 0;
+}
+
+int krylov_b200_shift_get_history(void* ws, int shift, double* out, int cap) {
+  Handle* h = lookup_shift(ws);
+  if (!h) return fail("krylov_b200_shift_get_history", "unknown shift workspace handle");
+  if (!out || cap < 0 || shift < 0 || shift >= shift_count(h))
+    return fail("krylov_b200_shift_get_history", "bad arguments (out is NULL, cap < 0 or shift out of range)");
+  const Stats& s = stats_any(h);
+  if (shift >= (int)s.shift_residuals.size()) return 0;
+  const std::vector<double>& v = s.shift_residuals[shift];
+  const int k = std::min((int)v.size(), cap);
+  for (int i = 0; i < k; i++) out[i] = v[i];
+  return k;
 }
 
 }  // extern "C"

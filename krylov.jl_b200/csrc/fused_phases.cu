@@ -1694,6 +1694,86 @@ template <class T> void proc_divide(Ctx& c, const ProcDivBody<T>& body) {
   launch_stream<T, 0>(c, std::max(body.n1, body.out2 ? body.n2 : 0), body, NoFin());
 }
 
+// ===========================================================================
+// CG-Lanczos-shift and CGLS-Lanczos-shift  (src/cg_lanczos_shift.jl:206-268, src/cgls_lanczos_shift.jl:206-260)
+// ===========================================================================
+// The shift update both solvers share, for up to kShiftPass active shifts per launch: v is read once (the first launch
+// of an iteration may scale it by 1/beta and store it back, kdiv!(n, v, β)), then for every shift i of the launch
+// x_i += gamma_i p_i ; p_i = sigma_i v + omega_i p_i: the reference's kaxpy! and kaxpby!, operation by operation.  The
+// columns and scalars of the launch's shifts travel by value, so converged shifts cost no bytes.
+template <class T> struct ShiftUpdBody {
+  T* v; T inv_beta; int scale; int cnt;
+  T* x[kShiftPass]; T* p[kShiftPass];
+  T gamma[kShiftPass], sigma[kShiftPass], omega[kShiftPass];
+  __device__ __forceinline__ void operator()(int j, T*) const {
+    T vj = v[j];
+    if (scale) { vj = mul_rn(inv_beta, vj); v[j] = vj; }
+#pragma unroll
+    for (int i = 0; i < kShiftPass; i++) {
+      if (i < cnt) {
+        const T pi = p[i][j];
+        x[i][j] = add_rn(x[i][j], mul_rn(gamma[i], pi));
+        p[i][j] = add_rn(mul_rn(sigma[i], vj), mul_rn(omega[i], pi));
+      }
+    }
+  }
+};
+template <class T>
+void shift_fused_update(Workspace<T>& ws, T* v, bool scale, T beta, int cnt, T* const* x, T* const* p, const T* gamma,
+                        const T* sigma, const T* omega) {
+  // with no active shift a requested scaling still runs (a pass over v alone), so v leaves every iteration scaled
+  for (int base = 0; base < cnt || (base == 0 && scale); base += kShiftPass) {
+    ShiftUpdBody<T> body{};
+    body.v = v; body.inv_beta = T(1) / beta; body.scale = (scale && base == 0) ? 1 : 0;
+    body.cnt = std::min(kShiftPass, cnt - base);
+    for (int i = 0; i < kShiftPass; i++) {
+      const bool live = base + i < cnt;
+      const int k = live ? base + i : std::max(cnt - 1, 0);
+      body.x[i] = cnt > 0 ? x[k] : v; body.p[i] = cnt > 0 ? p[k] : v;     // not read unless live
+      body.gamma[i] = live ? gamma[k] : T(0); body.sigma[i] = live ? sigma[k] : T(0); body.omega[i] = live ? omega[k] : T(0);
+    }
+    launch_stream<T, 0>(ws.ctx, ws.n, body, NoFin());
+  }
+}
+
+// The Golub-Kahan-like half of CGLS-Lanczos-shift, M = I, A and A^T CSR operators.  The u vectors stay unscaled until
+// read: ws.u holds ũ_k = β_k u_k, and the u pass forms u_k = (1/β_k) ũ_k, the reference's kdiv!(m, u_next, β) of the
+// previous iteration, with the same product.
+template <class T> struct ShiftGkState { T uu, vv; };
+template <class T> struct ShiftGkAvEpi {           // u_next = A v ; <u_next, u_next>
+  T* un;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const { un[row] = acc; d[0] += acc * acc; }
+};
+template <class T> struct ShiftGkUBody {           // u_k = s_u ũ_k ; u_next -= delta u_k ; u_next -= beta u_prev ; u_prev = u_k
+  T* un; const T* ut; T* up; T s_u; T delta; T beta;
+  __device__ __forceinline__ void operator()(int j, T*) const {
+    const T uk = mul_rn(s_u, ut[j]);
+    T t = add_rn(un[j], mul_rn(-delta, uk));
+    t = add_rn(t, mul_rn(-beta, up[j]));
+    un[j] = t;
+    up[j] = uk;
+  }
+};
+template <class T> struct ShiftGkAtuEpi {          // v = A^T u_next ; <v, v>
+  T* v;
+  __device__ __forceinline__ void operator()(int row, T acc, T* d) const { v[row] = acc; d[0] += acc * acc; }
+};
+template <class T> struct ShiftGkFin {
+  T* dst;
+  __device__ void operator()(const T* tot) const { *dst = tot[0]; }
+};
+template <class T> T shift_gk_delta(Workspace<T>& ws, const Csr<T>& A) {
+  StateBlock<ShiftGkState, T> sb(ws);
+  launch_spmv_epi<T, 1>(ws.ctx, A, ws.v, ShiftGkAvEpi<T>{ws.u_next}, ShiftGkFin<T>{&sb.dev->uu});
+  return sb.read().uu;
+}
+template <class T> T shift_gk_next(Workspace<T>& ws, const Csr<T>& At, T s_u, T delta, T beta) {
+  StateBlock<ShiftGkState, T> sb(ws);
+  launch_stream<T, 0>(ws.ctx, ws.m, ShiftGkUBody<T>{ws.u_next, ws.u, ws.u_prev, s_u, delta, beta}, NoFin());
+  launch_spmv_epi<T, 1>(ws.ctx, At, ws.u_next, ShiftGkAtuEpi<T>{ws.v}, ShiftGkFin<T>{&sb.dev->vv});
+  return sb.read().vv;
+}
+
 int gmres_fused_max() { return kGmresMaxFused; }
 
 #define INST(T)                                                                                                      \
@@ -1741,7 +1821,10 @@ int gmres_fused_max() { return kGmresMaxFused; }
   template void crmr_fused_iteration<T>(Workspace<T>&, const Csr<T>&, const Csr<T>&, bool, T, T*, T*);          \
   template void proc_spmv<T>(Ctx&, const Csr<T>&, const T*, const T*, const ProcEpi<T>&, const ProcFin<T>&);       \
   template void proc_stream<T>(Ctx&, int, const ProcUpdBody<T>&, const ProcFin<T>&);                                \
-  template void proc_divide<T>(Ctx&, const ProcDivBody<T>&);
+  template void proc_divide<T>(Ctx&, const ProcDivBody<T>&);                                                         \
+  template void shift_fused_update<T>(Workspace<T>&, T*, bool, T, int, T* const*, T* const*, const T*, const T*, const T*); \
+  template T shift_gk_delta<T>(Workspace<T>&, const Csr<T>&);                                                        \
+  template T shift_gk_next<T>(Workspace<T>&, const Csr<T>&, T, T, T);
 INST(double)
 INST(float)
 #undef INST

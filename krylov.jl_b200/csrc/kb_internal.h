@@ -208,6 +208,8 @@ struct Stats {
   std::vector<double> err_lbnds, err_ubnds_lq, err_ubnds_cg;
   bool solved_primal = false, solved_dual = false;   // AdjointStats (bilqr!, trilqr!): residuals holds residuals_primal
   std::vector<double> residuals_dual;
+  std::vector<std::vector<double>> shift_residuals;  // LanczosShiftStats (cg_lanczos_shift!, cgls_lanczos_shift!):
+  std::vector<unsigned char> shift_indefinite;       // one history and one flag per shift
   std::string status = "unknown";
   void reset() {
     residuals.clear(); Aresiduals.clear(); Acond.clear(); indefinite = false; npcCount = 0;
@@ -219,7 +221,8 @@ struct Stats {
 // values of KrylovSolverType (interfaces/include/krylov.h:48-83); cg_lanczos has no slot in the reference's C enum
 enum SolverKind { S_CG = 0, S_CR = 1, S_MINRES = 3, S_DIOM = 5, S_DQGMRES = 6, S_FOM = 7, S_GMRES = 8, S_FGMRES = 9, S_BICGSTAB = 10,
                   S_CGS = 11, S_BILQ = 12, S_QMR = 13, S_TRILQR = 18, S_BILQR = 19, S_LSLQ = 20, S_LSQR = 21, S_LSMR = 22, S_CGLS = 24, S_CRLS = 25,
-                  S_CGNE = 26, S_CRMR = 27, S_CRAIG = 28, S_CRAIGMR = 29, S_LNLQ = 30, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100 };
+                  S_CGNE = 26, S_CRMR = 27, S_CRAIG = 28, S_CRAIGMR = 29, S_LNLQ = 30, S_CAR = 32, S_MINARES = 33, S_CG_LANCZOS = 100,
+                  S_CG_LANCZOS_SHIFT = 101, S_CGLS_LANCZOS_SHIFT = 102 };   // the shift solvers: their own handle kind
 // The interface facts of each solver the C ABI serves, one row per SolverKind (capi.cu reads them; ws_create `rect`).
 enum PrecondUse : unsigned char {
   P_ON_N,        // takes the preconditioner on the n-dimensional space (the square solvers: n = m)
@@ -357,6 +360,9 @@ struct Workspace {
                                        // CRLS: Ar (n), Ms in Mr (m, lazy) (+ x, p, q: n; r, Ap, s: m)
                                        // CGNE: Aᴴz in Ar (+ x, p: n; r, q: m; s, z: m, lazy)
                                        // CRMR: Aᴴr in Ar, Nq in z (m, lazy) (+ x, p: n; r, q: m; s: m, lazy)
+  T *Xs = nullptr, *Ps = nullptr;      // shift solvers: x_i and p_i, column-major n x nshifts blocks
+  T *u_next = nullptr;                 // CGLS-Lanczos-shift (+ v: n; u_prev, u: m)
+  int nshifts = 0;
   std::vector<T*> V;
   std::vector<T*> Z;                   // FGMRES: Z[k] = N_k V[k];  DQGMRES / DIOM: the direction stack P
   std::vector<T> c, sgiv, zg, R;       // GMRES host-side Givens data
@@ -423,6 +429,14 @@ template <class T> void cr_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b
 template <class T> void car_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
 // minares! takes no preconditioner (the reference refuses M != I); o.lambda shifts A, o.axtol holds its Artol
 template <class T> void minares_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const LinOp<T>& M, const SolveOpts& o);
+// The shift solvers (shift.cu): one Lanczos process for the p systems (A + σᵢ I) xᵢ = b (CG-Lanczos-shift, M on
+// the n-space) or (AᵀA + σᵢ I) xᵢ = Aᵀb (CGLS-Lanczos-shift, no M; At: A^T as a CSR operator or a callback m -> n).
+// Their workspace holds X and P (n x nshifts) besides the Lanczos vectors; stats.shift_* the per-shift results.
+template <class T> Workspace<T>* shift_ws_create(SolverKind kind, int m, int n, int nshifts, int device);
+template <class T> void cg_lanczos_shift_solve(Workspace<T>& ws, const LinOp<T>& A, const T* b, const T* shifts,
+                                               const LinOp<T>& M, const SolveOpts& o);
+template <class T> void cgls_lanczos_shift_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b,
+                                                 const T* shifts, const SolveOpts& o);
 // Least squares on an m x n operator (lsq.cu).  At: the adjoint (a CSR operator holding A^T, or a callback m -> n).
 template <class T> void lsqr_solve(Workspace<T>& ws, const LinOp<T>& A, const LinOp<T>& At, const T* b, const LinOp<T>& M,
                                    const LinOp<T>& N, const SolveOpts& o);
@@ -507,6 +521,15 @@ template <class T> void cgs_fused_directions(Workspace<T>& ws, T beta);
 template <class T> T lanczos_fused_delta(Workspace<T>& ws, const Csr<T>& A);
 template <class T> T lanczos_fused_recur(Workspace<T>& ws, T delta, T beta, bool later);
 template <class T> void lanczos_fused_update(Workspace<T>& ws, T beta, T gamma, T sigma, T omega);
+// Shift solvers (fused_phases.cu).  The shift update of cnt active shifts (columns x[i], p[i] and their scalars), in
+// ceil(cnt / kShiftPass) streaming passes over n; `scale`: the first pass sets v = v / beta first.
+constexpr int kShiftPass = 16;
+template <class T> void shift_fused_update(Workspace<T>& ws, T* v, bool scale, T beta, int cnt, T* const* x, T* const* p,
+                                           const T* gamma, const T* sigma, const T* omega);
+// CGLS-Lanczos-shift, M = I, A and A^T CSR operators: u_next = A v, returns <u_next, u_next> (one read-back) ...
+template <class T> T shift_gk_delta(Workspace<T>& ws, const Csr<T>& A);
+// ... then u_k = s_u ũ_k, u_next -= delta u_k + beta u_prev, u_prev = u_k over m, and v = A^T u_next; returns <v, v>.
+template <class T> T shift_gk_next(Workspace<T>& ws, const Csr<T>& At, T s_u, T delta, T beta);
 template <class T> void cr_fused_step(Workspace<T>& ws, const Csr<T>& A, T alpha, T* xx, T* rr, T* ArAr, T* rAr);
 template <class T> T cr_fused_directions(Workspace<T>& ws, T beta);
 // CAR (fused_phases.cu), M = I.  C1: x += alpha p ; r -= alpha q ; s -= alpha u, one read-back of ||r||^2, ||s||^2.

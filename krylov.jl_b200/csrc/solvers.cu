@@ -126,7 +126,7 @@ template <class T> void ws_destroy(Workspace<T>* ws) {
   T* vecs[] = {ws->x, ws->dx, ws->r, ws->p, ws->Ap, ws->z, ws->npc_dir, ws->p2, ws->v, ws->s, ws->qd, ws->t, ws->yz,
                ws->r1, ws->r2, ws->w1, ws->w2, ws->y, ws->vv, ws->w, ws->q, ws->pp, ws->bbuf, ws->cbuf,
                ws->u, ws->ts, ws->vw, ws->Mv, ws->Mv_prev, ws->Mv_next, ws->Nv, ws->Mu, ws->Av, ws->Atu, ws->h, ws->hbar,
-               ws->Ar, ws->Mr, ws->u_prev, ws->v_prev, ws->d1, ws->d2, ws->dy};
+               ws->Ar, ws->Mr, ws->u_prev, ws->v_prev, ws->d1, ws->d2, ws->dy, ws->Xs, ws->Ps, ws->u_next};
   for (T* p : vecs) dev_free(p);
   for (T* p : ws->V) dev_free(p);
   for (T* p : ws->Z) dev_free(p);

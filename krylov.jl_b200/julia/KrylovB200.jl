@@ -699,6 +699,92 @@ function Krylov.block_gmres!(ws::Krylov.BlockGmresWorkspace{T,T,B200Vector{T},B2
   Krylov.block_gmres!(ws, A, B; kw...)
 end
 
+# ---- cg_lanczos_shift! / cgls_lanczos_shift! (src/cg_lanczos_shift.jl, src/cgls_lanczos_shift.jl): one shift handle per
+# workspace (include/krylov_b200.h, krylov_b200_shift_*), one krylov_b200_shift_solve per solve; ws.x[i] is filled by a
+# device-to-device copy and the LanczosShiftStats by one stats call and one history call per shift.
+const SHIFT_ID = Dict(:cg_lanczos_shift => 101, :cgls_lanczos_shift => 102)
+function shift_handle_for(method::Symbol, ws, A::B200CSR{T}, nshifts::Int) where T
+  h = get(HANDLES, ws, nothing)
+  if h === nothing
+    out = Ref{Ptr{Cvoid}}(C_NULL)
+    rc = ccall((:krylov_b200_shift_workspace_create, lib), Cint, (Cint, Cint, Cint, Cint, Cint, Cint, Ptr{Ptr{Cvoid}}),
+               SHIFT_ID[method], A.m, A.n, nshifts, dtype_id(T), 1, out)                # KRYLOV_CUDA = 1
+    rc == 0 || error("krylov_b200_shift_workspace_create -> $rc: " * unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    h = Handle(out[], C_NULL, false)
+    finalizer(x -> (x.ptr != C_NULL && ccall((:krylov_b200_shift_workspace_free, lib), Cint, (Ptr{Cvoid},), x.ptr); x.ptr = C_NULL), h)
+    HANDLES[ws] = h
+  end
+  if h.op != A.handle
+    check(ccall((:krylov_b200_attach_csr, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, A.handle))
+    h.op = A.handle
+  end
+  h
+end
+
+function shift_solve!(method::Symbol, ws, A::B200CSR{T}, b::B200Vector{T}, shifts::AbstractVector{T}, M, ldiv::Bool,
+                      check_curvature::Bool, atol::T, rtol::T, itmax::Int, timemax::Float64, verbose::Int, history::Bool,
+                      callback) where T
+  nshifts = length(shifts)
+  nshifts == ws.nshifts || error("workspace.nshifts = $(ws.nshifts) is inconsistent with length(shifts) = $nshifts")
+  h = shift_handle_for(method, ws, A, nshifts)
+  set_precond!(h, 0, M)
+  user = Ref{Any}((callback, ws))
+  cb = @cfunction(_cb_tramp, Cint, (Ptr{Cvoid}, Ptr{Cvoid}))
+  ext = Ref(CExt(history, ldiv, NaN, NaN, 1, 0, cb, Base.unsafe_convert(Ptr{Cvoid}, user), 0, check_curvature, NaN, NaN, NaN, 0.0, NaN, 0, 1))
+  o = Ref(COpts(atol, rtol, itmax, verbose, 0.0, NaN, NaN, isinf(timemax) ? NaN : timemax, 0.0, false, false, false))
+  sh = Cdouble.(shifts)
+  GC.@preserve user ext o sh begin
+    check(ccall((:krylov_b200_set_options, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.ptr, ext))
+    rc = ccall((:krylov_b200_shift_solve, lib), Cint,
+               (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cdouble}, Ptr{Cvoid}, Ptr{Cvoid}),
+               h.ptr, C_NULL, C_NULL, C_NULL, b.ptr, sh, C_NULL, o)
+    rc == 0 || error(unsafe_string(ccall((:krylov_b200_last_error, lib), Cstring, ())))
+    for i in 1:nshifts
+      check(ccall((:krylov_b200_shift_get_x, lib), Cint, (Ptr{Cvoid}, Cint, Ptr{Cvoid}, Cint), h.ptr, i - 1, ws.x[i].ptr, A.n))
+    end
+  end
+  niter, solved, timer = Ref{Cint}(0), Ref{Cint}(0), Ref{Cdouble}(0)
+  status = Vector{UInt8}(undef, 96)
+  indef, hlen = Vector{Cint}(undef, nshifts), Vector{Cint}(undef, nshifts)
+  check(ccall((:krylov_b200_shift_get_stats, lib), Cint,
+              (Ptr{Cvoid}, Ptr{Cint}, Ptr{Cint}, Ptr{Cdouble}, Ptr{UInt8}, Cint, Ptr{Cint}, Ptr{Cint}),
+              h.ptr, niter, solved, timer, status, 96, indef, hlen))
+  st = ws.stats                                   # LanczosShiftStats (src/krylov_stats.jl:169-179)
+  st.niter = niter[]; st.solved = solved[] != 0; st.timer = timer[]
+  z = findfirst(==(0x00), status)
+  st.status = String(status[1:(z === nothing ? length(status) : z - 1)])
+  for i in 1:nshifts
+    st.indefinite[i] = indef[i] != 0
+    buf = Vector{Cdouble}(undef, hlen[i])
+    got = hlen[i] == 0 ? 0 : ccall((:krylov_b200_shift_get_history, lib), Cint, (Ptr{Cvoid}, Cint, Ptr{Cdouble}, Cint),
+                                   h.ptr, i - 1, buf, hlen[i])
+    empty!(st.residuals[i]); append!(st.residuals[i], T.(buf[1:got]))
+  end
+  ws
+end
+
+# keywords: def_kwargs_cg_lanczos_shift (src/cg_lanczos_shift.jl:89-99)
+function Krylov.cg_lanczos_shift!(ws::Krylov.CgLanczosShiftWorkspace{T,T,B200Vector{T}}, A::B200CSR{T}, b::B200Vector{T},
+                                  shifts::AbstractVector{T}; M = I, ldiv::Bool = false, check_curvature::Bool = false,
+                                  atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0, timemax::Float64 = Inf,
+                                  verbose::Int = 0, history::Bool = false, callback = workspace -> false,
+                                  iostream::IO = stdout) where T
+  A.m == A.n || error("System must be square")
+  length(b) == A.n || error("Inconsistent problem size")
+  shift_solve!(:cg_lanczos_shift, ws, A, b, shifts, M, ldiv, check_curvature, atol, rtol, itmax, timemax, verbose, history, callback)
+end
+
+# keywords: def_kwargs_cgls_lanczos_shift (src/cgls_lanczos_shift.jl:91-100); M other than I is refused by the library
+function Krylov.cgls_lanczos_shift!(ws::Krylov.CglsLanczosShiftWorkspace{T,T,B200Vector{T},B200Vector{T}}, A::B200CSR{T},
+                                    b::B200Vector{T}, shifts::AbstractVector{T}; M = I, ldiv::Bool = false,
+                                    atol::T = √eps(T), rtol::T = √eps(T), itmax::Int = 0, timemax::Float64 = Inf,
+                                    verbose::Int = 0, history::Bool = false, callback = workspace -> false,
+                                    iostream::IO = stdout) where T
+  M === I || error("Preconditioner `M` is not supported.")
+  length(b) == A.m || error("Inconsistent problem size")
+  shift_solve!(:cgls_lanczos_shift, ws, A, b, shifts, M, ldiv, false, atol, rtol, itmax, timemax, verbose, history, callback)
+end
+
 # ---- Krylov processes (src/krylov_processes.jl): one kb200_<process> call each, every step enqueued on the GPU with the
 # coefficients kept on the device and read back once (DESIGN.md §3i).  Bases come back as B200Matrix{T} (column-major,
 # k + 1 columns), T / Tᴴ / L as SparseMatrixCSC{T,Int} with the reference's colptr / rowval, H as a dense Matrix{T}.

@@ -750,6 +750,191 @@ def block_gmres_(ws: BlockGmresWorkspace, A, B, X0=None, **kw):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# The shift solvers: one Lanczos process for p shifted systems, p solutions (their own handle kind in the C ABI).
+# ---------------------------------------------------------------------------------------------------------------------
+@dataclass
+class LanczosShiftStats:
+    """src/krylov_stats.jl:169-179: one residual history (`residuals`) and one `indefinite` flag per shift; Anorm and
+    Acond stay NaN, as the reference leaves them."""
+    niter: int = 0
+    solved: bool = False
+    residuals: list = field(default_factory=list)
+    indefinite: list = field(default_factory=list)
+    Anorm: float = math.nan
+    Acond: float = math.nan
+    allocation_timer: float = 0.0
+    timer: float = 0.0
+    status: str = "unknown"
+
+
+_SHIFT_KW = dict(M=None, ldiv=False, atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False,
+                 callback=None, fused=True)
+
+
+class _ShiftWorkspace(KrylovWorkspace):
+    """Workspace of a shift solver: X and P hold n x nshifts entries besides the Lanczos vectors."""
+
+    solver_id = 0
+    rect = False            # A is m x n and its adjoint is applied (CGLS-Lanczos-shift)
+    keywords = _SHIFT_KW
+
+    def __init__(self, m, n, nshifts, dtype=np.float64, *, device: str = "host"):
+        self.m, self.n, self.nshifts = int(m), int(n), int(nshifts)
+        self.dtype = np.dtype(dtype)
+        self.device = device
+        self._keep = []
+        self._cb = None
+        self._h = C.c_void_p()
+        rc = lib().krylov_b200_shift_workspace_create(self.solver_id, self.m, self.n, self.nshifts, _dtype_id(self.dtype),
+                                                      KRYLOV_CUDA if device == "cuda" else KRYLOV_CPU, C.byref(self._h))
+        if rc != 0:
+            raise B200Error(f"krylov_b200_shift_workspace_create({self.solver}) -> {rc}: {_lib.last_error()}")
+        self._ext = lib().krylov_b200_default_options()
+        self._op_id = None
+
+    def free(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            lib().krylov_b200_shift_workspace_free(self._h)
+            self._h = C.c_void_p()
+
+    def solve(self, A, b, shifts, **kw):
+        """solver!(ws, A, b, shifts; kwargs...): the keywords of the class's `keywords`.  A: a SciPy matrix, a
+        CsrOperator or a (rowptr, colind, values) tuple; or a host callable (CG-Lanczos-shift), a LinearOperator or a
+        (matvec, rmatvec) pair (CGLS-Lanczos-shift).  M: None, a 1-D diagonal, (nblocks, bs, bs) block-Jacobi blocks or
+        a host callable (CG-Lanczos-shift only)."""
+        name = self.solver
+        if kw.keys() - self.keywords.keys():
+            raise B200Error(f"{name}!: unsupported keyword argument(s) {', '.join(sorted(kw.keys() - self.keywords.keys()))}")
+        kw = {**self.keywords, **kw}
+        M, callback = kw.pop("M"), kw.pop("callback")
+        shifts = np.ascontiguousarray(shifts.cpu().numpy() if _is_torch(shifts) else shifts, dtype=np.float64).ravel()
+        if shifts.shape[0] != self.nshifts:
+            raise B200Error(f"workspace.nshifts = {self.nshifts} is inconsistent with length(shifts) = {shifts.shape[0]}")
+        if self.rect and M is not None:
+            raise B200Error("Preconditioner `M` is not supported.")
+        o, e = _options(kw, self.keywords)
+        keep = [self._set_options(e, callback)]
+        m, n = self.m, self.n
+        fA = fAt = fM = None
+        if self.rect:
+            if hasattr(A, "matvec") and hasattr(A, "rmatvec") and not isinstance(A, CsrOperator):   # LinearOperator
+                A = (A.matvec, A.rmatvec)
+            if isinstance(A, tuple) and len(A) == 2 and all(callable(f) for f in A):
+                fA, fAt = self._wrap(A[0], n, m), self._wrap(A[1], m, n)
+        elif callable(A) and not hasattr(A, "shape"):
+            fA = self._wrap(A, n, n)
+        if fA is None and A is not None:
+            self.set_operator(A)
+        if callable(M) and not hasattr(M, "shape"):
+            fM = self._wrap(M, n, n)
+            self._set_diag(0, None)
+        else:
+            self._set_diag(0, M)
+        keep += [fA, fAt, fM]
+        if not _is_torch(b):
+            b = np.ascontiguousarray(b, dtype=self.dtype)
+            if self.device == "cuda":
+                raise B200Error("ktypeof(b) must be a device vector for a device workspace")
+        elif self.device != "cuda":
+            raise B200Error("ktypeof(b) must be a host vector for a host workspace")
+        if b.shape[0] != m:
+            raise B200Error("Inconsistent problem size")
+        pb, kb_ = _ptr(b)
+        self._order_after(kb_)
+        null = _lib.MATVEC()
+        sh = (C.c_double * self.nshifts)(*shifts.tolist())
+        rc = lib().krylov_b200_shift_solve(self._h, fA or null, fAt or null, fM or null, pb, sh, None, C.byref(o))
+        del keep
+        if self._cb_error is not None:
+            raise self._cb_error
+        if rc != 0:
+            raise B200Error(_lib.last_error())
+        return self
+
+    @property
+    def x(self):
+        """solution(ws): the nshifts solutions, host arrays (or torch CUDA tensors for device workspaces)."""
+        out = []
+        for i in range(self.nshifts):
+            if self.device == "cuda":
+                import torch
+                xi = torch.empty(self.n, dtype=torch.float64 if self.dtype == np.float64 else torch.float32, device="cuda")
+                p = C.c_void_p(xi.data_ptr())
+            else:
+                xi = np.empty(self.n, dtype=self.dtype)
+                p = xi.ctypes.data_as(C.c_void_p)
+            if lib().krylov_b200_shift_get_x(self._h, i, p, self.n) != 0:
+                raise B200Error(_lib.last_error())
+            out.append(xi)
+        return out
+
+    @property
+    def stats(self) -> LanczosShiftStats:
+        p = self.nshifts
+        niter, solved, timer = C.c_int(), C.c_int(), C.c_double()
+        status = C.create_string_buffer(96)
+        indef, hlen = (C.c_int * p)(), (C.c_int * p)()
+        if lib().krylov_b200_shift_get_stats(self._h, C.byref(niter), C.byref(solved), C.byref(timer), status, 96, indef,
+                                             hlen) != 0:
+            raise B200Error(_lib.last_error())
+        res = []
+        for i in range(p):
+            buf = (C.c_double * max(hlen[i], 1))()
+            k = lib().krylov_b200_shift_get_history(self._h, i, buf, hlen[i])
+            res.append(list(buf[:max(k, 0)]))
+        s = KrylovB200Stats()
+        lib().krylov_b200_get_stats(self._h, C.byref(s))
+        return LanczosShiftStats(niter.value, bool(solved.value), res, [bool(v) for v in indef], math.nan, math.nan,
+                                 s.allocation_timer, timer.value, status.value.decode("utf-8"))
+
+
+class CgLanczosShiftWorkspace(_ShiftWorkspace):
+    """CgLanczosShiftWorkspace(m, n, nshifts, dtype) (src/krylov_workspaces.jl:604-660): cg_lanczos_shift! solves
+    (A + σᵢ I) xᵢ = b for every shift σᵢ with one Lanczos process; m == n."""
+    solver, solver_id = "cg_lanczos_shift", _lib.KRYLOV_B200_CG_LANCZOS_SHIFT
+    keywords = dict(_SHIFT_KW, check_curvature=False)
+
+
+class CglsLanczosShiftWorkspace(_ShiftWorkspace):
+    """CglsLanczosShiftWorkspace(m, n, nshifts, dtype): cgls_lanczos_shift! solves (AᵀA + σᵢ I) xᵢ = Aᵀb for every
+    shift σᵢ, A m x n (b: m entries, xᵢ: n); no preconditioner."""
+    solver, solver_id, rect = "cgls_lanczos_shift", _lib.KRYLOV_B200_CGLS_LANCZOS_SHIFT, True
+
+
+def _make_shift(name, cls):
+    def inplace(ws, A, b, shifts, **kw):
+        if ws.solver != name:
+            raise B200Error(f"{name}! needs a {cls.__name__}")
+        return ws.solve(A, b, shifts, **kw)
+
+    def outofplace(A, b, shifts, **kw):
+        n = _columns(name, A, kw.pop("n", None)) if cls.rect else b.shape[0]
+        if _is_torch(b):
+            import torch
+            dt = {torch.float32: np.float32, torch.float64: np.float64}.get(b.dtype, np.float64)
+        else:
+            dt = np.asarray(b).dtype
+        if dt not in (np.float32, np.float64):
+            dt = np.float64
+        ws = cls(b.shape[0], int(n), len(shifts), dt, device="cuda" if _is_torch(b) else "host")
+        try:
+            ws.solve(A, b, shifts, **kw)
+            return ws.x, ws.stats
+        finally:
+            ws.free()
+    inplace.__name__, outofplace.__name__ = name + "_", name
+    inplace.__doc__ = f"{name}!(workspace, A, b, shifts; kwargs...)"
+    outofplace.__doc__ = f"(xs, stats) = {name}(A, b, shifts; kwargs...): xs holds one solution per shift"
+    return inplace, outofplace
+
+
+cg_lanczos_shift_, cg_lanczos_shift = _make_shift("cg_lanczos_shift", CgLanczosShiftWorkspace)
+cgls_lanczos_shift_, cgls_lanczos_shift = _make_shift("cgls_lanczos_shift", CglsLanczosShiftWorkspace)
+__all__ += ["LanczosShiftStats", "CgLanczosShiftWorkspace", "CglsLanczosShiftWorkspace", "cg_lanczos_shift",
+            "cg_lanczos_shift_", "cgls_lanczos_shift", "cgls_lanczos_shift_"]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # The solvers: one row each.  The workspace class, solver! and solver of every row are made from it below.
 # ---------------------------------------------------------------------------------------------------------------------
 _COMMON = dict(atol=None, rtol=None, itmax=0, timemax=math.inf, verbose=0, history=False, callback=None, fused=True,

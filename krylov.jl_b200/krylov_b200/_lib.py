@@ -25,6 +25,8 @@ SOLVER_IDS = {"lslq": KRYLOV_LSLQ, "lsqr": KRYLOV_LSQR, "lsmr": KRYLOV_LSMR, "cg
               "cr": KRYLOV_CR, "diom": KRYLOV_DIOM, "dqgmres": KRYLOV_DQGMRES, "bilq": 12, "qmr": 13,
               "car": 32, "minares": 33, "trilqr": 18, "bilqr": 19, "craig": 28, "craigmr": 29, "lnlq": 30,
               "cgne": 26, "crmr": 27}
+# the shift solvers have their own handle kind (krylov_b200_shift_workspace_create), outside SOLVER_IDS
+KRYLOV_B200_CG_LANCZOS_SHIFT, KRYLOV_B200_CGLS_LANCZOS_SHIFT = 101, 102
 
 MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p)
 BLOCK_MATVEC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p)
@@ -151,6 +153,13 @@ SIGNATURES = {
     "kb200_golub_kahan": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, C.POINTER(_D), C.POINTER(_D), _I]),
     "kb200_nonhermitian_lanczos": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P] + [C.POINTER(_D)] * 4 + [_I]),
     "kb200_saunders_simon_yip": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P] + [C.POINTER(_D)] * 4 + [_I]),
+    "krylov_b200_shift_workspace_create": (_I, [_I, _I, _I, _I, _I, _I, C.POINTER(_P)]),
+    "krylov_b200_shift_workspace_free": (_I, [_P]),
+    "krylov_b200_shift_solve": (_I, [_P, MATVEC, MATVEC, MATVEC, _P, C.POINTER(_D), _P, C.POINTER(KrylovOptions)]),
+    "krylov_b200_shift_get_x": (_I, [_P, _I, _P, _I]),
+    "krylov_b200_shift_get_stats": (_I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_D), C.c_char_p, _I, C.POINTER(_I),
+                                         C.POINTER(_I)]),
+    "krylov_b200_shift_get_history": (_I, [_P, _I, C.POINTER(_D), _I]),
 }
 
 _LIB = None
